@@ -751,8 +751,8 @@ int tbvh_build_tlas( tbvh_bvh t, const void* instances, uint32_t inst_stride, ui
 		{ tbvh_set_error( "TLAS: BLAS %u holds no triangle tree (IntersectTLAS walks LAYOUT_BVH BLASses, tiny_bvh.h:3341; traverse_tlas.cl CWBVH ones)", k ); return TBVH_E_STATE; }
 		if (has_bvh && b->info.max_depth + 1 > TBVH_STACK) { tbvh_set_error( "TLAS: BLAS %u has depth %u, the two-level kernel walks a BLAS with a %d-entry stack", k, b->info.max_depth, TBVH_STACK ); return TBVH_E_LIMIT; }
 		if (has_cw && b->cw_depth + 1 > 128) { tbvh_set_error( "TLAS: the wide tree of BLAS %u has depth %u (128 pending node groups per ray, tiny_bvh.h:7048)", k, b->cw_depth ); return TBVH_E_LIMIT; }
-		refs[k].trav = has_bvh ? b->d_trav : 0, refs[k].tris = has_bvh ? b->d_leaf_tris : 0, refs[k].root_ref = b->root_ref, refs[k].root_count = b->root_count, refs[k].pad0 = refs[k].pad1 = 0;
-		refs[k].cw_nodes = has_cw ? b->d_cw_trav : 0, refs[k].cw_tris = has_cw ? b->d_cw_tris : 0;
+		refs[k].trav = has_bvh ? b->d_trav : 0, refs[k].tris = has_bvh ? b->d_leaf_tris : 0, refs[k].root_ref = b->root_ref, refs[k].root_count = b->root_count, refs[k].pad1 = 0;
+		refs[k].cw_nodes = has_cw ? b->d_cw_trav : 0, refs[k].cw_tris = has_cw ? b->d_cw_tris : 0, refs[k].cw_rd_limit = has_cw ? b->cw_rd_limit : -1.0f;
 		blas_layouts &= (has_bvh ? 1u << TBVH_LAYOUT_BVH : 0u) | (has_cw ? 1u << TBVH_LAYOUT_CWBVH : 0u);
 	}
 	for (uint32_t i = 0; i < inst_count; i++)

@@ -94,6 +94,7 @@ struct tbvh_bvh_t
 	float4* d_cw_tris = 0;     // 3 float4 per triangle
 	float4* d_cw_trav = 0;     // traversal nodes derived from d_cw_nodes (trace_cwbvh.cu cw_make_trav): 10 float4 per node
 	uint32_t cw_depth = 0;     // depth of the wide tree (root = 0)
+	float cw_rd_limit = -1.0f; // rays with |rD| up to this (and |O| <= 2^126) take the integer-ordered slab test (cw_walk.cuh cw_ray_fits); < 0: none
 	uint32_t generation = 0;   // renewed (tbvh_next_generation) whenever the arrays a TLAS may point at are replaced (build, upload, refit, convert)
 	// TLAS (BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) :2221): nodes / primIdx over instance boxes + device tables
 	float4* d_aabbs = 0;       // instance boxes the TLAS was built over (2 float4 per instance)
@@ -149,7 +150,7 @@ int build_hq_launch( tbvh_bvh b, float c_trav, float c_int );
 int refit_launch( tbvh_bvh b, cudaStream_t s );
 int tlas_trace_launch( tbvh_bvh b, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s );
 struct TlasInst { float inv[16]; uint32_t blasIdx, mask, pad0, pad1; };                                  // 80 bytes
-struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root_count, pad0, pad1; const float4* cw_nodes; const float4* cw_tris; }; // 48 bytes: BVH-layout arrays, CWBVH traversal nodes + bvh8Tris (0 when absent)
+struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root_count; float cw_rd_limit; uint32_t pad1; const float4* cw_nodes; const float4* cw_tris; }; // 48 bytes: BVH-layout arrays, CWBVH traversal nodes + bvh8Tris (0 when absent) and their rD limit
 int make_leaf_tris( tbvh_bvh b, cudaStream_t s );
 int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used_nodes_gpu, cudaStream_t s );
 int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s );

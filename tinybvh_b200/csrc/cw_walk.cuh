@@ -28,12 +28,22 @@ __device__ __forceinline__ float2 fma2( const float2 a, const float2 b, const fl
 	return make_float2( __fmaf_rn( a.x, b.x, c.x ), __fmaf_rn( a.y, b.y, c.y ) );
 }
 
-// one pair of children against one ray: `near` / `far` words already chosen by the ray's signs
-__device__ __forceinline__ uint32_t pair_hits( const uint32_t wnx, const uint32_t wny, const uint32_t wnz, const uint32_t wfx, const uint32_t wfy, const uint32_t wfz,
+// one pair of children against one ray: `near` / `far` words already chosen by the ray's signs.  IORD: the slab test on the bit
+// patterns of the plane values as signed integers (cw_ray_fits states when that gives the float test's result)
+template <bool IORD> __device__ __forceinline__ uint32_t pair_hits( const uint32_t wnx, const uint32_t wny, const uint32_t wnz, const uint32_t wfx, const uint32_t wfy, const uint32_t wfz,
 	const uint32_t bits_a, const uint32_t bits_b, const float2 ax, const float2 ay, const float2 az, const float2 bx, const float2 by, const float2 bz, const float t )
 {
 	const float2 tnx = fma2( widen( wnx ), ax, bx ), tny = fma2( widen( wny ), ay, by ), tnz = fma2( widen( wnz ), az, bz );
 	const float2 tfx = fma2( widen( wfx ), ax, bx ), tfy = fma2( widen( wfy ), ay, by ), tfz = fma2( widen( wfz ), az, bz );
+	if (IORD)
+	{
+		// max( tn, +0 ) and min( tf ) in two three-input integer instructions each; `!( in > t )` lets a NaN t pass as fminf ignores it
+		const int in_a = __vimax3_s32_relu( __float_as_int( tnx.x ), __float_as_int( tny.x ), __float_as_int( tnz.x ) );
+		const int in_b = __vimax3_s32_relu( __float_as_int( tnx.y ), __float_as_int( tny.y ), __float_as_int( tnz.y ) );
+		const int out_a = __vimin3_s32( __float_as_int( tfx.x ), __float_as_int( tfy.x ), __float_as_int( tfz.x ) );
+		const int out_b = __vimin3_s32( __float_as_int( tfx.y ), __float_as_int( tfy.y ), __float_as_int( tfz.y ) );
+		return (in_a <= out_a && !(__int_as_float( in_a ) > t) ? bits_a : 0u) | (in_b <= out_b && !(__int_as_float( in_b ) > t) ? bits_b : 0u);
+	}
 	const float in_a = fmaxf( fmaxf( fmaxf( tnx.x, tny.x ), tnz.x ), 0.0f ), out_a = fminf( fminf( fminf( tfx.x, tfy.x ), tfz.x ), t );
 	const float in_b = fmaxf( fmaxf( fmaxf( tnx.y, tny.y ), tnz.y ), 0.0f ), out_b = fminf( fminf( fminf( tfx.y, tfy.y ), tfz.y ), t );
 	return (in_a <= out_a ? bits_a : 0u) | (in_b <= out_b ? bits_b : 0u);
@@ -49,19 +59,41 @@ __device__ __forceinline__ uint32_t slots_to_order( const uint32_t w, const uint
 	return top << 24;
 }
 
-// All child pairs of one node against one ray -> the node's hit word in traversal order (inner children in bits 24..31 by
-// s ^ o, triangles in bits 0..23).  OCT < 0: the ray's own signs (per lane); OCT = 0..7: every ray of the warp has negative
-// x / y / z direction components as bits 2 / 1 / 0 of OCT say - plane choice and bit order are then compile-time.
-template <int OCT> __device__ __forceinline__ uint32_t node_hits( const float4* __restrict__ np, const uint32_t pairs, const bool negx, const bool negy, const bool negz, const uint32_t o,
-	const float ax1, const float ay1, const float az1, const float bx1, const float by1, const float bz1, const float t )
+// The integer-ordered slab test (pair_hits<true>) gives the float test's result when no plane value is NaN and no far plane is -0:
+// the bit patterns of non-negative floats order as signed integers do, every negative float sorts below every non-negative one
+// (so it still fails `in <= out` against in >= +0, as in float), and the RELU's 0 is +0.  -0 is excluded by adding +0 to
+// ( p - O ) * rD (node_hits), which changes no comparison: fma( q, a, b ) is then -0 for no q.  NaN is excluded per ray and tree:
+// a plane value fma( q, 2^e * rD, ( p - O ) * rD ) with q in 0..255 is not NaN when 2^e * rD is finite and ( p - O ) * rD is not
+// NaN, which holds when |rD| <= rd_limit = 2^( 127 - largest e ) and |O|, |p| <= 2^126.  cw_make_trav finds the largest e and
+// |p| of the tree and sets rd_limit < 0 (no ray fits) for a tree that has e = -128 (2^e is stored as -inf, :7072-7074) or
+// |p| > 2^126.  A NaN running t is not excluded: `!( in > t )` passes it, as fminf( out, NaN ) ignores it.
+#define CW_ORIGIN_LIMIT 8.5070592e37f // 2^126
+__device__ __forceinline__ bool cw_ray_fits( const float ox, const float oy, const float oz, const float rdx, const float rdy, const float rdz, const float rd_limit )
 {
+	return fabsf( rdx ) <= rd_limit && fabsf( rdy ) <= rd_limit && fabsf( rdz ) <= rd_limit && // NaN fails every comparison
+		fabsf( ox ) <= CW_ORIGIN_LIMIT && fabsf( oy ) <= CW_ORIGIN_LIMIT && fabsf( oz ) <= CW_ORIGIN_LIMIT;
+}
+
+// One traversal node against one ray -> the node's hit word in traversal order (inner children in bits 24..31 by s ^ o, triangles
+// in bits 0..23).  h0 / h1: the node's header, already loaded.  OCT < 0: the ray's own signs (per lane); OCT = 0..7: every ray of
+// the warp has negative x / y / z direction components as bits 2 / 1 / 0 of OCT say - plane choice and bit order are then
+// compile-time.  IORD: the integer-ordered slab test, for rays that pass cw_ray_fits.
+template <int OCT, bool IORD> __device__ __forceinline__ uint32_t node_hits( const float4* __restrict__ np, const float4 h0, const float4 h1,
+	const float ox, const float oy, const float oz, const float rdx, const float rdy, const float rdz, const bool negx, const bool negy, const bool negz, const uint32_t o, const float t )
+{
+	// scale = 2^e as a float bit pattern, ( e + 127 ) << 23 (:7072-7074), stored by cw_make_trav as top halves
+	const uint32_t sxy = __float_as_uint( h0.w ), szm = __float_as_uint( h1.z );
+	const float scx = __uint_as_float( sxy << 16 ), scy = __uint_as_float( sxy & 0xffff0000u ), scz = __uint_as_float( szm << 16 );
+	const float ax1 = __fmul_rn( scx, rdx ), ay1 = __fmul_rn( scy, rdy ), az1 = __fmul_rn( scz, rdz );
+	// + 0: -0 becomes +0 (see cw_ray_fits)
+	const float bx1 = __fadd_rn( __fmul_rn( -__fsub_rn( ox, h0.x ), rdx ), 0.0f ), by1 = __fadd_rn( __fmul_rn( -__fsub_rn( oy, h0.y ), rdy ), 0.0f );
+	const float bz1 = __fadd_rn( __fmul_rn( -__fsub_rn( oz, h0.z ), rdz ), 0.0f );
 	const bool nx = OCT < 0 ? negx : (OCT & 4) != 0, ny = OCT < 0 ? negy : (OCT & 2) != 0, nz = OCT < 0 ? negz : (OCT & 1) != 0;
 	const float2 ax = make_float2( ax1, ax1 ), ay = make_float2( ay1, ay1 ), az = make_float2( az1, az1 );
 	const float2 bx = make_float2( bx1, bx1 ), by = make_float2( by1, by1 ), bz = make_float2( bz1, bz1 );
 	// All four pair records, unconditionally: a node visited on the way to a hit is almost always full (3.83 of 4 pair steps per visited
-	// node on Bistro camera rays), the records behind `pairs` are zero (no bits, so whatever their planes say contributes nothing), and
-	// without the four branch regions the eight loads leave together.
-	(void)pairs;
+	// node on Bistro camera rays), the records behind the node's pair count are zero (no bits, so whatever their planes say contributes
+	// nothing), and without the four branch regions the eight loads leave together.
 	float4 A[4], B[4];
 	#pragma unroll
 	for (int j = 0; j < 4; j++) A[j] = __ldg( np + 2 + 2 * j ), B[j] = __ldg( np + 3 + 2 * j );
@@ -71,7 +103,7 @@ template <int OCT> __device__ __forceinline__ uint32_t node_hits( const float4* 
 	{
 		const uint32_t lx = __float_as_uint( A[j].x ), ly = __float_as_uint( A[j].y ), lz = __float_as_uint( A[j].z );
 		const uint32_t hx = __float_as_uint( A[j].w ), hy = __float_as_uint( B[j].x ), hz = __float_as_uint( B[j].y );
-		got |= pair_hits( nx ? hx : lx, ny ? hy : ly, nz ? hz : lz, nx ? lx : hx, ny ? ly : hy, nz ? lz : hz,
+		got |= pair_hits<IORD>( nx ? hx : lx, ny ? hy : ly, nz ? hz : lz, nx ? lx : hx, ny ? ly : hy, nz ? lz : hz,
 			__float_as_uint( B[j].z ), __float_as_uint( B[j].w ), ax, ay, az, bx, by, bz, t );
 	}
 	return slots_to_order( got, OCT < 0 ? o : (uint32_t)(7 - OCT) ) | (got & 0x00ffffffu);

@@ -23,8 +23,11 @@
 //    integer-to-float on the quarter-rate unit, no magic-number subtraction).
 //  * Near / far planes are picked by the sign of rD once per pair on the packed words, inner-child bits are accumulated in slot order
 //    and moved to octant order by one 3-stage bit butterfly per node - and when every ray of a warp points into the same direction
-//    octant (camera and shadow rays), a warp-uniform switch runs the node step through the instance compiled for that octant, where
-//    both are compile-time (node_hits<OCT>).
+//    octant (camera and shadow rays), one warp-uniform switch before the walk picks the walk compiled for that octant, where both
+//    are compile-time (cw_trace<OCT>, node_hits<OCT>).
+//  * The slab test's max / min chains run on the bit patterns of the plane values as signed integers, two three-input integer
+//    min / max instructions per child (cw_walk.cuh pair_hits<true>); warps with a ray for which that could differ from the float
+//    test (cw_ray_fits) run the float test.
 //  * The per-axis scales 2^e are stored as the top halves of their float patterns: one shift or mask each instead of a byte decode.
 //
 // Triangles are the reference's 48-byte records (e2, e1, v0 | primIdx) read straight from bvh8Tris.
@@ -34,11 +37,20 @@
 // ---- bvh8Data -> traversal nodes ------------------------------------------------------------------------------------
 // One thread per node.  Slot i of the source node: meta byte i (n1.z / n1.w), quantised bounds byte i of the six 8-byte rows at
 // bytes 32..79 (lo.x, lo.y, lo.z, hi.x, hi.y, hi.z) - layout in SURVEY.md 8(a), written by BVH8_CWBVH::ConvertFrom (tiny_bvh.h:5948-6015).
-__global__ void k_cw_expand( const uint4* __restrict__ src, uint4* __restrict__ dst, uint32_t* __restrict__ parent, const uint32_t count )
+// range: max over the nodes of 128 + the largest exponent byte, or 256 for a node with e = -128 or |p| > 2^126 (cw_ray_fits)
+__global__ void k_cw_expand( const uint4* __restrict__ src, uint4* __restrict__ dst, uint32_t* __restrict__ parent, uint32_t* __restrict__ range, const uint32_t count )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= count) return;
 	const uint4 n0 = src[(size_t)x * 5], n1 = src[(size_t)x * 5 + 1], n2 = src[(size_t)x * 5 + 2], n3 = src[(size_t)x * 5 + 3], n4 = src[(size_t)x * 5 + 4];
+	{
+		const int ex = (int8_t)(n0.w & 255u), ey = (int8_t)((n0.w >> 8) & 255u), ez = (int8_t)((n0.w >> 16) & 255u);
+		const bool p_ok = fabsf( __uint_as_float( n0.x ) ) <= CW_ORIGIN_LIMIT && fabsf( __uint_as_float( n0.y ) ) <= CW_ORIGIN_LIMIT && fabsf( __uint_as_float( n0.z ) ) <= CW_ORIGIN_LIMIT;
+		const bool bad = !p_ok || ex == -128 || ey == -128 || ez == -128;
+		const uint32_t key = bad ? 256u : (uint32_t)(128 + max( ex, max( ey, ez ) ));
+		const uint32_t m = __reduce_max_sync( __activemask(), key );
+		if ((threadIdx.x & 31) == __ffs( __activemask() ) - 1) atomicMax( range, m );
+	}
 	const uint32_t row[6][2] = { { n2.x, n2.y }, { n2.z, n2.w }, { n3.x, n3.y }, { n3.z, n3.w }, { n4.x, n4.y }, { n4.z, n4.w } };
 	const uint32_t meta[2] = { n1.z, n1.w };
 	uint32_t word[4][8]; // pair records under construction
@@ -98,41 +110,101 @@ int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth )
 	if (b->d_cw_trav) cudaFree( b->d_cw_trav ), b->d_cw_trav = 0;
 	const uint32_t count = b->info.used_blocks / 5;
 	if (count == 0) { tbvh_set_error( "cw_make_trav: no CWBVH nodes" ); return TBVH_E_STATE; }
-	CUDA_TRY( cudaMalloc( &b->d_cw_trav, (size_t)count * CW_NODE_F4 * 16 ) );
-	if (known_depth >= 0)
-	{
-		k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, 0, count ); LAUNCHED();
-		b->cw_depth = (uint32_t)known_depth;
-		return TBVH_OK;
-	}
-	// uploaded data: the depth of the wide tree is not known - every node notes its parent, then walks up to the root
+	// one float4 past the nodes holds the tree's exponent / |p| range while it is found
+	CUDA_TRY( cudaMalloc( &b->d_cw_trav, ((size_t)count * CW_NODE_F4 + 1) * 16 ) );
+	uint32_t* d_range = (uint32_t*)(b->d_cw_trav + (size_t)count * CW_NODE_F4);
+	uint32_t range = 256;
+	b->cw_rd_limit = -1.0f;
+	CUDA_TRY( cudaMemsetAsync( d_range, 0, 4, s ) );
 	uint32_t* d_parent = 0;
-	CUDA_TRY( cudaMalloc( &d_parent, ((size_t)count + 1) * 4 ) );
-	uint32_t depth = 0;
+	uint32_t depth = (uint32_t)known_depth;
 	auto body = [&]() -> int
 	{
-		CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)count * 4, s ) );
-		CUDA_TRY( cudaMemsetAsync( d_parent + count, 0, 4, s ) );
-		k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_parent, count ); LAUNCHED();
-		k_cw_depth<<<(count + 127) / 128, 128, 0, s>>>( d_parent, count, d_parent + count ); LAUNCHED();
-		CUDA_TRY( cudaMemcpyAsync( &depth, d_parent + count, 4, cudaMemcpyDeviceToHost, s ) );
+		if (known_depth >= 0) k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, 0, d_range, count );
+		else
+		{
+			// uploaded data: the depth of the wide tree is not known - every node notes its parent, then walks up to the root
+			CUDA_TRY( cudaMalloc( &d_parent, ((size_t)count + 1) * 4 ) );
+			CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)count * 4, s ) );
+			CUDA_TRY( cudaMemsetAsync( d_parent + count, 0, 4, s ) );
+			k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_parent, d_range, count ); LAUNCHED();
+			k_cw_depth<<<(count + 127) / 128, 128, 0, s>>>( d_parent, count, d_parent + count );
+			CUDA_TRY( cudaMemcpyAsync( &depth, d_parent + count, 4, cudaMemcpyDeviceToHost, s ) );
+		}
+		LAUNCHED();
+		CUDA_TRY( cudaMemcpyAsync( &range, d_range, 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
 	};
 	const int rc = body();
-	cudaFree( d_parent );
+	if (d_parent) cudaFree( d_parent );
 	b->cw_depth = depth;
+	// |rD| <= 2^( 127 - largest e ) keeps 2^e * rD finite (cw_ray_fits); 2^127 at most, and no ray fits a tree that has range 256
+	if (rc == TBVH_OK && range < 256) b->cw_rd_limit = ldexpf( 1.0f, 127 - max( 0, (int)range - 128 ) );
 	return rc;
 }
 
 // ---- traversal ------------------------------------------------------------------------------------------------------
 
-// OCTSW = 1: warps whose rays all point into one direction octant (camera and shadow rays: nearly all of them) run the node step
-// through the instance compiled for that octant, picked by a warp-uniform switch; mixed warps use the per-lane form.
+// One ray's walk from the root with one instance of the node step (OCT, IORD: node_hits).  Returns true on an any-hit; closest hits
+// update t / hu / hv / hprim.
+template <bool ANYHIT, bool STATS, int OCT, bool IORD> __device__ __forceinline__ bool cw_trace( const float4* __restrict__ nodes, const float4* __restrict__ tris,
+	const float ox, const float oy, const float oz, const float dx, const float dy, const float dz, const float rdx, const float rdy, const float rdz,
+	const uint32_t o, const bool negx, const bool negy, const bool negz, float& t, float& hu, float& hv, uint32_t& hprim, uint2* pending, unsigned long long* __restrict__ stats )
+{
+	int depth = 0;
+	uint32_t base = 0, word = 0x80000000u; // the root as a one-child group: bit 31, no siblings
+	unsigned long long nsteps = 0, ntris = 0, npairs = 0;
+	bool occluded = false;
+	while (true)
+	{
+		// ---- enter the pending inner child with the highest bit
+		const uint32_t bit = 31u - __clz( word );
+		const uint32_t rest = word & ~(1u << bit);
+		if (rest > 0x00ffffffu) pending[depth++] = make_uint2( base, rest );
+		const uint32_t slot = (bit - 24u) ^ (OCT < 0 ? o : (uint32_t)(7 - OCT));
+		const uint32_t nidx = base + __popc( word & ~(0xffffffffu << slot) );
+		const float4* np = nodes + (size_t)nidx * CW_NODE_F4;
+		const float4 h0 = __ldg( np ), h1 = __ldg( np + 1 );
+		const uint32_t szm = __float_as_uint( h1.z );
+		if (STATS) nsteps++, npairs += szm >> 24;
+		const uint32_t got = node_hits<OCT, IORD>( np, h0, h1, ox, oy, oz, rdx, rdy, rdz, negx, negy, negz, o, t );
+		base = __float_as_uint( h1.x );
+		word = (got & 0xff000000u) | ((szm >> 16) & 255u);
+		// ---- triangles of the leaf children that were hit, highest bit first (:7132-7142)
+		uint32_t tmask = got & 0x00ffffffu;
+		const float4* tbase = tris + __float_as_uint( h1.y );
+		while (tmask)
+		{
+			const uint32_t k = 31u - __clz( tmask );
+			tmask &= ~(1u << k);
+			const float4* tp = tbase + k * 3;
+			const float4 e2 = __ldg( tp ), e1 = __ldg( tp + 1 ), v0 = __ldg( tp + 2 );
+			if (STATS) ntris++;
+			float tt, u, v;
+			if (mt_test( ox, oy, oz, dx, dy, dz, v0, e1, e2, t, tt, u, v ))
+			{
+				if (ANYHIT) { occluded = true; break; }
+				t = tt, hu = u, hv = v, hprim = __float_as_uint( v0.w );
+			}
+		}
+		if (ANYHIT && occluded) break;
+		if (word > 0x00ffffffu) continue;
+		if (depth == 0) break;
+		const uint2 e = pending[--depth];
+		base = e.x, word = e.y;
+	}
+	if (STATS) { atomicAdd( &stats[0], nsteps ); atomicAdd( &stats[1], ntris ); atomicAdd( &stats[2], npairs ); }
+	return occluded;
+}
+
+// OCTSW = 1: warps whose rays all point into one direction octant (camera and shadow rays: nearly all of them) walk with the
+// instance compiled for that octant, picked once per warp before the walk; mixed warps use the per-lane form.  Warps in which
+// every ray passes cw_ray_fits (rd_limit: cw_make_trav) run the integer-ordered slab test; any other warp runs the float test.
 template <bool ANYHIT, bool STATS, int OCTSW>
 __global__ void __launch_bounds__( 128 ) k_trace_wide( const float4* __restrict__ nodes, const float4* __restrict__ tris,
 	const char* rays, const uint32_t stride, char* hits, const uint32_t hit_stride, uint32_t* __restrict__ bits, const uint64_t n,
-	unsigned long long* __restrict__ stats )
+	unsigned long long* __restrict__ stats, const float rd_limit )
 {
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	bool occluded = false;
@@ -156,81 +228,35 @@ __global__ void __launch_bounds__( 128 ) k_trace_wide( const float4* __restrict_
 		const uint32_t oct0 = __shfl_sync( 0xffffffffu, oct, vm ? __ffs( vm ) - 1 : 0 );
 		uni = __all_sync( 0xffffffffu, !valid || (oct == oct0 && o == 7u - oct) );
 	}
+	const bool iord = __all_sync( 0xffffffffu, !valid || cw_ray_fits( ox, oy, oz, rdx, rdy, rdz, rd_limit ) );
 	if (valid)
 	{
 		float t = rh4.x, hu = rh4.y, hv = rh4.z;
 		uint32_t hprim = __float_as_uint( rh4.w );
 		uint2 pending[CW_STACK];
-		int depth = 0;
-		uint32_t base = 0, word = 0x80000000u; // the root as a one-child group: bit 31, no siblings
-		unsigned long long nsteps = 0, ntris = 0, npairs = 0;
-		while (true)
+		#define TRACE( O, I ) occluded = cw_trace<ANYHIT, STATS, O, I>( nodes, tris, ox, oy, oz, dx, dy, dz, rdx, rdy, rdz, o, negx, negy, negz, t, hu, hv, hprim, pending, stats )
+		if (OCTSW && uni && iord)
 		{
-			// ---- enter the pending inner child with the highest bit
-			const uint32_t bit = 31u - __clz( word );
-			const uint32_t rest = word & ~(1u << bit);
-			if (rest > 0x00ffffffu) pending[depth++] = make_uint2( base, rest );
-			const uint32_t slot = (bit - 24u) ^ o;
-			const uint32_t nidx = base + __popc( word & ~(0xffffffffu << slot) );
-			const float4* np = nodes + (size_t)nidx * CW_NODE_F4;
-			const float4 h0 = __ldg( np ), h1 = __ldg( np + 1 );
-			if (STATS) nsteps++;
-			// scale = 2^e as a float bit pattern, ( e + 127 ) << 23 (:7072-7074), stored by cw_make_trav as top halves
-			const uint32_t sxy = __float_as_uint( h0.w ), szm = __float_as_uint( h1.z );
-			const float scx = __uint_as_float( sxy << 16 ), scy = __uint_as_float( sxy & 0xffff0000u ), scz = __uint_as_float( szm << 16 );
-			const float ax1 = __fmul_rn( scx, rdx ), ay1 = __fmul_rn( scy, rdy ), az1 = __fmul_rn( scz, rdz );
-			const float bx1 = __fmul_rn( -__fsub_rn( ox, h0.x ), rdx ), by1 = __fmul_rn( -__fsub_rn( oy, h0.y ), rdy ), bz1 = __fmul_rn( -__fsub_rn( oz, h0.z ), rdz );
-			const uint32_t pairs = szm >> 24;
-			if (STATS) npairs += pairs;
-			uint32_t got;
-			#define NODE_HITS( O ) got = node_hits<O>( np, pairs, negx, negy, negz, o, ax1, ay1, az1, bx1, by1, bz1, t )
-			if (OCTSW && uni)
+			switch (oct)
 			{
-				switch (oct)
-				{
-				case 0: NODE_HITS( 0 ); break;
-				case 1: NODE_HITS( 1 ); break;
-				case 2: NODE_HITS( 2 ); break;
-				case 3: NODE_HITS( 3 ); break;
-				case 4: NODE_HITS( 4 ); break;
-				case 5: NODE_HITS( 5 ); break;
-				case 6: NODE_HITS( 6 ); break;
-				default: NODE_HITS( 7 ); break;
-				}
+			case 0: TRACE( 0, true ); break;
+			case 1: TRACE( 1, true ); break;
+			case 2: TRACE( 2, true ); break;
+			case 3: TRACE( 3, true ); break;
+			case 4: TRACE( 4, true ); break;
+			case 5: TRACE( 5, true ); break;
+			case 6: TRACE( 6, true ); break;
+			default: TRACE( 7, true ); break;
 			}
-			else NODE_HITS( -1 );
-			#undef NODE_HITS
-			base = __float_as_uint( h1.x );
-			word = (got & 0xff000000u) | ((szm >> 16) & 255u);
-			// ---- triangles of the leaf children that were hit, highest bit first (:7132-7142)
-			uint32_t tmask = got & 0x00ffffffu;
-			const float4* tbase = tris + __float_as_uint( h1.y );
-			while (tmask)
-			{
-				const uint32_t k = 31u - __clz( tmask );
-				tmask &= ~(1u << k);
-				const float4* tp = tbase + k * 3;
-				const float4 e2 = __ldg( tp ), e1 = __ldg( tp + 1 ), v0 = __ldg( tp + 2 );
-				if (STATS) ntris++;
-				float tt, u, v;
-				if (mt_test( ox, oy, oz, dx, dy, dz, v0, e1, e2, t, tt, u, v ))
-				{
-					if (ANYHIT) { occluded = true; break; }
-					t = tt, hu = u, hv = v, hprim = __float_as_uint( v0.w );
-				}
-			}
-			if (ANYHIT && occluded) break;
-			if (word > 0x00ffffffu) continue;
-			if (depth == 0) break;
-			const uint2 e = pending[--depth];
-			base = e.x, word = e.y;
 		}
+		else if (iord) TRACE( -1, true );
+		else TRACE( -1, false );
+		#undef TRACE
 		if (!ANYHIT)
 		{
 			float4* hp = (float4*)(hits + i * hit_stride);
 			*hp = make_float4( t, hu, hv, __uint_as_float( hprim ) );
 		}
-		if (STATS) { atomicAdd( &stats[0], nsteps ); atomicAdd( &stats[1], ntris ); atomicAdd( &stats[2], npairs ); }
 	}
 	if (ANYHIT)
 	{
@@ -250,7 +276,7 @@ int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d
 	if (grid > 0x7fffffffull) { tbvh_set_error( "ray batch too large for one launch" ); return TBVH_E_ARG; }
 	const int sw = b->ctx->trace_variant == 0 ? 0 : 1; // trace_variant 0: the per-lane form only (A/B switch for measurements)
 	#define LAUNCH( A, S, O ) k_trace_wide<A, S, O><<<(uint32_t)grid, block, 0, s>>>( b->d_cw_trav, b->d_cw_tris, (const char*)d_rays, stride, \
-		(char*)d_hits, hit_stride, d_bits, n, d_stats )
+		(char*)d_hits, hit_stride, d_bits, n, d_stats, b->cw_rd_limit )
 	if (anyhit) { if (d_stats) LAUNCH( true, true, 0 ); else if (sw) LAUNCH( true, false, 1 ); else LAUNCH( true, false, 0 ); }
 	else { if (d_stats) LAUNCH( false, true, 0 ); else if (sw) LAUNCH( false, false, 1 ); else LAUNCH( false, false, 0 ); }
 	#undef LAUNCH

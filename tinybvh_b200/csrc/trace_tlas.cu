@@ -82,10 +82,10 @@ template <bool ANYHIT> __device__ bool trace_blas( const BlasRef B, const float 
 	return false;
 }
 
-// one BLAS in its CWBVH layout, walked as k_trace_wide walks it (trace_cwbvh.cu) in the per-lane form.  BVH8_CWBVH::Intersect starts from
+// one BLAS in its CWBVH layout, walked as k_trace_wide walks it (trace_cwbvh.cu) in the per-lane form; IORD as node_hits.  BVH8_CWBVH::Intersect starts from
 // the running hit distance and the two-level walk keeps its result only when it ends BELOW that distance (`blasHit.x < hit.x`): a
 // triangle met at exactly the running distance changes nothing.
-template <bool ANYHIT> __device__ bool trace_blas_cw( const float4* __restrict__ nodes, const float4* __restrict__ tris, const float ox, const float oy, const float oz,
+template <bool ANYHIT, bool IORD> __device__ bool trace_blas_cw( const float4* __restrict__ nodes, const float4* __restrict__ tris, const float ox, const float oy, const float oz,
 	const float dx, const float dy, const float dz, const float rdx, const float rdy, const float rdz, float& tmax, float& hu, float& hv, uint32_t& hprim, bool& hit, uint2* pending )
 {
 	const uint32_t o = 7u - ((dx < 0 ? 4u : 0u) | (dy < 0 ? 2u : 0u) | (dz < 0 ? 1u : 0u)); // octinv (:7053, signs of D)
@@ -104,11 +104,8 @@ template <bool ANYHIT> __device__ bool trace_blas_cw( const float4* __restrict__
 		const uint32_t nidx = base + __popc( word & ~(0xffffffffu << slot) );
 		const float4* np = nodes + (size_t)nidx * CW_NODE_F4;
 		const float4 h0 = __ldg( np ), h1 = __ldg( np + 1 );
-		const uint32_t sxy = __float_as_uint( h0.w ), szm = __float_as_uint( h1.z );
-		const float scx = __uint_as_float( sxy << 16 ), scy = __uint_as_float( sxy & 0xffff0000u ), scz = __uint_as_float( szm << 16 );
-		const float ax1 = __fmul_rn( scx, rdx ), ay1 = __fmul_rn( scy, rdy ), az1 = __fmul_rn( scz, rdz );
-		const float bx1 = __fmul_rn( -__fsub_rn( ox, h0.x ), rdx ), by1 = __fmul_rn( -__fsub_rn( oy, h0.y ), rdy ), bz1 = __fmul_rn( -__fsub_rn( oz, h0.z ), rdz );
-		const uint32_t got = node_hits<-1>( np, szm >> 24, negx, negy, negz, o, ax1, ay1, az1, bx1, by1, bz1, t );
+		const uint32_t szm = __float_as_uint( h1.z );
+		const uint32_t got = node_hits<-1, IORD>( np, h0, h1, ox, oy, oz, rdx, rdy, rdz, negx, negy, negz, o, t );
 		base = __float_as_uint( h1.x );
 		word = (got & 0xff000000u) | ((szm >> 16) & 255u);
 		uint32_t tmask = got & 0x00ffffffu;
@@ -193,8 +190,12 @@ template <bool ANYHIT, bool CW> __global__ void __launch_bounds__( 128 ) k_trace
 					const float tdz = __fmaf_rn( r2.z, dz, __fmaf_rn( r2.x, dx, __fmul_rn( r2.y, dy ) ) );
 					bool hit = false;
 					const BlasRef B = blas[__float_as_uint( meta.x )];
-					const bool occ = CW ? trace_blas_cw<ANYHIT>( B.cw_nodes, B.cw_tris, tox, toy, toz, tdx, tdy, tdz, safercp( tdx ), safercp( tdy ), safercp( tdz ), tmax, hu, hv, hprim, hit, bstack )
-						: trace_blas<ANYHIT>( B, tox, toy, toz, tdx, tdy, tdz, safercp( tdx ), safercp( tdy ), safercp( tdz ), tmax, hu, hv, hprim, hit, bstack );
+					const float trdx = safercp( tdx ), trdy = safercp( tdy ), trdz = safercp( tdz );
+					bool occ;
+					if (!CW) occ = trace_blas<ANYHIT>( B, tox, toy, toz, tdx, tdy, tdz, trdx, trdy, trdz, tmax, hu, hv, hprim, hit, bstack );
+					else if (cw_ray_fits( tox, toy, toz, trdx, trdy, trdz, B.cw_rd_limit ))
+						occ = trace_blas_cw<ANYHIT, true>( B.cw_nodes, B.cw_tris, tox, toy, toz, tdx, tdy, tdz, trdx, trdy, trdz, tmax, hu, hv, hprim, hit, bstack );
+					else occ = trace_blas_cw<ANYHIT, false>( B.cw_nodes, B.cw_tris, tox, toy, toz, tdx, tdy, tdz, trdx, trdy, trdz, tmax, hu, hv, hprim, hit, bstack );
 					if (occ)
 					{
 						occluded = true;
