@@ -158,6 +158,22 @@ int tbvh_build_tlas( tbvh_bvh tlas, const void* instances, uint32_t inst_stride,
  * SBVH") or when no BVH-layout tree is resident.  Derived layouts on the handle are dropped; tbvh_convert again. */
 int tbvh_refit( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_count, int space );
 
+/* Refit that keeps the derived layouts: tbvh_refit's BVH::Refit, then every layout the handle holds brought up to date in place
+ * instead of dropped, with the same arguments.
+ *  - BVH_GPU: BVH_GPU::ConvertFrom (tiny_bvh.h:4612) of the refitted tree, byte for byte (the conversion is a pure relayout).
+ *  - CWBVH: the 8-wide collapse of the last tbvh_convert is kept - which BVH2 nodes are the children of each wide node, in
+ *    adoption order.  The boxes come from the refitted BVH2 after SplitLeafs(3) (chain leaves keep their refitted parent leaf's
+ *    box); BVH8_CWBVH::ConvertFrom's greedy slot assignment, stack-order addresses and quantised encode (:5884) run on that, and
+ *    bvh8Tris is taken from the new vertices.  The wide-node count and depth stay; slot assignment and node addresses may change.
+ *    Every frame uses the collapse of the conversion, not that of the previous frame, so a long animation keeps the tree quality
+ *    of its first frame: call tbvh_convert again to collapse anew.
+ *  - info.build_ms is the device time of the call, aabb_min / aabb_max the new root box.
+ * Refusals leave the handle unmodified: TBVH_E_STATE for an SBVH, a TLAS, no BVH-layout tree, or a CWBVH that tbvh_convert did not
+ * produce from the resident tree (tbvh_upload_cwbvh, a group replica); TBVH_E_ARG for another prim_count.
+ * As after every refit, a TLAS over this BLAS is stale (its instance boxes are) until tbvh_build_tlas runs again, and group
+ * replicas keep the old boxes until tbvh_group_replicate runs again. */
+int tbvh_refit_layouts( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_count, int space );
+
 /* consume a tree built elsewhere, in the reference's own layouts (the public members bvhNode / primIdx /
  * verts of tiny_bvh.h:952-964, BVH_GPU::bvhNode :1124, BVH8_CWBVH::bvh8Data / bvh8Tris :1356-1357) */
 int tbvh_upload_bvh( tbvh_bvh bvh, const void* nodes32, uint32_t used_nodes, const uint32_t* prim_idx, uint32_t idx_count,

@@ -48,6 +48,7 @@ SYMBOLS = {
     "tbvh_instance_update_box": (i32, [vp, vp, vp]),
     "tbvh_build_tlas": (i32, [vp, vp, u32, u32, vp, u32, f32, f32]),
     "tbvh_refit": (i32, [vp, vp, u32, u32, i32]),
+    "tbvh_refit_layouts": (i32, [vp, vp, u32, u32, i32]),
     "tbvh_build_indexed": (i32, [vp, vp, u32, u32, vp, u32, i32, f32, f32, i32]),
     "tbvh_upload_bvh": (i32, [vp, vp, u32, vp, u32, vp, u32, u32, i32]),
     "tbvh_upload_bvh_gpu": (i32, [vp, vp, u32, vp, u32, vp, u32, u32, i32]),

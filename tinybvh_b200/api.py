@@ -244,6 +244,12 @@ class TLAS(BVH):
         return self
 
 
+def _refit_layouts(obj, vertices):
+    p, stride, nv, space, keep = _verts_arg(vertices)
+    check(_lib.lib().tbvh_refit_layouts(obj.h, p, stride, nv // 3, space))
+    return obj
+
+
 class BVH_GPU(_Base):
     """tinybvh::BVH_GPU (tiny_bvh.h:1092-1127): Aila-Laine 64-byte nodes."""
     layout = LAYOUT_BVH_GPU
@@ -259,6 +265,11 @@ class BVH_GPU(_Base):
         self._build(vertices, primCount, _lib.BUILD_HQ, indices)
         check(_lib.lib().tbvh_convert(self.h, LAYOUT_BVH_GPU))
         return self
+
+    def Refit(self, vertices):
+        """BVH::Refit of the underlying tree, then ConvertFrom again on the device (tbvh_refit_layouts): same triangles, new
+        positions, numpy or torch CUDA vertices as BVH.Refit."""
+        return _refit_layouts(self, vertices)
 
     def upload(self, nodes, primIdx, vertices):
         p, stride, nv, space, keep = _verts_arg(vertices)
@@ -290,6 +301,12 @@ class BVH8_CWBVH(_Base):
         self._build(vertices, primCount, _lib.BUILD_HQ, indices)
         check(_lib.lib().tbvh_convert(self.h, LAYOUT_CWBVH))
         return self
+
+    def Refit(self, vertices):
+        """Refit without a new collapse (tbvh_refit_layouts): BVH::Refit of the underlying tree, then BVH8_CWBVH::ConvertFrom of the
+        8-wide collapse kept from the last conversion with the refitted boxes - same wide-node count, in place.  The reference has no
+        BVH8_CWBVH::Refit; it refits the BVH2 and converts again (Build once more for that)."""
+        return _refit_layouts(self, vertices)
 
     def upload(self, bvh8Data, bvh8Tris):
         """bvh8Data: float32 [usedBlocks,4]; bvh8Tris: float32 [3*triCount,4] (public members :1356-1357)."""

@@ -386,6 +386,7 @@ static void free_layouts( tbvh_bvh b )
 	b->d_verts = 0, b->d_nodes = 0, b->d_prim_idx = 0, b->d_leaf_tris = 0, b->d_nodes_gpu = 0, b->d_cw_nodes = 0, b->d_cw_tris = 0, b->d_cw_trav = 0, b->d_trav = 0, b->leaf_tris_count = 0;
 	b->d_aabbs = 0, b->d_inst = 0, b->d_blas = 0, b->inst_count = 0, b->blas_count = 0, b->cw_depth = 0, b->tlas_blas_layouts = 0;
 	b->links.clear();
+	cw_keep_free( b );
 	b->generation = tbvh_next_generation(); // a TLAS built over the old arrays must notice (tlas_check)
 	memset( &b->info, 0, sizeof( b->info ) );
 	b->refittable = true;
@@ -604,6 +605,7 @@ int tbvh_upload_cwbvh( tbvh_bvh b, const void* bvh8_data, uint32_t used_blocks, 
 	if (b->d_cw_tris) cudaFree( b->d_cw_tris );
 	if (b->d_cw_trav) cudaFree( b->d_cw_trav );
 	b->d_cw_nodes = 0, b->d_cw_tris = 0, b->d_cw_trav = 0;
+	cw_keep_free( b ); // these arrays were not converted from the resident tree: tbvh_refit_layouts refuses them
 	CUDA_TRY( cudaMalloc( &b->d_cw_nodes, (size_t)used_blocks * 16 ) );
 	CUDA_TRY( cudaMalloc( &b->d_cw_tris, (size_t)tri_count * 48 ) );
 	CUDA_TRY( cudaMemcpyAsync( b->d_cw_nodes, bvh8_data, (size_t)used_blocks * 16, kind, s ) );
@@ -804,9 +806,40 @@ int tbvh_refit( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_co
 	if (b->d_cw_nodes) cudaFree( b->d_cw_nodes ), b->d_cw_nodes = 0;
 	if (b->d_cw_tris) cudaFree( b->d_cw_tris ), b->d_cw_tris = 0;
 	if (b->d_cw_trav) cudaFree( b->d_cw_trav ), b->d_cw_trav = 0;
+	cw_keep_free( b );
 	b->info.layouts = 1u << TBVH_LAYOUT_BVH, b->info.used_nodes_gpu = 0, b->info.used_blocks = 0, b->info.cwbvh_tri_count = 0;
 	TRY( make_leaf_tris( b, s ) );
 	CUDA_TRY( cudaStreamSynchronize( s ) );
+	return TBVH_OK;
+}
+
+// BVH::Refit, then every derived layout brought up to date in place (include/tinybvh_b200.h)
+int tbvh_refit_layouts( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space )
+{
+	ARG_CHECK( b && verts, "NULL argument" );
+	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
+	// every refusal comes before the vertex copy: a refused call leaves the handle as it was
+	if (!(b->info.layouts & (1u << TBVH_LAYOUT_BVH)) || !b->d_nodes || b->d_trav != b->d_nodes) { tbvh_set_error( "tbvh_refit_layouts: no BVH-layout tree on this handle" ); return TBVH_E_STATE; }
+	if (!b->refittable) { tbvh_set_error( b->d_inst ? "tbvh_refit_layouts: a TLAS is rebuilt, not refitted (tiny_bvh.h:3060)" : "tbvh_refit_layouts: refitting an SBVH (BVH::Refit, tiny_bvh.h:3057)" ); return TBVH_E_STATE; }
+	if ((b->info.layouts & (1u << TBVH_LAYOUT_CWBVH)) && !b->cw_keep)
+	{ tbvh_set_error( "tbvh_refit_layouts: the CWBVH on this handle was not converted from the resident tree (tbvh_convert)" ); return TBVH_E_STATE; }
+	ARG_CHECK( prim_count == b->info.prim_count && stride >= 12 && (stride & 3) == 0, "tbvh_refit_layouts: the vertex slice must describe the same triangles" );
+	cudaStream_t s = b->ctx->stream;
+	const size_t nv = (size_t)prim_count * 3;
+	const cudaMemcpyKind kind = space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+	if (stride == 16) CUDA_TRY( cudaMemcpyAsync( b->d_verts, verts, nv * 16, kind, s ) );
+	else CUDA_TRY( cudaMemcpy2DAsync( b->d_verts, 16, verts, stride, stride < 16 ? stride : 16, nv, kind, s ) );
+	// the arrays keep their addresses, but a TLAS over this BLAS holds its old root box in the instance records: stale until rebuilt
+	b->generation = tbvh_next_generation();
+	if (b->cw_keep) TRY( cwbvh_refit( b, s ) );
+	else
+	{
+		TRY( refit_launch( b, s ) );
+		TRY( make_leaf_tris( b, s ) );
+		CUDA_TRY( cudaStreamSynchronize( s ) );
+	}
+	// BVH_GPU::ConvertFrom is a pure relayout of the refitted tree
+	if (b->info.layouts & (1u << TBVH_LAYOUT_BVH_GPU)) TRY( bvh_to_bvh_gpu( b, s ) );
 	return TBVH_OK;
 }
 

@@ -104,6 +104,7 @@ struct tbvh_bvh_t
 	uint32_t tlas_blas_layouts = 0; // TLAS only: layouts EVERY BLAS held at build time (bit TBVH_LAYOUT_BVH / TBVH_LAYOUT_CWBVH)
 	std::vector<BlasLink> links; // TLAS only: the BLAS handles it points into, with the generation they had at build time
 	bool refittable = true;    // BVHBase::refittable (:811): false after BuildHQ ("can't refit an SBVH", :3027)
+	struct CwKeep* cw_keep = 0; // refittable trees: the 8-wide collapse of the last tbvh_convert to CWBVH (convert_cwbvh.cu), for tbvh_refit_layouts
 	// statistics
 	int stats = 0;
 	unsigned long long* d_stats = 0; // [0]=steps [1]=tris, accumulated over every launch of one API call
@@ -144,10 +145,13 @@ __device__ __forceinline__ float key2f( uint32_t k ) { return __uint_as_float( (
 int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
 int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
 int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth = -1 ); // known_depth < 0: measured on the device
+int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range ); // cw_make_trav's node expansion into the existing d_cw_trav
+float cw_rd_limit_for( uint32_t range );                               // cw_rd_limit of a tree whose expansion found `range`
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)
 int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour );
 int build_hq_launch( tbvh_bvh b, float c_trav, float c_int );
 int refit_launch( tbvh_bvh b, cudaStream_t s );
+int refit_enqueue( tbvh_bvh b, cudaStream_t s, uint32_t* parent, uint32_t* arrive, bool fill_parent );
 int tlas_trace_launch( tbvh_bvh b, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s );
 struct TlasInst { float inv[16]; uint32_t blasIdx, mask, pad0, pad1; };                                  // 80 bytes
 struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root_count; float cw_rd_limit; uint32_t pad1; const float4* cw_nodes; const float4* cw_tris; }; // 48 bytes: BVH-layout arrays, CWBVH traversal nodes + bvh8Tris (0 when absent) and their rD limit
@@ -155,5 +159,7 @@ int make_leaf_tris( tbvh_bvh b, cudaStream_t s );
 int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used_nodes_gpu, cudaStream_t s );
 int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s );
 int bvh_to_cwbvh( tbvh_bvh b, cudaStream_t s );
+int cwbvh_refit( tbvh_bvh b, cudaStream_t s );  // tbvh_refit_layouts over b->cw_keep (convert_cwbvh.cu)
+void cw_keep_free( tbvh_bvh b );                // drop b->cw_keep: wherever the CWBVH arrays are replaced or dropped
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)
 int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint32_t n, cudaStream_t s );

@@ -28,6 +28,11 @@ __device__ __forceinline__ float2 fma2( const float2 a, const float2 b, const fl
 	return make_float2( __fmaf_rn( a.x, b.x, c.x ), __fmaf_rn( a.y, b.y, c.y ) );
 }
 
+// tinybvh_max / tinybvh_min (tiny_bvh.h:432-433), which the float slab test must use: a NaN plane (0 * inf where 2^e * rD overflows)
+// in the second operand is returned, where fmaxf / fminf would drop it and keep the other side
+__device__ __forceinline__ float ref_max( const float a, const float b ) { return a > b ? a : b; }
+__device__ __forceinline__ float ref_min( const float a, const float b ) { return a < b ? a : b; }
+
 // one pair of children against one ray: `near` / `far` words already chosen by the ray's signs.  IORD: the slab test on the bit
 // patterns of the plane values as signed integers (cw_ray_fits states when that gives the float test's result)
 template <bool IORD> __device__ __forceinline__ uint32_t pair_hits( const uint32_t wnx, const uint32_t wny, const uint32_t wnz, const uint32_t wfx, const uint32_t wfy, const uint32_t wfz,
@@ -44,8 +49,9 @@ template <bool IORD> __device__ __forceinline__ uint32_t pair_hits( const uint32
 		const int out_b = __vimin3_s32( __float_as_int( tfx.y ), __float_as_int( tfy.y ), __float_as_int( tfz.y ) );
 		return (in_a <= out_a && !(__int_as_float( in_a ) > t) ? bits_a : 0u) | (in_b <= out_b && !(__int_as_float( in_b ) > t) ? bits_b : 0u);
 	}
-	const float in_a = fmaxf( fmaxf( fmaxf( tnx.x, tny.x ), tnz.x ), 0.0f ), out_a = fminf( fminf( fminf( tfx.x, tfy.x ), tfz.x ), t );
-	const float in_b = fmaxf( fmaxf( fmaxf( tnx.y, tny.y ), tnz.y ), 0.0f ), out_b = fminf( fminf( fminf( tfx.y, tfy.y ), tfz.y ), t );
+	// (a NaN t still passes, through fminf, as in the integer form)
+	const float in_a = ref_max( ref_max( ref_max( tnx.x, tny.x ), tnz.x ), 0.0f ), out_a = fminf( ref_min( ref_min( tfx.x, tfy.x ), tfz.x ), t );
+	const float in_b = ref_max( ref_max( ref_max( tnx.y, tny.y ), tnz.y ), 0.0f ), out_b = fminf( ref_min( ref_min( tfx.y, tfy.y ), tfz.y ), t );
 	return (in_a <= out_a ? bits_a : 0u) | (in_b <= out_b ? bits_b : 0u);
 }
 

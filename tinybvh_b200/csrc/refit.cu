@@ -58,6 +58,17 @@ __global__ void k_refit( float4* nodes, const uint32_t* __restrict__ prim_idx, c
 }
 } // namespace
 
+// enqueue BVH::Refit on s (d_verts already holds the new positions).  parent / arrive: `used` words each; parent depends on the
+// topology only, so it is filled only when fill_parent (a caller may keep it between refits)
+int refit_enqueue( tbvh_bvh b, cudaStream_t s, uint32_t* parent, uint32_t* arrive, bool fill_parent )
+{
+	const uint32_t used = b->info.used_nodes;
+	CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)used * 4, s ) );
+	if (fill_parent) { k_refit_parents<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes, parent, used ); LAUNCHED(); }
+	k_refit<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes, b->d_prim_idx, b->d_verts, parent, arrive, used ); LAUNCHED();
+	return TBVH_OK;
+}
+
 // d_verts already holds the new positions
 int refit_launch( tbvh_bvh b, cudaStream_t s )
 {
@@ -70,9 +81,7 @@ int refit_launch( tbvh_bvh b, cudaStream_t s )
 		CUDA_TRY( cudaMalloc( &d_arrive, (size_t)used * 4 ) );
 		CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) );
 		CUDA_TRY( cudaEventRecord( e0, s ) );
-		CUDA_TRY( cudaMemsetAsync( d_arrive, 0, (size_t)used * 4, s ) );
-		k_refit_parents<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes, d_parent, used ); LAUNCHED();
-		k_refit<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes, b->d_prim_idx, b->d_verts, d_parent, d_arrive, used ); LAUNCHED();
+		{ const int r = refit_enqueue( b, s, d_parent, d_arrive, true ); if (r != TBVH_OK) return r; }
 		CUDA_TRY( cudaEventRecord( e1, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		float ms = 0;

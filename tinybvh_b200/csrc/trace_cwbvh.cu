@@ -105,6 +105,17 @@ __global__ void k_cw_depth( const uint32_t* __restrict__ parent, const uint32_t 
 	atomicMax( max_depth, d );
 }
 
+// k_cw_expand of every node of d_cw_nodes into the allocated d_cw_trav; *d_range (zeroed by the caller) receives the tree's range
+int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range )
+{
+	const uint32_t count = b->info.used_blocks / 5;
+	k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, 0, d_range, count ); LAUNCHED();
+	return TBVH_OK;
+}
+
+// |rD| <= 2^( 127 - largest e ) keeps 2^e * rD finite (cw_ray_fits); 2^127 at most, and no ray fits a tree that has range 256
+float cw_rd_limit_for( uint32_t range ) { return range < 256 ? ldexpf( 1.0f, 127 - max( 0, (int)range - 128 ) ) : -1.0f; }
+
 int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth )
 {
 	if (b->d_cw_trav) cudaFree( b->d_cw_trav ), b->d_cw_trav = 0;
@@ -120,7 +131,7 @@ int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth )
 	uint32_t depth = (uint32_t)known_depth;
 	auto body = [&]() -> int
 	{
-		if (known_depth >= 0) k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, 0, d_range, count );
+		if (known_depth >= 0) { const int r = cw_expand_launch( b, s, d_range ); if (r != TBVH_OK) return r; }
 		else
 		{
 			// uploaded data: the depth of the wide tree is not known - every node notes its parent, then walks up to the root
@@ -128,10 +139,9 @@ int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth )
 			CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)count * 4, s ) );
 			CUDA_TRY( cudaMemsetAsync( d_parent + count, 0, 4, s ) );
 			k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_parent, d_range, count ); LAUNCHED();
-			k_cw_depth<<<(count + 127) / 128, 128, 0, s>>>( d_parent, count, d_parent + count );
+			k_cw_depth<<<(count + 127) / 128, 128, 0, s>>>( d_parent, count, d_parent + count ); LAUNCHED();
 			CUDA_TRY( cudaMemcpyAsync( &depth, d_parent + count, 4, cudaMemcpyDeviceToHost, s ) );
 		}
-		LAUNCHED();
 		CUDA_TRY( cudaMemcpyAsync( &range, d_range, 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
@@ -139,8 +149,7 @@ int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth )
 	const int rc = body();
 	if (d_parent) cudaFree( d_parent );
 	b->cw_depth = depth;
-	// |rD| <= 2^( 127 - largest e ) keeps 2^e * rD finite (cw_ray_fits); 2^127 at most, and no ray fits a tree that has range 256
-	if (rc == TBVH_OK && range < 256) b->cw_rd_limit = ldexpf( 1.0f, 127 - max( 0, (int)range - 128 ) );
+	if (rc == TBVH_OK) b->cw_rd_limit = cw_rd_limit_for( range );
 	return rc;
 }
 
