@@ -408,3 +408,35 @@ def test_reference_layouts_disagree_on_a_pinned_set_of_rays(ntris, seed, res, pr
     a, b = d["diffuse"].copy(), d["diffuse"].copy()
     cw.intersect(a), o.intersect(b)
     assert dis(a, b) == diffuse
+
+
+@pytest.mark.skipif(not refpy.available(), reason="oracle/_ref not built (needs /root/reference)")
+@pytest.mark.parametrize("fam", ["zero:random", "zero:order", "scale:-126", "scale:-6", "scale:24", "scale:40", "scale:90", "shift:1048576", "shift:-12582912"])
+@pytest.mark.parametrize("mode", [0, 1, 2])
+def test_port_matches_reference_on_offatrium_families(mode, fam):
+    """The restatement against the compiled reference on the off-atrium families (tests/test_offatrium_gpu.py): signed zeros,
+    power-of-two scales on both sides of the scale-invariance window, large translations.  Trees byte for byte, BVH and CWBVH walks
+    bit for bit on camera, axis (+-0 directions, rD = +-inf) and all-octant rays."""
+    from tests.test_offatrium_gpu import family, unit_rays
+    v = family(fam, 2000)
+    ref = refpy.RefBVH(v, mode=mode, threaded=False)
+    if mode == 2:
+        nodes, idx, ic = portpy.build_hq(v)
+        assert np.array_equal(ref.nodes.view(np.uint8), nodes.view(np.uint8)) and np.array_equal(ref.prim_idx[: idx.shape[0]], idx)
+        port = portpy.PortBVH(v, nodes=nodes, prim_idx=idx)
+    else:
+        port = portpy.PortBVH(v, avx=mode == 1)
+        assert np.array_equal(ref.nodes.view(np.uint8), port.nodes.view(np.uint8)) and np.array_equal(ref.prim_idx, port.prim_idx)
+    r = unit_rays(fam, 2000)
+    a, b = r.copy(), r.copy()
+    ref.intersect(a, threads=2), port.intersect(b, threads=2)
+    assert util.compare_hits(a, b) == {"prim": 0, "t": 0, "u": 0, "v": 0}
+    cw_mode = {0: 2, 1: 0, 2: 1}[mode]
+    rc, pc = refpy.RefCWBVH(v, mode=cw_mode), None
+    tree = portpy.PortBVH(v, avx=mode == 1) if mode != 2 else port
+    used = int(tree.nodes["triCount"].sum())
+    pc = portpy.PortCWBVH(tree.nodes, tree.prim_idx[:used], v, idx_count=ic if mode == 2 else tree.prim_idx.shape[0])
+    assert np.array_equal(np.ascontiguousarray(rc.nodes).view(np.uint8), np.ascontiguousarray(pc.nodes).view(np.uint8))
+    a, b = r.copy(), r.copy()
+    rc.intersect(a), pc.intersect(b)
+    assert util.compare_hits(a, b) == {"prim": 0, "t": 0, "u": 0, "v": 0}

@@ -123,6 +123,16 @@ def bits_u32(a):
     return np.ascontiguousarray(a).view(np.uint32)
 
 
+def nan_canonical(r):
+    """A copy with every NaN t / u / v set to one pattern.  A hit with a NaN distance (Moeller-Trumbore overflowing on huge
+    coordinates: 0 * inf) is accepted by the reference's `t < 0 || t > tmax` test; the NaN's bits are the floating-point unit's
+    (0xffc00000 on x86, 0x7fffffff on the GPU), not the reference's."""
+    r = r.copy()
+    for f in ("t", "u", "v"):
+        r[f][np.isnan(r[f])] = np.float32(np.nan)
+    return r
+
+
 def compare_hits(got, want):
     """-> dict of mismatch counts between two traced ray arrays (bit-exact fields)."""
     return {
@@ -163,3 +173,234 @@ def random_transforms(count, seed, spread=60.0):
         m[:3, 3] = (rng.random(3) - 0.5) * spread
         out[i] = m.astype(np.float32).reshape(-1)
     return out
+
+
+# ---- input families away from the procedural atrium: signed zeros, power-of-two scales, large translations, long leaves
+# Every family is seeded and deterministic.  The seeded scenes above all live in about [-40,40] x [0,30] x [-20,20] and hold no -0.
+
+NEG_ZERO = np.float32(-0.0)
+
+
+def signed_zero(v, mode, seed=0, frac=0.1):
+    """Snap the coordinates nearest the floor plane y = 0 and the wall x = 0 (the `frac` of each closest to zero) to exact zeros.
+    mode: "pos" all +0, "neg" all -0, "random" a seeded sign per vertex, "order" the sign triple of triangle t is the bit pattern of
+    t % 8, so every vertex order of -0 and +0 occurs."""
+    v = np.array(v, np.float32).reshape(-1, 4)
+    rng = np.random.default_rng(seed)
+    tri = np.arange(v.shape[0]) // 3
+    for axis in (0, 1):
+        a = np.abs(v[:, axis])
+        snap = a <= np.quantile(a, frac)
+        if mode == "pos":
+            neg = np.zeros(v.shape[0], bool)
+        elif mode == "neg":
+            neg = np.ones(v.shape[0], bool)
+        elif mode == "random":
+            neg = rng.random(v.shape[0]) < 0.5
+        elif mode == "order":
+            neg = (((tri + axis) % 8) >> (np.arange(v.shape[0]) % 3)) & 1 == 1
+        else:
+            raise ValueError(mode)
+        v[snap, axis] = np.where(neg[snap], NEG_ZERO, np.float32(0))
+    return v
+
+
+def count_neg_zero(a):
+    a = np.ascontiguousarray(a, np.float32)
+    return int(((a == 0) & np.signbit(a)).sum())
+
+
+def zero_tri_cases():
+    """The two orders of one triangle with a -0 and a +0 x-coordinate: BVH::Build's root aabbMin.x is the sign of the LAST one."""
+    a = np.array([[NEG_ZERO, 0, 0, 0], [0, 1, 0, 0], [1, 0, 1, 0]], np.float32)
+    b = a[[1, 0, 2]].copy()
+    return a, b
+
+
+def scaled(v, k):
+    """Positions multiplied by exactly 2^k (float32 ldexp: subnormals round, as the scaled scene would)."""
+    v = np.array(v, np.float32).reshape(-1, 4)
+    v[:, :3] = np.ldexp(v[:, :3], k)
+    return v
+
+
+def scaled_rays(r, k):
+    """Rays made at unit scale, moved to scale 2^k: O * 2^k, D and rD unchanged, t = 1e30."""
+    r = r.copy()
+    r["O"] = np.ldexp(r["O"], k)
+    r["t"] = np.float32(1e30)
+    return r
+
+
+def translated(v, shift):
+    """Positions plus `shift` in float32: far from the origin rounding merges vertices and makes zero-area triangles."""
+    v = np.array(v, np.float32).reshape(-1, 4)
+    v[:, :3] = v[:, :3] + np.float32(shift)
+    return v
+
+
+ONE_TRI = np.array([[0, 0, 0, 0], [1, 0, 0, 0], [0, 1, 0, 0]], np.float32)
+
+
+def long_leaf_scene(name):
+    """Trees whose CWBVH holds long chains of 3-triangle leaves (SplitLeafs of one big leaf):
+    "identical": 700 identical triangles; "clusters": two clusters of 3,000 identical triangles 5 units apart;
+    "collapsed": the 6,000-triangle scene at 2^40, where the SAH costs overflow and the tree collapses into a few huge leaves."""
+    if name == "identical":
+        return np.tile(ONE_TRI, (700, 1))
+    if name == "clusters":
+        a = np.tile(ONE_TRI, (3000, 1))
+        b = a.copy()
+        b[:, 0] += 5
+        return np.concatenate([a, b])
+    if name == "collapsed":
+        return scaled(scenes.procedural_scene(6000, 7), 40)
+    raise ValueError(name)
+
+
+def cw_parents(nodes):
+    """-> (parent of every wide node (-1 for the root and unreferenced records), inner-child count of every node) of bvh8Data."""
+    n = np.ascontiguousarray(nodes).view(np.uint8).reshape(-1, 80)
+    w = n.view(np.uint32).reshape(-1, 20)
+    cnt = n.shape[0]
+    ninner = ((n[:, 24:32] & 0x18) == 0x18).sum(1).astype(np.int64)
+    parent = np.full(cnt, -1, np.int64)
+    for x in range(cnt):
+        for c in range(int(ninner[x])):
+            if w[x, 4] + c < cnt:
+                parent[w[x, 4] + c] = x
+    return parent, ninner
+
+
+def cw_depth_and_pending(nodes):
+    """-> (depth of the wide tree, pending bound): the most ancestors with two or more inner children on a path from the root,
+    the number of node groups the walk can hold at once."""
+    parent, ninner = cw_parents(nodes)
+    depth = pend = 0
+    for x in range(parent.shape[0]):
+        d = p = 0
+        m = x
+        while parent[m] >= 0:
+            m = parent[m]
+            d += 1
+            p += int(ninner[m] >= 2)
+        depth, pend = max(depth, d), max(pend, p)
+    return depth, pend
+
+
+def cw_exponents(nodes):
+    """-> int8 [nodes, 3] exponent bytes of bvh8Data."""
+    return np.ascontiguousarray(nodes).view(np.uint8).reshape(-1, 80)[:, 12:15].view(np.int8)
+
+
+def cw_rd_limit(nodes):
+    """The |rD| up to which a ray takes the CWBVH walk's integer slab test, from the bytes alone: 2^(127 - max(0, largest e)), or
+    None when some e = -128 or some node origin |p| > 2^126."""
+    e = cw_exponents(nodes).astype(np.int64)
+    p = np.ascontiguousarray(nodes).view(np.float32).reshape(-1, 20)[:, :3]
+    if (e == -128).any() or (np.abs(p) > np.float32(2.0 ** 126)).any():
+        return None
+    return np.float32(np.ldexp(1.0, 127 - max(0, int(e.max()))))
+
+
+def octant_dirs():
+    """The 8 direction octants as sign triples (+1 / -1), octant index = 4 * (x < 0) + 2 * (y < 0) + (z < 0)."""
+    return np.array([[-1 if (o >> 2) & 1 else 1, -1 if (o >> 1) & 1 else 1, -1 if o & 1 else 1] for o in range(8)], np.float32)
+
+
+def axis_rays(lo, hi, per_axis=16, seed=0):
+    """Axis-aligned rays into a box, in all 8 octants: direction +-1 on one axis and zeros carrying the octant's sign on the
+    others (rD = safercp(D), so +-1e30 there), origins outside the box on the travel axis, across the box and on its zero planes."""
+    rng = np.random.default_rng(seed)
+    lo, hi = np.asarray(lo, np.float32), np.asarray(hi, np.float32)
+    ext = np.maximum(hi - lo, np.float32(1e-30))
+    O, D = [], []
+    for o, s in enumerate(octant_dirs()):
+        for a in range(3):
+            d = np.where(s < 0, NEG_ZERO, np.float32(0)).astype(np.float32)
+            d[a] = s[a]
+            for j in range(per_axis):
+                p = (lo + ext * rng.random(3).astype(np.float32)).astype(np.float32)
+                if j % 4 == 0:
+                    p[(a + 1) % 3] = 0   # on a zero plane of the scene
+                if j % 8 == 0:
+                    p[(a + 2) % 3] = NEG_ZERO
+                p[a] = lo[a] - ext[a] if s[a] > 0 else hi[a] + ext[a]
+                O.append(p), D.append(d)
+    r = R.make_rays(np.array(O), np.array(D), normalized=True)
+    return r
+
+
+def octant_rays(lo, hi, per_octant=64, seed=0):
+    """Rays from points inside a box in random directions of every octant, per_octant each: the two test cameras never put a warp
+    of rays into the octants with negative x and positive z."""
+    rng = np.random.default_rng(seed)
+    lo, hi = np.asarray(lo, np.float32), np.asarray(hi, np.float32)
+    O, D = [], []
+    for s in octant_dirs():
+        O.append(lo + (hi - lo) * rng.random((per_octant, 3)).astype(np.float32))
+        D.append(s * (np.float32(0.05) + rng.random((per_octant, 3)).astype(np.float32)))
+    return R.make_rays(np.concatenate(O).astype(np.float32), np.concatenate(D).astype(np.float32))
+
+
+def with_inf_rd(r):
+    """The same rays with a user-supplied rD = 1 / D: +-inf on every zero direction component."""
+    r = r.copy()
+    with np.errstate(divide="ignore"):
+        r["rD"] = (np.float32(1) / r["D"]).astype(np.float32)
+    return r
+
+
+def octant_blocks(r, seed=0):
+    """Rays reordered into blocks of 32: blocks whose rays share one octant (every octant that occurs) alternating with blocks
+    that mix octants, so every octant instance of the CWBVH walk and its per-lane form run."""
+    oct_ = ((r["D"][:, 0] < 0) * 4 + (r["D"][:, 1] < 0) * 2 + (r["D"][:, 2] < 0)).astype(np.int64)
+    rng = np.random.default_rng(seed)
+    uni, mixed = [], []
+    for o in range(8):
+        idx = np.nonzero(oct_ == o)[0]
+        full = idx.shape[0] // 32 * 32
+        uni += [idx[k:k + 32] for k in range(0, full, 32)]
+        mixed += list(idx[full:])
+    mixed = np.array(mixed, np.int64)
+    rng.shuffle(mixed)
+    mixed = [mixed[k:k + 32] for k in range(0, mixed.shape[0], 32)]
+    order = []
+    for k in range(max(len(uni), len(mixed))):
+        if k < len(uni):
+            order.append(uni[k])
+        if k < len(mixed):
+            order.append(mixed[k])
+    return r[np.concatenate(order)] if order else r
+
+
+def rd_limit_rays(r, limit, seed=0):
+    """Rays around the integer-slab-test bound: |rD.x| set to limit, the next float above it, 2 * limit - ulp, 2 * limit and inf
+    (sign of D.x kept), in warps of their own and as one lane per warp of unchanged rays; plus origins at 2^126 and the next float."""
+    rng = np.random.default_rng(seed)
+    lim = np.float32(limit if limit is not None else 2.0 ** 127)
+    with np.errstate(over="ignore"):
+        two = np.float32(2) * lim   # inf when the bound is 2^127
+    vals = [lim, np.nextafter(lim, np.float32(np.inf)), np.nextafter(two, np.float32(0)), two, np.float32(np.inf)]
+    out = []
+    for v in vals:
+        for own in (True, False):
+            s = r[rng.integers(0, r.shape[0], 64)].copy()
+            sel = np.ones(64, bool) if own else (np.arange(64) % 32 == 7)
+            sgn = np.where(s["D"][:, 0] < 0, np.float32(-1), np.float32(1))
+            with np.errstate(over="ignore"):
+                s["rD"][sel, 0] = (sgn[sel] * v).astype(np.float32)
+            out.append(s)
+    for o in (np.float32(2.0 ** 126), np.nextafter(np.float32(2.0 ** 126), np.float32(np.inf))):
+        s = r[rng.integers(0, r.shape[0], 32)].copy()
+        s["O"][:, 0] = -o
+        out.append(s)
+    return np.concatenate(out)
+
+
+def shadow_at_hits(traced):
+    """Shadow rays whose tmax is exactly the hit distance of a traced set (the any-hit test's t <= tmax edge)."""
+    s = traced[traced["t"] < 1e30].copy()
+    s["u"] = s["v"] = 0
+    s["prim"] = 0
+    return s

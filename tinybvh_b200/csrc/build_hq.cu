@@ -54,6 +54,8 @@ struct HQCounters
 	uint32_t failed_splits;  // ":2939 spatial split failed" leaves
 	uint32_t overflow;       // a task stack / fragment pool ran out (cannot happen within the reference's own bounds)
 	uint32_t root_key[6];
+	uint32_t root_zpos[6];   // signed zeros (k_hq_root_zero): position word of the last fragment with a zero bound, per root bound
+	uint32_t negzero;        // some fragment bound is -0
 	float root_area;
 	float min_dim[3];
 	unsigned long long prof[32]; // TBVH_HQ_PROFILE=1: leader-thread cycles per phase, [0..15] level phase, [16..31] subtree phase
@@ -941,6 +943,8 @@ __global__ void k_hq_init( HQArgs A )
 	HQCounters* c = A.ctr;
 	c->node_ptr = 2, c->frag_ptr = A.n, c->next_big = 0, c->small_roots = 0, c->max_depth = 0, c->next_max = 0, c->failed_splits = 0, c->overflow = 0;
 	for (int k = 0; k < 3; k++) c->root_key[k] = f2key( BVH_FAR ), c->root_key[3 + k] = f2key( -BVH_FAR );
+	for (int k = 0; k < 6; k++) c->root_zpos[k] = 0;
+	c->negzero = 0;
 	for (int k = 0; k < 32; k++) c->prof[k] = 0;
 }
 
@@ -958,6 +962,10 @@ __global__ void k_hq_fragments( HQArgs A )
 		A.frag_max[i] = make_float4( mx[0], mx[1], mx[2], __uint_as_float( 0u ) );
 		A.prim_idx[i] = i;
 	}
+	// a -0 bound anywhere: the root's zero bounds take their sign in k_hq_root_zero (without one the keys are exact)
+	const bool neg = (mn[0] == 0 && signbit( mn[0] )) || (mn[1] == 0 && signbit( mn[1] )) || (mn[2] == 0 && signbit( mn[2] ))
+		|| (mx[0] == 0 && signbit( mx[0] )) || (mx[1] == 0 && signbit( mx[1] )) || (mx[2] == 0 && signbit( mx[2] ));
+	if (__any_sync( 0xffffffffu, neg ) && (threadIdx.x & 31) == 0) A.ctr->negzero = 1;
 	#pragma unroll
 	for (int k = 0; k < 3; k++)
 	{
@@ -967,11 +975,32 @@ __global__ void k_hq_fragments( HQArgs A )
 	}
 }
 
+// With a -0 fragment bound only: each root bound that is a zero takes the sign of the last fragment with a zero there, as
+// PrepareHQBuild's fold gives it (common.cuh zpos_word; build_sah.cu k_root_zero)
+__global__ void __launch_bounds__( 256 ) k_hq_root_zero( HQArgs A )
+{
+	if (!A.ctr->negzero) return;
+	uint32_t zw[6] = { 0, 0, 0, 0, 0, 0 };
+	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < A.n; i += gridDim.x * blockDim.x)
+	{
+		const float4 lo = A.frag_min[i], hi = A.frag_max[i];
+		const float f[6] = { lo.x, lo.y, lo.z, hi.x, hi.y, hi.z };
+		#pragma unroll
+		for (int k = 0; k < 6; k++) if (f[k] == 0) zw[k] = max( zw[k], zpos_word( i, f[k] ) );
+	}
+	#pragma unroll
+	for (int k = 0; k < 6; k++)
+	{
+		const uint32_t w = __reduce_max_sync( 0xffffffffu, zw[k] );
+		if ((threadIdx.x & 31) == 0 && w) atomicMax( &A.ctr->root_zpos[k], w );
+	}
+}
+
 __global__ void k_hq_root( HQArgs A )
 {
 	HQCounters* c = A.ctr;
 	float mn[3], mx[3];
-	for (int k = 0; k < 3; k++) mn[k] = key2f( c->root_key[k] ), mx[k] = key2f( c->root_key[3 + k] );
+	for (int k = 0; k < 3; k++) mn[k] = key2f( zero_resolve( c->root_key[k], c->root_zpos[k] ) ), mx[k] = key2f( zero_resolve( c->root_key[3 + k], c->root_zpos[3 + k] ) );
 	A.tmp_nodes[0] = make_float4( mn[0], mn[1], mn[2], __uint_as_float( 0u ) );
 	A.tmp_nodes[1] = make_float4( mx[0], mx[1], mx[2], __uint_as_float( A.n ) );
 	A.tmp_nodes[2] = A.tmp_nodes[3] = make_float4( 0, 0, 0, 0 );
@@ -1133,6 +1162,7 @@ int build_hq_launch( tbvh_bvh b, float c_trav, float c_int )
 		CUDA_TRY( cudaMemsetAsync( A.arrive, 0, (size_t)A.node_cap * 4, s ) );
 		k_hq_init<<<1, 1, 0, s>>>( A ); LAUNCHED();
 		k_hq_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+		k_hq_root_zero<<<b->ctx->sm_count, 256, 0, s>>>( A ); LAUNCHED();
 		k_hq_root<<<1, 1, 0, s>>>( A ); LAUNCHED();
 		uint32_t num = n > A.small_t ? 1 : 0, level = 0, max_count = n;
 		uint32_t max_cluster = (uint32_t)(b->ctx->hq_cluster < 1 ? 1 : b->ctx->hq_cluster > HQ_MAX_CLUSTER ? HQ_MAX_CLUSTER : b->ctx->hq_cluster);

@@ -27,6 +27,7 @@
 #define BIN_WORDS 168        // 3 axes x 8 bins x (3 min keys, 3 max keys, count)
 #define BIN_STRIDE 192       // + 3 x 8 counts of the PARTITION's own bin function (BuildAVX flavour, see bin_part_avx)
 __device__ __forceinline__ uint32_t bin_init_word( const uint32_t k ) { return (k < BIN_WORDS && (k % 7) < 3) ? 0xffffffffu : 0u; }
+#define ZPOS_WORDS 144       // 3 axes x 8 bins x (3 min, 3 max)
 #define SCAN_TILE 2048
 
 struct LargeNode { uint32_t tmp, first, count, depth; };
@@ -43,7 +44,9 @@ struct Counters
 	uint32_t lvl_chunks[2];
 	uint32_t levels;         // persistent large phase: levels run
 	uint32_t root_key[6];    // root AABB as ordered keys: min xyz, max xyz
-	uint32_t pad[4];
+	uint32_t root_zpos[6];   // position word (common.cuh zpos_word) of the last fragment with a zero bound, per root bound
+	uint32_t negzero;        // some fragment bound is -0: bins need the signed-zero pass (bin_zero_chunk, k_build_small)
+	uint32_t pad[3];
 };
 
 struct BuildArgs
@@ -57,6 +60,7 @@ struct BuildArgs
 	uint32_t* chunk_pre;     // persistent large phase: exclusive prefix of the per-chunk flag totals (chunks + 1 entries)
 	float4* tmp_nodes; uint32_t* node_first; uint32_t* node_depth;
 	LargeNode* lvl[2]; uint32_t* chunk_start; uint32_t* chunk_start_next; uint32_t* bins; SplitInfo* split;
+	uint32_t* zpos;          // per large node, ZPOS_WORDS position words of zero bin bounds (bin_zero_chunk); the sweep reads and clears them
 	SmallRoot* small;
 	Counters* ctr;
 	uint32_t n;
@@ -101,23 +105,35 @@ __device__ __forceinline__ float half_area( const float ex, const float ey, cons
 	return __fmaf_rn( ez, ex, __fmaf_rn( ey, ex, __fmul_rn( ey, ez ) ) );
 }
 
-struct SweepResult { bool split; uint32_t axis, pos, lN; float l1[3], l2[3], r1[3], r2[3]; };
+struct SweepResult { bool split, rotate; uint32_t axis, pos, lN; float l1[3], l2[3], r1[3], r2[3]; };
 
 // One warp evaluates the 21 candidate planes of a node from its bin table (ordered keys + counts) - the sweep,
 // termination test and child bounds of tiny_bvh.h:2380-2412.  All lanes return the same result.
-__device__ __forceinline__ SweepResult sweep_node( uint32_t* bins /* BIN_WORDS, shared or global; decoded in place */, const float4 nmin, const float4 nmax,
-	const uint32_t count, const float3 min_dim, const float c_trav, const float c_int, const uint32_t flavour )
+// NEGZERO: some fragment bound is -0 (Counters::negzero), so bin bounds are folded with the reference's tie rule; without a -0
+// fminf / fmaxf give the same bits.
+template <bool NEGZERO> __device__ __forceinline__ SweepResult sweep_node( uint32_t* bins /* BIN_WORDS, shared or global; decoded in place */, const float4 nmin, const float4 nmax,
+	const uint32_t count, const float3 min_dim, const float c_trav, const float c_int, const uint32_t flavour, uint32_t* zpos /* ZPOS_WORDS or 0 */, const bool root )
 {
 	const uint32_t lane = threadIdx.x & 31;
 	// decode pass: lanes 0..23 turn the six ordered keys of "their" bin back into floats, once, instead of every one of
-	// the 7 candidate lanes of an axis decoding all 8 bins again
+	// the 7 candidate lanes of an axis decoding all 8 bins again; a zero bound takes the sign its position word gives (and the
+	// word is cleared for the next level)
 	if (lane < 3 * BINS)
 	{
 		uint32_t* w = bins + lane * 7;
 		if (w[6] != 0)
 		{
 			#pragma unroll
-			for (int k = 0; k < 6; k++) w[k] = __float_as_uint( key2f( w[k] ) );
+			for (int k = 0; k < 6; k++)
+			{
+				uint32_t key = w[k];
+				if (zpos && zero_key( key ))
+				{
+					uint32_t* z = zpos + lane * 6 + k;
+					key = zero_resolve( key, *z ), *z = 0;
+				}
+				w[k] = __float_as_uint( key2f( key ) );
+			}
 		}
 	}
 	__syncwarp();
@@ -134,6 +150,9 @@ __device__ __forceinline__ SweepResult sweep_node( uint32_t* bins /* BIN_WORDS, 
 		const float md = a == 0 ? min_dim.x : a == 1 ? min_dim.y : min_dim.z;
 		if (ext > md)
 		{
+			// the reference folds the left side over bins 0..i and the right side over bins 7 down to i+1 (:2383-2388, :6601-6602),
+			// and a tie goes to the bin folded last.  Here both run upwards: the right side with the operands swapped keeps the
+			// first (lowest) tied bin instead, which is the one the reference's downward fold ends on.
 			for (uint32_t b = 0; b < BINS; b++)
 			{
 				const uint32_t* w = bins + (a * BINS + b) * 7;
@@ -143,13 +162,19 @@ __device__ __forceinline__ SweepResult sweep_node( uint32_t* bins /* BIN_WORDS, 
 				const float mxx = __uint_as_float( w[3] ), mxy = __uint_as_float( w[4] ), mxz = __uint_as_float( w[5] );
 				if (b <= i)
 				{
-					l1[0] = fminf( l1[0], mnx ), l1[1] = fminf( l1[1], mny ), l1[2] = fminf( l1[2], mnz );
-					l2[0] = fmaxf( l2[0], mxx ), l2[1] = fmaxf( l2[1], mxy ), l2[2] = fmaxf( l2[2], mxz ), lN += c;
+					if (NEGZERO) l1[0] = ref_min( l1[0], mnx ), l1[1] = ref_min( l1[1], mny ), l1[2] = ref_min( l1[2], mnz );
+					else l1[0] = fminf( l1[0], mnx ), l1[1] = fminf( l1[1], mny ), l1[2] = fminf( l1[2], mnz );
+					if (NEGZERO) l2[0] = ref_max( l2[0], mxx ), l2[1] = ref_max( l2[1], mxy ), l2[2] = ref_max( l2[2], mxz );
+					else l2[0] = fmaxf( l2[0], mxx ), l2[1] = fmaxf( l2[1], mxy ), l2[2] = fmaxf( l2[2], mxz );
+					lN += c;
 				}
 				else
 				{
-					r1[0] = fminf( r1[0], mnx ), r1[1] = fminf( r1[1], mny ), r1[2] = fminf( r1[2], mnz );
-					r2[0] = fmaxf( r2[0], mxx ), r2[1] = fmaxf( r2[1], mxy ), r2[2] = fmaxf( r2[2], mxz ), rN += c;
+					if (NEGZERO) r1[0] = ref_min( mnx, r1[0] ), r1[1] = ref_min( mny, r1[1] ), r1[2] = ref_min( mnz, r1[2] );
+					else r1[0] = fminf( r1[0], mnx ), r1[1] = fminf( r1[1], mny ), r1[2] = fminf( r1[2], mnz );
+					if (NEGZERO) r2[0] = ref_max( mxx, r2[0] ), r2[1] = ref_max( mxy, r2[1] ), r2[2] = ref_max( mxz, r2[2] );
+					else r2[0] = fmaxf( r2[0], mxx ), r2[1] = fmaxf( r2[1], mxy ), r2[2] = fmaxf( r2[2], mxz );
+					rN += c;
 				}
 			}
 			const float aL = half_area( __fsub_rn( l2[0], l1[0] ), __fsub_rn( l2[1], l1[1] ), __fsub_rn( l2[2], l1[2] ) );
@@ -186,14 +211,30 @@ __device__ __forceinline__ SweepResult sweep_node( uint32_t* bins /* BIN_WORDS, 
 	SweepResult R;
 	R.axis = win / 7, R.pos = __shfl_sync( 0xffffffffu, i, win );
 	R.lN = __shfl_sync( 0xffffffffu, lN, win );
-	// BuildAVX: if its partition puts everything on one side the reference leaves the node a leaf (:6639; it has by then
-	// permuted primIdx and burnt two node slots - "should not happen", not reproduced)
+	// If the partition puts everything on one side the reference leaves the node a leaf (:2423; BuildAVX :6639, which also burns
+	// two node slots - "should not happen", not reproduced)
 	R.split = found && !(splitCost >= noSplitCost) && R.lN != 0 && R.lN != count;
+	R.rotate = false;
 	#pragma unroll
 	for (int k = 0; k < 3; k++)
 	{
 		R.l1[k] = __shfl_sync( 0xffffffffu, l1[k], win ), R.l2[k] = __shfl_sync( 0xffffffffu, l2[k], win );
 		R.r1[k] = __shfl_sync( 0xffffffffu, r1[k], win ), R.r2[k] = __shfl_sync( 0xffffffffu, r2[k], win );
+	}
+	if (!found && root) // warp-uniform, and rare
+	{
+		// No candidate below BVH_FAR (every cost overflows, on scenes scaled far up): the reference still splits when the cost test
+		// passes, on axis 0 at plane 0, with the child boxes its best-split variables hold from EARLIER candidates (:2396-2404).  At
+		// the root those are the initial zeros - and children with zero boxes are leaves.  Further down they come from whichever node
+		// the reference swept last; the engine does not know them and leaves the node a leaf.
+		R.axis = 0, R.pos = 0, R.lN = __shfl_sync( 0xffffffffu, lN, flavour ? 5u : 0u ); // the lane of axis 0, plane 0
+		const bool ok = !(splitCost >= noSplitCost);
+		R.split = ok && R.lN != 0 && R.lN != count;
+		// a partition that sends everything right still runs its swap loop before the node becomes a leaf (:2414-2423): the range
+		// ends up rotated left by one
+		R.rotate = ok && R.lN == 0;
+		#pragma unroll
+		for (int k = 0; k < 3; k++) R.l1[k] = R.l2[k] = R.r1[k] = R.r2[k] = 0.0f;
 	}
 	return R;
 }
@@ -268,11 +309,16 @@ __global__ void __launch_bounds__( 256 ) k_fragments( BuildArgs A )
 	else if (i < A.n)
 	{
 		const float4 v0 = __ldg( A.verts + (size_t)i * 3 ), v1 = __ldg( A.verts + (size_t)i * 3 + 1 ), v2 = __ldg( A.verts + (size_t)i * 3 + 2 );
-		mn[0] = fminf( v0.x, fminf( v1.x, v2.x ) ), mn[1] = fminf( v0.y, fminf( v1.y, v2.y ) ), mn[2] = fminf( v0.z, fminf( v1.z, v2.z ) );
-		mx[0] = fmaxf( v0.x, fmaxf( v1.x, v2.x ) ), mx[1] = fmaxf( v0.y, fmaxf( v1.y, v2.y ) ), mx[2] = fmaxf( v0.z, fmaxf( v1.z, v2.z ) );
+		mn[0] = ref_min( v0.x, ref_min( v1.x, v2.x ) ), mn[1] = ref_min( v0.y, ref_min( v1.y, v2.y ) ), mn[2] = ref_min( v0.z, ref_min( v1.z, v2.z ) );
+		mx[0] = ref_max( v0.x, ref_max( v1.x, v2.x ) ), mx[1] = ref_max( v0.y, ref_max( v1.y, v2.y ) ), mx[2] = ref_max( v0.z, ref_max( v1.z, v2.z ) );
 		A.frag_min[i] = make_float4( mn[0], mn[1], mn[2], 0 ), A.frag_max[i] = make_float4( mx[0], mx[1], mx[2], 0 );
 		A.idx[0][i] = i;
 	}
+	// signed zeros: a -0 bound anywhere switches on the sign passes (k_root_zero, the bins' zero pass); without one every zero
+	// bound is +0 and the ordered keys below are exact
+	const bool neg = (mn[0] == 0 && signbit( mn[0] )) || (mn[1] == 0 && signbit( mn[1] )) || (mn[2] == 0 && signbit( mn[2] ))
+		|| (mx[0] == 0 && signbit( mx[0] )) || (mx[1] == 0 && signbit( mx[1] )) || (mx[2] == 0 && signbit( mx[2] ));
+	if (__any_sync( 0xffffffffu, neg ) && (threadIdx.x & 31) == 0) A.ctr->negzero = 1;
 	#pragma unroll
 	for (int k = 0; k < 3; k++) for (int o = 16; o > 0; o >>= 1)
 		mn[k] = fminf( mn[k], __shfl_xor_sync( 0xffffffffu, mn[k], o ) ), mx[k] = fmaxf( mx[k], __shfl_xor_sync( 0xffffffffu, mx[k], o ) );
@@ -286,18 +332,46 @@ __global__ void __launch_bounds__( 256 ) k_fragments( BuildArgs A )
 	else if (threadIdx.x < 6) atomicMax( &A.ctr->root_key[threadIdx.x], s_key[threadIdx.x] );
 }
 
+// Scenes with a -0 fragment bound only (the others return at once): each root bound that is a zero takes the sign of the last
+// fragment with a zero there - a max over position words (common.cuh zpos_word) - and the large phase's zero-position table is
+// cleared for bin_zero_chunk.
+__global__ void __launch_bounds__( 256 ) k_root_zero( BuildArgs A, const size_t zpos_words )
+{
+	if (!A.ctr->negzero) return;
+	const size_t stride = (size_t)gridDim.x * blockDim.x;
+	for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < zpos_words; k += stride) A.zpos[k] = 0;
+	uint32_t zw[6] = { 0, 0, 0, 0, 0, 0 };
+	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < A.n; i += (uint32_t)stride)
+	{
+		const float4 lo = A.frag_min[i], hi = A.frag_max[i];
+		const float f[6] = { lo.x, lo.y, lo.z, hi.x, hi.y, hi.z };
+		#pragma unroll
+		for (int k = 0; k < 6; k++) if (f[k] == 0) zw[k] = max( zw[k], zpos_word( i, f[k] ) );
+	}
+	#pragma unroll
+	for (int k = 0; k < 6; k++)
+	{
+		const uint32_t w = __reduce_max_sync( 0xffffffffu, zw[k] );
+		if ((threadIdx.x & 31) == 0 && w) atomicMax( &A.ctr->root_zpos[k], w );
+	}
+}
+
 __global__ void k_init_counters( BuildArgs A )
 {
 	Counters* c = A.ctr;
 	c->tmp_nodes = 2, c->next_large = 0, c->small_roots = 0, c->max_depth = 0, c->total_chunks = 0, c->lvl_num[0] = c->lvl_num[1] = 0, c->lvl_chunks[0] = c->lvl_chunks[1] = 0, c->levels = 0;
 	for (int k = 0; k < 3; k++) c->root_key[k] = 0xffffffffu, c->root_key[3 + k] = 0;
+	for (int k = 0; k < 6; k++) c->root_zpos[k] = 0;
+	c->negzero = 0;
 }
 
 __global__ void k_init_root( BuildArgs A )
 {
 	Counters* c = A.ctr;
-	const float4 mn = make_float4( key2f( c->root_key[0] ), key2f( c->root_key[1] ), key2f( c->root_key[2] ), __uint_as_float( 0u ) );
-	const float4 mx = make_float4( key2f( c->root_key[3] ), key2f( c->root_key[4] ), key2f( c->root_key[5] ), __uint_as_float( A.n ) );
+	float r[6];
+	for (int k = 0; k < 6; k++) r[k] = key2f( zero_resolve( c->root_key[k], c->root_zpos[k] ) );
+	const float4 mn = make_float4( r[0], r[1], r[2], __uint_as_float( 0u ) );
+	const float4 mx = make_float4( r[3], r[4], r[5], __uint_as_float( A.n ) );
 	A.tmp_nodes[0] = mn, A.tmp_nodes[1] = mx;
 	A.tmp_nodes[2] = make_float4( 0, 0, 0, 0 ), A.tmp_nodes[3] = make_float4( 0, 0, 0, 0 ); // node 1 stays unused (:2285)
 	A.node_first[0] = 0, A.node_depth[0] = 0, A.node_first[1] = 0, A.node_depth[1] = 0;
@@ -387,6 +461,58 @@ __global__ void __launch_bounds__( CHUNK ) k_bin( BuildArgs A, const LargeNode* 
 	bin_chunk( A, A.chunk_start, cur, num, idx_in, blockIdx.x, s_bins, s_slot );
 }
 
+// the bin of a fragment on each axis, as bin_chunk finds it
+__device__ __forceinline__ void sweep_bins( const uint32_t flavour, const float4 nmin, const float4 nmax, const float4 fmn, const float4 fmx, uint32_t b3[3] )
+{
+	if (flavour)
+	{
+		b3[0] = bin_of_avx( fmn.x, fmx.x, __fmul_rn( nmin.x, 2.0f ), rpd_avx( __fsub_rn( nmax.x, nmin.x ) ) );
+		b3[1] = bin_of_avx( fmn.y, fmx.y, __fmul_rn( nmin.y, 2.0f ), rpd_avx( __fsub_rn( nmax.y, nmin.y ) ) );
+		b3[2] = bin_of_avx( fmn.z, fmx.z, __fmul_rn( nmin.z, 2.0f ), rpd_avx( __fsub_rn( nmax.z, nmin.z ) ) );
+	}
+	else
+	{
+		b3[0] = bin_of( fmn.x, fmx.x, nmin.x, __fdiv_rn( (float)BINS, __fsub_rn( nmax.x, nmin.x ) ) );
+		b3[1] = bin_of( fmn.y, fmx.y, nmin.y, __fdiv_rn( (float)BINS, __fsub_rn( nmax.y, nmin.y ) ) );
+		b3[2] = bin_of( fmn.z, fmx.z, nmin.z, __fdiv_rn( (float)BINS, __fsub_rn( nmax.z, nmin.z ) ) );
+	}
+}
+
+// Signed zeros, for scenes with a -0 fragment bound (Counters::negzero) only.  Once a node's bin table is complete, every fragment
+// with a zero bound where its bin's bound is zero offers its position in the node's primIdx order; the sweep gives the bound the
+// sign of the highest (the reference's fold over the node's primitives, :2371-2375, lets the last tied one win).
+__device__ __forceinline__ void bin_zero_chunk( const BuildArgs& A, const uint32_t* cs, const LargeNode* cur, const uint32_t num, const uint32_t* idx_in, const uint32_t vb, uint32_t& s_slot )
+{
+	__syncthreads();
+	if (threadIdx.x == 0) s_slot = find_slot( cs, num, vb );
+	__syncthreads();
+	const uint32_t j = s_slot;
+	const LargeNode nd = cur[j];
+	const uint32_t off = (vb - LD( cs + j )) * CHUNK + threadIdx.x;
+	if (off >= nd.count) return;
+	const float4 fmn = __ldg( A.frag_min + LD( idx_in + nd.first + off ) ), fmx = __ldg( A.frag_max + LD( idx_in + nd.first + off ) );
+	const float f[6] = { fmn.x, fmn.y, fmn.z, fmx.x, fmx.y, fmx.z };
+	if (f[0] != 0 && f[1] != 0 && f[2] != 0 && f[3] != 0 && f[4] != 0 && f[5] != 0) return;
+	uint32_t b3[3];
+	sweep_bins( A.flavour, LD( A.tmp_nodes + (size_t)nd.tmp * 2 ), LD( A.tmp_nodes + (size_t)nd.tmp * 2 + 1 ), fmn, fmx, b3 );
+	#pragma unroll
+	for (int a = 0; a < 3; a++)
+	{
+		const uint32_t w = (a * BINS + b3[a]);
+		#pragma unroll
+		for (int k = 0; k < 6; k++)
+			if (f[k] == 0 && zero_key( LD( A.bins + (size_t)j * BIN_STRIDE + w * 7 + k ) ))
+				atomicMax( A.zpos + (size_t)j * ZPOS_WORDS + w * 6 + k, zpos_word( off, f[k] ) );
+	}
+}
+// a grid-stride loop over the level's chunks: the launch for the first level, made before the host knows whether it is needed,
+// costs one wave of blocks that return at once
+__global__ void __launch_bounds__( CHUNK ) k_bin_zero( BuildArgs A, const LargeNode* cur, const uint32_t num, const uint32_t* idx_in, const uint32_t chunks )
+{
+	__shared__ uint32_t s_slot;
+	if (A.ctr->negzero) for (uint32_t c = blockIdx.x; c < chunks; c += gridDim.x) bin_zero_chunk( A, A.chunk_start, cur, num, idx_in, c, s_slot );
+}
+
 // append the two children of a split node: bigger than SMALL_T -> next level's list, else -> warp-built subtree
 __device__ __forceinline__ void emit_child( const BuildArgs& A, LargeNode* next, const uint32_t tmp, const uint32_t first, const uint32_t count, const uint32_t depth, const uint32_t out_buf )
 {
@@ -402,12 +528,15 @@ __device__ __forceinline__ void sweep_one( const BuildArgs& A, const LargeNode* 
 	const float4 rmin = A.tmp_nodes[0], rmax = A.tmp_nodes[1];
 	const float mdf = A.flavour ? 1e-7f : 1e-20f; // minDim (:2346 / :6555)
 	const float3 min_dim = make_float3( __fmul_rn( __fsub_rn( rmax.x, rmin.x ), mdf ), __fmul_rn( __fsub_rn( rmax.y, rmin.y ), mdf ), __fmul_rn( __fsub_rn( rmax.z, rmin.z ), mdf ) );
-	const SweepResult R = sweep_node( A.bins + (size_t)j * BIN_STRIDE, nmin, nmax, nd.count, min_dim, A.c_trav, A.c_int, A.flavour );
+	// the position table is cleared (k_root_zero) and filled (bin_zero_chunk) only with a -0
+	uint32_t* const bins = A.bins + (size_t)j * BIN_STRIDE;
+	const SweepResult R = A.ctr->negzero ? sweep_node<true>( bins, nmin, nmax, nd.count, min_dim, A.c_trav, A.c_int, A.flavour, A.zpos + (size_t)j * ZPOS_WORDS, nd.tmp == 0 )
+		: sweep_node<false>( bins, nmin, nmax, nd.count, min_dim, A.c_trav, A.c_int, A.flavour, 0, nd.tmp == 0 );
 	if (!R.split)
 	{
 		// leaf: its range is final (tiny_bvh.h:2409-2412); publish the order it has in the current buffer
 		if (lane == 0) A.split[j] = SplitInfo{ 0, 0, 0, 0 };
-		for (uint32_t k = lane; k < nd.count; k += 32) A.idx_final[nd.first + k] = idx_in[nd.first + k];
+		for (uint32_t k = lane; k < nd.count; k += 32) A.idx_final[nd.first + k] = idx_in[nd.first + (R.rotate && k + 1 < nd.count ? k + 1 : R.rotate ? 0 : k)];
 		return;
 	}
 	if (lane == 0)
@@ -653,6 +782,11 @@ __global__ void __launch_bounds__( CHUNK ) k_large_phase( BuildArgs A )
 		// ---- 1. bin tables of the level's nodes
 		for (uint32_t c = blockIdx.x; c < chunks; c += gridDim.x) bin_chunk( A, cs, cur, num, idx_in, c, s_bins, s_slot );
 		grid.sync();
+		if (C->negzero) // written before the launch: uniform over the grid
+		{
+			for (uint32_t c = blockIdx.x; c < chunks; c += gridDim.x) bin_zero_chunk( A, cs, cur, num, idx_in, c, s_slot );
+			grid.sync();
+		}
 		// ---- 2. one warp per node: sweep, termination, children
 		for (uint32_t j = gwarp; j < num; j += gwarps) sweep_one( A, cur, next, j, idx_in, lp ^ 1 );
 		grid.sync();
@@ -735,10 +869,53 @@ template <bool FRAGS> struct SmallSmemT
 	uint32_t st_tmp[12]; uint32_t st_rng[12]; uint32_t st_db[12]; // stack: tmp node, lo | n << 16, depth | buf << 16
 };
 
+// Signed zeros in a warp-built node (bin_zero_chunk): the warp revisits the node's primitives in order, and of the lanes with a
+// zero where their bin's bound is zero the highest one writes its sign, so the last fragment in primIdx order wins.  The bins
+// come from S.posbl, where the binning loop left them.  Compiled into an instance of k_build_small of its own (NEGZERO): the
+// ordinary instance keeps its registers.
+template <class SmallSmem, bool FRAGS> __device__ __forceinline__ void small_bin_zero( const BuildArgs& A, SmallSmem& S, const uint32_t lo, const uint32_t n, const uint32_t buf )
+{
+	const uint32_t lane = threadIdx.x & 31;
+	for (uint32_t base = 0; base < n; base += 32)
+	{
+		const uint32_t k = base + lane;
+		float f[6] = { 1, 1, 1, 1, 1, 1 };
+		uint32_t bb = 0;
+		if (k < n)
+		{
+			const uint32_t sl = S.idx[buf][lo + k];
+			if (FRAGS) for (int c = 0; c < 3; c++) f[c] = S.fmn[sl][c], f[3 + c] = S.fmx[sl][c];
+			else
+			{
+				const float4 mn = __ldg( A.frag_min + S.gid[sl] ), mx = __ldg( A.frag_max + S.gid[sl] );
+				f[0] = mn.x, f[1] = mn.y, f[2] = mn.z, f[3] = mx.x, f[4] = mx.y, f[5] = mx.z;
+			}
+			bb = S.posbl[lo + k];
+		}
+		#pragma unroll
+		for (int a = 0; a < 3; a++)
+		{
+			const uint32_t b = (bb >> (3 * a)) & 7u;
+			#pragma unroll
+			for (int c = 0; c < 6; c++)
+			{
+				uint32_t* w = S.bins + (a * BINS + b) * 7 + c;
+				const bool z = k < n && f[c] == 0 && zero_key( *w );
+				const uint32_t m = __match_any_sync( 0xffffffffu, z ? b : BINS + lane );
+				if (z && lane == 31u - __clz( m )) *w = f2key( f[c] );
+			}
+		}
+		__syncwarp();
+	}
+}
+
 // FRAGS: stage the subtree's fragment boxes in shared memory (no global gathers per level, fewer resident warps).
 // AGG:   warp-aggregated bin updates for batches of a node with >= 64 primitives (small nodes use plain shared atomics:
 //        with a handful of active lanes the match/redux sequence costs more than the conflicts it removes).
-template <bool FRAGS, bool AGG>
+// NEGZERO: the signed-zero pass (small_bin_zero) and the tie-rule fold, for scenes with a -0 fragment bound (Counters::negzero);
+// also the instance that builds the tree's root (scenes of at most small_t primitives), which needs sweep_node's root rule.
+// The other instance carries neither.
+template <bool FRAGS, bool AGG, bool NEGZERO>
 __global__ void __launch_bounds__( SMALL_WARPS * 32 ) k_build_small( BuildArgs A, const uint32_t num_roots )
 {
 	typedef SmallSmemT<FRAGS> SmallSmem;
@@ -804,6 +981,7 @@ __global__ void __launch_bounds__( SMALL_WARPS * 32 ) k_build_small( BuildArgs A
 					b3[0] = bin_of( mnx, mxx, nmin.x, rpx ), b3[1] = bin_of( mny, mxy, nmin.y, rpy ), b3[2] = bin_of( mnz, mxz, nmin.z, rpz );
 					S.bid[lo + k] = (uint16_t)(b3[0] | (b3[1] << 3) | (b3[2] << 6));
 				}
+				if (NEGZERO) S.posbl[lo + k] = (uint16_t)(b3[0] | (b3[1] << 3) | (b3[2] << 6)); // for small_bin_zero: posbl is free until the partition
 				kmn[0] = f2key( mnx ), kmn[1] = f2key( mny ), kmn[2] = f2key( mnz ), kmx[0] = f2key( mxx ), kmx[1] = f2key( mxy ), kmx[2] = f2key( mxz );
 			}
 			if (AGG && n >= 64)
@@ -824,11 +1002,12 @@ __global__ void __launch_bounds__( SMALL_WARPS * 32 ) k_build_small( BuildArgs A
 			}
 		}
 		__syncwarp();
-		const SweepResult R = sweep_node( S.bins, nmin, nmax, n, min_dim, A.c_trav, A.c_int, A.flavour );
+		if (NEGZERO) small_bin_zero<SmallSmem, FRAGS>( A, S, lo, n, buf );
+		const SweepResult R = sweep_node<NEGZERO>( S.bins, nmin, nmax, n, min_dim, A.c_trav, A.c_int, A.flavour, 0, NEGZERO && tmp == 0 );
 		bool pop = false;
 		if (!R.split)
 		{
-			for (uint32_t k = lane; k < n; k += 32) A.idx_final[root.first + lo + k] = S.gid[S.idx[buf][lo + k]];
+			for (uint32_t k = lane; k < n; k += 32) A.idx_final[root.first + lo + k] = S.gid[S.idx[buf][lo + (R.rotate && k + 1 < n ? k + 1 : R.rotate ? 0 : k)]];
 			pop = true;
 		}
 		else
@@ -1016,6 +1195,7 @@ int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
 		DEV_ALLOC( A.tmp_nodes, max_nodes * 32 ); DEV_ALLOC( A.node_first, max_nodes * 4 ); DEV_ALLOC( A.node_depth, max_nodes * 4 );
 		DEV_ALLOC( A.lvl[0], max_large * sizeof( LargeNode ) ); DEV_ALLOC( A.lvl[1], max_large * sizeof( LargeNode ) );
 		DEV_ALLOC( A.chunk_start, (max_large + 1) * 4 ); DEV_ALLOC( A.chunk_start_next, (max_large + 1) * 4 ); DEV_ALLOC( A.bins, max_large * BIN_STRIDE * 4 ); DEV_ALLOC( A.split, max_large * sizeof( SplitInfo ) );
+		DEV_ALLOC( A.zpos, max_large * ZPOS_WORDS * 4 ); // cleared by k_root_zero, with a -0 only
 		DEV_ALLOC( A.chunk_pre, (flag_words / CHUNK + 2) * 4 );
 		DEV_ALLOC( A.small, ((size_t)n + 1) * sizeof( SmallRoot ) );
 		DEV_ALLOC( A.ctr, sizeof( Counters ) );
@@ -1025,6 +1205,7 @@ int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
 		CUDA_TRY( cudaEventRecord( e0, s ) );
 		k_init_counters<<<1, 1, 0, s>>>( A ); LAUNCHED();
 		k_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+		k_root_zero<<<b->ctx->sm_count, 256, 0, s>>>( A, max_large * ZPOS_WORDS ); LAUNCHED();
 		k_init_root<<<1, 256, 0, s>>>( A ); LAUNCHED();
 		uint32_t num = n > A.small_t ? 1 : 0, chunks = (n + CHUNK - 1) / CHUNK, level = 0;
 		// Large phase.  The first levels of a big scene are bandwidth work over all primitives: one launch per stage, every CTA the
@@ -1067,6 +1248,7 @@ int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
 			const uint32_t* idx_in = A.idx[level & 1];
 			uint32_t* idx_out = A.idx[(level + 1) & 1];
 			k_bin<<<chunks, CHUNK, 0, s>>>( A, cur, num, idx_in ); LAUNCHED();
+			if (level == 0 || h_ctr->negzero) { k_bin_zero<<<min( chunks, (uint32_t)b->ctx->sm_count ), CHUNK, 0, s>>>( A, cur, num, idx_in, chunks ); LAUNCHED(); }
 			k_sweep<<<(num * 32 + 255) / 256, 256, 0, s>>>( A, cur, next, num, idx_in, (level + 1) & 1 ); LAUNCHED();
 			k_flags<<<chunks, CHUNK, 0, s>>>( A, cur, num ); LAUNCHED();
 			{ const int r = exclusive_scan( A.flags, A.scan, tile_sum, chunks * CHUNK, s ); if (r != TBVH_OK) return r; }
@@ -1091,10 +1273,13 @@ int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
 		if (roots)
 		{
 			const uint32_t g = (roots + SMALL_WARPS - 1) / SMALL_WARPS, mode = (uint32_t)b->ctx->small_mode;
-			if (mode == 0) k_build_small<false, false><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots );
-			else if (mode == 1) k_build_small<true, false><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots );
-			else if (mode == 2) k_build_small<false, true><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots );
-			else k_build_small<true, true><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots );
+			#define SMALL( F, G ) do { if (h_ctr->negzero || n <= A.small_t) k_build_small<F, G, true><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); \
+				else k_build_small<F, G, false><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); } while (0)
+			if (mode == 0) SMALL( false, false );
+			else if (mode == 1) SMALL( true, false );
+			else if (mode == 2) SMALL( false, true );
+			else SMALL( true, true );
+			#undef SMALL
 			LAUNCHED();
 		}
 		CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( Counters ), cudaMemcpyDeviceToHost, s ) );

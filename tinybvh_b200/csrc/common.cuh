@@ -93,7 +93,7 @@ struct tbvh_bvh_t
 	float4* d_cw_nodes = 0;    // 5 float4 per node
 	float4* d_cw_tris = 0;     // 3 float4 per triangle
 	float4* d_cw_trav = 0;     // traversal nodes derived from d_cw_nodes (trace_cwbvh.cu cw_make_trav): 10 float4 per node
-	uint32_t cw_depth = 0;     // depth of the wide tree (root = 0)
+	uint32_t cw_pending = 0;   // most node groups a walk of the wide tree can leave pending (trace_cwbvh.cu k_cw_pending)
 	float cw_rd_limit = -1.0f; // rays with |rD| up to this (and |O| <= 2^126) take the integer-ordered slab test (cw_walk.cuh cw_ray_fits); < 0: none
 	uint32_t generation = 0;   // renewed (tbvh_next_generation) whenever the arrays a TLAS may point at are replaced (build, upload, refit, convert)
 	// TLAS (BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) :2221): nodes / primIdx over instance boxes + device tables
@@ -115,9 +115,9 @@ struct tbvh_bvh_t
 // contraction (-fmad) cannot change the rounding.
 
 // MOLLER_TRUMBORE_TEST tiny_bvh.h:1644-1656 with e1,e2 precomputed (identical bits: v1-v0 is exact-rounded once).
-// Returns true when the triangle is accepted for [0, tmax]; writes t,u,v.
+// Returns true when the triangle is accepted for [0, tmax] ([0, tmax) with below_tmax); writes t,u,v.
 __device__ __forceinline__ bool mt_test( const float ox, const float oy, const float oz, const float dx, const float dy, const float dz,
-	const float4 v0, const float4 e1, const float4 e2, const float tmax, float& t, float& u, float& v )
+	const float4 v0, const float4 e1, const float4 e2, const float tmax, float& t, float& u, float& v, const bool below_tmax = false )
 {
 	const float hx = __fmaf_rn( dy, e2.z, -__fmul_rn( dz, e2.y ) );
 	const float hy = __fmaf_rn( dz, e2.x, -__fmul_rn( dx, e2.z ) );
@@ -133,18 +133,29 @@ __device__ __forceinline__ bool mt_test( const float ox, const float oy, const f
 	v = __fmul_rn( f, __fmaf_rn( dz, qz, __fmaf_rn( dy, qy, __fmul_rn( dx, qx ) ) ) );
 	if (u < 0 || v < 0 || __fadd_rn( u, v ) > 1) return false;
 	t = __fmul_rn( f, __fmaf_rn( e2.z, qz, __fmaf_rn( e2.x, qx, __fmul_rn( e2.y, qy ) ) ) );
-	return !(t < 0 || t > tmax);
+	return !(t < 0 || (below_tmax ? t >= tmax : t > tmax));
 }
 
 // order-preserving float <-> uint key for atomicMin/Max on floats
 __device__ __forceinline__ uint32_t f2key( float f ) { uint32_t u = __float_as_uint( f ); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
 __device__ __forceinline__ float key2f( uint32_t k ) { return __uint_as_float( (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k ); }
 
+// Signed zeros.  The reference folds bounds with tinybvh_min / tinybvh_max (tiny_bvh.h:445-446), a < b ? a : b and a > b ? a : b:
+// on a tie the second operand wins, so of several zero bounds the one folded LAST gives the result its sign.  The key reductions
+// above find the value in any order (key(-0) = 0x7fffffff sits just below key(+0) = 0x80000000); where that value is a zero, the
+// builders take the sign from a position word, ((fold position + 1) << 1) | sign bit, reduced with a max.
+__device__ __forceinline__ float ref_min( const float a, const float b ) { return a < b ? a : b; }
+__device__ __forceinline__ float ref_max( const float a, const float b ) { return a > b ? a : b; }
+__device__ __forceinline__ bool zero_key( const uint32_t k ) { return k == 0x7fffffffu || k == 0x80000000u; }
+__device__ __forceinline__ uint32_t zpos_word( const uint32_t pos, const float f ) { return ((pos + 1u) << 1) | (__float_as_uint( f ) >> 31); }
+// the key of a zero bound whose sign a position word decided (0: no word, keep the key)
+__device__ __forceinline__ uint32_t zero_resolve( const uint32_t key, const uint32_t zw ) { return (zw && zero_key( key )) ? ((zw & 1u) ? 0x7fffffffu : 0x80000000u) : key; }
+
 // ---- internal entry points (one per .cu) -------------------------------------------------------------------
 // d_stats: NULL, or two counters the launch ADDS its node visits / triangle tests to (the caller zeroes them once per API call)
 int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
 int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
-int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth = -1 ); // known_depth < 0: measured on the device
+int cw_make_trav( tbvh_bvh b, cudaStream_t s ); // traversal nodes, cw_rd_limit and cw_pending of b's CWBVH
 int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range ); // cw_make_trav's node expansion into the existing d_cw_trav
 float cw_rd_limit_for( uint32_t range );                               // cw_rd_limit of a tree whose expansion found `range`
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)

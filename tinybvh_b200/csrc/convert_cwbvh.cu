@@ -392,8 +392,8 @@ int bvh_to_cwbvh( tbvh_bvh b, cudaStream_t s )
 		CUDA_TRY( cudaMalloc( &b->d_cw_tris, (size_t)idx_count * 48 ) );
 		{ const int r = cw_assign_encode( b, s, ext, lists, adopt, ifirst, off, wide ); if (r != TBVH_OK) return r; }
 		b->info.used_blocks = wide_count * 5, b->info.cwbvh_tri_count = idx_count;
-		// the traversal nodes the kernels read (trace_cwbvh.cu); the wide tree has `levels` levels
-		{ const int r = cw_make_trav( b, s, (int)levels - 1 ); if (r != TBVH_OK) return r; }
+		// the traversal nodes the kernels read and the pending bound of the wide tree (trace_cwbvh.cu)
+		{ const int r = cw_make_trav( b, s ); if (r != TBVH_OK) return r; }
 		if (b->refittable)
 		{
 			// keep the collapse for tbvh_refit_layouts, sized to the wide tree

@@ -144,7 +144,7 @@ int tbvh_group_replicate( tbvh_group g, tbvh_bvh src, double* ms_out )
 		{
 			CUDA_TRY( cudaSetDevice( c->device ) );
 			cudaStream_t s = c->stream;
-			r->info = src->info, r->root_ref = src->root_ref, r->root_count = src->root_count, r->refittable = src->refittable, r->cw_depth = src->cw_depth, r->cw_rd_limit = src->cw_rd_limit;
+			r->info = src->info, r->root_ref = src->root_ref, r->root_count = src->root_count, r->refittable = src->refittable, r->cw_pending = src->cw_pending, r->cw_rd_limit = src->cw_rd_limit;
 			const size_t nodes_b = (size_t)(src->info.used_nodes < 2 ? 2 : src->info.used_nodes) * 32;
 			TRY( peer_clone( (void**)&r->d_verts, c->device, src->d_verts, sdev, (size_t)src->info.prim_count * 48, s ) );
 			TRY( peer_clone( (void**)&r->d_prim_idx, c->device, src->d_prim_idx, sdev, (size_t)src->info.idx_count * 4, s ) );

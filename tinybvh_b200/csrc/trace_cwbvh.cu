@@ -91,18 +91,43 @@ __global__ void k_cw_expand( const uint4* __restrict__ src, uint4* __restrict__ 
 		o[2 + 2 * j] = make_uint4( word[j][0], word[j][1], word[j][2], word[j][3] );
 		o[3 + 2 * j] = make_uint4( word[j][4], word[j][5], word[j][6], word[j][7] );
 	}
-	// inner children sit at n1.x + 0 .. inner-1 (node units): note their parent for the depth pass
-	if (parent) for (uint32_t c = 0; c < inner; c++) if (n1.x + c < count) parent[n1.x + c] = x;
+	// inner children sit at n1.x + 0 .. inner-1 (node units): note their parent, and whether it has siblings to leave pending, for
+	// the pending pass
+	if (parent) for (uint32_t c = 0; c < inner; c++) if (n1.x + c < count) parent[n1.x + c] = x | (inner >= 2 ? 0x80000000u : 0u);
 }
 
-__global__ void k_cw_depth( const uint32_t* __restrict__ parent, const uint32_t count, uint32_t* __restrict__ max_depth )
+// The walk pushes a node group only when the node it enters has inner siblings still to visit (cw_trace: rest > 0x00ffffff), so
+// at a node it holds at most one group per ancestor with two or more inner children.  The largest such count over the nodes is
+// what the pending stack must hold - on a chain (the 3-triangle leaves SplitLeafs makes of a long leaf) far less than the depth.
+// It is found by pointer jumping: every node keeps an ancestor and the count of flagged nodes up to it, and each pass doubles
+// the distance (anc' = anc(anc), cnt' = cnt + cnt(anc)), so ceil( log2( count ) ) + 1 passes reach the root from any node.  A node
+// still short of the root then lies on a cycle (uploaded data): the tree is reported as such.
+#define CW_ROOT 0xffffffffu   // ancestor past the root
+#define CW_CYCLE 0xffffffffu  // cw_pending of a tree with a cycle
+__global__ void k_cw_jump_init( const uint32_t* __restrict__ parent, const uint32_t count, uint32_t* __restrict__ anc, uint32_t* __restrict__ cnt )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= count) return;
-	uint32_t d = 0, n = x;
-	while (n != 0 && n < count && d < 4096) n = parent[n], d++; // n >= count: a record no node points at (0xffffffff)
-	if (n != 0) return;
-	atomicMax( max_depth, d );
+	const uint32_t p = parent[x];
+	// the root steps past itself - unless some node names it as a child, a cycle a walk would never leave: it then stays on itself;
+	// a record no node points at (0xffffffff) gets ancestor `count` (out of range) and is not counted
+	anc[x] = x == 0 ? (p == 0xffffffffu ? CW_ROOT : 0u) : p == 0xffffffffu ? count : (p & 0x7fffffffu), cnt[x] = (x == 0 || p == 0xffffffffu) ? 0u : p >> 31;
+}
+__global__ void k_cw_jump( const uint32_t count, const uint32_t* __restrict__ anc, const uint32_t* __restrict__ cnt, uint32_t* __restrict__ anc2, uint32_t* __restrict__ cnt2 )
+{
+	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+	if (x >= count) return;
+	const uint32_t a = anc[x];
+	if (a < count) anc2[x] = anc[a], cnt2[x] = min( cnt[x] + cnt[a], 0x40000000u );
+	else anc2[x] = a, cnt2[x] = cnt[x];
+}
+__global__ void k_cw_pending( const uint32_t count, const uint32_t* __restrict__ anc, const uint32_t* __restrict__ cnt, uint32_t* __restrict__ max_pending )
+{
+	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+	if (x >= count) return;
+	const uint32_t a = anc[x];
+	if (a == CW_ROOT) atomicMax( max_pending, cnt[x] );
+	else if (a < count) atomicMax( max_pending, CW_CYCLE );
 }
 
 // k_cw_expand of every node of d_cw_nodes into the allocated d_cw_trav; *d_range (zeroed by the caller) receives the tree's range
@@ -116,7 +141,7 @@ int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range )
 // |rD| <= 2^( 127 - largest e ) keeps 2^e * rD finite (cw_ray_fits); 2^127 at most, and no ray fits a tree that has range 256
 float cw_rd_limit_for( uint32_t range ) { return range < 256 ? ldexpf( 1.0f, 127 - max( 0, (int)range - 128 ) ) : -1.0f; }
 
-int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth )
+int cw_make_trav( tbvh_bvh b, cudaStream_t s )
 {
 	if (b->d_cw_trav) cudaFree( b->d_cw_trav ), b->d_cw_trav = 0;
 	const uint32_t count = b->info.used_blocks / 5;
@@ -128,27 +153,29 @@ int cw_make_trav( tbvh_bvh b, cudaStream_t s, int known_depth )
 	b->cw_rd_limit = -1.0f;
 	CUDA_TRY( cudaMemsetAsync( d_range, 0, 4, s ) );
 	uint32_t* d_parent = 0;
-	uint32_t depth = (uint32_t)known_depth;
+	uint32_t pending = 0xffffffffu;
 	auto body = [&]() -> int
 	{
-		if (known_depth >= 0) { const int r = cw_expand_launch( b, s, d_range ); if (r != TBVH_OK) return r; }
-		else
-		{
-			// uploaded data: the depth of the wide tree is not known - every node notes its parent, then walks up to the root
-			CUDA_TRY( cudaMalloc( &d_parent, ((size_t)count + 1) * 4 ) );
-			CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)count * 4, s ) );
-			CUDA_TRY( cudaMemsetAsync( d_parent + count, 0, 4, s ) );
-			k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_parent, d_range, count ); LAUNCHED();
-			k_cw_depth<<<(count + 127) / 128, 128, 0, s>>>( d_parent, count, d_parent + count ); LAUNCHED();
-			CUDA_TRY( cudaMemcpyAsync( &depth, d_parent + count, 4, cudaMemcpyDeviceToHost, s ) );
-		}
+		// every node notes its parent, then the counts of ancestors that leave node groups pending are summed up to the root
+		CUDA_TRY( cudaMalloc( &d_parent, ((size_t)count * 5 + 1) * 4 ) );
+		uint32_t* const anc[2] = { d_parent + count, d_parent + 2 * (size_t)count }, * const cnt[2] = { d_parent + 3 * (size_t)count, d_parent + 4 * (size_t)count };
+		uint32_t* const d_pending = d_parent + 5 * (size_t)count;
+		CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)count * 4, s ) );
+		CUDA_TRY( cudaMemsetAsync( d_pending, 0, 4, s ) );
+		const uint32_t g = (count + 127) / 128;
+		k_cw_expand<<<g, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_parent, d_range, count ); LAUNCHED();
+		k_cw_jump_init<<<g, 128, 0, s>>>( d_parent, count, anc[0], cnt[0] ); LAUNCHED();
+		int cur = 0;
+		for (uint32_t reach = 1; reach < 2 * count; reach *= 2, cur ^= 1) { k_cw_jump<<<g, 128, 0, s>>>( count, anc[cur], cnt[cur], anc[cur ^ 1], cnt[cur ^ 1] ); LAUNCHED(); }
+		k_cw_pending<<<g, 128, 0, s>>>( count, anc[cur], cnt[cur], d_pending ); LAUNCHED();
+		CUDA_TRY( cudaMemcpyAsync( &pending, d_pending, 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaMemcpyAsync( &range, d_range, 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
 	};
 	const int rc = body();
 	if (d_parent) cudaFree( d_parent );
-	b->cw_depth = depth;
+	b->cw_pending = pending;
 	if (rc == TBVH_OK) b->cw_rd_limit = cw_rd_limit_for( range );
 	return rc;
 }
@@ -191,7 +218,9 @@ template <bool ANYHIT, bool STATS, int OCT, bool IORD> __device__ __forceinline_
 			const float4 e2 = __ldg( tp ), e1 = __ldg( tp + 1 ), v0 = __ldg( tp + 2 );
 			if (STATS) ntris++;
 			float tt, u, v;
-			if (mt_test( ox, oy, oz, dx, dy, dz, v0, e1, e2, t, tt, u, v ))
+			// any-hit is BVH8_CWBVH::IsOccluded, FALLBACK_SHADOW_QUERY (tiny_bvh.h:312): Intersect, then hit.t < tmax - a triangle
+			// exactly at tmax does not occlude (boxes are still culled at tmax)
+			if (mt_test( ox, oy, oz, dx, dy, dz, v0, e1, e2, t, tt, u, v, ANYHIT ))
 			{
 				if (ANYHIT) { occluded = true; break; }
 				t = tt, hu = u, hv = v, hprim = __float_as_uint( v0.w );
@@ -263,6 +292,9 @@ __global__ void __launch_bounds__( 128 ) k_trace_wide( const float4* __restrict_
 		#undef TRACE
 		if (!ANYHIT)
 		{
+			// the reference stores t, but u, v and prim only when t < BVH_FAR (end of :7046-7154): a NaN or infinite distance (Moeller-Trumbore
+			// overflowing on huge coordinates) leaves the ray's own u, v, prim
+			if (!(t < BVH_FAR)) hu = rh4.y, hv = rh4.z, hprim = __float_as_uint( rh4.w );
 			float4* hp = (float4*)(hits + i * hit_stride);
 			*hp = make_float4( t, hu, hv, __uint_as_float( hprim ) );
 		}
@@ -279,7 +311,8 @@ int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d
 {
 	if (!b->d_cw_trav || !b->d_cw_tris) { tbvh_set_error( "CWBVH layout not resident" ); return TBVH_E_STATE; }
 	if (n == 0) return TBVH_OK;
-	if (b->cw_depth + 1 > CW_STACK) { tbvh_set_error( "wide-tree depth %u exceeds the %d pending node groups a ray can hold (the reference's own limit)", b->cw_depth, CW_STACK ); return TBVH_E_LIMIT; }
+	if (b->cw_pending == CW_CYCLE) { tbvh_set_error( "the wide tree's inner-child links form a cycle" ); return TBVH_E_ARG; }
+	if (b->cw_pending > CW_STACK) { tbvh_set_error( "the wide tree can leave %u node groups pending, more than the %d a ray can hold (the reference's own limit)", b->cw_pending, CW_STACK ); return TBVH_E_LIMIT; }
 	const uint32_t block = 128;
 	const uint64_t grid = (n + block - 1) / block;
 	if (grid > 0x7fffffffull) { tbvh_set_error( "ray batch too large for one launch" ); return TBVH_E_ARG; }
