@@ -1,10 +1,15 @@
 """Every tuning variant (tbvh_set_option) must give the oracle's results: the traversal-kernel variants change which
 lane / code path runs a ray, never its arithmetic or order; the host-path modes change how bytes cross PCIe."""
+from types import SimpleNamespace
+
 import numpy as np
 import pytest
 
-from tinybvh_b200 import api, rays as R, scenes
+from tinybvh_b200 import _lib, api, rays as R, scenes
+from tinybvh_b200._lib import BUILD_REFERENCE
 from tests import util
+from tests.test_oracle_pin import tlas_case
+from tests.test_tlas_gpu import words
 
 pytestmark = pytest.mark.gpu
 ZERO = {"prim": 0, "t": 0, "u": 0, "v": 0}
@@ -50,25 +55,130 @@ def test_trace_variants_are_bit_exact(gpu, world, variant):
         api.set_option("trace_variant", 3)
 
 
-@pytest.mark.parametrize("mode", [0, 1, 2, 3])
-def test_host_path_modes_return_the_same_hits(gpu, world, mode):
+N_HOST = 65536 + 4096 + 100   # with 4096-ray chunks: 18 chunks (more than TBVH_SLOTS = 4), a ragged last chunk and occlusion word,
+                              # and past d2h_mode 2's host-scatter threshold of 65,536 rays
+STRIDES = (128, 64, 144, 136)  # 136 is not a multiple of 16: the gather (host_path 1) and the scatter (d2h_mode 3) must step aside
+SENTINEL = np.uint32(0x5A5A5A5A)
+
+
+def hit_words(records):
+    """bytes 48..63 (t, u, v, prim) of every record of a [n, stride] byte array, as uint32 [n, 4]"""
+    return np.ascontiguousarray(records[:, 48:64]).view(np.uint32)
+
+
+@pytest.fixture(scope="module")
+def host_world(world):
+    """N_HOST camera and shadow rays with the oracle's hits and occlusion words in each layout, the engines, and a TLAS per layout with
+    the device path's in-place results (held to the oracle in test_tlas_gpu.py)."""
+    import torch
     v, primary, d, want = world
+    rays, shadow = primary[:N_HOST].copy(), d["shadow"][:N_HOST].copy()
+    cw, _ = util.oracle_cwbvh(v, mode=2)
+    traced = rays.copy()
+    cw.intersect(traced)
+    tr = shadow.copy()
+    cw.intersect(tr)
+    occ_cw = tr["t"] < shadow["t"]   # BVH8_CWBVH::IsOccluded is FALLBACK_SHADOW_QUERY (tiny_bvh.h:312)
+    bvh_words = hit_words(want["primary"][:N_HOST].view(np.uint8).reshape(-1, 128))
+    bvh_bits = util.oracle_bvh(v).occluded(shadow.copy())
+    cw_bits = np.packbits(np.concatenate([occ_cw, np.zeros(-N_HOST % 32, bool)]).astype(np.uint8), bitorder="little").view(np.uint32)
+    engines = {}
+    for name, cls in (("BVH", api.BVH), ("BVH_GPU", api.BVH_GPU), ("CWBVH", api.BVH8_CWBVH)):
+        e = cls()
+        e.build_flavour = BUILD_REFERENCE   # the derived layouts over BVH::Build's tree, which the oracles convert
+        e.Build(v)
+        engines[name] = e
+    want_layout = {"BVH": (bvh_words, bvh_bits), "BVH_GPU": (bvh_words, bvh_bits), "CWBVH": (hit_words(traced.view(np.uint8).reshape(-1, 128)), cw_bits)}
+    tv, inst, O, D = tlas_case(93, 24)
+    blas = [api.BVH8_CWBVH().Build(x) for x in tv]
+    t_bvh = api.TLAS().Build(inst.copy(), blas)
+    t_cw = api.TLAS().Build(inst.copy(), blas, blas_layout=api.LAYOUT_CWBVH)
+    t_rays = R.make_rays(O, D)
+    tlas = {}
+    for name, t in (("BVH", t_bvh), ("CWBVH", t_cw)):
+        dev = torch.from_numpy(t_rays.view(np.uint8).reshape(-1, 128).copy()).cuda()
+        t.Intersect(dev)
+        tlas[name] = (t, words(dev.cpu().numpy().view(R.RAY_DTYPE).reshape(-1)))
+    tlas["BVH_GPU"] = tlas["BVH"]
+    return SimpleNamespace(rays=rays, shadow=shadow, engines=engines, want=want_layout, tlas=tlas, t_rays=t_rays, blas=blas)
+
+
+def strided(rays, stride, pinned):
+    """bytes 0..63 of every 128-byte record in records of `stride` bytes, page-locked or pageable; bytes 64.. carry a pattern"""
+    n = rays.shape[0]
+    buf = api.pinned_empty(n * stride, np.uint8).reshape(n, stride) if pinned else np.empty((n, stride), np.uint8)
+    buf[:, :64] = rays.view(np.uint8).reshape(-1, 128)[:, :64]
+    buf[:, 64:] = (np.arange(n)[:, None] * 13 + np.arange(stride - 64)[None, :]) & 255
+    return buf
+
+
+@pytest.mark.parametrize("chunk", [4096, 1 << 19])
+@pytest.mark.parametrize("h2d_split", [1, 3])
+@pytest.mark.parametrize("host_path", [0, 1, 2])
+@pytest.mark.parametrize("layout", ["BVH", "BVH_GPU", "CWBVH"])
+@pytest.mark.parametrize("mode", [0, 1, 2, 3])
+def test_host_path_modes_return_the_same_hits(gpu, host_world, mode, layout, host_path, h2d_split, chunk):
+    """tbvh_intersect (in place), tbvh_intersect_packed and tbvh_occluded on host records of 128, 64, 144 and 136 bytes, page-locked and
+    pageable, under every d2h_mode, host_path, h2d_split and chunk size: the oracle's hits and occlusion words; in place only bytes
+    48..63 of a record change, the packed call and the any-hit call change no byte of the rays, and exactly (n+31)/32 words are
+    written.  A TLAS traces in place under each mode, and its packed call is refused."""
+    L = _lib.lib()
+    w = host_world
+    e, lay = w.engines[layout], getattr(api, "LAYOUT_" + layout)
+    want_hits, want_bits = w.want[layout]
+    n, nw = N_HOST, (N_HOST + 31) // 32
     api.set_option("d2h_mode", mode)
+    api.set_option("host_path", host_path)
+    api.set_option("h2d_split", h2d_split)
+    api.set_option("chunk_rays", chunk)
     try:
-        e = api.BVH().Build(v)
-        n = primary.shape[0]
-        pinned = api.pinned_empty(n, R.RAY_DTYPE)
-        pinned[:] = primary
-        e.Intersect(pinned)
-        assert util.compare_hits(pinned, want["primary"]) == ZERO, f"d2h_mode {mode} (pinned)"
-        pageable = primary.copy()
-        e.Intersect(pageable)
-        assert util.compare_hits(pageable, want["primary"]) == ZERO, f"d2h_mode {mode} (pageable)"
-        hits = e.IntersectPacked(primary)   # packed return path: rays untouched, 16-byte hits
-        assert np.array_equal(hits["t"].view(np.uint32), want["primary"]["t"].view(np.uint32)) and np.array_equal(hits["prim"], want["primary"]["prim"])
-        api.pinned_free(pinned)
+        for stride in STRIDES:
+            for pinned in (True, False):
+                label = f"{layout} d2h_mode {mode} host_path {host_path} h2d_split {h2d_split} chunk {chunk} stride {stride} {'pinned' if pinned else 'pageable'}"
+                buf = strided(w.rays, stride, pinned)
+                try:
+                    before = buf.copy()
+                    api.check(L.tbvh_intersect(e.h, lay, buf.ctypes.data, stride, n))
+                    bad = np.nonzero((hit_words(buf) != want_hits).any(1))[0]
+                    assert bad.size == 0, f"{label}: in-place hits differ on {bad.size} rays, first {bad[:5]}"
+                    assert np.array_equal(buf[:, :48], before[:, :48]) and np.array_equal(buf[:, 64:], before[:, 64:]), f"{label}: bytes outside 48..63 changed"
+                    buf[:] = before
+                    hits = np.zeros((n, 4), np.uint32)
+                    api.check(L.tbvh_intersect_packed(e.h, lay, buf.ctypes.data, stride, n, hits.ctypes.data))
+                    assert np.array_equal(hits, want_hits), f"{label}: packed hits differ on {(hits != want_hits).any(1).sum()} rays"
+                    assert np.array_equal(buf, before), f"{label}: the packed call changed the rays"
+                finally:
+                    if pinned:
+                        api.pinned_free(buf)
+                sh = strided(w.shadow, stride, pinned)
+                try:
+                    before = sh.copy()
+                    bits = np.full(nw + 1, SENTINEL, np.uint32)
+                    api.check(L.tbvh_occluded(e.h, lay, sh.ctypes.data, stride, n, bits.ctypes.data))
+                    assert np.array_equal(bits[:nw], want_bits), f"{label}: {np.unpackbits((bits[:nw] ^ want_bits).view(np.uint8)).sum()} occlusion bits differ"
+                    assert bits[nw] == SENTINEL, f"{label}: the word after (n+31)/32 was written"
+                    assert np.array_equal(sh, before), f"{label}: the any-hit call changed the rays"
+                finally:
+                    if pinned:
+                        api.pinned_free(sh)
+        t, t_want = w.tlas[layout]
+        for pinned in (True, False):
+            tr = api.pinned_empty(w.t_rays.shape[0], R.RAY_DTYPE) if pinned else np.empty_like(w.t_rays)
+            try:
+                tr[:] = w.t_rays
+                t.Intersect(tr)
+                assert np.array_equal(words(tr), t_want), f"TLAS over {layout} BLASses, d2h_mode {mode} host_path {host_path}: hits differ"
+            finally:
+                if pinned:
+                    api.pinned_free(tr)
+        with pytest.raises(api.TbvhError):
+            t.IntersectPacked(w.t_rays)   # TLAS hits carry the instance: in place only
     finally:
         api.set_option("d2h_mode", 1)
+        api.set_option("host_path", 0)
+        api.set_option("h2d_split", 1)
+        api.set_option("chunk_rays", 1 << 19)
+        api.set_option("trace_variant", 3)
 
 
 @pytest.mark.parametrize("small_t", [8, 64, 256])

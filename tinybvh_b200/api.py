@@ -51,6 +51,14 @@ def _is_torch(x) -> bool:
     return type(x).__module__.startswith("torch")
 
 
+def _stream_arg(stream, device):
+    """cudaStream_t of a `stream` argument: a torch.cuda.Stream, a raw handle, or None for torch's current stream on `device`."""
+    import torch
+    if stream is None:
+        return torch.cuda.current_stream(device).cuda_stream
+    return getattr(stream, "cuda_stream", stream)
+
+
 def _verts_arg(verts):
     """-> (pointer, stride, vertex count, space, keepalive)"""
     if _is_torch(verts):
@@ -112,14 +120,14 @@ class _Base:
     # -- traversal over batches
     def Intersect(self, rays, hits=None, stream=None):
         """Closest hit for every ray, in place (t,u,v,prim at bytes 48..63).  numpy -> host path (copies inside);
-        torch CUDA tensor -> device path, asynchronous on `stream` (default: torch's current stream)."""
+        torch CUDA tensor -> device path, asynchronous on `stream` (a torch.cuda.Stream or a raw cudaStream_t; default: torch's
+        current stream)."""
         L = _lib.lib()
         if _is_torch(rays):
-            import torch
             assert rays.is_cuda and rays.is_contiguous()
             stride = rays.stride(0) * rays.element_size() if rays.dim() > 1 else None
             assert stride in (64, 128), "ray tensor must be [n, 64|128 bytes]"
-            st = stream if stream is not None else torch.cuda.current_stream(rays.device).cuda_stream
+            st = _stream_arg(stream, rays.device)
             hp = C.c_void_p(hits.data_ptr()) if hits is not None else None
             check(L.tbvh_intersect_device(self.h, self.layout, C.c_void_p(rays.data_ptr()), stride, hp, rays.shape[0], C.c_void_p(st)))
             return rays if hits is None else hits
@@ -146,7 +154,7 @@ class _Base:
             n = rays.shape[0]
             if bits is None:
                 bits = torch.empty((n + 31) // 32, dtype=torch.int32, device=rays.device)
-            st = stream if stream is not None else torch.cuda.current_stream(rays.device).cuda_stream
+            st = _stream_arg(stream, rays.device)
             check(L.tbvh_occluded_device(self.h, self.layout, C.c_void_p(rays.data_ptr()), stride, C.c_void_p(bits.data_ptr()), n, C.c_void_p(st)))
             return bits
         assert rays.dtype.itemsize in (64, 128) and rays.flags.c_contiguous
