@@ -138,7 +138,10 @@ int tbvh_build_indexed( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32
  * BVH2 TLAS, per-instance ray transform, CWBVH BLASses, a BLAS hit kept when it is closer, the instance attached), semantics of
  * BVH8_CWBVH::Intersect (:7046) per BLAS.  A BLAS may hold either layout or both (CWBVH: tbvh_convert / tbvh_upload_cwbvh BEFORE
  * tbvh_build_tlas - the TLAS records the arrays each BLAS holds at that moment); walking a layout some BLAS did not hold is
- * TBVH_E_STATE, and so is walking a TLAS after one of its BLASses was rebuilt, re-converted, re-uploaded or destroyed. */
+ * TBVH_E_STATE, and so is walking a TLAS after one of its BLASses was rebuilt, re-converted, re-uploaded or destroyed.
+ * The two-level kernel walks a BVH-layout BLAS with a 64-entry stack: a BLAS whose BVH2 has depth 64 or more is refused
+ * (TBVH_E_LIMIT) unless it also holds its CWBVH; then the TLAS is built, walks in TBVH_LAYOUT_CWBVH run, and walks in
+ * TBVH_LAYOUT_BVH are refused with TBVH_E_LIMIT. */
 /* BVH::SAHCost( 0 ) tiny_bvh.h:1889-1897: the tree's SAH cost, host recursion over the (downloaded) 32-byte node array in the
  * reference's own order and rounding - the number the speedtest prints after every build.  _nodes works on a host array. */
 int tbvh_sah_cost( tbvh_bvh bvh, float c_trav, float c_int, float* out );

@@ -385,6 +385,7 @@ static void free_layouts( tbvh_bvh b )
 	for (void* q : p) if (q) cudaFree( q );
 	b->d_verts = 0, b->d_nodes = 0, b->d_prim_idx = 0, b->d_leaf_tris = 0, b->d_nodes_gpu = 0, b->d_cw_nodes = 0, b->d_cw_tris = 0, b->d_cw_trav = 0, b->d_trav = 0, b->leaf_tris_count = 0;
 	b->d_aabbs = 0, b->d_inst = 0, b->d_blas = 0, b->inst_count = 0, b->blas_count = 0, b->cw_pending = 0, b->tlas_blas_layouts = 0;
+	b->tlas_deep_blas = 0, b->tlas_deep_depth = 0;
 	b->links.clear();
 	cw_keep_free( b );
 	b->generation = tbvh_next_generation(); // a TLAS built over the old arrays must notice (tlas_check)
@@ -748,10 +749,18 @@ int tbvh_build_tlas( tbvh_bvh t, const void* instances, uint32_t inst_stride, ui
 	{
 		const tbvh_bvh b = blasses[k];
 		ARG_CHECK( b && b != t && b->ctx == t->ctx, "TLAS: a BLAS handle is NULL or lives in another context" );
-		const bool has_bvh = (b->info.layouts & (1u << TBVH_LAYOUT_BVH)) && b->d_trav && b->d_leaf_tris, has_cw = b->d_cw_trav && b->d_cw_tris;
+		bool has_bvh = (b->info.layouts & (1u << TBVH_LAYOUT_BVH)) && b->d_trav && b->d_leaf_tris;
+		const bool has_cw = b->d_cw_trav && b->d_cw_tris;
 		if (b->d_inst || (!has_bvh && !has_cw))
 		{ tbvh_set_error( "TLAS: BLAS %u holds no triangle tree (IntersectTLAS walks LAYOUT_BVH BLASses, tiny_bvh.h:3341; traverse_tlas.cl CWBVH ones)", k ); return TBVH_E_STATE; }
-		if (has_bvh && b->info.max_depth + 1 > TBVH_STACK) { tbvh_set_error( "TLAS: BLAS %u has depth %u, the two-level kernel walks a BLAS with a %d-entry stack", k, b->info.max_depth, TBVH_STACK ); return TBVH_E_LIMIT; }
+		if (has_bvh && b->info.max_depth + 1 > TBVH_STACK)
+		{
+			// the two-level kernel walks a BVH2 BLAS with a TBVH_STACK-entry stack; the CWBVH walk does not use it, so a BLAS that
+			// also holds its CWBVH stays usable through that layout, and a LAYOUT_BVH walk of the TLAS is refused (tlas_check)
+			if (!has_cw) { tbvh_set_error( "TLAS: BLAS %u has depth %u, the two-level kernel walks a BLAS with a %d-entry stack", k, b->info.max_depth, TBVH_STACK ); return TBVH_E_LIMIT; }
+			if (!t->tlas_deep_blas) t->tlas_deep_blas = k + 1, t->tlas_deep_depth = b->info.max_depth;
+			has_bvh = false;
+		}
 		if (has_cw && b->cw_pending == 0xffffffffu) { tbvh_set_error( "TLAS: the wide tree of BLAS %u has a cycle in its inner-child links", k ); return TBVH_E_ARG; }
 		if (has_cw && b->cw_pending > 128) { tbvh_set_error( "TLAS: the wide tree of BLAS %u can leave %u node groups pending (128 per ray, tiny_bvh.h:7048)", k, b->cw_pending ); return TBVH_E_LIMIT; }
 		refs[k].trav = has_bvh ? b->d_trav : 0, refs[k].tris = has_bvh ? b->d_leaf_tris : 0, refs[k].root_ref = b->root_ref, refs[k].root_count = b->root_count, refs[k].pad1 = 0;
@@ -918,6 +927,8 @@ static int tlas_check( tbvh_bvh t, int layout )
 	// the layout argument of a traversal call on a TLAS names the layout the BLASses are walked in (trace_tlas.cu)
 	const uint32_t want = layout == TBVH_LAYOUT_CWBVH ? 1u << TBVH_LAYOUT_CWBVH : 1u << TBVH_LAYOUT_BVH;
 	if (layout != TBVH_LAYOUT_CWBVH && layout != TBVH_LAYOUT_BVH && layout != TBVH_LAYOUT_BVH_GPU) { tbvh_set_error( "unknown layout %d", layout ); return TBVH_E_ARG; }
+	if (!(t->tlas_blas_layouts & want) && want == (1u << TBVH_LAYOUT_BVH) && t->tlas_deep_blas)
+	{ tbvh_set_error( "TLAS: BLAS %u has depth %u, the two-level kernel walks a BVH-layout BLAS with a %d-entry stack (walk its CWBVH layout)", t->tlas_deep_blas - 1, t->tlas_deep_depth, TBVH_STACK ); return TBVH_E_LIMIT; }
 	if (!(t->tlas_blas_layouts & want))
 	{ tbvh_set_error( "TLAS: not every BLAS held its %s layout when the TLAS was built", layout == TBVH_LAYOUT_CWBVH ? "CWBVH" : "BVH" ); return TBVH_E_STATE; }
 	std::lock_guard<std::mutex> lk( g_live_mutex );

@@ -102,6 +102,7 @@ struct tbvh_bvh_t
 	void* d_blas = 0;          // BlasRef records (traversal arrays of every BLAS)
 	uint32_t inst_count = 0, blas_count = 0;
 	uint32_t tlas_blas_layouts = 0; // TLAS only: layouts EVERY BLAS held at build time (bit TBVH_LAYOUT_BVH / TBVH_LAYOUT_CWBVH)
+	uint32_t tlas_deep_blas = 0, tlas_deep_depth = 0; // TLAS only: 1 + the first BLAS whose BVH2 is too deep for the two-level walk (0: none), and its depth
 	std::vector<BlasLink> links; // TLAS only: the BLAS handles it points into, with the generation they had at build time
 	bool refittable = true;    // BVHBase::refittable (:811): false after BuildHQ ("can't refit an SBVH", :3027)
 	struct CwKeep* cw_keep = 0; // refittable trees: the 8-wide collapse of the last tbvh_convert to CWBVH (convert_cwbvh.cu), for tbvh_refit_layouts
