@@ -8,6 +8,7 @@
 //
 // What is exposed (all cited lines are /root/reference/tiny_bvh.h):
 //   ref_bvh_build        -> BVH::Build  (:2124, scalar binned SAH "reference builder"), BuildAVX (:6351), BuildHQ (:2623)
+//   ref_bvh_optimize     -> BVH::Build (:2124) followed by BVH::Optimize (:3043, BVH_Verbose::Optimize :4338)
 //   ref_bvh_intersect    -> BVH::Intersect (:3222)      ref_bvh_occluded -> BVH::IsOccluded (:3382)
 //   ref_bvhgpu_*         -> BVH_GPU::ConvertFrom (:4612), BVH_GPU::Intersect (:4657)
 //   ref_cwbvh_*          -> BVH8_CWBVH::Build/BuildHQ (:5822-5866), ConvertFrom (:5884), CPU Intersect (:7046)
@@ -90,6 +91,16 @@ float ref_bvh_sah_cost( void* h ) { return ((BVH*)h)->SAHCost(); }
 void ref_bvh_compact( void* h ) { ((BVH*)h)->Compact(); }
 void ref_bvh_refit( void* h ) { ((BVH*)h)->Refit(); } // the caller has already moved the vertices in the array the BVH points at
 void ref_bvh_split_leafs( void* h, uint32_t maxPrims ) { ((BVH*)h)->SplitLeafs( maxPrims ); }
+// BVH::Build, then the reference's own reinsertion optimiser: the tree the shim's BVH::Optimize uploads (subtrees moved, every leaf
+// keeps its firstTri, so the leaf ranges are no longer in DFS order)
+void* ref_bvh_optimize( const float* verts, uint32_t primCount, uint32_t iterations, int extreme, int stochastic )
+{
+	BVH* b = new BVH();
+	b->threadedBuild = false;
+	b->Build( (const bvhvec4*)verts, primCount );
+	b->Optimize( iterations, extreme != 0, stochastic != 0 );
+	return b;
+}
 // wrap externally produced arrays (e.g. a GPU-built tree) so the reference can traverse / score them.
 void* ref_bvh_from_arrays( const void* nodes, uint32_t usedNodes, const uint32_t* primIdx, uint32_t idxCount, const float* verts, uint32_t primCount )
 {

@@ -40,6 +40,7 @@ def lib():
             "ref_bvh_sah_cost": (C.c_float, [vp]),
             "ref_bvh_compact": (None, [vp]), "ref_bvh_refit": (None, [vp]), "ref_bvh_split_leafs": (None, [vp, u32]),
             "ref_bvh_from_arrays": (vp, [vp, u32, vp, u32, vp, u32]),
+            "ref_bvh_optimize": (vp, [vp, u32, u32, i32, i32]),
             "ref_bvh_intersect": (None, [vp, vp, u64, i32]),
             "ref_bvh_intersect_cost": (u64, [vp, vp, u64, i32]),
             "ref_bvh_occluded": (None, [vp, vp, u64, vp, i32]),
@@ -127,6 +128,16 @@ class RefBVH(_Traceable):
         prim_idx = np.ascontiguousarray(prim_idx, np.uint32)
         self.h = lib().ref_bvh_from_arrays(_ptr(nodes), nodes.shape[0], _ptr(prim_idx), prim_idx.shape[0],
                                            _ptr(self.verts), self.verts.shape[0] // 3)
+        self._own = True
+        return self
+
+    @classmethod
+    def optimized(cls, verts, iterations: int = 25, extreme: bool = False, stochastic: bool = False):
+        """BVH::Build followed by the reference's BVH::Optimize( iterations, extreme, stochastic ) (ref_bvh_optimize)."""
+        self = cls.__new__(cls)
+        self._owner = None
+        self.verts = np.array(verts, np.float32, copy=True).reshape(-1, 4)
+        self.h = lib().ref_bvh_optimize(_ptr(self.verts), self.verts.shape[0] // 3, int(iterations), int(extreme), int(stochastic))
         self._own = True
         return self
 

@@ -96,6 +96,277 @@ def renumber_bfs(nodes):
     return out
 
 
+# ---- trees no builder makes: the same triangles under other valid BVH2s, for the consumers of an uploaded tree
+# Every family keeps node 1 unused, children behind their parent (BVH::Refit walks the nodes backwards) and every primIdx entry a
+# valid triangle number.  A tree is (nodes NODE32, primIdx[idx_count], idx_count).
+
+def source_tree(verts, builder):
+    """BVH::Build / BuildAVX / BuildHQ of a scene as an uploadable tree: primIdx padded with zeros to idxCount (the SBVH's tail)."""
+    o = oracle_tree(verts, {"Build": 0, "BuildAVX": 1, "BuildHQ": 2}[builder])
+    ic = int(getattr(o, "idx_count", o.prim_idx.shape[0]))
+    idx = np.zeros(ic, np.uint32)
+    idx[: o.prim_idx.shape[0]] = o.prim_idx
+    return np.ascontiguousarray(o.nodes).view(portpy.NODE32).reshape(-1).copy(), idx, ic
+
+
+def optimized_tree(verts, iterations=25):
+    """BVH::Build followed by the reference's own BVH::Optimize (needs oracle/_ref): the tree the shim's BVH::Optimize uploads."""
+    o = refpy.RefBVH.optimized(verts, iterations)
+    return np.ascontiguousarray(o.nodes).view(portpy.NODE32).reshape(-1).copy(), o.prim_idx.copy(), int(o.idx_count)
+
+
+def tree_levels(nodes):
+    """-> list of node-index arrays per depth (root = level 0), over the nodes reachable from the root."""
+    frontier, out = np.zeros(1, np.int64), []
+    while frontier.size:
+        out.append(frontier)
+        inner = frontier[nodes["triCount"][frontier] == 0]
+        first = nodes["leftFirst"][inner].astype(np.int64)
+        frontier = np.stack([first, first + 1], 1).reshape(-1)
+    return out
+
+
+def tree_depth(nodes):
+    return len(tree_levels(nodes)) - 1
+
+
+def dfs_leaves(nodes):
+    """-> leaf node indices in DFS order (left child first)."""
+    out, stack = [], [0]
+    lf, tc = nodes["leftFirst"], nodes["triCount"]
+    while stack:
+        x = stack.pop()
+        if tc[x]:
+            out.append(x)
+        else:
+            stack += [int(lf[x]) + 1, int(lf[x])]
+    return np.array(out, np.int64)
+
+
+def leaf_order_is_dfs(nodes):
+    """True when firstTri grows along the DFS leaf order: the order every builder leaves and BVH_GPU::ConvertFrom's old closed form
+    assumed."""
+    f = nodes["leftFirst"][dfs_leaves(nodes)].astype(np.int64)
+    return bool((np.diff(f) > 0).all())
+
+
+def refold_boxes(nodes):
+    """Interior boxes recomputed bottom-up from the leaf boxes with the reference's tinybvh_min / tinybvh_max (a < b ? a : b,
+    a > b ? a : b; left child first), in place."""
+    for lvl in reversed(tree_levels(nodes)):
+        inner = lvl[nodes["triCount"][lvl] == 0]
+        if inner.size == 0:
+            continue
+        c = nodes["leftFirst"][inner].astype(np.int64)
+        lmin, rmin = nodes["aabbMin"][c], nodes["aabbMin"][c + 1]
+        lmax, rmax = nodes["aabbMax"][c], nodes["aabbMax"][c + 1]
+        nodes["aabbMin"][inner] = np.where(lmin < rmin, lmin, rmin)
+        nodes["aabbMax"][inner] = np.where(lmax > rmax, lmax, rmax)
+    return nodes
+
+
+def swapped(tree, seed, frac):
+    """Family A: the two child records of a seeded share `frac` of the interior nodes exchanged (at least one; frac = 1 mirrors the
+    tree).  Numbering, boxes and primIdx stay; the DFS leaf order changes."""
+    nodes, idx, ic = tree
+    nodes = nodes.copy()
+    inner = np.concatenate(tree_levels(nodes))
+    inner = inner[nodes["triCount"][inner] == 0]
+    if inner.size:
+        rng = np.random.default_rng(seed)
+        pick = rng.permutation(inner)[: max(1, int(round(frac * inner.size)))]
+        c = nodes["leftFirst"][pick].astype(np.int64)
+        nodes[c], nodes[c + 1] = nodes[c + 1].copy(), nodes[c].copy()
+    return nodes, idx.copy(), ic
+
+
+def write_dfs(nodes, left, right, root):
+    """A tree given as child lists written back as BVH::ConvertFrom( BVH_Verbose ) writes it: DFS preorder, the k-th interior node's
+    children at 2 + 2k and 3 + 2k, leaves keep firstTri / triCount / box; interior boxes refolded."""
+    out = np.zeros(nodes.shape[0], portpy.NODE32)
+    nxt, stack = 2, [(root, 0)]
+    while stack:
+        s, d = stack.pop()
+        if left[s] < 0:
+            out[d] = nodes[s]
+            continue
+        out[d]["leftFirst"], out[d]["triCount"] = nxt, 0
+        stack += [(right[s], nxt + 1), (left[s], nxt)]
+        nxt += 2
+    assert nxt == nodes.shape[0], "the tree has holes"
+    return refold_boxes(out)
+
+
+def reinserted(tree, seed, k, max_depth=63, grow_to=None):
+    """Family B, the shape BVH::Optimize leaves: k seeded subtree reinsertions.  Subtree X leaves its parent P, X's sibling takes
+    P's place, and P becomes the parent of X and a node Y outside X's subtree (in either slot order).  A reinsertion that would
+    make the tree deeper than max_depth is not made.  grow_to: Y is the deepest leaf and X a leaf off its path, until the tree is
+    that deep (the 64..255 range of the 256-entry walk).  Written back in ConvertFrom( BVH_Verbose )'s numbering; leaves keep
+    firstTri, so the DFS leaf order no longer follows primIdx (more reinsertions are made until it does not)."""
+    nodes, idx, ic = tree
+    rng = np.random.default_rng(seed)
+    n = nodes.shape[0]
+    left, right, parent, height = [-1] * n, [-1] * n, [-1] * n, [0] * n
+    levels = tree_levels(nodes)
+    for lvl in reversed(levels):
+        for x in lvl.tolist():
+            if nodes["triCount"][x] == 0:
+                c = int(nodes["leftFirst"][x])
+                left[x], right[x], parent[c], parent[c + 1] = c, c + 1, x, x
+                height[x] = 1 + max(height[c], height[c + 1])
+    reach = np.concatenate(levels).tolist()
+    leaves = [x for x in reach if left[x] < 0]
+    if len(leaves) < 2:
+        return nodes.copy(), idx.copy(), ic
+    root = 0
+
+    def path(y):   # -> ancestors of y, nearest first
+        out = []
+        while parent[y] >= 0:
+            y = parent[y]
+            out.append(y)
+        return out
+
+    def replace(q, old, new):
+        if left[q] == old:
+            left[q] = new
+        else:
+            right[q] = new
+
+    def fix_heights(a):
+        while a >= 0:
+            height[a] = 1 + max(height[left[a]], height[right[a]])
+            a = parent[a]
+
+    def move(x, y):
+        nonlocal root
+        p = parent[x]
+        s = right[p] if left[p] == x else left[p]
+        g = parent[p]
+        if g < 0:
+            root, parent[s] = s, -1
+        else:
+            replace(g, p, s)
+            parent[s] = g
+        q = parent[y]
+        if q < 0:
+            root, parent[p] = p, -1
+        else:
+            replace(q, y, p)
+            parent[p] = q
+        left[p], right[p] = (x, y) if rng.random() < 0.5 else (y, x)
+        parent[x] = parent[y] = p
+        fix_heights(g)
+        fix_heights(p)
+
+    def try_move(x, y, limit):
+        if x == root or y == parent[x] or y == x:
+            return False
+        anc = path(y)
+        if x in anc:
+            return False
+        d = len(anc) - (parent[x] in anc)
+        if d + 1 + max(height[x], height[y]) > limit:
+            return False
+        move(x, y)
+        return True
+
+    def dfs_sorted():
+        order, stack = [], [root]
+        while stack:
+            a = stack.pop()
+            if left[a] < 0:
+                order.append(int(nodes["leftFirst"][a]))
+            else:
+                stack += [right[a], left[a]]
+        return all(order[i] < order[i + 1] for i in range(len(order) - 1))
+
+    done = tries = 0
+    while (done < k or dfs_sorted()) and tries < 50 * k + 1000:
+        tries += 1
+        done += try_move(reach[rng.integers(len(reach))], reach[rng.integers(len(reach))], max_depth)
+    while grow_to is not None and height[root] < grow_to:
+        y = root
+        while left[y] >= 0:
+            y = left[y] if height[left[y]] >= height[right[y]] else right[y]
+        try_move(leaves[rng.integers(len(leaves))], y, grow_to)
+    return write_dfs(nodes, left, right, root), idx.copy(), ic
+
+
+def shuffled_ranges(tree, seed, gap=0):
+    """Family C: the leaf blocks placed in primIdx in a seeded order (never the DFS order), leftFirst updated.  gap > 0: 1 .. gap
+    unreferenced entries holding triangle 0 after every block, so idxCount exceeds the referenced entries.  The source's tail of
+    unreferenced entries (an SBVH's) is kept."""
+    nodes, idx, ic = tree
+    nodes = nodes.copy()
+    leaves = dfs_leaves(nodes)
+    rng = np.random.default_rng(seed)
+    perm = rng.permutation(leaves.size)
+    if leaves.size > 1 and (np.diff(perm) > 0).all():
+        perm = np.roll(perm, 1)
+    parts, pos = [], 0
+    for j in perm.tolist():
+        x = leaves[j]
+        f, c = int(nodes["leftFirst"][x]), int(nodes["triCount"][x])
+        parts.append(idx[f:f + c])
+        nodes["leftFirst"][x] = pos
+        pos += c
+        if gap:
+            g = int(rng.integers(1, gap + 1))
+            parts.append(np.zeros(g, np.uint32))
+            pos += g
+    used = int(nodes["triCount"][leaves].sum())
+    parts.append(np.zeros(ic - used, np.uint32))
+    out = np.concatenate(parts).astype(np.uint32)
+    return nodes, out, out.shape[0]
+
+
+def renumbered(tree):
+    """Family D's last step: sibling pairs numbered breadth-first (renumber_bfs)."""
+    nodes, idx, ic = tree
+    return renumber_bfs(nodes), idx.copy(), ic
+
+
+FAMILIES = ["A0.3", "A1", "B", "C0", "C3", "DA", "DB", "DC"]
+
+
+def family_tree(tree, fam, seed):
+    """A tree of family `fam` (FAMILIES) made from a builder's tree: A0.3 / A1 swapped(0.3 / 1), B reinserted, C0 / C3
+    shuffled_ranges(0 / 3), DA / DB / DC the BFS renumbering of swapped(0.3), reinserted and shuffled_ranges(3)."""
+    if fam.startswith("D"):
+        return renumbered(family_tree(tree, {"DA": "A0.3", "DB": "B", "DC": "C3"}[fam], seed))
+    if fam.startswith("A"):
+        return swapped(tree, seed, float(fam[1:]))
+    if fam == "B":
+        nodes = tree[0]
+        return reinserted(tree, seed, max(4, min(400, nodes.shape[0] // 8)))
+    return shuffled_ranges(tree, seed, int(fam[1:]))
+
+
+def check_tree(tree, ntris):
+    """The structural claims of every family: every node reachable exactly once (node 1 unused), leaf ranges disjoint and inside
+    primIdx, children behind their parent, every primIdx entry a triangle, every interior box the fold of its children's.
+    -> the tree's depth."""
+    nodes, idx, ic = tree
+    assert idx.shape[0] == ic and (idx < ntris).all()
+    levels = tree_levels(nodes)
+    reach = np.concatenate(levels)
+    want = np.ones(nodes.shape[0], np.int64)
+    want[1:2] = 0
+    assert np.array_equal(np.bincount(reach, minlength=nodes.shape[0]), want), "every node but node 1 reachable exactly once"
+    leaf = reach[nodes["triCount"][reach] > 0]
+    inner = reach[nodes["triCount"][reach] == 0]
+    c = nodes["leftFirst"][inner].astype(np.int64)
+    assert (c > inner).all() and (c % 2 == 0).all(), "children sit behind their parent, in pairs from 2"
+    f, n = nodes["leftFirst"][leaf].astype(np.int64), nodes["triCount"][leaf].astype(np.int64)
+    o = np.argsort(f)
+    assert (f + n <= ic).all() and (f[o][1:] >= (f + n)[o][:-1]).all(), "leaf ranges in bounds and disjoint"
+    lmin, rmin, lmax, rmax = nodes["aabbMin"][c], nodes["aabbMin"][c + 1], nodes["aabbMax"][c], nodes["aabbMax"][c + 1]
+    assert np.array_equal(bits_u32(nodes["aabbMin"][inner]), bits_u32(np.where(lmin < rmin, lmin, rmin)))
+    assert np.array_equal(bits_u32(nodes["aabbMax"][inner]), bits_u32(np.where(lmax > rmax, lmax, rmax)))
+    return len(levels) - 1
+
+
 def small_scene(ntris=6000, seed=7):
     return scenes.procedural_scene(ntris, seed)
 

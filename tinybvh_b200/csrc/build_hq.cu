@@ -1077,23 +1077,11 @@ __global__ void __launch_bounds__( HQ_SMALL_WARPS * 32, 6 ) k_hq_subtrees( HQArg
 // bottom-up: number of interior nodes / of leaf index entries per subtree (second arrival at a parent carries on)
 __global__ void k_hq_up( HQArgs A, const uint32_t tmp_count )
 {
-	uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= tmp_count || x == 1) return;
 	const uint32_t cnt = __float_as_uint( A.tmp_nodes[(size_t)x * 2 + 1].w );
 	if (cnt == 0) return; // interior
-	A.sub_int[x] = 0, A.sub_prims[x] = cnt;
-	for (;;)
-	{
-		const uint32_t p = A.parent[x];
-		if (p == 0xffffffffu) break;
-		__threadfence();
-		if (atomicAdd( &A.arrive[p], 1u ) == 0) break;
-		__threadfence();
-		const uint32_t lc = __float_as_uint( A.tmp_nodes[(size_t)p * 2].w );
-		const volatile uint32_t* si = A.sub_int; const volatile uint32_t* sp = A.sub_prims;
-		A.sub_int[p] = si[lc] + si[lc + 1] + 1, A.sub_prims[p] = sp[lc] + sp[lc + 1];
-		x = p;
-	}
+	dfs_sizes_up( A.tmp_nodes, A.parent, A.arrive, A.sub_int, A.sub_prims, x, cnt );
 }
 // top-down by walking to the root: K = interior nodes before x in DFS preorder, O = leaf index entries before x
 __global__ void k_hq_down( HQArgs A, const uint32_t tmp_count, float4* out_nodes, uint32_t* out_idx )
@@ -1101,15 +1089,8 @@ __global__ void k_hq_down( HQArgs A, const uint32_t tmp_count, float4* out_nodes
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= tmp_count) return;
 	if (x == 1) { out_nodes[2] = out_nodes[3] = make_float4( 0, 0, 0, 0 ); return; }
-	uint32_t K = 0, O = 0, c = x, Kparent = 0;
-	while (c != 0)
-	{
-		const uint32_t p = A.parent[c], lc = __float_as_uint( A.tmp_nodes[(size_t)p * 2].w );
-		uint32_t add = 1;
-		if (c == lc + 1) add += A.sub_int[lc], O += A.sub_prims[lc];
-		if (c == x) Kparent = add; // K(parent) = K(x) - add, fixed up below
-		K += add, c = p;
-	}
+	uint32_t K, O, Kparent; // K(parent) = K(x) - Kparent
+	dfs_rank( A.tmp_nodes, A.parent, A.sub_int, A.sub_prims, x, K, O, Kparent );
 	const uint32_t dst = x == 0 ? 0u : 2u + 2u * (K - Kparent) + ((x & 1u) ? 1u : 0u); // pairs start at even temp indices: odd = right child
 	const float4 a = A.tmp_nodes[(size_t)x * 2], b = A.tmp_nodes[(size_t)x * 2 + 1];
 	const uint32_t cnt = __float_as_uint( b.w );

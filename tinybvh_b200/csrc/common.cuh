@@ -152,6 +152,44 @@ __device__ __forceinline__ uint32_t zpos_word( const uint32_t pos, const float f
 // the key of a zero bound whose sign a position word decided (0: no word, keep the key)
 __device__ __forceinline__ uint32_t zero_resolve( const uint32_t key, const uint32_t zw ) { return (zw && zero_key( key )) ? ((zw & 1u) ? 0x7fffffffu : 0x80000000u) : key; }
 
+// ---- DFS preorder of a BVH2 in the reference's layout (node 1 unused, children paired at leftFirst), whatever its numbering and
+// whatever the order of its leaf ranges in primIdx.  Used by BuildHQ's Compact() (build_hq.cu) and BVH_GPU::ConvertFrom (convert.cu).
+// parent[]: the parent of every reachable node, 0xffffffff for the root.
+// Bottom-up from leaf x carrying weight w: sub_int[] = interior nodes per subtree, sub_w[] = summed leaf weights per subtree.  The
+// second arrival at a parent (arrive[] zeroed beforehand) sums both children and carries on, as refit.cu climbs.
+__device__ __forceinline__ void dfs_sizes_up( const float4* nodes, const uint32_t* parent, uint32_t* arrive, uint32_t* sub_int, uint32_t* sub_w,
+	uint32_t x, const uint32_t w )
+{
+	sub_int[x] = 0, sub_w[x] = w;
+	for (;;)
+	{
+		const uint32_t p = parent[x];
+		if (p == 0xffffffffu) break;
+		__threadfence();
+		if (atomicAdd( &arrive[p], 1u ) == 0) break;
+		__threadfence();
+		const uint32_t lc = __float_as_uint( nodes[(size_t)p * 2].w );
+		const volatile uint32_t* si = sub_int; const volatile uint32_t* sw = sub_w;
+		sub_int[p] = si[lc] + si[lc + 1] + 1, sub_w[p] = sw[lc] + sw[lc + 1];
+		x = p;
+	}
+}
+// Top-down by walking x's path to the root: K = interior nodes before x in DFS preorder, O = leaf weights before x, Kp = the part of
+// K that x's own step added (K of x's parent is K - Kp).  With every leaf weighing 1, x's preorder index is K + O.
+__device__ __forceinline__ void dfs_rank( const float4* nodes, const uint32_t* parent, const uint32_t* sub_int, const uint32_t* sub_w,
+	const uint32_t x, uint32_t& K, uint32_t& O, uint32_t& Kp )
+{
+	K = 0, O = 0, Kp = 0;
+	for (uint32_t c = x; c != 0;)
+	{
+		const uint32_t p = parent[c], lc = __float_as_uint( nodes[(size_t)p * 2].w );
+		uint32_t add = 1;
+		if (c == lc + 1) add += sub_int[lc], O += sub_w[lc];
+		if (c == x) Kp = add;
+		K += add, c = p;
+	}
+}
+
 // ---- internal entry points (one per .cu) -------------------------------------------------------------------
 // d_stats: NULL, or two counters the launch ADDS its node visits / triangle tests to (the caller zeroes them once per API call)
 int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );

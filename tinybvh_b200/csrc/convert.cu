@@ -66,14 +66,11 @@ int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used, cudaStream_t s )
 }
 
 // ---- BVH -> BVH_GPU (BVH_GPU::ConvertFrom, tiny_bvh.h:4612-4655) --------------------------------------------------
-// The reference re-lays the tree out in DFS preorder (node, left subtree, right subtree).  With f = first primitive of a
-// node's range, the preorder index of a node is
-//     (#interior nodes before it) + (#leaves before it)
-//   = prefI[f] + chainpos + prefL[f]                 for an interior node
-//   = prefI[f] + cntI[f]  + prefL[f]                 for a leaf
-// where cntI[f] = number of interior nodes whose range starts at f (the left-spine chain above the leaf starting at f),
-// chainpos = position in that chain counted from its top, and prefI / prefL are exclusive prefix sums over positions.
-// Every leaf walks its own left spine, so all of this is atomics-free.
+// The reference re-lays the tree out in DFS preorder (node, left subtree, right subtree) with an explicit stack.  Here the preorder
+// index of every node comes from subtree sizes (dfs_sizes_up / dfs_rank in common.cuh, shared with BuildHQ's Compact):
+//     pre(left) = pre(p) + 1,   pre(right) = pre(p) + 1 + size(left)
+// so it depends on the tree's shape alone: neither on the node numbering nor on the order of the leaf ranges in primIdx (a tree
+// after BVH::Optimize, or uploaded from elsewhere, has its leaf ranges out of DFS order).
 __global__ void k_gpu_parents( const float4* __restrict__ nodes, uint32_t* __restrict__ parent, const uint32_t used )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
@@ -84,51 +81,37 @@ __global__ void k_gpu_parents( const float4* __restrict__ nodes, uint32_t* __res
 	parent[c] = x, parent[c + 1] = x;
 }
 
-__global__ void k_gpu_spines( const float4* __restrict__ nodes, const uint32_t* __restrict__ parent, uint32_t* __restrict__ first,
-	uint32_t* __restrict__ chainpos, uint32_t* __restrict__ cntL, uint32_t* __restrict__ cntI, const uint32_t used )
+// bottom-up from every leaf: interior nodes and leaves per subtree (every leaf weighs 1)
+__global__ void k_gpu_sizes( const float4* __restrict__ nodes, const uint32_t* __restrict__ parent, uint32_t* arrive, uint32_t* sub_int, uint32_t* sub_leaves,
+	const uint32_t used )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= used || x == 1) return;
 	if (__float_as_uint( nodes[(size_t)x * 2 + 1].w ) == 0) return; // leaves only
-	const uint32_t f = __float_as_uint( nodes[(size_t)x * 2].w );
-	first[x] = f, cntL[f] = 1;
-	uint32_t len = 0;
-	for (uint32_t a = x; a != 0; len++)
-	{
-		const uint32_t p = parent[a];
-		if (__float_as_uint( nodes[(size_t)p * 2].w ) != a) break; // a is a right child: chain ends
-		a = p;
-	}
-	cntI[f] = len;
-	uint32_t a = x;
-	for (uint32_t k = len; k > 0; k--)
-	{
-		const uint32_t p = parent[a];
-		first[p] = f, chainpos[p] = k - 1;
-		a = p;
-	}
+	dfs_sizes_up( nodes, parent, arrive, sub_int, sub_leaves, x, 1u );
 }
 
-__global__ void k_gpu_emit( const float4* __restrict__ nodes, const uint32_t* __restrict__ first, const uint32_t* __restrict__ chainpos,
-	const uint32_t* __restrict__ cntI, const uint32_t* __restrict__ prefL, const uint32_t* __restrict__ prefI, float4* __restrict__ out, const uint32_t used )
+// one thread per node: its preorder index from its path to the root; an interior node's left child follows it, its right child
+// follows the left subtree (sub_int + sub_leaves nodes)
+__global__ void k_gpu_emit( const float4* __restrict__ nodes, const uint32_t* __restrict__ parent, const uint32_t* __restrict__ sub_int,
+	const uint32_t* __restrict__ sub_leaves, float4* __restrict__ out, const uint32_t used )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= used || x == 1) return;
 	const float4 a = nodes[(size_t)x * 2], b = nodes[(size_t)x * 2 + 1];
-	const uint32_t f = first[x], cnt = __float_as_uint( b.w );
+	uint32_t K, L, Kp;
+	dfs_rank( nodes, parent, sub_int, sub_leaves, x, K, L, Kp );
+	const uint32_t idx = K + L, cnt = __float_as_uint( b.w );
 	const float4 z = make_float4( 0, 0, 0, 0 );
 	if (cnt)
 	{
-		const uint32_t idx = prefI[f] + cntI[f] + prefL[f];
 		out[(size_t)idx * 4] = z, out[(size_t)idx * 4 + 1] = z;
 		out[(size_t)idx * 4 + 2] = make_float4( 0, 0, 0, __uint_as_float( cnt ) ), out[(size_t)idx * 4 + 3] = make_float4( 0, 0, 0, a.w );
 		return;
 	}
-	const uint32_t idx = prefI[f] + chainpos[x] + prefL[f];
 	const uint32_t c = __float_as_uint( a.w );
 	const float4 l0 = nodes[(size_t)c * 2], l1 = nodes[(size_t)c * 2 + 1], r0 = nodes[(size_t)c * 2 + 2], r1 = nodes[(size_t)c * 2 + 3];
-	const uint32_t fr = first[c + 1];
-	const uint32_t ridx = prefI[fr] + (__float_as_uint( r1.w ) ? cntI[fr] : chainpos[c + 1]) + prefL[fr];
+	const uint32_t ridx = idx + 1 + sub_int[c] + sub_leaves[c];
 	out[(size_t)idx * 4] = make_float4( l0.x, l0.y, l0.z, __uint_as_float( idx + 1 ) );
 	out[(size_t)idx * 4 + 1] = make_float4( l1.x, l1.y, l1.z, __uint_as_float( ridx ) );
 	out[(size_t)idx * 4 + 2] = make_float4( r0.x, r0.y, r0.z, __uint_as_float( 0u ) );
@@ -137,25 +120,22 @@ __global__ void k_gpu_emit( const float4* __restrict__ nodes, const uint32_t* __
 
 int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s )
 {
-	const uint32_t used = b->info.used_nodes, n = b->info.idx_count;
+	const uint32_t used = b->info.used_nodes;
 	if (b->d_nodes_gpu) cudaFree( b->d_nodes_gpu );
 	b->d_nodes_gpu = 0;
 	CUDA_TRY( cudaMalloc( &b->d_nodes_gpu, (size_t)used * 64 ) );
-	uint32_t* w = 0; // workspace: parent, first, chainpos [used] ; cntL, cntI, prefL, prefI [n+1] ; tile sums
-	const size_t words = (size_t)used * 3 + ((size_t)n + 1) * 4 + (n / 2048 + 2);
+	uint32_t* w = 0; // workspace: parent, arrive, sub_int, sub_leaves [used]
+	const size_t words = (size_t)used * 4;
 	CUDA_TRY( cudaMalloc( &w, words * 4 ) );
-	uint32_t* parent = w, * first = w + used, * chainpos = first + used, * cntL = chainpos + used, * cntI = cntL + (n + 1);
-	uint32_t* prefL = cntI + (n + 1), * prefI = prefL + (n + 1), * tile = prefI + (n + 1);
+	uint32_t* parent = w, * arrive = w + used, * sub_int = arrive + used, * sub_leaves = sub_int + used;
 	int rc = TBVH_OK;
 	auto body = [&]() -> int
 	{
 		CUDA_TRY( cudaMemsetAsync( w, 0, words * 4, s ) );
 		const uint32_t g = (used + 255) / 256;
 		k_gpu_parents<<<g, 256, 0, s>>>( b->d_nodes, parent, used ); LAUNCHED();
-		k_gpu_spines<<<g, 256, 0, s>>>( b->d_nodes, parent, first, chainpos, cntL, cntI, used ); LAUNCHED();
-		{ const int r = exclusive_scan( cntL, prefL, tile, n, s ); if (r != TBVH_OK) return r; }
-		{ const int r = exclusive_scan( cntI, prefI, tile, n, s ); if (r != TBVH_OK) return r; }
-		k_gpu_emit<<<g, 256, 0, s>>>( b->d_nodes, first, chainpos, cntI, prefL, prefI, b->d_nodes_gpu, used ); LAUNCHED();
+		k_gpu_sizes<<<g, 256, 0, s>>>( b->d_nodes, parent, arrive, sub_int, sub_leaves, used ); LAUNCHED();
+		k_gpu_emit<<<g, 256, 0, s>>>( b->d_nodes, parent, sub_int, sub_leaves, b->d_nodes_gpu, used ); LAUNCHED();
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
 	};
