@@ -124,6 +124,29 @@ int tbvh_build_flavour( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32
 int tbvh_build_indexed( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space,
 	float c_trav, float c_int, int flavour );
 
+/* Many meshes in one call: a binned-SAH tree per mesh, as the reference's scene code builds one BLAS per mesh (tiny_scene.h,
+ * tmpl8/game.cpp).  bvhs[i] receives the tree of meshes[i] and ends up exactly as tbvh_build_flavour (or, with indices,
+ * tbvh_build_indexed) of that mesh alone would leave it: nodes, primIdx and leaf triangles byte for byte, the same info (build_ms is
+ * the device time of the whole batch), layout TBVH_LAYOUT_BVH, refittable, and a TLAS built over its old arrays is stale.  The
+ * trees are built together by the same kernels, so the fixed cost of a build (allocations, launches, host round trips) is paid once
+ * per batch instead of once per mesh; the order of `meshes` changes no tree.  All meshes are in one `space`; device-space inputs
+ * follow the rule above.
+ *  flavour: TBVH_BUILD_REFERENCE or TBVH_BUILD_AVX; TBVH_BUILD_HQ is TBVH_E_UNSUPPORTED (one SBVH per tbvh_build_flavour call).
+ *  Refusals come before any handle is touched, so every handle keeps its previous tree: TBVH_E_ARG for count 0, a NULL or repeated
+ *  handle, handles of different contexts, prim_count 0, a bad stride, or any index >= vert_count; TBVH_E_LIMIT when the meshes
+ *  hold more than TBVH_BATCH_MAX_PRIMS triangles together (positions of one shared index space must fit the builder's 32-bit
+ *  encodings).  A failure after the device work started leaves every handle of the batch empty, as a failed build does. */
+typedef struct tbvh_mesh
+{
+	const void* verts;          /* as for tbvh_build (flat: 3 * prim_count vertices) or tbvh_build_indexed (vert_count vertices) */
+	uint32_t stride;            /* bytes between vertices, a multiple of 4, at least 12 */
+	uint32_t vert_count;        /* used with indices only */
+	const uint32_t* indices;    /* NULL: flat triangle soup; else 3 * prim_count vertex indices, in the same space as verts */
+	uint32_t prim_count;
+} tbvh_mesh;
+#define TBVH_BATCH_MAX_PRIMS (1u << 30)
+int tbvh_build_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int, int flavour );
+
 /* TLAS: BVH::Build( BLASInstance* instances, instCount, BVHBase** blasses, blasCount ) tiny_bvh.h:2221, traversed by
  * BVH::IntersectTLAS (:3306) / IsOccludedTLAS (:3455) whenever tbvh_intersect / tbvh_occluded (or the _device forms) are
  * called on the handle.  instances: inst_count records of the reference's 192-byte BLASInstance (:1443), inst_stride bytes

@@ -58,6 +58,11 @@ inline tbvh_ctx context( int device = -1 )
 inline void* malloc_pinned( size_t bytes ) { void* p = 0; TBVH_FATAL_IF( tbvh_host_alloc( bytes, &p ), "malloc_pinned" ); return p; }
 inline void free_pinned( void* p ) { tbvh_host_free( p ); }
 
+// Many meshes in one call (tbvh_build_batch): objs[i] ends up as if its own Build( vertices[i], primCounts[i] ) had run - the tree,
+// Refit and Optimize working from the caller's arrays, the public counters.  flavour: TBVH_BUILD_REFERENCE (BVH::Build) or
+// TBVH_BUILD_AVX; by default the builder the class's own Build uses.  BVH_GPU / BVH8_CWBVH objects are converted afterwards.
+template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* const* vertices, const uint32_t* primCounts, uint32_t count, int flavour = -1 );
+
 class BVHBase
 {
 public:
@@ -143,11 +148,13 @@ protected:
 	bool own = true;
 	friend class BVH_GPU;
 	friend class BVH8_CWBVH;
+	template <class T, class Vec4> friend void BuildBatch( T* const*, const Vec4* const*, const uint32_t*, uint32_t, int );
 };
 
 class BVH : public BVHBase
 {
 public:
+	static constexpr int defaultFlavour = TBVH_BUILD_REFERENCE; // BVH::Build
 	BVH() : BVHBase( TBVH_LAYOUT_BVH ) {}
 	// BVH::Build( const bvhvec4* vertices, uint32_t primCount ) tiny_bvh.h:2124 - binned SAH on the GPU
 	template <class Vec4> void Build( const Vec4* vertices, const uint32_t primCount )
@@ -275,6 +282,8 @@ public:
 	}
 #endif
 private:
+	template <class T, class Vec4> friend void BuildBatch( T* const*, const Vec4* const*, const uint32_t*, uint32_t, int );
+	void batch_built( const void* v, uint32_t stride, uint32_t prims ) { remember( v, stride, 0, prims ), sync_info(); }
 	void remember( const void* v, uint32_t stride, const uint32_t* idx, uint32_t prims ) { vertsPtr = v, vertsStride = stride, vertIdx = idx, vertsPrims = prims; }
 	const void* vertsPtr = 0; const uint32_t* vertIdx = 0; // BVHBase::verts / vertIdx (:806-807): pointers to the caller's arrays, for Refit
 	uint32_t vertsStride = 16, vertsPrims = 0;
@@ -283,6 +292,7 @@ private:
 class BVH_GPU : public BVHBase
 {
 public:
+	static constexpr int defaultFlavour = TBVH_BUILD_AVX; // BuildDefault on x86 (tiny_bvh.h:1817-1832)
 	BVH_GPU() : BVHBase( TBVH_LAYOUT_BVH_GPU ) {}
 	template <class Vec4> void Build( const Vec4* vertices, const uint32_t primCount )
 	{
@@ -318,11 +328,15 @@ public:
 		sync_info();
 	}
 	void Download( void* bvhNode ) const { TBVH_FATAL_IF( tbvh_download_bvh_gpu( h, bvhNode, TBVH_HOST ), "BVH_GPU::Download" ); }
+private:
+	template <class T, class Vec4> friend void BuildBatch( T* const*, const Vec4* const*, const uint32_t*, uint32_t, int );
+	void batch_built( const void*, uint32_t, uint32_t ) { TBVH_FATAL_IF( tbvh_convert( h, TBVH_LAYOUT_BVH_GPU ), "BuildBatch" ); sync_info(); }
 };
 
 class BVH8_CWBVH : public BVHBase
 {
 public:
+	static constexpr int defaultFlavour = TBVH_BUILD_AVX; // BuildDefault on x86 (tiny_bvh.h:5830)
 	BVH8_CWBVH() : BVHBase( TBVH_LAYOUT_CWBVH ) {}
 	uint32_t usedBlocks = 0;
 	template <class Vec4> void Build( const Vec4* vertices, const uint32_t primCount )
@@ -386,7 +400,26 @@ public:
 		return true;
 	}
 #endif
+private:
+	template <class T, class Vec4> friend void BuildBatch( T* const*, const Vec4* const*, const uint32_t*, uint32_t, int );
+	void batch_built( const void*, uint32_t, uint32_t ) { TBVH_FATAL_IF( tbvh_convert( h, TBVH_LAYOUT_CWBVH ), "BuildBatch" ); sync_info(), usedBlocks = Info().used_blocks; }
 };
+
+template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* const* vertices, const uint32_t* primCounts, uint32_t count, int flavour )
+{
+	tbvh_bvh* hs = (tbvh_bvh*)malloc( sizeof( tbvh_bvh ) * (count ? count : 1) );
+	tbvh_mesh* ms = (tbvh_mesh*)calloc( count ? count : 1, sizeof( tbvh_mesh ) );
+	for (uint32_t k = 0; k < count; k++)
+	{
+		hs[k] = objs[k] ? objs[k]->handle() : 0;
+		ms[k].verts = vertices[k], ms[k].stride = (uint32_t)sizeof( Vec4 ), ms[k].prim_count = primCounts[k];
+	}
+	const int rc = tbvh_build_batch( hs, ms, count, TBVH_HOST, count && objs[0] ? objs[0]->c_trav : 1.0f, count && objs[0] ? objs[0]->c_int : 1.0f,
+		flavour < 0 ? T::defaultFlavour : flavour );
+	free( hs ), free( ms );
+	TBVH_FATAL_IF( rc, "BuildBatch" );
+	for (uint32_t k = 0; k < count; k++) objs[k]->batch_built( vertices[k], (uint32_t)sizeof( Vec4 ), primCounts[k] );
+}
 
 } // namespace tinybvh_b200
 

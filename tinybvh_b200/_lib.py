@@ -10,6 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "libtinybvh_b200.so")
 
 OK, HOST, DEVICE = 0, 0, 1
+E_CUDA, E_ARG, E_STATE, E_LIMIT, E_UNSUPPORTED = -1, -2, -3, -4, -5
 LAYOUT_BVH, LAYOUT_BVH_GPU, LAYOUT_CWBVH = 1, 5, 10
 BUILD_REFERENCE, BUILD_AVX, BUILD_HQ = 0, 1, 2
 
@@ -23,6 +24,11 @@ class Info(C.Structure):
                 ("used_nodes_gpu", C.c_uint32), ("used_blocks", C.c_uint32), ("cwbvh_tri_count", C.c_uint32),
                 ("max_depth", C.c_uint32), ("layouts", C.c_uint32),
                 ("aabb_min", C.c_float * 3), ("aabb_max", C.c_float * 3), ("build_ms", C.c_double)]
+
+
+class Mesh(C.Structure):
+    """tbvh_mesh: one mesh of a tbvh_build_batch call"""
+    _fields_ = [("verts", C.c_void_p), ("stride", C.c_uint32), ("vert_count", C.c_uint32), ("indices", C.c_void_p), ("prim_count", C.c_uint32)]
 
 
 # every symbol include/tinybvh_b200.h declares: name -> (restype, argtypes)
@@ -50,6 +56,7 @@ SYMBOLS = {
     "tbvh_refit": (i32, [vp, vp, u32, u32, i32]),
     "tbvh_refit_layouts": (i32, [vp, vp, u32, u32, i32]),
     "tbvh_build_indexed": (i32, [vp, vp, u32, u32, vp, u32, i32, f32, f32, i32]),
+    "tbvh_build_batch": (i32, [vp, vp, u32, i32, f32, f32, i32]),
     "tbvh_upload_bvh": (i32, [vp, vp, u32, vp, u32, vp, u32, u32, i32]),
     "tbvh_upload_bvh_gpu": (i32, [vp, vp, u32, vp, u32, vp, u32, u32, i32]),
     "tbvh_upload_cwbvh": (i32, [vp, vp, u32, vp, u32, i32]),

@@ -331,6 +331,47 @@ class BVH8_CWBVH(_Base):
         return d, t
 
 
+def build_batch(bvhs, meshes, flavour: int = _lib.BUILD_REFERENCE, indices=None):
+    """tbvh_build_batch: one binned-SAH tree per mesh, all built in one call.  bvhs[i] ends up as bvhs[i].Build(meshes[i]) (flavour
+    BUILD_REFERENCE) or .BuildAVX (BUILD_AVX) would leave it.  `meshes`: numpy vertex arrays, or torch CUDA tensors - one space per
+    call; `indices`: None, or one entry per mesh (None for a flat mesh, else its vertex indices in the same space).  BVH_GPU and
+    BVH8_CWBVH objects are converted afterwards, as their Build does.  A refused batch raises TbvhError and leaves every object as
+    it was."""
+    bvhs, meshes = list(bvhs), list(meshes)
+    if len(bvhs) != len(meshes):
+        raise TbvhError("build_batch: one object per mesh")
+    indices = [None] * len(meshes) if indices is None else list(indices)
+    if len(indices) != len(meshes):
+        raise TbvhError("build_batch: one index entry per mesh")
+    if len({_is_torch(m) for m in meshes}) > 1:
+        raise TbvhError("build_batch: host and device meshes in one call")
+    recs = (_lib.Mesh * max(len(meshes), 1))()
+    keep, space = [], HOST
+    for r, m, ix in zip(recs, meshes, indices):
+        p, stride, nv, space, k = _verts_arg(m)
+        keep.append(k)
+        r.verts, r.stride = p.value, stride
+        if ix is None:
+            r.vert_count, r.indices, r.prim_count = 0, None, nv // 3
+            continue
+        if _is_torch(ix):
+            assert space == DEVICE and ix.is_cuda and ix.is_contiguous() and ix.element_size() == 4
+            r.indices, n = ix.data_ptr(), ix.numel()
+        else:
+            assert space == HOST, "device vertices need device indices"
+            ix = np.ascontiguousarray(ix, np.uint32).reshape(-1)
+            r.indices, n = ix.ctypes.data, ix.shape[0]
+        keep.append(ix)
+        r.vert_count, r.prim_count = nv, n // 3
+    hs = (C.c_void_p * max(len(bvhs), 1))(*[b.h for b in bvhs]) if bvhs else None
+    c0 = bvhs[0] if bvhs else None
+    check(_lib.lib().tbvh_build_batch(hs, recs, len(meshes), space, c0.c_trav if c0 else 1.0, c0.c_int if c0 else 1.0, flavour))
+    for b in bvhs:
+        if b.layout != LAYOUT_BVH:
+            check(_lib.lib().tbvh_convert(b.h, b.layout))
+    return bvhs
+
+
 def pinned_empty(n: int, dtype, device: int = None, node: int = None) -> np.ndarray:
     """numpy array in page-locked host memory on the NUMA node of `device` (default: the current CUDA device): full-speed DMA
     for the host path (tbvh_host_alloc / tbvh_host_alloc_near)."""

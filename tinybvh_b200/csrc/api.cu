@@ -4,6 +4,7 @@
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <vector>
 #include <thread>
 #include <atomic>
@@ -431,18 +432,23 @@ int tbvh_get_stats_ex( tbvh_bvh b, uint64_t out[4] )
 // ---- uploads ------------------------------------------------------------------------------------------------
 
 // vertices -> engine-owned float4 array (xyz of each vertex, w copied when the stride holds it)
+static int copy_verts( float4* dst, const void* verts, uint32_t stride, size_t nv, int space, cudaStream_t s )
+{
+	const cudaMemcpyKind kind = space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+	if (stride == 16) CUDA_TRY( cudaMemcpyAsync( dst, verts, nv * 16, kind, s ) );
+	else
+	{
+		CUDA_TRY( cudaMemsetAsync( dst, 0, nv * 16, s ) );
+		CUDA_TRY( cudaMemcpy2DAsync( dst, 16, verts, stride, stride < 16 ? stride : 16, nv, kind, s ) );
+	}
+	return TBVH_OK;
+}
 static int upload_verts( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space, cudaStream_t s )
 {
 	ARG_CHECK( verts && stride >= 12 && (stride & 3) == 0 && prim_count > 0, "bad vertex slice" );
 	const size_t nv = (size_t)prim_count * 3;
 	CUDA_TRY( cudaMalloc( &b->d_verts, nv * 16 ) );
-	const cudaMemcpyKind kind = space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-	if (stride == 16) CUDA_TRY( cudaMemcpyAsync( b->d_verts, verts, nv * 16, kind, s ) );
-	else
-	{
-		CUDA_TRY( cudaMemsetAsync( b->d_verts, 0, nv * 16, s ) );
-		CUDA_TRY( cudaMemcpy2DAsync( b->d_verts, 16, verts, stride, stride < 16 ? stride : 16, nv, kind, s ) );
-	}
+	TRY( copy_verts( b->d_verts, verts, stride, nv, space, s ) );
 	b->info.prim_count = prim_count;
 	return TBVH_OK;
 }
@@ -458,36 +464,45 @@ __global__ void k_gather_verts( const float4* __restrict__ src, const uint32_t* 
 	if (v >= vert_count) { atomicAdd( bad, 1u ); dst[i] = make_float4( 0, 0, 0, 0 ); return; }
 	dst[i] = src[v];
 }
-static int upload_verts_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space, cudaStream_t s )
+// the gather into dst; indices past vert_count are counted into d_bad.  Synchronises the stream.
+static int gather_verts( float4* dst, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space, cudaStream_t s, uint32_t* d_bad )
 {
-	ARG_CHECK( verts && indices && stride >= 12 && (stride & 3) == 0 && prim_count > 0 && vert_count > 0, "bad indexed vertex slice" );
 	const size_t nv = (size_t)prim_count * 3;
 	const cudaMemcpyKind kind = space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-	float4* d_src = 0; uint32_t* d_idx = 0; uint32_t* d_bad = 0;
-	int rc = TBVH_OK;
+	float4* d_src = 0; uint32_t* d_idx = 0;
 	auto body = [&]() -> int
 	{
 		CUDA_TRY( cudaMalloc( &d_src, (size_t)vert_count * 16 ) );
 		CUDA_TRY( cudaMalloc( &d_idx, nv * 4 ) );
+		TRY( copy_verts( d_src, verts, stride, vert_count, space, s ) );
+		CUDA_TRY( cudaMemcpyAsync( d_idx, indices, nv * 4, kind, s ) );
+		k_gather_verts<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>( d_src, d_idx, dst, (uint32_t)nv, vert_count, d_bad ); LAUNCHED();
+		return TBVH_OK;
+	};
+	const int rc = body();
+	cudaStreamSynchronize( s );
+	cudaFree( d_src ), cudaFree( d_idx );
+	return rc;
+}
+static int upload_verts_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space, cudaStream_t s )
+{
+	ARG_CHECK( verts && indices && stride >= 12 && (stride & 3) == 0 && prim_count > 0 && vert_count > 0, "bad indexed vertex slice" );
+	const size_t nv = (size_t)prim_count * 3;
+	uint32_t* d_bad = 0;
+	int rc = TBVH_OK;
+	auto body = [&]() -> int
+	{
 		CUDA_TRY( cudaMalloc( &d_bad, 4 ) );
 		CUDA_TRY( cudaMalloc( &b->d_verts, nv * 16 ) );
 		CUDA_TRY( cudaMemsetAsync( d_bad, 0, 4, s ) );
-		if (stride == 16) CUDA_TRY( cudaMemcpyAsync( d_src, verts, (size_t)vert_count * 16, kind, s ) );
-		else
-		{
-			CUDA_TRY( cudaMemsetAsync( d_src, 0, (size_t)vert_count * 16, s ) );
-			CUDA_TRY( cudaMemcpy2DAsync( d_src, 16, verts, stride, stride < 16 ? stride : 16, vert_count, kind, s ) );
-		}
-		CUDA_TRY( cudaMemcpyAsync( d_idx, indices, nv * 4, kind, s ) );
-		k_gather_verts<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>( d_src, d_idx, b->d_verts, (uint32_t)nv, vert_count, d_bad ); LAUNCHED();
+		TRY( gather_verts( b->d_verts, verts, stride, vert_count, indices, prim_count, space, s, d_bad ) );
 		uint32_t bad = 0;
-		CUDA_TRY( cudaMemcpyAsync( &bad, d_bad, 4, cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
+		CUDA_TRY( cudaMemcpy( &bad, d_bad, 4, cudaMemcpyDeviceToHost ) );
 		if (bad) { tbvh_set_error( "indexed build: %u indices point past the %u vertices", bad, vert_count ); return TBVH_E_ARG; }
 		return TBVH_OK;
 	};
 	rc = body();
-	cudaFree( d_src ), cudaFree( d_idx ), cudaFree( d_bad );
+	cudaFree( d_bad );
 	b->info.prim_count = prim_count;
 	return rc;
 }
@@ -624,7 +639,7 @@ int tbvh_build_flavour( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t
 	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
 	free_layouts( b );
 	TRY( upload_verts( b, verts, stride, prim_count, space, b->ctx->stream ) );
-	if (flavour == TBVH_BUILD_HQ) TRY( build_hq_launch( b, c_trav, c_int ) ); else TRY( build_sah_launch( b, c_trav, c_int, flavour ) );
+	if (flavour == TBVH_BUILD_HQ) TRY( build_hq_launch( b, c_trav, c_int ) ); else TRY( build_sah_launch( &b, 1, c_trav, c_int, flavour ) );
 	b->info.layouts = 1u << TBVH_LAYOUT_BVH, b->refittable = flavour != TBVH_BUILD_HQ;
 	return TBVH_OK;
 }
@@ -788,7 +803,7 @@ int tbvh_build_tlas( tbvh_bvh t, const void* instances, uint32_t inst_stride, ui
 	CUDA_TRY( cudaMemcpyAsync( t->d_blas, refs.data(), refs.size() * sizeof( BlasRef ), cudaMemcpyHostToDevice, s ) );
 	CUDA_TRY( cudaStreamSynchronize( s ) ); // the host vectors go out of scope
 	t->info.prim_count = inst_count, t->inst_count = inst_count, t->blas_count = blas_count, t->tlas_blas_layouts = blas_layouts;
-	TRY( build_sah_launch( t, c_trav, c_int, TBVH_BUILD_REFERENCE ) ); // "Build(); // or BuildAVX, for large TLAS." :2258
+	TRY( build_sah_launch( &t, 1, c_trav, c_int, TBVH_BUILD_REFERENCE ) ); // "Build(); // or BuildAVX, for large TLAS." :2258
 	t->info.layouts = 1u << TBVH_LAYOUT_BVH, t->refittable = false; // "do not refit a TLAS, use Build(..)" :3060
 	if (t->info.max_depth + 1 > TBVH_STACK) { tbvh_set_error( "TLAS depth %u exceeds the %d-entry stack of IntersectTLAS (tiny_bvh.h:3308)", t->info.max_depth, TBVH_STACK ); return TBVH_E_LIMIT; }
 	// the device table holds raw addresses of the BLAS arrays: remember which generation of each BLAS they belong to
@@ -861,9 +876,80 @@ int tbvh_build_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t
 	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
 	free_layouts( b );
 	TRY( upload_verts_indexed( b, verts, stride, vert_count, indices, prim_count, space, b->ctx->stream ) );
-	if (flavour == TBVH_BUILD_HQ) TRY( build_hq_launch( b, c_trav, c_int ) ); else TRY( build_sah_launch( b, c_trav, c_int, flavour ) );
+	if (flavour == TBVH_BUILD_HQ) TRY( build_hq_launch( b, c_trav, c_int ) ); else TRY( build_sah_launch( &b, 1, c_trav, c_int, flavour ) );
 	b->info.layouts = 1u << TBVH_LAYOUT_BVH, b->refittable = flavour != TBVH_BUILD_HQ;
 	return TBVH_OK;
+}
+
+// Many meshes, one build (include/tinybvh_b200.h).  Every refusal comes before any handle is touched, the vertex staging included:
+// each mesh's vertices go into a fresh array first, and only when every index has been found in range do the handles drop their
+// old arrays and adopt the new ones.
+int tbvh_build_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int, int flavour )
+{
+	ARG_CHECK( bvhs && meshes && count > 0, "no meshes" );
+	if (flavour == TBVH_BUILD_HQ) { tbvh_set_error( "tbvh_build_batch: BuildHQ (SBVH) builds one tree per call" ); return TBVH_E_UNSUPPORTED; }
+	ARG_CHECK( flavour == TBVH_BUILD_REFERENCE || flavour == TBVH_BUILD_AVX, "unknown builder flavour" );
+	ARG_CHECK( space == TBVH_HOST || space == TBVH_DEVICE, "unknown space" );
+	for (uint32_t k = 0; k < count; k++) ARG_CHECK( bvhs[k] && bvhs[k]->ctx == bvhs[0]->ctx, "a handle is NULL or lives in another context" );
+	{
+		std::vector<tbvh_bvh> sorted( bvhs, bvhs + count );
+		std::sort( sorted.begin(), sorted.end() );
+		ARG_CHECK( std::adjacent_find( sorted.begin(), sorted.end() ) == sorted.end(), "the same handle twice" );
+	}
+	uint64_t total = 0;
+	for (uint32_t k = 0; k < count; k++)
+	{
+		const tbvh_mesh& m = meshes[k];
+		ARG_CHECK( m.verts && m.stride >= 12 && (m.stride & 3) == 0 && m.prim_count > 0 && (!m.indices || m.vert_count > 0), "bad vertex slice" );
+		total += m.prim_count;
+		if (m.indices && space == TBVH_HOST)
+			for (size_t i = 0; i < (size_t)m.prim_count * 3; i++)
+				if (m.indices[i] >= m.vert_count) { tbvh_set_error( "tbvh_build_batch: mesh %u: index %u points past the %u vertices", k, m.indices[i], m.vert_count ); return TBVH_E_ARG; }
+	}
+	if (total > TBVH_BATCH_MAX_PRIMS) { tbvh_set_error( "tbvh_build_batch: %llu triangles in one batch (at most %u)", (unsigned long long)total, (unsigned)TBVH_BATCH_MAX_PRIMS ); return TBVH_E_LIMIT; }
+	const tbvh_ctx ctx = bvhs[0]->ctx;
+	CUDA_TRY( cudaSetDevice( ctx->device ) );
+	cudaStream_t s = ctx->stream;
+	std::vector<float4*> staged( count, (float4*)0 );
+	uint32_t* d_bad = 0;
+	auto stage = [&]() -> int
+	{
+		CUDA_TRY( cudaMalloc( &d_bad, 4 ) );
+		CUDA_TRY( cudaMemsetAsync( d_bad, 0, 4, s ) );
+		for (uint32_t k = 0; k < count; k++)
+		{
+			const tbvh_mesh& m = meshes[k];
+			CUDA_TRY( cudaMalloc( &staged[k], (size_t)m.prim_count * 3 * 16 ) );
+			if (m.indices) TRY( gather_verts( staged[k], m.verts, m.stride, m.vert_count, m.indices, m.prim_count, space, s, d_bad ) );
+			else TRY( copy_verts( staged[k], m.verts, m.stride, (size_t)m.prim_count * 3, space, s ) );
+		}
+		uint32_t bad = 0;
+		CUDA_TRY( cudaMemcpyAsync( &bad, d_bad, 4, cudaMemcpyDeviceToHost, s ) );
+		CUDA_TRY( cudaStreamSynchronize( s ) );
+		if (bad) { tbvh_set_error( "tbvh_build_batch: %u indices point past their mesh's vertices", bad ); return TBVH_E_ARG; }
+		return TBVH_OK;
+	};
+	int rc = stage();
+	if (d_bad) cudaFree( d_bad );
+	if (rc != TBVH_OK)
+	{
+		cudaStreamSynchronize( s );
+		for (float4* p : staged) if (p) cudaFree( p );
+		return rc;
+	}
+	for (uint32_t k = 0; k < count; k++)
+	{
+		const tbvh_bvh b = bvhs[k];
+		free_layouts( b );
+		b->d_verts = staged[k], b->info.prim_count = meshes[k].prim_count;
+	}
+	rc = build_sah_launch( bvhs, count, c_trav, c_int, flavour );
+	for (uint32_t k = 0; k < count; k++)
+	{
+		if (rc != TBVH_OK) free_layouts( bvhs[k] ); // as a failed build leaves its handle: empty
+		else bvhs[k]->info.layouts = 1u << TBVH_LAYOUT_BVH, bvhs[k]->refittable = true;
+	}
+	return rc;
 }
 
 int tbvh_build( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space, float c_trav, float c_int )

@@ -16,9 +16,16 @@
 //   k_build_small   one warp per subtree of <= SMALL_T primitives, whole subtree built out of shared memory
 //   relayout        DFS-preorder numbering from (first, depth) of every interior node: rank = #interior nodes that
 //                   start earlier + position in the chain of nodes starting at the same primitive
+//
+// Batches (tbvh_build_batch): K trees are built by the same launches.  Tree t owns the primitive positions
+// [tree_base[t], tree_base[t+1]) of one shared index space, its root is temporary node 2t (2t+1 is its unused "node 1"),
+// and nodes never straddle two trees because a partition stays inside its node's range.  What is per build in the
+// reference is per tree here (TreeState: root box keys and signed-zero words, max depth, node count); the relayout ranks
+// a tree's interior nodes by the global prefix minus the prefix at the tree's first primitive.  A single build is K = 1.
 #include "common.cuh"
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <vector>
 
 #define BINS 8
@@ -38,21 +45,33 @@ struct Counters
 	uint32_t tmp_nodes;      // temp node records allocated (pairs)
 	uint32_t next_large;     // nodes appended to the next level's list
 	uint32_t small_roots;    // subtree roots for k_build_small
-	uint32_t max_depth;
 	uint32_t total_chunks;   // chunks of the current level list
 	uint32_t lvl_num[2];     // persistent large phase: nodes / chunks of the level with parity 0 / 1
 	uint32_t lvl_chunks[2];
 	uint32_t levels;         // persistent large phase: levels run
-	uint32_t root_key[6];    // root AABB as ordered keys: min xyz, max xyz
-	uint32_t root_zpos[6];   // position word (common.cuh zpos_word) of the last fragment with a zero bound, per root bound
-	uint32_t negzero;        // some fragment bound is -0: bins need the signed-zero pass (bin_zero_chunk, k_build_small)
-	uint32_t pad[3];
+	uint32_t negzero;        // some fragment bound is -0: bins need the signed-zero pass (bin_zero_chunk, k_build_small); on a tree
+	                         // without a -0 that pass gives the bits of the plain one, so one flag serves a whole batch
+	uint32_t pad[2];
 };
+
+// what the reference keeps per build, kept per tree
+struct TreeState
+{
+	uint32_t key[6];         // root AABB as ordered keys: min xyz, max xyz
+	uint32_t zpos[6];        // position word (common.cuh zpos_word) of the last fragment with a zero bound, per root bound
+	uint32_t max_depth, used_nodes, pad[2];
+	float4 root[2];          // the root node in the output numbering
+};
+// where a tree's inputs come from and its results go (the handle's own arrays)
+struct TreeIO { const float4* verts; float4* nodes; uint32_t* prim_idx; float4* leaf_tris; };
 
 struct BuildArgs
 {
-	const float4* verts;
 	const float4* aabbs;     // TLAS build (BVH::Build( BLASInstance*, .. ) :2243-2255): fragment i = box (aabbs[2i], aabbs[2i+1]) instead of a triangle's
+	uint32_t trees;          // K: roots are temporary nodes 0, 2, .., 2K-2
+	const uint32_t* tree_base; // K + 1 entries: tree t owns primitive positions [tree_base[t], tree_base[t+1])
+	const TreeIO* io;
+	TreeState* ts;
 	float4* frag_min; float4* frag_max;
 	uint32_t* idx[2]; uint32_t* idx_final;
 	uint16_t* bin_ids;
@@ -69,6 +88,21 @@ struct BuildArgs
 	uint32_t level0;         // persistent large phase: the level it starts at (the launch-per-stage path may have run the first ones)
 	float c_trav, c_int;
 };
+
+// the tree that owns primitive position p
+__device__ __forceinline__ uint32_t tree_of( const BuildArgs& A, const uint32_t p )
+{
+	uint32_t lo = 0, hi = A.trees; // largest t with tree_base[t] <= p
+	while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (A.tree_base[mid] <= p) lo = mid; else hi = mid; }
+	return lo;
+}
+// minDim of the tree (:2346 / :6555): a fraction of its root box's extent
+__device__ __forceinline__ float3 tree_min_dim( const BuildArgs& A, const uint32_t t )
+{
+	const float4 rmin = A.tmp_nodes[(size_t)t * 4], rmax = A.tmp_nodes[(size_t)t * 4 + 1];
+	const float mdf = A.flavour ? 1e-7f : 1e-20f;
+	return make_float3( __fmul_rn( __fsub_rn( rmax.x, rmin.x ), mdf ), __fmul_rn( __fsub_rn( rmax.y, rmin.y ), mdf ), __fmul_rn( __fsub_rn( rmax.z, rmin.z ), mdf ) );
+}
 
 // ---------------------------------------------------------------------------------------------- shared math
 
@@ -298,6 +332,9 @@ __global__ void __launch_bounds__( 256 ) k_fragments( BuildArgs A )
 {
 	// PrepareBuild :2300-2308: bmin = min(v0, min(v1, v2)), bmax likewise; root box = union; primIdx[i] = i
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	// trees of the block's first and last primitive: uniform over the block
+	const uint32_t t0 = tree_of( A, blockIdx.x * blockDim.x ), t1 = tree_of( A, min( (blockIdx.x + 1) * blockDim.x, A.n ) - 1 );
+	const uint32_t t = t0 == t1 || i >= A.n ? t0 : tree_of( A, i );
 	float mn[3] = { BVH_FAR, BVH_FAR, BVH_FAR }, mx[3] = { -BVH_FAR, -BVH_FAR, -BVH_FAR };
 	if (i < A.n && A.aabbs)
 	{
@@ -308,7 +345,8 @@ __global__ void __launch_bounds__( 256 ) k_fragments( BuildArgs A )
 	}
 	else if (i < A.n)
 	{
-		const float4 v0 = __ldg( A.verts + (size_t)i * 3 ), v1 = __ldg( A.verts + (size_t)i * 3 + 1 ), v2 = __ldg( A.verts + (size_t)i * 3 + 2 );
+		const float4* v = A.io[t].verts + (size_t)(i - A.tree_base[t]) * 3;
+		const float4 v0 = __ldg( v ), v1 = __ldg( v + 1 ), v2 = __ldg( v + 2 );
 		mn[0] = ref_min( v0.x, ref_min( v1.x, v2.x ) ), mn[1] = ref_min( v0.y, ref_min( v1.y, v2.y ) ), mn[2] = ref_min( v0.z, ref_min( v1.z, v2.z ) );
 		mx[0] = ref_max( v0.x, ref_max( v1.x, v2.x ) ), mx[1] = ref_max( v0.y, ref_max( v1.y, v2.y ) ), mx[2] = ref_max( v0.z, ref_max( v1.z, v2.z ) );
 		A.frag_min[i] = make_float4( mn[0], mn[1], mn[2], 0 ), A.frag_max[i] = make_float4( mx[0], mx[1], mx[2], 0 );
@@ -319,6 +357,20 @@ __global__ void __launch_bounds__( 256 ) k_fragments( BuildArgs A )
 	const bool neg = (mn[0] == 0 && signbit( mn[0] )) || (mn[1] == 0 && signbit( mn[1] )) || (mn[2] == 0 && signbit( mn[2] ))
 		|| (mx[0] == 0 && signbit( mx[0] )) || (mx[1] == 0 && signbit( mx[1] )) || (mx[2] == 0 && signbit( mx[2] ));
 	if (__any_sync( 0xffffffffu, neg ) && (threadIdx.x & 31) == 0) A.ctr->negzero = 1;
+	if (t0 != t1)
+	{
+		// the block spans trees (a batch of small meshes): lanes of one tree reduce together, one atomic per tree and warp
+		const bool valid = i < A.n;
+		const uint32_t m = __match_any_sync( 0xffffffffu, valid ? t : 0xffffffffu );
+		const bool leader = valid && (threadIdx.x & 31) == (uint32_t)(__ffs( m ) - 1);
+		#pragma unroll
+		for (int k = 0; k < 3; k++)
+		{
+			const uint32_t lo = __reduce_min_sync( m, f2key( mn[k] ) ), hi = __reduce_max_sync( m, f2key( mx[k] ) );
+			if (leader) atomicMin( &A.ts[t].key[k], lo ), atomicMax( &A.ts[t].key[3 + k], hi );
+		}
+		return;
+	}
 	#pragma unroll
 	for (int k = 0; k < 3; k++) for (int o = 16; o > 0; o >>= 1)
 		mn[k] = fminf( mn[k], __shfl_xor_sync( 0xffffffffu, mn[k], o ) ), mx[k] = fmaxf( mx[k], __shfl_xor_sync( 0xffffffffu, mx[k], o ) );
@@ -328,8 +380,8 @@ __global__ void __launch_bounds__( 256 ) k_fragments( BuildArgs A )
 	if ((threadIdx.x & 31) == 0)
 		for (int k = 0; k < 3; k++) atomicMin( &s_key[k], f2key( mn[k] ) ), atomicMax( &s_key[3 + k], f2key( mx[k] ) );
 	__syncthreads();
-	if (threadIdx.x < 3) atomicMin( &A.ctr->root_key[threadIdx.x], s_key[threadIdx.x] );
-	else if (threadIdx.x < 6) atomicMax( &A.ctr->root_key[threadIdx.x], s_key[threadIdx.x] );
+	if (threadIdx.x < 3) atomicMin( &A.ts[t0].key[threadIdx.x], s_key[threadIdx.x] );
+	else if (threadIdx.x < 6) atomicMax( &A.ts[t0].key[threadIdx.x], s_key[threadIdx.x] );
 }
 
 // Scenes with a -0 fragment bound only (the others return at once): each root bound that is a zero takes the sign of the last
@@ -340,53 +392,66 @@ __global__ void __launch_bounds__( 256 ) k_root_zero( BuildArgs A, const size_t 
 	if (!A.ctr->negzero) return;
 	const size_t stride = (size_t)gridDim.x * blockDim.x;
 	for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < zpos_words; k += stride) A.zpos[k] = 0;
-	uint32_t zw[6] = { 0, 0, 0, 0, 0, 0 };
-	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < A.n; i += (uint32_t)stride)
+	// per tree: the lanes of one tree reduce together (positions are global, which orders a tree's own primitives as local ones do)
+	for (uint32_t base = blockIdx.x * blockDim.x; base < A.n; base += (uint32_t)stride)
 	{
-		const float4 lo = A.frag_min[i], hi = A.frag_max[i];
-		const float f[6] = { lo.x, lo.y, lo.z, hi.x, hi.y, hi.z };
+		const uint32_t i = base + threadIdx.x;
+		const bool valid = i < A.n;
+		uint32_t zw[6] = { 0, 0, 0, 0, 0, 0 };
+		if (valid)
+		{
+			const float4 lo = A.frag_min[i], hi = A.frag_max[i];
+			const float f[6] = { lo.x, lo.y, lo.z, hi.x, hi.y, hi.z };
+			#pragma unroll
+			for (int k = 0; k < 6; k++) if (f[k] == 0) zw[k] = zpos_word( i, f[k] );
+		}
+		const uint32_t t = valid ? tree_of( A, i ) : 0xffffffffu;
+		const uint32_t m = __match_any_sync( 0xffffffffu, t );
+		const bool leader = valid && (threadIdx.x & 31) == (uint32_t)(__ffs( m ) - 1);
 		#pragma unroll
-		for (int k = 0; k < 6; k++) if (f[k] == 0) zw[k] = max( zw[k], zpos_word( i, f[k] ) );
-	}
-	#pragma unroll
-	for (int k = 0; k < 6; k++)
-	{
-		const uint32_t w = __reduce_max_sync( 0xffffffffu, zw[k] );
-		if ((threadIdx.x & 31) == 0 && w) atomicMax( &A.ctr->root_zpos[k], w );
+		for (int k = 0; k < 6; k++)
+		{
+			const uint32_t w = __reduce_max_sync( m, zw[k] );
+			if (leader && w) atomicMax( &A.ts[t].zpos[k], w );
+		}
 	}
 }
 
-__global__ void k_init_counters( BuildArgs A )
+// counters and per-tree state; the first level's node lists come from the host (build_sah_launch)
+__global__ void k_init_counters( BuildArgs A, const uint32_t small_roots )
 {
-	Counters* c = A.ctr;
-	c->tmp_nodes = 2, c->next_large = 0, c->small_roots = 0, c->max_depth = 0, c->total_chunks = 0, c->lvl_num[0] = c->lvl_num[1] = 0, c->lvl_chunks[0] = c->lvl_chunks[1] = 0, c->levels = 0;
-	for (int k = 0; k < 3; k++) c->root_key[k] = 0xffffffffu, c->root_key[3 + k] = 0;
-	for (int k = 0; k < 6; k++) c->root_zpos[k] = 0;
-	c->negzero = 0;
+	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t == 0)
+	{
+		Counters* c = A.ctr;
+		c->tmp_nodes = 2 * A.trees, c->next_large = 0, c->small_roots = small_roots, c->total_chunks = 0, c->lvl_num[0] = c->lvl_num[1] = 0, c->lvl_chunks[0] = c->lvl_chunks[1] = 0, c->levels = 0;
+		c->negzero = 0;
+	}
+	if (t < A.trees)
+	{
+		TreeState& s = A.ts[t];
+		for (int k = 0; k < 3; k++) s.key[k] = 0xffffffffu, s.key[3 + k] = 0;
+		for (int k = 0; k < 6; k++) s.zpos[k] = 0;
+		s.max_depth = 0, s.used_nodes = 0;
+	}
 }
 
-__global__ void k_init_root( BuildArgs A )
+// every tree's root (temporary node 2t, its node 2t+1 stays unused as node 1 does, :2285) and the bin tables of the first level
+__global__ void __launch_bounds__( 256 ) k_init_root( BuildArgs A, const uint32_t large_roots )
 {
-	Counters* c = A.ctr;
-	float r[6];
-	for (int k = 0; k < 6; k++) r[k] = key2f( zero_resolve( c->root_key[k], c->root_zpos[k] ) );
-	const float4 mn = make_float4( r[0], r[1], r[2], __uint_as_float( 0u ) );
-	const float4 mx = make_float4( r[3], r[4], r[5], __uint_as_float( A.n ) );
-	A.tmp_nodes[0] = mn, A.tmp_nodes[1] = mx;
-	A.tmp_nodes[2] = make_float4( 0, 0, 0, 0 ), A.tmp_nodes[3] = make_float4( 0, 0, 0, 0 ); // node 1 stays unused (:2285)
-	A.node_first[0] = 0, A.node_depth[0] = 0, A.node_first[1] = 0, A.node_depth[1] = 0;
-	if (A.n > A.small_t)
+	const uint32_t stride = gridDim.x * blockDim.x;
+	for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < A.trees; t += stride)
 	{
-		A.lvl[0][0] = LargeNode{ 0, 0, A.n, 0 };
-		A.chunk_start[0] = 0, A.chunk_start[1] = (A.n + CHUNK - 1) / CHUNK;
-		c->total_chunks = (A.n + CHUNK - 1) / CHUNK, c->lvl_num[0] = 1, c->lvl_chunks[0] = (A.n + CHUNK - 1) / CHUNK;
-		for (int k = threadIdx.x; k < BIN_STRIDE; k += blockDim.x) A.bins[k] = bin_init_word( k );
+		const TreeState& s = A.ts[t];
+		const uint32_t first = A.tree_base[t], count = A.tree_base[t + 1] - first;
+		float r[6];
+		for (int k = 0; k < 6; k++) r[k] = key2f( zero_resolve( s.key[k], s.zpos[k] ) );
+		A.tmp_nodes[(size_t)t * 4] = make_float4( r[0], r[1], r[2], __uint_as_float( first ) );
+		A.tmp_nodes[(size_t)t * 4 + 1] = make_float4( r[3], r[4], r[5], __uint_as_float( count ) );
+		A.tmp_nodes[(size_t)t * 4 + 2] = make_float4( 0, 0, 0, 0 ), A.tmp_nodes[(size_t)t * 4 + 3] = make_float4( 0, 0, 0, 0 );
+		A.node_first[2 * t] = first, A.node_depth[2 * t] = 0, A.node_first[2 * t + 1] = first, A.node_depth[2 * t + 1] = 0;
 	}
-	else if (threadIdx.x == 0)
-	{
-		A.small[0] = SmallRoot{ 0, 0, A.n, 0 };
-		c->small_roots = 1;
-	}
+	for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < large_roots * BIN_STRIDE; k += stride) A.bins[k] = bin_init_word( k % BIN_STRIDE );
 }
 
 // ---------------------------------------------------------------------------------------------- large phase
@@ -525,13 +590,13 @@ __device__ __forceinline__ void sweep_one( const BuildArgs& A, const LargeNode* 
 	const uint32_t lane = threadIdx.x & 31;
 	const LargeNode nd = cur[j];
 	const float4 nmin = A.tmp_nodes[(size_t)nd.tmp * 2], nmax = A.tmp_nodes[(size_t)nd.tmp * 2 + 1];
-	const float4 rmin = A.tmp_nodes[0], rmax = A.tmp_nodes[1];
-	const float mdf = A.flavour ? 1e-7f : 1e-20f; // minDim (:2346 / :6555)
-	const float3 min_dim = make_float3( __fmul_rn( __fsub_rn( rmax.x, rmin.x ), mdf ), __fmul_rn( __fsub_rn( rmax.y, rmin.y ), mdf ), __fmul_rn( __fsub_rn( rmax.z, rmin.z ), mdf ) );
+	const uint32_t t = tree_of( A, nd.first );
+	const float3 min_dim = tree_min_dim( A, t );
+	const bool root = nd.tmp < 2 * A.trees;
 	// the position table is cleared (k_root_zero) and filled (bin_zero_chunk) only with a -0
 	uint32_t* const bins = A.bins + (size_t)j * BIN_STRIDE;
-	const SweepResult R = A.ctr->negzero ? sweep_node<true>( bins, nmin, nmax, nd.count, min_dim, A.c_trav, A.c_int, A.flavour, A.zpos + (size_t)j * ZPOS_WORDS, nd.tmp == 0 )
-		: sweep_node<false>( bins, nmin, nmax, nd.count, min_dim, A.c_trav, A.c_int, A.flavour, 0, nd.tmp == 0 );
+	const SweepResult R = A.ctr->negzero ? sweep_node<true>( bins, nmin, nmax, nd.count, min_dim, A.c_trav, A.c_int, A.flavour, A.zpos + (size_t)j * ZPOS_WORDS, root )
+		: sweep_node<false>( bins, nmin, nmax, nd.count, min_dim, A.c_trav, A.c_int, A.flavour, 0, root );
 	if (!R.split)
 	{
 		// leaf: its range is final (tiny_bvh.h:2409-2412); publish the order it has in the current buffer
@@ -549,7 +614,7 @@ __device__ __forceinline__ void sweep_one( const BuildArgs& A, const LargeNode* 
 		A.node_first[n] = nd.first, A.node_first[n + 1] = nd.first + R.lN, A.node_depth[n] = d, A.node_depth[n + 1] = d;
 		// parent becomes interior: leftFirst = child pair, triCount = 0 (:2432)
 		A.tmp_nodes[(size_t)nd.tmp * 2].w = __uint_as_float( n ), A.tmp_nodes[(size_t)nd.tmp * 2 + 1].w = __uint_as_float( 0u );
-		atomicMax( &A.ctr->max_depth, d );
+		atomicMax( &A.ts[t].max_depth, d );
 		A.split[j] = SplitInfo{ 1, R.axis, R.pos, R.lN };
 		emit_child( A, next, n, nd.first, R.lN, d, out_buf );
 		emit_child( A, next, n + 1, nd.first + R.lN, nd.count - R.lN, d, out_buf );
@@ -939,9 +1004,7 @@ __global__ void __launch_bounds__( SMALL_WARPS * 32 ) k_build_small( BuildArgs A
 			S.fmn[k][0] = mn.x, S.fmn[k][1] = mn.y, S.fmn[k][2] = mn.z, S.fmx[k][0] = mx.x, S.fmx[k][1] = mx.y, S.fmx[k][2] = mx.z;
 		}
 	}
-	const float4 rmin = A.tmp_nodes[0], rmax = A.tmp_nodes[1];
-	const float mdf = A.flavour ? 1e-7f : 1e-20f; // minDim (:2346 / :6555)
-	const float3 min_dim = make_float3( __fmul_rn( __fsub_rn( rmax.x, rmin.x ), mdf ), __fmul_rn( __fsub_rn( rmax.y, rmin.y ), mdf ), __fmul_rn( __fsub_rn( rmax.z, rmin.z ), mdf ) );
+	const float3 min_dim = tree_min_dim( A, tree_of( A, root.first ) );
 	uint32_t sp = 0, local_max_depth = 0;
 	uint32_t tmp = root.tmp, lo = 0, n = root.count, depth = root.depth_buf & 0xffffu, buf = 0;
 	__syncwarp();
@@ -1003,7 +1066,7 @@ __global__ void __launch_bounds__( SMALL_WARPS * 32 ) k_build_small( BuildArgs A
 		}
 		__syncwarp();
 		if (NEGZERO) small_bin_zero<SmallSmem, FRAGS>( A, S, lo, n, buf );
-		const SweepResult R = sweep_node<NEGZERO>( S.bins, nmin, nmax, n, min_dim, A.c_trav, A.c_int, A.flavour, 0, NEGZERO && tmp == 0 );
+		const SweepResult R = sweep_node<NEGZERO>( S.bins, nmin, nmax, n, min_dim, A.c_trav, A.c_int, A.flavour, 0, NEGZERO && tmp < 2 * A.trees );
 		bool pop = false;
 		if (!R.split)
 		{
@@ -1103,7 +1166,7 @@ __global__ void __launch_bounds__( SMALL_WARPS * 32 ) k_build_small( BuildArgs A
 			__syncwarp();
 		}
 	}
-	if (lane == 0) atomicMax( &A.ctr->max_depth, local_max_depth );
+	if (lane == 0) atomicMax( &A.ts[tree_of( A, root.first )].max_depth, local_max_depth ); // looked up again: not held over the loop
 }
 
 // ---------------------------------------------------------------------------------------------- relayout
@@ -1112,40 +1175,60 @@ __global__ void __launch_bounds__( SMALL_WARPS * 32 ) k_build_small( BuildArgs A
 __global__ void k_rank_count( BuildArgs A, const uint32_t tmp_count, uint32_t* __restrict__ cnt, uint32_t* __restrict__ min_depth )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= tmp_count || x == 1) return;
+	if (x >= tmp_count || (x < 2 * A.trees && (x & 1))) return; // the trees' unused nodes
 	if (__float_as_uint( A.tmp_nodes[(size_t)x * 2 + 1].w ) != 0) return; // leaf
 	const uint32_t f = A.node_first[x];
 	atomicAdd( cnt + f, 1u );
 	atomicMin( min_depth + f, A.node_depth[x] );
 }
 
-// final index of the child pair of interior node x: 2 + 2 * (DFS-preorder rank among interior nodes)
-__device__ __forceinline__ uint32_t final_pair( const BuildArgs& A, const uint32_t x, const uint32_t* __restrict__ prefix, const uint32_t* __restrict__ min_depth )
+// final index of the child pair of interior node x: 2 + 2 * (DFS-preorder rank among its tree's interior nodes); p0 = prefix at the
+// tree's first primitive (the interior nodes of the trees before it)
+__device__ __forceinline__ uint32_t final_pair( const BuildArgs& A, const uint32_t x, const uint32_t* __restrict__ prefix, const uint32_t* __restrict__ min_depth, const uint32_t p0 )
 {
 	const uint32_t f = A.node_first[x];
-	return 2u + 2u * (prefix[f] + A.node_depth[x] - min_depth[f]);
+	return 2u + 2u * (prefix[f] - p0 + A.node_depth[x] - min_depth[f]);
 }
 
-__global__ void k_relayout( BuildArgs A, const uint32_t tmp_count, const uint32_t* __restrict__ prefix, const uint32_t* __restrict__ min_depth, float4* __restrict__ out )
+// into each tree's own node array; leaf firstTri becomes local to the tree
+__global__ void k_relayout( BuildArgs A, const uint32_t tmp_count, const uint32_t* __restrict__ prefix, const uint32_t* __restrict__ min_depth )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= tmp_count || x == 1) return;
+	if (x >= tmp_count || (x < 2 * A.trees && (x & 1))) return;
 	float4 a = A.tmp_nodes[(size_t)x * 2], b = A.tmp_nodes[(size_t)x * 2 + 1];
-	const bool interior = __float_as_uint( b.w ) == 0;
-	if (x == 0)
+	const bool interior = __float_as_uint( b.w ) == 0, root = x < 2 * A.trees;
+	if (!interior && !root) return;
+	const uint32_t t = root ? x / 2 : tree_of( A, A.node_first[x] ), base = A.tree_base[t], p0 = prefix[base];
+	float4* __restrict__ out = A.io[t].nodes;
+	if (root)
 	{
-		if (interior) a.w = __uint_as_float( final_pair( A, 0, prefix, min_depth ) );
+		a.w = __uint_as_float( interior ? final_pair( A, x, prefix, min_depth, p0 ) : __float_as_uint( a.w ) - base );
 		out[0] = a, out[1] = b, out[2] = make_float4( 0, 0, 0, 0 ), out[3] = make_float4( 0, 0, 0, 0 );
+		TreeState& s = A.ts[t];
+		s.root[0] = a, s.root[1] = b, s.used_nodes = 2 + 2 * (prefix[A.tree_base[t + 1]] - p0);
 	}
 	if (!interior) return;
 	// copy this node's two children to their final pair, re-pointing interior children at their own final pairs
-	const uint32_t c = __float_as_uint( A.tmp_nodes[(size_t)x * 2].w ), dst = final_pair( A, x, prefix, min_depth );
+	const uint32_t c = __float_as_uint( A.tmp_nodes[(size_t)x * 2].w ), dst = final_pair( A, x, prefix, min_depth, p0 );
 	for (uint32_t s = 0; s < 2; s++)
 	{
 		float4 ca = A.tmp_nodes[(size_t)(c + s) * 2], cb = A.tmp_nodes[(size_t)(c + s) * 2 + 1];
-		if (__float_as_uint( cb.w ) == 0) ca.w = __uint_as_float( final_pair( A, c + s, prefix, min_depth ) );
+		ca.w = __uint_as_float( __float_as_uint( cb.w ) == 0 ? final_pair( A, c + s, prefix, min_depth, p0 ) : __float_as_uint( ca.w ) - base );
 		out[(size_t)(dst + s) * 2] = ca, out[(size_t)(dst + s) * 2 + 1] = cb;
 	}
+}
+
+// primIdx local to each tree (a batch only: a single build's leaves wrote the handle's array directly) and the leaf-ordered
+// triangle records of every tree in one launch (make_leaf_tris)
+__global__ void __launch_bounds__( 256 ) k_tree_outputs( BuildArgs A, const bool write_idx )
+{
+	const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+	if (p >= A.n) return;
+	const uint32_t t = tree_of( A, p ), base = A.tree_base[t];
+	const TreeIO io = A.io[t];
+	const uint32_t pi = A.idx_final[p] - base;
+	if (write_idx) io.prim_idx[p - base] = pi;
+	if (io.leaf_tris) leaf_tri_record( io.verts, pi, io.leaf_tris, p - base );
 }
 
 // ---------------------------------------------------------------------------------------------- host driver
@@ -1164,28 +1247,56 @@ int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint3
 
 #define DEV_ALLOC( ptr, bytes ) do { CUDA_TRY( cudaMalloc( (void**)&(ptr), (bytes) ) ); scratch.push_back( (void*)(ptr) ); } while (0)
 
-int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
+// bs[0 .. trees): handles of one context holding their primitives (d_verts, or d_aabbs for a TLAS, which is built alone) and
+// info.prim_count; on success each holds its tree as a build of its own would leave it.  On failure the caller empties them.
+int build_sah_launch( const tbvh_bvh* bs, const uint32_t trees, float c_trav, float c_int, int flavour )
 {
-	const uint32_t n = b->info.prim_count;
-	cudaStream_t s = b->ctx->stream;
+	const tbvh_ctx ctx = bs[0]->ctx;
+	cudaStream_t s = ctx->stream;
 	std::vector<void*> scratch;
 	BuildArgs A = {};
-	A.verts = b->d_verts, A.aabbs = b->d_aabbs, A.n = n, A.c_trav = c_trav, A.c_int = c_int, A.flavour = (uint32_t)flavour;
+	A.aabbs = bs[0]->d_aabbs, A.trees = trees, A.c_trav = c_trav, A.c_int = c_int, A.flavour = (uint32_t)flavour;
 	{
-		const int t = b->ctx->small_t; // threads per CTA of the warp-subtree kernel (tbvh_set_option "small_t")
+		const int t = ctx->small_t; // threads per CTA of the warp-subtree kernel (tbvh_set_option "small_t")
 		A.small_t = (uint32_t)(t < 8 ? 8 : t > SMALL_T ? SMALL_T : t);
 	}
-	const size_t max_nodes = (size_t)2 * n + 2, max_large = n / A.small_t + 2;
+	// the shared primitive index space and the first level: trees above small_t start in the large phase's list, the others are
+	// warp subtrees from the start
+	std::vector<uint32_t> base( (size_t)trees + 1, 0 ), chunk0( 1, 0 );
+	std::vector<LargeNode> large;
+	std::vector<SmallRoot> small;
+	for (uint32_t t = 0; t < trees; t++)
+	{
+		const uint32_t nt = bs[t]->info.prim_count;
+		base[t + 1] = base[t] + nt;
+		if (nt > A.small_t) large.push_back( LargeNode{ 2 * t, base[t], nt, 0 } ), chunk0.push_back( chunk0.back() + (nt + CHUNK - 1) / CHUNK );
+		else small.push_back( SmallRoot{ 2 * t, base[t], nt, 0 } );
+	}
+	const uint32_t n = base[trees];
+	A.n = n;
+	const size_t max_nodes = (size_t)2 * n + 2 * (size_t)trees, max_large = n / A.small_t + 2;
 	int rc = TBVH_OK;
 	uint32_t* tile_sum = 0;
 	Counters* h_ctr = 0;
 	cudaEvent_t e0 = 0, e1 = 0;
-	// outputs (kept by the handle)
-	CUDA_TRY( cudaMalloc( &b->d_nodes, max_nodes * 32 ) );
-	CUDA_TRY( cudaMalloc( &b->d_prim_idx, (size_t)n * 4 ) );
-	A.idx_final = b->d_prim_idx;
+	// outputs (kept by the handles)
+	std::vector<TreeIO> io( trees );
+	for (uint32_t t = 0; t < trees; t++)
+	{
+		const tbvh_bvh b = bs[t];
+		const size_t nt = b->info.prim_count;
+		CUDA_TRY( cudaMalloc( &b->d_nodes, (2 * nt + 2) * 32 ) );
+		CUDA_TRY( cudaMalloc( &b->d_prim_idx, nt * 4 ) );
+		if (!b->d_aabbs) { CUDA_TRY( cudaMalloc( &b->d_leaf_tris, nt * 48 ) ); b->leaf_tris_count = (uint32_t)nt; } // a TLAS has no triangles of its own
+		io[t] = TreeIO{ b->d_verts, b->d_nodes, b->d_prim_idx, b->d_leaf_tris };
+	}
+	A.idx_final = bs[0]->d_prim_idx; // one tree: the leaves write the handle's primIdx directly
 	auto body = [&]() -> int
 	{
+		uint32_t* d_base = 0; TreeIO* d_io = 0;
+		DEV_ALLOC( d_base, base.size() * 4 ); DEV_ALLOC( d_io, io.size() * sizeof( TreeIO ) ); DEV_ALLOC( A.ts, (size_t)trees * sizeof( TreeState ) );
+		A.tree_base = d_base, A.io = d_io;
+		if (trees > 1) DEV_ALLOC( A.idx_final, (size_t)n * 4 ); // global positions, made local by k_tree_outputs
 		DEV_ALLOC( A.frag_min, (size_t)n * 16 ); DEV_ALLOC( A.frag_max, (size_t)n * 16 );
 		DEV_ALLOC( A.idx[0], (size_t)n * 4 ); DEV_ALLOC( A.idx[1], (size_t)n * 4 );
 		DEV_ALLOC( A.bin_ids, (size_t)n * 2 );
@@ -1202,23 +1313,34 @@ int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
 		DEV_ALLOC( tile_sum, (flag_words / SCAN_TILE + 2) * 4 );
 		CUDA_TRY( cudaMallocHost( &h_ctr, sizeof( Counters ) ) );
 		CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) );
+		CUDA_TRY( cudaMemcpyAsync( d_base, base.data(), base.size() * 4, cudaMemcpyHostToDevice, s ) );
+		CUDA_TRY( cudaMemcpyAsync( d_io, io.data(), io.size() * sizeof( TreeIO ), cudaMemcpyHostToDevice, s ) );
+		if (!large.empty())
+		{
+			CUDA_TRY( cudaMemcpyAsync( A.lvl[0], large.data(), large.size() * sizeof( LargeNode ), cudaMemcpyHostToDevice, s ) );
+			CUDA_TRY( cudaMemcpyAsync( A.chunk_start, chunk0.data(), chunk0.size() * 4, cudaMemcpyHostToDevice, s ) );
+		}
+		if (!small.empty()) CUDA_TRY( cudaMemcpyAsync( A.small, small.data(), small.size() * sizeof( SmallRoot ), cudaMemcpyHostToDevice, s ) );
 		CUDA_TRY( cudaEventRecord( e0, s ) );
-		k_init_counters<<<1, 1, 0, s>>>( A ); LAUNCHED();
+		k_init_counters<<<(trees + 255) / 256, 256, 0, s>>>( A, (uint32_t)small.size() ); LAUNCHED();
 		k_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
-		k_root_zero<<<b->ctx->sm_count, 256, 0, s>>>( A, max_large * ZPOS_WORDS ); LAUNCHED();
-		k_init_root<<<1, 256, 0, s>>>( A ); LAUNCHED();
-		uint32_t num = n > A.small_t ? 1 : 0, chunks = (n + CHUNK - 1) / CHUNK, level = 0;
+		k_root_zero<<<ctx->sm_count, 256, 0, s>>>( A, max_large * ZPOS_WORDS ); LAUNCHED();
+		{
+			const size_t work = std::max( (size_t)trees, large.size() * BIN_STRIDE );
+			k_init_root<<<(uint32_t)std::min( (work + 255) / 256, (size_t)ctx->sm_count * 8 ), 256, 0, s>>>( A, (uint32_t)large.size() ); LAUNCHED();
+		}
+		uint32_t num = (uint32_t)large.size(), chunks = chunk0.back(), level = 0;
 		// Large phase.  The first levels of a big scene are bandwidth work over all primitives: one launch per stage, every CTA the
 		// device can hold.  Once a level is down to a few chunks per SM the stages are launch-latency sized, and the rest of the
 		// phase runs inside ONE persistent cooperative launch (k_large_phase) without further host round trips.
 		int per_sm = 0;
 		uint32_t pgrid = 0;
-		if (num && b->ctx->build_mode == 0)
+		if (num && ctx->build_mode == 0)
 		{
 			CUDA_TRY( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &per_sm, k_large_phase, CHUNK, 0 ) );
-			const int want = b->ctx->build_ctas > 0 ? b->ctx->build_ctas : 4;
+			const int want = ctx->build_ctas > 0 ? ctx->build_ctas : 4;
 			if (per_sm > want) per_sm = want;
-			pgrid = (uint32_t)(per_sm > 0 ? per_sm * b->ctx->sm_count : 0);
+			pgrid = (uint32_t)(per_sm > 0 ? per_sm * ctx->sm_count : 0);
 		}
 		const uint32_t persist_chunks = pgrid * 3;
 		while (num)
@@ -1248,7 +1370,7 @@ int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
 			const uint32_t* idx_in = A.idx[level & 1];
 			uint32_t* idx_out = A.idx[(level + 1) & 1];
 			k_bin<<<chunks, CHUNK, 0, s>>>( A, cur, num, idx_in ); LAUNCHED();
-			if (level == 0 || h_ctr->negzero) { k_bin_zero<<<min( chunks, (uint32_t)b->ctx->sm_count ), CHUNK, 0, s>>>( A, cur, num, idx_in, chunks ); LAUNCHED(); }
+			if (level == 0 || h_ctr->negzero) { k_bin_zero<<<min( chunks, (uint32_t)ctx->sm_count ), CHUNK, 0, s>>>( A, cur, num, idx_in, chunks ); LAUNCHED(); }
 			k_sweep<<<(num * 32 + 255) / 256, 256, 0, s>>>( A, cur, next, num, idx_in, (level + 1) & 1 ); LAUNCHED();
 			k_flags<<<chunks, CHUNK, 0, s>>>( A, cur, num ); LAUNCHED();
 			{ const int r = exclusive_scan( A.flags, A.scan, tile_sum, chunks * CHUNK, s ); if (r != TBVH_OK) return r; }
@@ -1272,8 +1394,9 @@ int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
 		const uint32_t roots = h_ctr->small_roots;
 		if (roots)
 		{
-			const uint32_t g = (roots + SMALL_WARPS - 1) / SMALL_WARPS, mode = (uint32_t)b->ctx->small_mode;
-			#define SMALL( F, G ) do { if (h_ctr->negzero || n <= A.small_t) k_build_small<F, G, true><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); \
+			const uint32_t g = (roots + SMALL_WARPS - 1) / SMALL_WARPS, mode = (uint32_t)ctx->small_mode;
+			// the signed-zero instance also carries the root rule, for trees whose root is a warp subtree
+			#define SMALL( F, G ) do { if (h_ctr->negzero || !small.empty()) k_build_small<F, G, true><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); \
 				else k_build_small<F, G, false><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); } while (0)
 			if (mode == 0) SMALL( false, false );
 			else if (mode == 1) SMALL( true, false );
@@ -1291,19 +1414,27 @@ int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour )
 		CUDA_TRY( cudaMemsetAsync( A.pos_bl, 0xff, ((size_t)n + 1) * 4, s ) );
 		k_rank_count<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count, A.flags, A.pos_bl ); LAUNCHED();
 		{ const int r = exclusive_scan( A.flags, A.scan, tile_sum, n, s ); if (r != TBVH_OK) return r; }
-		k_relayout<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count, A.scan, A.pos_bl, b->d_nodes ); LAUNCHED();
+		k_relayout<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count, A.scan, A.pos_bl ); LAUNCHED();
 		CUDA_TRY( cudaEventRecord( e1, s ) );
+		if (trees > 1 || !A.aabbs) { k_tree_outputs<<<(n + 255) / 256, 256, 0, s>>>( A, trees > 1 ); LAUNCHED(); }
+		std::vector<TreeState> ts( trees );
+		CUDA_TRY( cudaMemcpyAsync( ts.data(), A.ts, ts.size() * sizeof( TreeState ), cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		float ms = 0;
 		CUDA_TRY( cudaEventElapsedTime( &ms, e0, e1 ) );
-		b->info.build_ms = ms;
-		b->info.used_nodes = tmp_count, b->info.idx_count = n, b->info.max_depth = h_ctr->max_depth;
-		uint32_t rootw[8];
-		CUDA_TRY( cudaMemcpy( rootw, b->d_nodes, 32, cudaMemcpyDeviceToHost ) );
-		memcpy( b->info.aabb_min, rootw, 12 ), memcpy( b->info.aabb_max, rootw + 4, 12 );
-		b->root_ref = rootw[3], b->root_count = rootw[7];
-		b->d_trav = b->d_nodes;
-		return b->d_aabbs ? TBVH_OK : make_leaf_tris( b, s ); // a TLAS has no triangles of its own
+		for (uint32_t t = 0; t < trees; t++)
+		{
+			const tbvh_bvh b = bs[t];
+			uint32_t rootw[8];
+			memcpy( rootw, ts[t].root, 32 );
+			b->info.build_ms = ms;
+			b->info.used_nodes = ts[t].used_nodes, b->info.idx_count = b->info.prim_count, b->info.max_depth = ts[t].max_depth;
+			memcpy( b->info.aabb_min, rootw, 12 ), memcpy( b->info.aabb_max, rootw + 4, 12 );
+			b->root_ref = rootw[3], b->root_count = rootw[7];
+			b->d_trav = b->d_nodes;
+			b->generation = tbvh_next_generation(); // new arrays: a TLAS built over the old ones must notice (tlas_check)
+		}
+		return TBVH_OK;
 	};
 	rc = body();
 	cudaStreamSynchronize( s );

@@ -152,6 +152,16 @@ __device__ __forceinline__ uint32_t zpos_word( const uint32_t pos, const float f
 // the key of a zero bound whose sign a position word decided (0: no word, keep the key)
 __device__ __forceinline__ uint32_t zero_resolve( const uint32_t key, const uint32_t zw ) { return (zw && zero_key( key )) ? ((zw & 1u) ? 0x7fffffffu : 0x80000000u) : key; }
 
+// leaf-ordered triangle record p of a BVH2 (tbvh_bvh_t::d_leaf_tris) for primitive pi: 3 x 16 B gathered vertex reads, 3 x 16 B writes.
+// e1 = v1 - v0, e2 = v2 - v0 exactly as IntersectTri computes them per test (tiny_bvh.h:8510)
+__device__ __forceinline__ void leaf_tri_record( const float4* __restrict__ verts, const uint32_t pi, float4* __restrict__ out, const uint32_t p )
+{
+	const float4 v0 = __ldg( verts + (size_t)pi * 3 ), v1 = __ldg( verts + (size_t)pi * 3 + 1 ), v2 = __ldg( verts + (size_t)pi * 3 + 2 );
+	out[(size_t)p * 3] = make_float4( v0.x, v0.y, v0.z, __uint_as_float( pi ) );
+	out[(size_t)p * 3 + 1] = make_float4( __fsub_rn( v1.x, v0.x ), __fsub_rn( v1.y, v0.y ), __fsub_rn( v1.z, v0.z ), 0.0f );
+	out[(size_t)p * 3 + 2] = make_float4( __fsub_rn( v2.x, v0.x ), __fsub_rn( v2.y, v0.y ), __fsub_rn( v2.z, v0.z ), 0.0f );
+}
+
 // ---- DFS preorder of a BVH2 in the reference's layout (node 1 unused, children paired at leftFirst), whatever its numbering and
 // whatever the order of its leaf ranges in primIdx.  Used by BuildHQ's Compact() (build_hq.cu) and BVH_GPU::ConvertFrom (convert.cu).
 // parent[]: the parent of every reachable node, 0xffffffff for the root.
@@ -198,7 +208,8 @@ int cw_make_trav( tbvh_bvh b, cudaStream_t s ); // traversal nodes, cw_rd_limit 
 int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range ); // cw_make_trav's node expansion into the existing d_cw_trav
 float cw_rd_limit_for( uint32_t range );                               // cw_rd_limit of a tree whose expansion found `range`
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)
-int build_sah_launch( tbvh_bvh b, float c_trav, float c_int, int flavour );
+// binned-SAH builds of `trees` handles of one context at once (build_sah.cu); a single build is trees = 1
+int build_sah_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, int flavour );
 int build_hq_launch( tbvh_bvh b, float c_trav, float c_int );
 int refit_launch( tbvh_bvh b, cudaStream_t s );
 int refit_enqueue( tbvh_bvh b, cudaStream_t s, uint32_t* parent, uint32_t* arrive, bool fill_parent );
