@@ -137,6 +137,21 @@ __device__ __forceinline__ bool mt_test( const float ox, const float oy, const f
 	return !(t < 0 || (below_tmax ? t >= tmax : t > tmax));
 }
 
+// ray record i of a traversal batch: O | mask, D, rD | inst, hit (t, u, v, prim) - four 16-byte loads
+__device__ __forceinline__ void load_ray( const char* rays, const uint64_t i, const uint32_t stride, float4& ro4, float4& rd4, float4& rr4, float4& rh4 )
+{
+	const float4* rp = (const float4*)(rays + i * stride);
+	ro4 = rp[0], rd4 = rp[1], rr4 = rp[2], rh4 = rp[3];
+}
+
+// any-hit result of a one-ray-per-thread kernel: one ballot word per warp.  blockDim is a multiple of 32 and i is the global thread
+// index, so lane l of a warp holds ray 32*w + l; every lane of the warp must call it.
+__device__ __forceinline__ void store_occlusion_word( uint32_t* bits, const uint64_t i, const uint64_t n, const bool occluded )
+{
+	const uint32_t m = __ballot_sync( 0xffffffffu, occluded );
+	if ((threadIdx.x & 31) == 0 && (i & ~31ull) < n) bits[i >> 5] = m;
+}
+
 // order-preserving float <-> uint key for atomicMin/Max on floats
 __device__ __forceinline__ uint32_t f2key( float f ) { uint32_t u = __float_as_uint( f ); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
 __device__ __forceinline__ float key2f( uint32_t k ) { return __uint_as_float( (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k ); }
