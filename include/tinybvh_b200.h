@@ -209,8 +209,27 @@ int tbvh_upload_bvh_gpu( tbvh_bvh bvh, const void* nodes64, uint32_t used_nodes,
 int tbvh_upload_cwbvh( tbvh_bvh bvh, const void* bvh8_data, uint32_t used_blocks, const void* bvh8_tris, uint32_t tri_count, int space );
 
 /* layout conversion on the device: BVH_GPU::ConvertFrom tiny_bvh.h:4612; BVH8_CWBVH::Build's chain
- * Compact :3733 + SplitLeafs(3) :1988 + MBVH<8>::ConvertFrom :4975 + BVH8_CWBVH::ConvertFrom :5884 */
+ * Compact :3733 + SplitLeafs(3) :1988 + MBVH<8>::ConvertFrom :4975 + BVH8_CWBVH::ConvertFrom :5884.  A TLAS handle has no
+ * CWBVH (its leaves are instances, not triangles): TBVH_E_STATE.  A conversion to CWBVH that fails on the device leaves the
+ * handle without a CWBVH. */
 int tbvh_convert( tbvh_bvh bvh, int to_layout );
+
+/* Many trees converted to CWBVH in one call, as a scene converts every BLAS before a TLAS walks them in TBVH_LAYOUT_CWBVH.
+ * Afterwards each bvhs[i] holds exactly what tbvh_convert( bvhs[i], TBVH_LAYOUT_CWBVH ) would leave: bvh8Data and bvh8Tris byte
+ * for byte, the same info (build_ms untouched), layout bits and traversal limits, a renewed generation where it held a CWBVH before
+ * (a TLAS over the old arrays is stale), and on a refittable tree the collapse tbvh_refit_layouts reuses.  The trees are converted
+ * together by the same kernels, so the fixed cost of a conversion (allocations, launches, host round trips) is paid once per batch
+ * instead of once per tree; the order of `bvhs` and the other trees of the batch change no tree.  Any BVH_GPU layout stays.
+ *  to_layout: TBVH_LAYOUT_CWBVH; any other is TBVH_E_UNSUPPORTED (BVH_GPU::ConvertFrom is a relayout without a fixed cost worth
+ *  batching: tbvh_convert per handle).
+ *  Refusals come before any handle is touched, so every handle keeps its arrays and its generation: TBVH_E_ARG for count 0, a NULL
+ *  or repeated handle, or handles of different contexts; TBVH_E_STATE for a handle without a BVH-layout tree, or a TLAS (its leaves
+ *  are instances, not triangles); TBVH_E_LIMIT when the split trees together could hold more than TBVH_CONVERT_BATCH_MAX_NODES
+ *  nodes, counted as the sum of max( used_nodes, 2 ) + 2 * ceil( idx_count / 3 ) (node indices of the shared index space are 32-bit).  A
+ *  failure after the device work started leaves every handle of the batch with its BVH-layout tree and any other layout it had,
+ *  and without a CWBVH. */
+#define TBVH_CONVERT_BATCH_MAX_NODES (1u << 31)
+int tbvh_convert_batch( tbvh_bvh* bvhs, uint32_t count, int to_layout );
 
 /* read a layout back in the reference's format so SAHCost / Save / ConvertFrom / the CPU traversals can use a
  * GPU-built tree.  Buffers are sized from tbvh_bvh_info. */

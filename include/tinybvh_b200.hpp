@@ -142,6 +142,7 @@ protected:
 		for (size_t i = 0; i < (size_t)primCount * 3; i++) vmax = indices[i] > vmax ? indices[i] : vmax;
 		TBVH_FATAL_IF( tbvh_build_indexed( h, vertices, (uint32_t)sizeof( Vec4 ), vmax + 1, indices, primCount, TBVH_HOST, c_trav, c_int, flavour ), what );
 	}
+	static void batch_convert( tbvh_bvh*, uint32_t ) {} // BuildBatch: layouts converted for the whole batch at once (BVH8_CWBVH)
 	void adopt( const BVHBase& o ) { if (own) tbvh_bvh_destroy( h ); h = o.h, own = false; } // "both must be kept alive" (README.md:99)
 	tbvh_bvh h = 0;
 	int layout;
@@ -402,7 +403,8 @@ public:
 #endif
 private:
 	template <class T, class Vec4> friend void BuildBatch( T* const*, const Vec4* const*, const uint32_t*, uint32_t, int );
-	void batch_built( const void*, uint32_t, uint32_t ) { TBVH_FATAL_IF( tbvh_convert( h, TBVH_LAYOUT_CWBVH ), "BuildBatch" ); sync_info(), usedBlocks = Info().used_blocks; }
+	static void batch_convert( tbvh_bvh* hs, uint32_t count ) { TBVH_FATAL_IF( tbvh_convert_batch( hs, count, TBVH_LAYOUT_CWBVH ), "BuildBatch" ); }
+	void batch_built( const void*, uint32_t, uint32_t ) { sync_info(), usedBlocks = Info().used_blocks; }
 };
 
 template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* const* vertices, const uint32_t* primCounts, uint32_t count, int flavour )
@@ -416,8 +418,11 @@ template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* cons
 	}
 	const int rc = tbvh_build_batch( hs, ms, count, TBVH_HOST, count && objs[0] ? objs[0]->c_trav : 1.0f, count && objs[0] ? objs[0]->c_int : 1.0f,
 		flavour < 0 ? T::defaultFlavour : flavour );
-	free( hs ), free( ms );
+	free( ms );
+	if (rc != TBVH_OK) free( hs );
 	TBVH_FATAL_IF( rc, "BuildBatch" );
+	T::batch_convert( hs, count );
+	free( hs );
 	for (uint32_t k = 0; k < count; k++) objs[k]->batch_built( vertices[k], (uint32_t)sizeof( Vec4 ), primCounts[k] );
 }
 

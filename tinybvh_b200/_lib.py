@@ -61,6 +61,7 @@ SYMBOLS = {
     "tbvh_upload_bvh_gpu": (i32, [vp, vp, u32, vp, u32, vp, u32, u32, i32]),
     "tbvh_upload_cwbvh": (i32, [vp, vp, u32, vp, u32, i32]),
     "tbvh_convert": (i32, [vp, i32]),
+    "tbvh_convert_batch": (i32, [vp, u32, i32]),
     "tbvh_download_bvh": (i32, [vp, vp, vp, i32]),
     "tbvh_download_bvh_gpu": (i32, [vp, vp, i32]),
     "tbvh_download_cwbvh": (i32, [vp, vp, vp, i32]),

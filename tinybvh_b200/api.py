@@ -335,8 +335,8 @@ def build_batch(bvhs, meshes, flavour: int = _lib.BUILD_REFERENCE, indices=None)
     """tbvh_build_batch: one binned-SAH tree per mesh, all built in one call.  bvhs[i] ends up as bvhs[i].Build(meshes[i]) (flavour
     BUILD_REFERENCE) or .BuildAVX (BUILD_AVX) would leave it.  `meshes`: numpy vertex arrays, or torch CUDA tensors - one space per
     call; `indices`: None, or one entry per mesh (None for a flat mesh, else its vertex indices in the same space).  BVH_GPU and
-    BVH8_CWBVH objects are converted afterwards, as their Build does.  A refused batch raises TbvhError and leaves every object as
-    it was."""
+    BVH8_CWBVH objects are converted afterwards, as their Build does (the BVH8_CWBVH objects in one convert_batch).  A refused batch
+    raises TbvhError and leaves every object as it was."""
     bvhs, meshes = list(bvhs), list(meshes)
     if len(bvhs) != len(meshes):
         raise TbvhError("build_batch: one object per mesh")
@@ -366,10 +366,23 @@ def build_batch(bvhs, meshes, flavour: int = _lib.BUILD_REFERENCE, indices=None)
     hs = (C.c_void_p * max(len(bvhs), 1))(*[b.h for b in bvhs]) if bvhs else None
     c0 = bvhs[0] if bvhs else None
     check(_lib.lib().tbvh_build_batch(hs, recs, len(meshes), space, c0.c_trav if c0 else 1.0, c0.c_int if c0 else 1.0, flavour))
+    cw = [b for b in bvhs if b.layout == LAYOUT_CWBVH]
+    if cw:
+        convert_batch(cw)
     for b in bvhs:
-        if b.layout != LAYOUT_BVH:
+        if b.layout == LAYOUT_BVH_GPU:
             check(_lib.lib().tbvh_convert(b.h, b.layout))
     return bvhs
+
+
+def convert_batch(objs):
+    """tbvh_convert_batch: the CWBVH of every object's BVH-layout tree, all converted in one call.  Each object then holds what
+    tbvh_convert( h, LAYOUT_CWBVH ) of it alone leaves (BVH8_CWBVH.Build's conversion chain), whatever the other objects of the
+    call.  A refused call raises TbvhError and leaves every object as it was."""
+    objs = list(objs)
+    hs = (C.c_void_p * max(len(objs), 1))(*[b.h for b in objs])
+    check(_lib.lib().tbvh_convert_batch(hs, len(objs), LAYOUT_CWBVH))
+    return objs
 
 
 def pinned_empty(n: int, dtype, device: int = None, node: int = None) -> np.ndarray:

@@ -627,7 +627,7 @@ int tbvh_upload_cwbvh( tbvh_bvh b, const void* bvh8_data, uint32_t used_blocks, 
 	CUDA_TRY( cudaMemcpyAsync( b->d_cw_nodes, bvh8_data, (size_t)used_blocks * 16, kind, s ) );
 	CUDA_TRY( cudaMemcpyAsync( b->d_cw_tris, bvh8_tris, (size_t)tri_count * 48, kind, s ) );
 	b->info.used_blocks = used_blocks, b->info.cwbvh_tri_count = tri_count;
-	TRY( cw_make_trav( b, s ) ); // the traversal nodes the kernels read + the pending bound of the wide tree (synchronises the stream)
+	TRY( cw_make_trav( &b, 1, s ) ); // the traversal nodes the kernels read + the pending bound of the wide tree (synchronises the stream)
 	b->info.layouts |= 1u << TBVH_LAYOUT_CWBVH;
 	return TBVH_OK;
 }
@@ -963,9 +963,39 @@ int tbvh_convert( tbvh_bvh b, int to_layout )
 	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
 	if (!(b->info.layouts & (1u << TBVH_LAYOUT_BVH))) { tbvh_set_error( "tbvh_convert: source layout BVH not resident" ); return TBVH_E_STATE; }
 	if (to_layout == TBVH_LAYOUT_BVH_GPU) { TRY( bvh_to_bvh_gpu( b, b->ctx->stream ) ); b->info.layouts |= 1u << TBVH_LAYOUT_BVH_GPU; return TBVH_OK; }
-	if (to_layout == TBVH_LAYOUT_CWBVH) { TRY( bvh_to_cwbvh( b, b->ctx->stream ) ); b->info.layouts |= 1u << TBVH_LAYOUT_CWBVH; return TBVH_OK; }
+	if (to_layout == TBVH_LAYOUT_CWBVH)
+	{
+		// a TLAS's leaves are instances: there are no triangles to encode (its handle holds no vertices)
+		if (b->d_inst) { tbvh_set_error( "tbvh_convert: a TLAS has no CWBVH layout (convert its BLASses)" ); return TBVH_E_STATE; }
+		return bvh_to_cwbvh( &b, 1, b->ctx->stream );
+	}
 	tbvh_set_error( "tbvh_convert: unsupported target layout %d", to_layout );
 	return TBVH_E_UNSUPPORTED;
+}
+
+// Many trees, one conversion (include/tinybvh_b200.h).  Every refusal comes before any handle is touched.
+int tbvh_convert_batch( tbvh_bvh* bvhs, uint32_t count, int to_layout )
+{
+	ARG_CHECK( bvhs && count > 0, "no handles" );
+	for (uint32_t k = 0; k < count; k++) ARG_CHECK( bvhs[k] && bvhs[k]->ctx == bvhs[0]->ctx, "a handle is NULL or lives in another context" );
+	{
+		std::vector<tbvh_bvh> sorted( bvhs, bvhs + count );
+		std::sort( sorted.begin(), sorted.end() );
+		ARG_CHECK( std::adjacent_find( sorted.begin(), sorted.end() ) == sorted.end(), "the same handle twice" );
+	}
+	uint64_t nodes = 0;
+	for (uint32_t k = 0; k < count; k++)
+	{
+		const tbvh_bvh b = bvhs[k];
+		if (!(b->info.layouts & (1u << TBVH_LAYOUT_BVH))) { tbvh_set_error( "tbvh_convert_batch: handle %u holds no BVH-layout tree", k ); return TBVH_E_STATE; }
+		if (b->d_inst) { tbvh_set_error( "tbvh_convert_batch: handle %u is a TLAS, which has no CWBVH layout", k ); return TBVH_E_STATE; }
+		// at least two nodes per tree (a leaf root is wrapped into node 1); SplitLeafs(3) adds at most 2 nodes per 3 primitives
+		nodes += (uint64_t)std::max( b->info.used_nodes, 2u ) + 2 * (((uint64_t)b->info.idx_count + 2) / 3);
+	}
+	if (to_layout != TBVH_LAYOUT_CWBVH) { tbvh_set_error( "tbvh_convert_batch: target layout %d (only TBVH_LAYOUT_CWBVH converts in batches)", to_layout ); return TBVH_E_UNSUPPORTED; }
+	if (nodes > TBVH_CONVERT_BATCH_MAX_NODES) { tbvh_set_error( "tbvh_convert_batch: up to %llu split-tree nodes in one batch (at most %u)", (unsigned long long)nodes, (unsigned)TBVH_CONVERT_BATCH_MAX_NODES ); return TBVH_E_LIMIT; }
+	CUDA_TRY( cudaSetDevice( bvhs[0]->ctx->device ) );
+	return bvh_to_cwbvh( bvhs, count, bvhs[0]->ctx->stream );
 }
 
 static cudaMemcpyKind out_kind( int space ) { return space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost; }

@@ -219,7 +219,8 @@ __device__ __forceinline__ void dfs_rank( const float4* nodes, const uint32_t* p
 // d_stats: NULL, or two counters the launch ADDS its node visits / triangle tests to (the caller zeroes them once per API call)
 int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
 int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
-int cw_make_trav( tbvh_bvh b, cudaStream_t s ); // traversal nodes, cw_rd_limit and cw_pending of b's CWBVH
+// traversal nodes, cw_rd_limit and cw_pending of the CWBVH of each of bs[0 .. K), in one pass (trace_cwbvh.cu); synchronises s
+int cw_make_trav( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
 int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range ); // cw_make_trav's node expansion into the existing d_cw_trav
 float cw_rd_limit_for( uint32_t range );                               // cw_rd_limit of a tree whose expansion found `range`
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)
@@ -234,7 +235,8 @@ struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root
 int make_leaf_tris( tbvh_bvh b, cudaStream_t s );
 int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used_nodes_gpu, cudaStream_t s );
 int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s );
-int bvh_to_cwbvh( tbvh_bvh b, cudaStream_t s );
+// BVH8_CWBVH::Build's conversion chain for K handles of one context at once (convert_cwbvh.cu); tbvh_convert is K = 1
+int bvh_to_cwbvh( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
 int cwbvh_refit( tbvh_bvh b, cudaStream_t s );  // tbvh_refit_layouts over b->cw_keep (convert_cwbvh.cu)
 void cw_keep_free( tbvh_bvh b );                // drop b->cw_keep: wherever the CWBVH arrays are replaced or dropped
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)

@@ -17,7 +17,15 @@
 // On a refittable tree the collapse is kept (CwKeep), and tbvh_refit_layouts runs everything after it again over the refitted boxes
 // (cwbvh_refit): the result is BVH8_CWBVH::ConvertFrom of an MBVH<8> with the collapse of the conversion and the boxes of the
 // refitted tree, which tests/cwbvh_refit_oracle.c restates.
+//
+// Batches (tbvh_convert_batch; a single conversion is K = 1).  K trees share one index space per stage: tree t owns BVH2 nodes
+// nbase[t] .. nbase[t+1] of the SplitLeafs scan and split-tree nodes ext_base[t] .. ext_base[t+1] of one `ext` array, whose child
+// links are global.  Level 0 of the collapse holds the K roots; a level places every node's interior children by a scan over the
+// level in list order, so each level is grouped by tree in batch order and the lists are deterministic.  Every root gets address 0,
+// so addresses below it are local to its tree; the encode writes through a table of per-tree outputs (CwTree).  The fixed costs -
+// allocations, launches and host round trips - grow with the deepest tree's level count, not with K.
 #include "common.cuh"
+#include <algorithm>
 #include <new>
 #include <string.h>
 #include <vector>
@@ -43,6 +51,7 @@ struct CwKeep
 	uint32_t used = 0, total = 0, wide_count = 0; // BVH2 nodes, nodes after SplitLeafs(3), wide nodes
 	bool leaf_root = false;                       // the wide root wraps a leaf root (MBVH<8>::ConvertFrom :5036)
 	std::vector<uint32_t> off;                    // level l holds wide nodes off[l] .. off[l+1]
+	// one allocation, at base, holds the four arrays of the collapse
 	uint32_t* base = 0;                           // used + 1: k_split_count scan, where each split leaf's chain goes
 	uint32_t* list = 0;                           // wide_count: split-tree node of every wide node
 	uint32_t* adopt = 0;                          // wide_count * 8: its children in ADOPTION order (k_assign breaks ties by it)
@@ -59,12 +68,38 @@ void cw_keep_free( tbvh_bvh b )
 {
 	CwKeep* k = b->cw_keep;
 	if (!k) return;
-	void* p[] = { k->base, k->list, k->adopt, k->ifirst, k->ext, k->wide, k->parent, k->arrive, k->misc };
+	void* p[] = { k->base, k->ext, k->wide, k->parent, k->arrive, k->misc }; // base also holds list, adopt and ifirst
 	for (void* q : p) if (q) cudaFree( q );
 	if (k->e0) cudaEventDestroy( k->e0 );
 	if (k->e1) cudaEventDestroy( k->e1 );
 	delete k;
 	b->cw_keep = 0;
+}
+
+// one tree of a conversion: its BVH2, its outputs, and where it sits in the batch's index spaces (device table, indexed by tree)
+struct CwTree
+{
+	const float4* nodes;          // BVH2 nodes (d_nodes)
+	const uint32_t* prim_idx;     // the tree's own primIdx
+	const float4* verts;
+	float4* cw_nodes, * cw_tris;  // bvh8Data / bvh8Tris of the handle
+	uint32_t* keep;               // refittable: the handle's CwKeep block (base | list | adopt | ifirst), else NULL
+	uint32_t nbase, used;         // first BVH2 node in the batch's node index space, BVH2 nodes
+	uint32_t seg;                 // nodes the tree owns before its chain nodes: cw_seg( used )
+	uint32_t ext_base;            // first split-tree node (k_tree_bases)
+	uint32_t wide_count;          // wide nodes
+};
+
+// A tree owns at least two split-tree nodes before its chain nodes: a leaf root is wrapped into node 1 (wrap_leaf_root), which an
+// uploaded one-node tree does not have
+__host__ __device__ __forceinline__ uint32_t cw_seg( const uint32_t used ) { return used < 2 ? 2 : used; }
+
+// the tree that holds BVH2 node g of the batch (nbase rises strictly: every tree has a node)
+__device__ __forceinline__ uint32_t tree_of_node( const CwTree* __restrict__ T, const uint32_t K, const uint32_t g )
+{
+	uint32_t lo = 0, hi = K;
+	while (hi - lo > 1) { const uint32_t m = (lo + hi) >> 1; if (T[m].nbase <= g) lo = m; else hi = m; }
+	return lo;
 }
 
 // BVH::SA (tiny_bvh.h:8477) in the oracle's pairing
@@ -75,24 +110,40 @@ __device__ __forceinline__ float node_sa( const float4 mn, const float4 mx )
 }
 
 // ---- SplitLeafs(3): a leaf with c > 3 primitives becomes a right-leaning chain of ceil(c/3) leaves that all keep the
-// original bounds (:1996-2003).  New nodes are appended after the existing ones.
-__global__ void k_split_count( const float4* __restrict__ nodes, uint32_t* __restrict__ extra, const uint32_t used, const uint32_t max_prims )
+// original bounds (:1996-2003).  New nodes are appended after the tree's existing ones.
+__global__ void k_split_count( const CwTree* __restrict__ T, const uint32_t K, const uint32_t n, uint32_t* __restrict__ extra, const uint32_t max_prims )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= used) return;
-	const uint32_t c = x == 1 ? 0 : __float_as_uint( nodes[(size_t)x * 2 + 1].w );
-	extra[x] = c > max_prims ? 2 * ((c + max_prims - 1) / max_prims - 1) : 0;
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	const CwTree& tr = T[tree_of_node( T, K, g )];
+	const uint32_t x = g - tr.nbase;
+	const uint32_t c = x == 1 || x >= tr.used ? 0 : __float_as_uint( tr.nodes[(size_t)x * 2 + 1].w );
+	extra[g] = c > max_prims ? 2 * ((c + max_prims - 1) / max_prims - 1) : 0;
 }
 
-__global__ void k_split_emit( const float4* __restrict__ nodes, const uint32_t* __restrict__ base, float4* __restrict__ ext, const uint32_t used, const uint32_t max_prims )
+// first split-tree node of every tree, from the scan of k_split_count: the nodes and chain nodes of the trees before it
+__global__ void k_tree_bases( CwTree* __restrict__ T, const uint32_t K, const uint32_t* __restrict__ base, uint32_t* __restrict__ ext_base )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= used) return;
-	float4 a = nodes[(size_t)x * 2], b = nodes[(size_t)x * 2 + 1];
+	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= K) return;
+	const uint32_t nb = T[t].nbase;
+	T[t].ext_base = ext_base[t] = nb + base[nb];
+	if (t == K - 1) ext_base[K] = nb + T[t].seg + base[nb + T[t].seg];
+}
+
+// BVH2 node x (a, b) as split-tree node x + shift: a link to its children moves with it, and a long leaf's chain goes to the pairs
+// from `pair` on
+__device__ __forceinline__ void split_emit( float4 a, const float4 b, const uint32_t x, const uint32_t shift, uint32_t pair, float4* __restrict__ ext, const uint32_t max_prims )
+{
 	const uint32_t c = x == 1 ? 0 : __float_as_uint( b.w ), first = __float_as_uint( a.w );
-	if (c <= max_prims) { ext[(size_t)x * 2] = a, ext[(size_t)x * 2 + 1] = b; return; }
+	uint32_t cur = x + shift;
+	if (c <= max_prims)
+	{
+		if (__float_as_uint( b.w ) == 0) a.w = __uint_as_float( first + shift );
+		ext[(size_t)cur * 2] = a, ext[(size_t)cur * 2 + 1] = b;
+		return;
+	}
 	const uint32_t k = (c + max_prims - 1) / max_prims; // leaves in the chain
-	uint32_t cur = x, pair = used + base[x];
 	for (uint32_t j = 0; j + 1 < k; j++, pair += 2)
 	{
 		// `cur` becomes interior over (leaf of max_prims, rest)
@@ -106,46 +157,167 @@ __global__ void k_split_emit( const float4* __restrict__ nodes, const uint32_t* 
 	ext[(size_t)cur * 2 + 1] = make_float4( b.x, b.y, b.z, __uint_as_float( c - (k - 1) * max_prims ) );
 }
 
-// ---- MBVH<8>::ConvertFrom collapse for one level of wide nodes (:5010-5033): wide nodes lo .. lo+num-1 of `list`; their
-// interior children are appended to `list` as the next level, each node's contiguously and in adoption order
-__global__ void k_collapse( const float4* __restrict__ ext, uint32_t* __restrict__ list, const uint32_t lo, const uint32_t num, uint32_t* __restrict__ adopt,
-	uint32_t* __restrict__ ifirst, uint32_t* __restrict__ next_count )
+// one tree, with the tree's own scan (cwbvh_refit over CwKeep::base)
+__global__ void k_split_emit( const float4* __restrict__ nodes, const uint32_t* __restrict__ base, float4* __restrict__ ext, const uint32_t used, const uint32_t max_prims )
 {
-	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-	if (t >= num) return;
-	const uint32_t w = lo + t, x = list[w];
+	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+	if (x >= used) return;
+	split_emit( nodes[(size_t)x * 2], nodes[(size_t)x * 2 + 1], x, 0, cw_seg( used ) + base[x], ext, max_prims );
+}
+
+// every tree of a batch: tree t's chains follow its own nodes, at ext_base + seg + (base[g] - base[nbase]) = nbase + seg + base[g]
+__global__ void k_split_emit_batch( const CwTree* __restrict__ T, const uint32_t K, const uint32_t n, const uint32_t* __restrict__ base, float4* __restrict__ ext, const uint32_t max_prims )
+{
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	const CwTree& tr = T[tree_of_node( T, K, g )];
+	const uint32_t x = g - tr.nbase;
+	if (x >= tr.used) return; // node 1 of a one-node tree: only a leaf-root wrap writes it
+	split_emit( tr.nodes[(size_t)x * 2], tr.nodes[(size_t)x * 2 + 1], x, tr.ext_base, tr.nbase + tr.seg + base[g], ext, max_prims );
+}
+
+// MBVH<8>::ConvertFrom :5036-5044: a leaf root x is copied to node x + 1 (its tree's unused node 1), and x becomes a one-child
+// interior node (wide node w)
+__device__ __forceinline__ void wrap_leaf_root( float4* ext, uint32_t* adopt, const uint32_t x, const uint32_t w )
+{
+	ext[(size_t)(x + 1) * 2] = ext[(size_t)x * 2], ext[(size_t)(x + 1) * 2 + 1] = ext[(size_t)x * 2 + 1];
+	ext[(size_t)x * 2 + 1].w = __uint_as_float( 0u );
+	adopt[(size_t)w * 8] = x + 1;
+	for (int i = 1; i < 8; i++) adopt[(size_t)w * 8 + i] = 0;
+}
+__global__ void k_wrap_leaf_root( float4* ext, uint32_t* adopt ) { wrap_leaf_root( ext, adopt, 0, 0 ); }
+
+// ---- MBVH<8>::ConvertFrom collapse for one level of wide nodes (:5010-5033): wide nodes lo .. lo+num-1 of `list`; their interior
+// children are appended to `list` as the next level, each node's contiguously and in adoption order, the nodes in list order.  On
+// level 0 (roots = K) a leaf root is wrapped instead.  Where a node's children go is an exclusive scan of the interior-child counts
+// over the level: a block scan, then each block looks back over its predecessors' published sums (decoupled look-back).  Blocks
+// take their place in the level from a ticket, so every block a block waits for is already running.  look: one zeroed word per
+// block of the level; *next_count receives the size of the next level.  groups (a batch only): the first wide node of every run of
+// one tree's nodes on the level, as (tree, node), appended in any order at *ngroups.
+#define CW_LEVEL_T 256
+#define CW_MAX_LEVELS 4096
+__global__ void __launch_bounds__( CW_LEVEL_T ) k_collapse( float4* __restrict__ ext, uint32_t* __restrict__ list, uint32_t* __restrict__ wtree, const uint32_t lo,
+	const uint32_t num, const uint32_t roots, uint32_t* __restrict__ adopt, uint32_t* __restrict__ ifirst, uint32_t* __restrict__ leaf_root,
+	unsigned long long* look, uint32_t* ticket, uint32_t* __restrict__ next_count, uint2* __restrict__ groups, uint32_t* __restrict__ ngroups )
+{
+	__shared__ uint32_t s_blk, s_excl, s_warp[CW_LEVEL_T / 32];
+	if (threadIdx.x == 0) s_blk = atomicAdd( ticket, 1u );
+	__syncthreads();
+	const uint32_t blk = s_blk, t = blk * CW_LEVEL_T + threadIdx.x, w = lo + t;
 	uint32_t c[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-	uint32_t n = 2;
-	c[0] = __float_as_uint( ext[(size_t)x * 2].w ), c[1] = c[0] + 1;
-	while (n < 8)
+	uint32_t n = 0, ic = 0;
+	if (t < num)
 	{
-		int best = -1;
-		float bestSA = 0;
-		for (uint32_t i = 0; i < n; i++)
+		const uint32_t x = list[w];
+		if (groups && (t == 0 || wtree[w - 1] != wtree[w])) groups[atomicAdd( ngroups, 1u )] = make_uint2( wtree[w], w );
+		if (t < roots && __float_as_uint( ext[(size_t)x * 2 + 1].w ) != 0) wrap_leaf_root( ext, adopt, x, w ), leaf_root[t] = 1;
+		else
 		{
-			const float4 mn = ext[(size_t)c[i] * 2], mx = ext[(size_t)c[i] * 2 + 1];
-			if (__float_as_uint( mx.w ) != 0) continue; // leaf: cannot be adopted
-			const float sa = node_sa( mn, mx );
-			if (sa > bestSA) best = (int)i, bestSA = sa;
+			n = 2;
+			c[0] = __float_as_uint( ext[(size_t)x * 2].w ), c[1] = c[0] + 1;
+			while (n < 8)
+			{
+				int best = -1;
+				float bestSA = 0;
+				for (uint32_t i = 0; i < n; i++)
+				{
+					const float4 mn = ext[(size_t)c[i] * 2], mx = ext[(size_t)c[i] * 2 + 1];
+					if (__float_as_uint( mx.w ) != 0) continue; // leaf: cannot be adopted
+					const float sa = node_sa( mn, mx );
+					if (sa > bestSA) best = (int)i, bestSA = sa;
+				}
+				if (best < 0) break;
+				const uint32_t g = __float_as_uint( ext[(size_t)c[best] * 2].w );
+				c[best] = g, c[n++] = g + 1;
+			}
+			for (uint32_t i = 0; i < 8; i++)
+			{
+				adopt[(size_t)w * 8 + i] = c[i];
+				if (i < n && __float_as_uint( ext[(size_t)c[i] * 2 + 1].w ) == 0) ic++;
+			}
 		}
-		if (best < 0) break;
-		const uint32_t g = __float_as_uint( ext[(size_t)c[best] * 2].w );
-		c[best] = g, c[n++] = g + 1;
 	}
-	uint32_t ic = 0;
-	for (uint32_t i = 0; i < 8; i++)
+	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	uint32_t inc = ic;
+	#pragma unroll
+	for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync( 0xffffffffu, inc, d ); if (lane >= d) inc += y; }
+	if (lane == 31) s_warp[warp] = inc;
+	__syncthreads();
+	if (threadIdx.x == 0)
 	{
-		adopt[(size_t)w * 8 + i] = c[i];
-		if (i < n && __float_as_uint( ext[(size_t)c[i] * 2 + 1].w ) == 0) ic++;
+		uint32_t agg = 0;
+		for (int i = 0; i < CW_LEVEL_T / 32; i++) { const uint32_t v = s_warp[i]; s_warp[i] = agg, agg += v; }
+		// look word: status (1 = this block's sum, 2 = the sum of every block up to and including it) << 32 | value
+		uint32_t excl = 0;
+		if (blk)
+		{
+			atomicExch( look + blk, (1ull << 32) | agg );
+			for (uint32_t p = blk - 1;; p--)
+			{
+				unsigned long long v;
+				do v = *(volatile unsigned long long*)(look + p); while ((v >> 32) == 0);
+				excl += (uint32_t)v;
+				if ((v >> 32) == 2) break;
+			}
+		}
+		atomicExch( look + blk, (2ull << 32) | (excl + agg) );
+		s_excl = excl;
+		if (blk == gridDim.x - 1) *next_count = excl + agg;
 	}
-	uint32_t at = lo + num + (ic ? atomicAdd( next_count, ic ) : 0u);
-	ifirst[w] = at;
-	for (uint32_t i = 0; i < n; i++) if (__float_as_uint( ext[(size_t)c[i] * 2 + 1].w ) == 0) list[at++] = c[i];
+	__syncthreads();
+	if (t < num)
+	{
+		uint32_t at = lo + num + s_excl + s_warp[warp] + inc - ic;
+		ifirst[w] = at;
+		const uint32_t tree = wtree[w];
+		for (uint32_t i = 0; i < n; i++) if (__float_as_uint( ext[(size_t)c[i] * 2 + 1].w ) == 0) list[at] = c[i], wtree[at] = tree, at++;
+	}
+}
+
+// the run of one tree's wide nodes that holds wide node w: runs are sorted by their first node (gfirst) and tile every level
+__device__ __forceinline__ uint32_t run_of( const uint32_t* __restrict__ gfirst, const uint32_t G, const uint32_t w )
+{
+	uint32_t lo = 0, hi = G;
+	while (hi - lo > 1) { const uint32_t m = (lo + hi) >> 1; if (gfirst[m] <= w) lo = m; else hi = m; }
+	return lo;
+}
+
+// the collapse of every refittable tree into its handle's CwKeep block, local to the tree: wide node w of run g is the tree's node
+// w - gfirst[g] + glocal[g], split-tree nodes lose ext_base, and the SplitLeafs scan starts at 0.  Threads 0 .. W-1 take the wide
+// nodes, W .. W+N-1 the BVH2 nodes.
+__global__ void k_keep( const CwTree* __restrict__ T, const uint32_t K, const uint32_t* __restrict__ wtree, const uint32_t* __restrict__ gfirst,
+	const uint32_t* __restrict__ glocal, const uint32_t G, const uint32_t W, const uint32_t* __restrict__ list, const uint32_t* __restrict__ adopt,
+	const uint32_t* __restrict__ ifirst, const uint32_t* __restrict__ base, const uint32_t N )
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < W)
+	{
+		const uint32_t t = wtree[i];
+		const CwTree& tr = T[t];
+		if (!tr.keep) return;
+		const uint32_t g = run_of( gfirst, G, i ), x = i - gfirst[g] + glocal[g];
+		uint32_t* kl = tr.keep + tr.used + 1, * ka = kl + tr.wide_count, * ki = ka + (size_t)8 * tr.wide_count;
+		kl[x] = list[i] - tr.ext_base;
+		for (int j = 0; j < 8; j++) { const uint32_t a = adopt[(size_t)i * 8 + j]; ka[(size_t)x * 8 + j] = a ? a - tr.ext_base : 0u; }
+		// read only for nodes with interior children, which are the tree's own nodes on the next level
+		const uint32_t c = ifirst[i], gc = c < W ? run_of( gfirst, G, c ) : 0;
+		ki[x] = c < W && wtree[c] == t ? c - gfirst[gc] + glocal[gc] : 0u;
+	}
+	else if (i - W < N)
+	{
+		const uint32_t g = i - W;
+		const CwTree& tr = T[tree_of_node( T, K, g )];
+		const uint32_t x = g - tr.nbase;
+		if (!tr.keep || x >= tr.used) return;
+		const uint32_t b0 = base[tr.nbase];
+		tr.keep[x] = base[g] - b0;
+		if (x + 1 == tr.used) tr.keep[tr.used] = base[g + 1] - b0;
+	}
 }
 
 // ---- BVH8_CWBVH::ConvertFrom, greedy child -> slot assignment (:5910-5946) and per-node child statistics, one thread per wide node
 __global__ void k_assign( const float4* __restrict__ ext, const uint32_t* __restrict__ list, const uint32_t* __restrict__ adopt, const uint32_t* __restrict__ ifirst,
-	const uint32_t num, WideNode* __restrict__ wide )
+	const uint32_t num, const uint32_t roots, WideNode* __restrict__ wide )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= num) return;
@@ -200,7 +372,7 @@ __global__ void k_assign( const float4* __restrict__ ext, const uint32_t* __rest
 		if (cnt == 0) w.wchild[s] = wi++, w.ichild++; else lt += cnt;
 	}
 	w.leaf_tris = lt, w.size = 1, w.tris = lt;
-	if (t == 0) w.cbase = 1; // root: node 0 at address 0, its children from node 1, its triangles from record 0
+	if (t < roots) w.cbase = 1; // a root (wide nodes 0 .. roots-1): node 0 of its tree, its children from node 1, its triangles from record 0
 	wide[t] = w;
 }
 
@@ -248,11 +420,16 @@ __device__ __forceinline__ int quant_exponent( const float extent )
 	return (int)(int8_t)(v & 0xff);
 }
 
+// T: the batch's trees, wide node t belongs to tree wtree[t]; T = NULL: every node belongs to `one`
 __global__ void k_encode( const float4* __restrict__ ext, const uint32_t* __restrict__ list, const uint32_t num, const WideNode* __restrict__ wide,
-	const uint32_t* __restrict__ prim_idx, const float4* __restrict__ verts, float4* __restrict__ out_nodes, float4* __restrict__ out_tris )
+	const CwTree* __restrict__ T, const uint32_t* __restrict__ wtree, const CwTree one )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= num) return;
+	const CwTree& io = T ? T[wtree[t]] : one;
+	const uint32_t* __restrict__ prim_idx = io.prim_idx;
+	const float4* __restrict__ verts = io.verts;
+	float4* __restrict__ out_nodes = io.cw_nodes, * __restrict__ out_tris = io.cw_tris;
 	const uint32_t x = list[t];
 	const WideNode w = wide[t];
 	const float4 lo = ext[(size_t)x * 2], hi = ext[(size_t)x * 2 + 1];
@@ -302,21 +479,14 @@ __global__ void k_encode( const float4* __restrict__ ext, const uint32_t* __rest
 	o[4] = make_float4( __uint_as_float( q[8] ), __uint_as_float( q[9] ), __uint_as_float( q[10] ), __uint_as_float( q[11] ) );
 }
 
-__global__ void k_wrap_leaf_root( float4* ext, uint32_t* adopt )
-{
-	// MBVH<8>::ConvertFrom :5036-5044: a leaf root is copied to node 1 and the root becomes a one-child interior node
-	ext[2] = ext[0], ext[3] = ext[1];
-	ext[1].w = __uint_as_float( 0u );
-	adopt[0] = 1;
-	for (int i = 1; i < 8; i++) adopt[i] = 0;
-}
 
-// slot assignment, subtree sizes (bottom-up), addresses (top-down), encode: everything after the collapse that depends on boxes
-static int cw_assign_encode( tbvh_bvh b, cudaStream_t s, const float4* ext, const uint32_t* list, const uint32_t* adopt, const uint32_t* ifirst,
-	const std::vector<uint32_t>& off, WideNode* wide )
+// slot assignment, subtree sizes (bottom-up), addresses (top-down), encode: everything after the collapse that depends on boxes.
+// Wide nodes 0 .. roots-1 are roots; T / wtree / one as for k_encode.
+static int cw_assign_encode( cudaStream_t s, const float4* ext, const uint32_t* list, const uint32_t* adopt, const uint32_t* ifirst,
+	const std::vector<uint32_t>& off, WideNode* wide, const uint32_t roots, const CwTree* T, const uint32_t* wtree, const CwTree& one )
 {
 	const uint32_t levels = (uint32_t)off.size() - 1, wide_count = off[levels];
-	k_assign<<<(wide_count + 127) / 128, 128, 0, s>>>( ext, list, adopt, ifirst, wide_count, wide ); LAUNCHED();
+	k_assign<<<(wide_count + 127) / 128, 128, 0, s>>>( ext, list, adopt, ifirst, wide_count, roots, wide ); LAUNCHED();
 	for (int l = (int)levels - 1; l >= 0; l--)
 	{
 		const uint32_t num = off[l + 1] - off[l];
@@ -327,97 +497,173 @@ static int cw_assign_encode( tbvh_bvh b, cudaStream_t s, const float4* ext, cons
 		const uint32_t num = off[l + 1] - off[l];
 		k_addresses<<<(num + 127) / 128, 128, 0, s>>>( off[l], num, wide ); LAUNCHED();
 	}
-	k_encode<<<(wide_count + 127) / 128, 128, 0, s>>>( ext, list, wide_count, wide, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris ); LAUNCHED();
+	k_encode<<<(wide_count + 127) / 128, 128, 0, s>>>( ext, list, wide_count, wide, T, wtree, one ); LAUNCHED();
 	return TBVH_OK;
 }
 
-int bvh_to_cwbvh( tbvh_bvh b, cudaStream_t s )
+// the CWBVH arrays of b and what refers to them go (a TLAS over them becomes stale)
+static void drop_cwbvh( tbvh_bvh b )
 {
-	const uint32_t used = b->info.used_nodes, idx_count = b->info.idx_count;
-	std::vector<void*> scratch;
-	#define CW_ALLOC( ptr, bytes ) do { CUDA_TRY( cudaMalloc( (void**)&(ptr), (bytes) ) ); scratch.push_back( (void*)(ptr) ); } while (0)
 	if (b->d_cw_trav || b->d_cw_tris) b->generation = tbvh_next_generation(); // a TLAS may hold these addresses (api.cu tlas_check)
 	if (b->d_cw_nodes) cudaFree( b->d_cw_nodes );
 	if (b->d_cw_tris) cudaFree( b->d_cw_tris );
 	if (b->d_cw_trav) cudaFree( b->d_cw_trav );
 	b->d_cw_nodes = 0, b->d_cw_tris = 0, b->d_cw_trav = 0;
 	cw_keep_free( b );
-	uint32_t* extra = 0, * base = 0, * tile = 0, * lists = 0, * adopt = 0, * ifirst = 0, * d_count = 0;
+}
+
+// bs[0 .. K): handles of one context holding BVH-layout trees.  On success each holds the CWBVH a conversion of its own tree gives;
+// on failure none holds a CWBVH.
+int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
+{
+	std::vector<CwTree> T( K );
+	uint32_t N = 0; // BVH2 nodes of the batch (the caller bounds the batch; a single tree's count is a uint32_t)
+	for (uint32_t t = 0; t < K; t++)
+	{
+		const tbvh_bvh b = bs[t];
+		drop_cwbvh( b );
+		b->info.layouts &= ~(1u << TBVH_LAYOUT_CWBVH);
+		T[t] = CwTree{ b->d_nodes, b->d_prim_idx, b->d_verts, 0, 0, 0, N, b->info.used_nodes, cw_seg( b->info.used_nodes ), 0, 0 };
+		N += T[t].seg;
+	}
+	std::vector<void*> scratch;
+	#define CW_ALLOC( ptr, bytes ) do { CUDA_TRY( cudaMalloc( (void**)&(ptr), (bytes) ) ); scratch.push_back( (void*)(ptr) ); } while (0)
+	// scratch of one stage carved from one allocation: fewer cudaMalloc / cudaFree pairs per call
+	size_t carve = 0;
+	char* blob = 0;
+	auto take = [&]( const size_t bytes ) { const size_t o = carve; carve += (bytes + 255) & ~(size_t)255; return o; };
+	CwTree* d_T = 0;
+	uint32_t* extra = 0, * base = 0, * tile = 0, * d_ext = 0, * lists = 0, * wtree = 0, * adopt = 0, * ifirst = 0, * leaf = 0, * tickets = 0, * counts = 0;
+	uint32_t* d_runs = 0, * ngroups = 0;
+	uint2* groups = 0;
+	unsigned long long* look = 0;
 	float4* ext = 0;
 	WideNode* wide = 0;
 	auto body = [&]() -> int
 	{
-		// ---- SplitLeafs(3)
-		CW_ALLOC( extra, ((size_t)used + 1) * 4 ); CW_ALLOC( base, ((size_t)used + 1) * 4 ); CW_ALLOC( tile, ((size_t)used / 2048 + 2) * 4 );
-		k_split_count<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes, extra, used, 3 ); LAUNCHED();
-		{ const int r = exclusive_scan( extra, base, tile, used, s ); if (r != TBVH_OK) return r; }
-		uint32_t n_extra = 0;
-		CUDA_TRY( cudaMemcpyAsync( &n_extra, base + used, 4, cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		const uint32_t total = used + n_extra;
-		CW_ALLOC( ext, (size_t)total * 32 );
-		k_split_emit<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes, base, ext, used, 3 ); LAUNCHED();
-		// ---- collapse to 8-wide, level by level (a wide node is an interior node of the split tree: fewer than total)
-		CW_ALLOC( lists, ((size_t)total + 1) * 4 );
-		CW_ALLOC( adopt, ((size_t)total + 1) * 32 );
-		CW_ALLOC( ifirst, ((size_t)total + 1) * 4 );
-		CW_ALLOC( d_count, 4 );
-		uint32_t rootw[8];
-		CUDA_TRY( cudaMemcpyAsync( rootw, ext, 32, cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		std::vector<uint32_t> off; // level l occupies lists[off[l] .. off[l+1])
-		const uint32_t zero = 0;
-		CUDA_TRY( cudaMemcpyAsync( lists, &zero, 4, cudaMemcpyHostToDevice, s ) ); // level 0 = { root }
-		off.push_back( 0 ), off.push_back( 1 );
-		const bool leaf_root = rootw[7] != 0;
-		if (leaf_root) { k_wrap_leaf_root<<<1, 1, 0, s>>>( ext, adopt ); LAUNCHED(); }
-		else
+		// ---- SplitLeafs(3) over every tree, and each tree's first split-tree node
 		{
-			while (off[off.size() - 1] > off[off.size() - 2])
-			{
-				const uint32_t lo = off[off.size() - 2], num = off[off.size() - 1] - lo;
-				CUDA_TRY( cudaMemsetAsync( d_count, 0, 4, s ) );
-				k_collapse<<<(num + 127) / 128, 128, 0, s>>>( ext, lists, lo, num, adopt, ifirst, d_count ); LAUNCHED();
-				uint32_t next = 0;
-				CUDA_TRY( cudaMemcpyAsync( &next, d_count, 4, cudaMemcpyDeviceToHost, s ) );
-				CUDA_TRY( cudaStreamSynchronize( s ) );
-				off.push_back( lo + num + next );
-				if (off.size() > 4096) { tbvh_set_error( "CWBVH conversion: runaway depth" ); return TBVH_E_LIMIT; }
-			}
-			off.pop_back(); // the last level is empty
+			carve = 0;
+			const size_t o_T = take( (size_t)K * sizeof( CwTree ) ), o_extra = take( ((size_t)N + 1) * 4 ), o_base = take( ((size_t)N + 1) * 4 );
+			const size_t o_tile = take( ((size_t)N / 2048 + 2) * 4 ), o_ext = take( ((size_t)K + 1) * 4 );
+			CW_ALLOC( blob, carve );
+			d_T = (CwTree*)(blob + o_T), extra = (uint32_t*)(blob + o_extra), base = (uint32_t*)(blob + o_base), tile = (uint32_t*)(blob + o_tile);
+			d_ext = (uint32_t*)(blob + o_ext);
 		}
-		const uint32_t levels = (uint32_t)off.size() - 1, wide_count = off[levels];
-		CW_ALLOC( wide, (size_t)wide_count * sizeof( WideNode ) );
-		CUDA_TRY( cudaMalloc( &b->d_cw_nodes, (size_t)wide_count * 80 ) );
-		CUDA_TRY( cudaMalloc( &b->d_cw_tris, (size_t)idx_count * 48 ) );
-		{ const int r = cw_assign_encode( b, s, ext, lists, adopt, ifirst, off, wide ); if (r != TBVH_OK) return r; }
-		b->info.used_blocks = wide_count * 5, b->info.cwbvh_tri_count = idx_count;
-		// the traversal nodes the kernels read and the pending bound of the wide tree (trace_cwbvh.cu)
-		{ const int r = cw_make_trav( b, s ); if (r != TBVH_OK) return r; }
-		if (b->refittable)
+		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
+		k_split_count<<<(N + 255) / 256, 256, 0, s>>>( d_T, K, N, extra, 3 ); LAUNCHED();
+		{ const int r = exclusive_scan( extra, base, tile, N, s ); if (r != TBVH_OK) return r; }
+		k_tree_bases<<<(K + 127) / 128, 128, 0, s>>>( d_T, K, base, d_ext ); LAUNCHED();
+		std::vector<uint32_t> ext_base( (size_t)K + 1 );
+		CUDA_TRY( cudaMemcpyAsync( ext_base.data(), d_ext, ((size_t)K + 1) * 4, cudaMemcpyDeviceToHost, s ) );
+		CUDA_TRY( cudaStreamSynchronize( s ) );
+		const uint32_t total = ext_base[K];
+		// the collapse's arrays (a wide node is an interior node of the split tree: fewer than total); leaf, tickets and look are zeroed
+		// together
+		const size_t look_words = (size_t)total / CW_LEVEL_T + CW_MAX_LEVELS + 1; // a block per CW_LEVEL_T nodes of each level
 		{
+			carve = 0;
+			const size_t o_ext = take( (size_t)total * 32 ), o_lists = take( ((size_t)total + 1) * 4 ), o_wtree = take( ((size_t)total + 1) * 4 );
+			const size_t o_adopt = take( ((size_t)total + 1) * 32 ), o_ifirst = take( ((size_t)total + 1) * 4 ), o_counts = take( CW_MAX_LEVELS * 4 );
+			const size_t o_groups = K > 1 ? take( ((size_t)total + 1) * 8 ) : 0; // a run per tree and level: at most one per wide node
+			const size_t o_leaf = take( (size_t)K * 4 ), o_tickets = take( (CW_MAX_LEVELS + 1) * 4 ), o_look = take( look_words * 8 );
+			CW_ALLOC( blob, carve );
+			ext = (float4*)(blob + o_ext), lists = (uint32_t*)(blob + o_lists), wtree = (uint32_t*)(blob + o_wtree), adopt = (uint32_t*)(blob + o_adopt);
+			ifirst = (uint32_t*)(blob + o_ifirst), counts = (uint32_t*)(blob + o_counts), groups = K > 1 ? (uint2*)(blob + o_groups) : 0;
+			leaf = (uint32_t*)(blob + o_leaf), tickets = (uint32_t*)(blob + o_tickets), look = (unsigned long long*)(blob + o_look);
+			CUDA_TRY( cudaMemsetAsync( blob + o_leaf, 0, carve - o_leaf, s ) );
+		}
+		ngroups = tickets + CW_MAX_LEVELS;
+		k_split_emit_batch<<<(N + 255) / 256, 256, 0, s>>>( d_T, K, N, base, ext, 3 ); LAUNCHED();
+		// ---- collapse to 8-wide, level by level from the K roots
+		std::vector<uint32_t> iota( K );
+		for (uint32_t t = 0; t < K; t++) iota[t] = t;
+		CUDA_TRY( cudaMemcpyAsync( lists, ext_base.data(), (size_t)K * 4, cudaMemcpyHostToDevice, s ) ); // level 0 = the roots
+		CUDA_TRY( cudaMemcpyAsync( wtree, iota.data(), (size_t)K * 4, cudaMemcpyHostToDevice, s ) );
+		std::vector<uint32_t> off; // level l occupies lists[off[l] .. off[l+1])
+		off.push_back( 0 ), off.push_back( K );
+		size_t look_used = 0;
+		while (off[off.size() - 1] > off[off.size() - 2])
+		{
+			const uint32_t level = (uint32_t)off.size() - 2, lo = off[level], num = off[level + 1] - lo, grid = (num + CW_LEVEL_T - 1) / CW_LEVEL_T;
+			k_collapse<<<grid, CW_LEVEL_T, 0, s>>>( ext, lists, wtree, lo, num, level == 0 ? K : 0, adopt, ifirst, leaf, look + look_used, tickets + level, counts + level,
+				groups, ngroups ); LAUNCHED();
+			look_used += grid;
+			uint32_t next = 0;
+			CUDA_TRY( cudaMemcpyAsync( &next, counts + level, 4, cudaMemcpyDeviceToHost, s ) );
+			CUDA_TRY( cudaStreamSynchronize( s ) );
+			off.push_back( lo + num + next );
+			if (off.size() > CW_MAX_LEVELS) { tbvh_set_error( "CWBVH conversion: runaway depth" ); return TBVH_E_LIMIT; }
+		}
+		off.pop_back(); // the last level is empty
+		const uint32_t levels = (uint32_t)off.size() - 1, W = off[levels];
+		// ---- each tree's runs of wide nodes, one per level it reaches: its wide-node count and its own level offsets (a CwKeep's off).
+		// Levels are grouped by tree in batch order, so sorted by first node the runs tile every level and a run ends where the next begins.
+		std::vector<uint32_t> h_leaf( K ), gfirst, glocal;
+		std::vector<uint2> runs;
+		uint32_t G = levels;
+		if (K > 1) CUDA_TRY( cudaMemcpyAsync( &G, ngroups, 4, cudaMemcpyDeviceToHost, s ) );
+		CUDA_TRY( cudaMemcpyAsync( h_leaf.data(), leaf, (size_t)K * 4, cudaMemcpyDeviceToHost, s ) );
+		CUDA_TRY( cudaStreamSynchronize( s ) );
+		if (K > 1)
+		{
+			runs.resize( G );
+			CUDA_TRY( cudaMemcpyAsync( runs.data(), groups, (size_t)G * 8, cudaMemcpyDeviceToHost, s ) );
+			CUDA_TRY( cudaStreamSynchronize( s ) );
+			std::sort( runs.begin(), runs.end(), []( const uint2& a, const uint2& b ) { return a.y < b.y; } );
+		}
+		else for (uint32_t l = 0; l < levels; l++) runs.push_back( make_uint2( 0, off[l] ) );
+		std::vector<std::vector<uint32_t>> toff( K, std::vector<uint32_t>( 1, 0 ) );
+		gfirst.resize( G ), glocal.resize( G );
+		for (uint32_t g = 0; g < G; g++)
+		{
+			const uint32_t t = runs[g].x, first = runs[g].y, end = g + 1 < G ? runs[g + 1].y : W;
+			gfirst[g] = first, glocal[g] = toff[t].back();
+			toff[t].push_back( toff[t].back() + (end - first) );
+		}
+		// ---- outputs, per handle
+		bool any_keep = false;
+		for (uint32_t t = 0; t < K; t++)
+		{
+			const tbvh_bvh b = bs[t];
+			const uint32_t wc = toff[t].back();
+			CUDA_TRY( cudaMalloc( &b->d_cw_nodes, (size_t)wc * 80 ) );
+			CUDA_TRY( cudaMalloc( &b->d_cw_tris, (size_t)b->info.idx_count * 48 ) );
+			T[t].cw_nodes = b->d_cw_nodes, T[t].cw_tris = b->d_cw_tris, T[t].ext_base = ext_base[t], T[t].wide_count = wc;
+			b->info.used_blocks = wc * 5, b->info.cwbvh_tri_count = b->info.idx_count;
+			if (!b->refittable) continue;
 			// keep the collapse for tbvh_refit_layouts, sized to the wide tree
 			CwKeep* k = new (std::nothrow) CwKeep();
 			if (!k) { tbvh_set_error( "CWBVH conversion: out of host memory" ); return TBVH_E_ARG; }
 			b->cw_keep = k;
-			k->used = used, k->total = total, k->wide_count = wide_count, k->leaf_root = leaf_root, k->off = off;
-			CUDA_TRY( cudaMalloc( &k->base, ((size_t)used + 1) * 4 ) );
-			CUDA_TRY( cudaMalloc( &k->list, (size_t)wide_count * 4 ) );
-			CUDA_TRY( cudaMalloc( &k->adopt, (size_t)wide_count * 32 ) );
-			CUDA_TRY( cudaMalloc( &k->ifirst, (size_t)wide_count * 4 ) );
-			CUDA_TRY( cudaMemcpyAsync( k->base, base, ((size_t)used + 1) * 4, cudaMemcpyDeviceToDevice, s ) );
-			CUDA_TRY( cudaMemcpyAsync( k->list, lists, (size_t)wide_count * 4, cudaMemcpyDeviceToDevice, s ) );
-			CUDA_TRY( cudaMemcpyAsync( k->adopt, adopt, (size_t)wide_count * 32, cudaMemcpyDeviceToDevice, s ) );
-			CUDA_TRY( cudaMemcpyAsync( k->ifirst, ifirst, (size_t)wide_count * 4, cudaMemcpyDeviceToDevice, s ) );
+			const uint32_t used = b->info.used_nodes;
+			k->used = used, k->total = ext_base[t + 1] - ext_base[t], k->wide_count = wc, k->leaf_root = h_leaf[t] != 0, k->off = toff[t];
+			CUDA_TRY( cudaMalloc( &k->base, ((size_t)used + 1 + (size_t)wc * 10) * 4 ) );
+			k->list = k->base + used + 1, k->adopt = k->list + wc, k->ifirst = k->adopt + (size_t)wc * 8;
+			T[t].keep = k->base, any_keep = true;
 		}
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		return TBVH_OK;
+		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
+		CW_ALLOC( wide, (size_t)W * sizeof( WideNode ) );
+		{ const int r = cw_assign_encode( s, ext, lists, adopt, ifirst, off, wide, K, d_T, wtree, CwTree{} ); if (r != TBVH_OK) return r; }
+		if (any_keep)
+		{
+			CW_ALLOC( d_runs, (size_t)G * 8 );
+			CUDA_TRY( cudaMemcpyAsync( d_runs, gfirst.data(), (size_t)G * 4, cudaMemcpyHostToDevice, s ) );
+			CUDA_TRY( cudaMemcpyAsync( d_runs + G, glocal.data(), (size_t)G * 4, cudaMemcpyHostToDevice, s ) );
+			k_keep<<<(uint32_t)(((size_t)W + N + 255) / 256), 256, 0, s>>>( d_T, K, wtree, d_runs, d_runs + G, G, W, lists, adopt, ifirst, base, N ); LAUNCHED();
+		}
+		// the traversal nodes the kernels read and the pending bound of every wide tree (trace_cwbvh.cu); synchronises the stream
+		return cw_make_trav( bs, K, s );
 	};
 	const int rc = body();
 	cudaStreamSynchronize( s );
 	for (void* p : scratch) cudaFree( p );
-	if (rc != TBVH_OK) cw_keep_free( b );
 	#undef CW_ALLOC
+	for (uint32_t t = 0; t < K; t++)
+	{
+		if (rc != TBVH_OK) drop_cwbvh( bs[t] ), bs[t]->info.used_blocks = 0, bs[t]->info.cwbvh_tri_count = 0;
+		else bs[t]->info.layouts |= 1u << TBVH_LAYOUT_CWBVH;
+	}
 	return rc;
 }
 
@@ -443,7 +689,7 @@ int cwbvh_refit( tbvh_bvh b, cudaStream_t s )
 	{ const int r = make_leaf_tris( b, s ); if (r != TBVH_OK) return r; }
 	k_split_emit<<<(k->used + 255) / 256, 256, 0, s>>>( b->d_nodes, k->base, k->ext, k->used, 3 ); LAUNCHED();
 	if (k->leaf_root) { k_wrap_leaf_root<<<1, 1, 0, s>>>( k->ext, k->adopt ); LAUNCHED(); }
-	{ const int r = cw_assign_encode( b, s, k->ext, k->list, k->adopt, k->ifirst, k->off, k->wide ); if (r != TBVH_OK) return r; }
+	{ const int r = cw_assign_encode( s, k->ext, k->list, k->adopt, k->ifirst, k->off, k->wide, 1, 0, 0, CwTree{ 0, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris } ); if (r != TBVH_OK) return r; }
 	CUDA_TRY( cudaMemsetAsync( k->misc + 8, 0, 4, s ) );
 	{ const int r = cw_expand_launch( b, s, k->misc + 8 ); if (r != TBVH_OK) return r; }
 	CUDA_TRY( cudaEventRecord( k->e1, s ) );

@@ -39,19 +39,42 @@
 // ---- bvh8Data -> traversal nodes ------------------------------------------------------------------------------------
 // One thread per node.  Slot i of the source node: meta byte i (n1.z / n1.w), quantised bounds byte i of the six 8-byte rows at
 // bytes 32..79 (lo.x, lo.y, lo.z, hi.x, hi.y, hi.z) - layout in SURVEY.md 8(a), written by BVH8_CWBVH::ConvertFrom (tiny_bvh.h:5948-6015).
-// range: max over the nodes of 128 + the largest exponent byte, or 256 for a node with e = -128 or |p| > 2^126 (cw_ray_fits)
-__global__ void k_cw_expand( const uint4* __restrict__ src, uint4* __restrict__ dst, uint32_t* __restrict__ parent, uint32_t* __restrict__ range, const uint32_t count )
+// One wide tree of a pass: its bvh8Data (src), its traversal nodes (dst), where its results go (res[0]: range, res[1]: pending
+// bound) and its first node in the pass's node index space (wbase).  A batch passes a device table of them, one tree `one`.
+struct CwTrav { const uint4* src; uint4* dst; uint32_t* res; uint32_t wbase, count; };
+
+// the tree that holds node g of a pass (wbase rises strictly: every tree has a node)
+__device__ __forceinline__ uint32_t trav_tree( const CwTrav* __restrict__ T, const uint32_t K, const uint32_t g )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= count) return;
+	uint32_t lo = 0, hi = K;
+	while (hi - lo > 1) { const uint32_t m = (lo + hi) >> 1; if (T[m].wbase <= g) lo = m; else hi = m; }
+	return lo;
+}
+
+// range: max over a tree's nodes of 128 + the largest exponent byte, or 256 for a node with e = -128 or |p| > 2^126 (cw_ray_fits)
+// BATCH: the trees of the table T; else the one tree `one`, whose pointers stay kernel parameters (read from a table, they make
+// nvcc keep the pair records below in local memory)
+template <bool BATCH>
+__global__ void k_cw_expand( const CwTrav* __restrict__ T, const uint32_t K, const CwTrav one, const uint32_t W, uint32_t* __restrict__ parent )
+{
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= W) return;
+	const uint32_t tree = BATCH ? trav_tree( T, K, g ) : 0;
+	const CwTrav* tr = BATCH ? T + tree : &one;
+	const uint4* __restrict__ src = tr->src;
+	uint4* __restrict__ dst = tr->dst;
+	uint32_t* const res = tr->res;
+	const uint32_t wbase = tr->wbase, x = g - wbase, count = tr->count;
 	const uint4 n0 = src[(size_t)x * 5], n1 = src[(size_t)x * 5 + 1], n2 = src[(size_t)x * 5 + 2], n3 = src[(size_t)x * 5 + 3], n4 = src[(size_t)x * 5 + 4];
 	{
 		const int ex = (int8_t)(n0.w & 255u), ey = (int8_t)((n0.w >> 8) & 255u), ez = (int8_t)((n0.w >> 16) & 255u);
 		const bool p_ok = fabsf( __uint_as_float( n0.x ) ) <= CW_ORIGIN_LIMIT && fabsf( __uint_as_float( n0.y ) ) <= CW_ORIGIN_LIMIT && fabsf( __uint_as_float( n0.z ) ) <= CW_ORIGIN_LIMIT;
 		const bool bad = !p_ok || ex == -128 || ey == -128 || ez == -128;
 		const uint32_t key = bad ? 256u : (uint32_t)(128 + max( ex, max( ey, ez ) ));
-		const uint32_t m = __reduce_max_sync( __activemask(), key );
-		if ((threadIdx.x & 31) == __ffs( __activemask() ) - 1) atomicMax( range, m );
+		// reduced over the lanes of the same tree only: one tree's exponents never reach another's limit
+		const uint32_t same = __match_any_sync( __activemask(), tree );
+		const uint32_t m = __reduce_max_sync( same, key );
+		if ((threadIdx.x & 31) == __ffs( same ) - 1) atomicMax( res, m );
 	}
 	const uint32_t row[6][2] = { { n2.x, n2.y }, { n2.z, n2.w }, { n3.x, n3.y }, { n3.z, n3.w }, { n4.x, n4.y }, { n4.z, n4.w } };
 	const uint32_t meta[2] = { n1.z, n1.w };
@@ -95,7 +118,7 @@ __global__ void k_cw_expand( const uint4* __restrict__ src, uint4* __restrict__ 
 	}
 	// inner children sit at n1.x + 0 .. inner-1 (node units): note their parent, and whether it has siblings to leave pending, for
 	// the pending pass
-	if (parent) for (uint32_t c = 0; c < inner; c++) if (n1.x + c < count) parent[n1.x + c] = x | (inner >= 2 ? 0x80000000u : 0u);
+	if (parent) for (uint32_t c = 0; c < inner; c++) if (n1.x + c < count) parent[wbase + n1.x + c] = x | (inner >= 2 ? 0x80000000u : 0u);
 }
 
 // The walk pushes a node group only when the node it enters has inner siblings still to visit (cw_trace: rest > 0x00ffffff), so
@@ -103,82 +126,99 @@ __global__ void k_cw_expand( const uint4* __restrict__ src, uint4* __restrict__ 
 // what the pending stack must hold - on a chain (the 3-triangle leaves SplitLeafs makes of a long leaf) far less than the depth.
 // It is found by pointer jumping: every node keeps an ancestor and the count of flagged nodes up to it, and each pass doubles
 // the distance (anc' = anc(anc), cnt' = cnt + cnt(anc)), so ceil( log2( count ) ) + 1 passes reach the root from any node.  A node
-// still short of the root then lies on a cycle (uploaded data): the tree is reported as such.
+// still short of the root then lies on a cycle (uploaded data): the tree is reported as such.  The trees of a batch jump together
+// over one index space (W nodes); parent links never leave a tree.
 #define CW_ROOT 0xffffffffu   // ancestor past the root
 #define CW_CYCLE 0xffffffffu  // cw_pending of a tree with a cycle
-__global__ void k_cw_jump_init( const uint32_t* __restrict__ parent, const uint32_t count, uint32_t* __restrict__ anc, uint32_t* __restrict__ cnt )
+__global__ void k_cw_jump_init( const CwTrav* __restrict__ T, const uint32_t K, const uint32_t* __restrict__ parent, const uint32_t W, uint32_t* __restrict__ anc, uint32_t* __restrict__ cnt )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= count) return;
-	const uint32_t p = parent[x];
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= W) return;
+	const uint32_t wb = T[trav_tree( T, K, g )].wbase, p = parent[g];
 	// the root steps past itself - unless some node names it as a child, a cycle a walk would never leave: it then stays on itself;
-	// a record no node points at (0xffffffff) gets ancestor `count` (out of range) and is not counted
-	anc[x] = x == 0 ? (p == 0xffffffffu ? CW_ROOT : 0u) : p == 0xffffffffu ? count : (p & 0x7fffffffu), cnt[x] = (x == 0 || p == 0xffffffffu) ? 0u : p >> 31;
+	// a record no node points at (0xffffffff) gets ancestor W (out of range) and is not counted
+	anc[g] = g == wb ? (p == 0xffffffffu ? CW_ROOT : g) : p == 0xffffffffu ? W : wb + (p & 0x7fffffffu), cnt[g] = (g == wb || p == 0xffffffffu) ? 0u : p >> 31;
 }
-__global__ void k_cw_jump( const uint32_t count, const uint32_t* __restrict__ anc, const uint32_t* __restrict__ cnt, uint32_t* __restrict__ anc2, uint32_t* __restrict__ cnt2 )
+__global__ void k_cw_jump( const uint32_t W, const uint32_t* __restrict__ anc, const uint32_t* __restrict__ cnt, uint32_t* __restrict__ anc2, uint32_t* __restrict__ cnt2 )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= count) return;
+	if (x >= W) return;
 	const uint32_t a = anc[x];
-	if (a < count) anc2[x] = anc[a], cnt2[x] = min( cnt[x] + cnt[a], 0x40000000u );
+	if (a < W) anc2[x] = anc[a], cnt2[x] = min( cnt[x] + cnt[a], 0x40000000u );
 	else anc2[x] = a, cnt2[x] = cnt[x];
 }
-__global__ void k_cw_pending( const uint32_t count, const uint32_t* __restrict__ anc, const uint32_t* __restrict__ cnt, uint32_t* __restrict__ max_pending )
+__global__ void k_cw_pending( const CwTrav* __restrict__ T, const uint32_t K, const uint32_t W, const uint32_t* __restrict__ anc, const uint32_t* __restrict__ cnt )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= count) return;
-	const uint32_t a = anc[x];
-	if (a == CW_ROOT) atomicMax( max_pending, cnt[x] );
-	else if (a < count) atomicMax( max_pending, CW_CYCLE );
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= W) return;
+	const uint32_t a = anc[g];
+	uint32_t* pending = T[trav_tree( T, K, g )].res + 1;
+	if (a == CW_ROOT) atomicMax( pending, cnt[g] );
+	else if (a < W) atomicMax( pending, CW_CYCLE );
 }
 
 // k_cw_expand of every node of d_cw_nodes into the allocated d_cw_trav; *d_range (zeroed by the caller) receives the tree's range
 int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range )
 {
 	const uint32_t count = b->info.used_blocks / 5;
-	k_cw_expand<<<(count + 127) / 128, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, 0, d_range, count ); LAUNCHED();
+	const CwTrav one = { (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_range, 0, count };
+	k_cw_expand<false><<<(count + 127) / 128, 128, 0, s>>>( 0, 1, one, count, 0 ); LAUNCHED();
 	return TBVH_OK;
 }
 
 // |rD| <= 2^( 127 - largest e ) keeps 2^e * rD finite (cw_ray_fits); 2^127 at most, and no ray fits a tree that has range 256
 float cw_rd_limit_for( uint32_t range ) { return range < 256 ? ldexpf( 1.0f, 127 - max( 0, (int)range - 128 ) ) : -1.0f; }
 
-int cw_make_trav( tbvh_bvh b, cudaStream_t s )
+int cw_make_trav( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 {
-	if (b->d_cw_trav) cudaFree( b->d_cw_trav ), b->d_cw_trav = 0;
-	const uint32_t count = b->info.used_blocks / 5;
-	if (count == 0) { tbvh_set_error( "cw_make_trav: no CWBVH nodes" ); return TBVH_E_STATE; }
-	// one float4 past the nodes holds the tree's exponent / |p| range while it is found
-	CUDA_TRY( cudaMalloc( &b->d_cw_trav, ((size_t)count * CW_NODE_F4 + 1) * 16 ) );
-	uint32_t* d_range = (uint32_t*)(b->d_cw_trav + (size_t)count * CW_NODE_F4);
-	uint32_t range = 256;
-	b->cw_rd_limit = -1.0f;
-	CUDA_TRY( cudaMemsetAsync( d_range, 0, 4, s ) );
+	std::vector<CwTrav> T( K );
+	uint32_t W = 0, most = 0; // nodes of the pass (the conversion's batch bound keeps it a uint32_t), nodes of the largest tree
+	for (uint32_t t = 0; t < K; t++)
+	{
+		const tbvh_bvh b = bs[t];
+		if (b->d_cw_trav) cudaFree( b->d_cw_trav ), b->d_cw_trav = 0;
+		b->cw_pending = 0xffffffffu, b->cw_rd_limit = -1.0f;
+		const uint32_t count = b->info.used_blocks / 5;
+		if (count == 0) { tbvh_set_error( "cw_make_trav: no CWBVH nodes" ); return TBVH_E_STATE; }
+		T[t] = CwTrav{ (const uint4*)b->d_cw_nodes, 0, 0, W, count };
+		W += count, most = max( most, count );
+	}
+	for (uint32_t t = 0; t < K; t++)
+	{
+		CUDA_TRY( cudaMalloc( &bs[t]->d_cw_trav, (size_t)T[t].count * CW_NODE_F4 * 16 ) );
+		T[t].dst = (uint4*)bs[t]->d_cw_trav;
+	}
+	CwTrav* d_T = 0;
 	uint32_t* d_parent = 0;
-	uint32_t pending = 0xffffffffu;
+	std::vector<uint32_t> res( (size_t)K * 2 ); // range, pending bound per tree
 	auto body = [&]() -> int
 	{
 		// every node notes its parent, then the counts of ancestors that leave node groups pending are summed up to the root
-		CUDA_TRY( cudaMalloc( &d_parent, ((size_t)count * 5 + 1) * 4 ) );
-		uint32_t* const anc[2] = { d_parent + count, d_parent + 2 * (size_t)count }, * const cnt[2] = { d_parent + 3 * (size_t)count, d_parent + 4 * (size_t)count };
-		uint32_t* const d_pending = d_parent + 5 * (size_t)count;
-		CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)count * 4, s ) );
-		CUDA_TRY( cudaMemsetAsync( d_pending, 0, 4, s ) );
-		const uint32_t g = (count + 127) / 128;
-		k_cw_expand<<<g, 128, 0, s>>>( (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_parent, d_range, count ); LAUNCHED();
-		k_cw_jump_init<<<g, 128, 0, s>>>( d_parent, count, anc[0], cnt[0] ); LAUNCHED();
+		const size_t words = (((size_t)W * 5 + (size_t)K * 2) + 63) & ~(size_t)63; // the tree table follows, 256-byte aligned
+		CUDA_TRY( cudaMalloc( &d_parent, words * 4 + (size_t)K * sizeof( CwTrav ) ) );
+		d_T = (CwTrav*)(d_parent + words);
+		uint32_t* const anc[2] = { d_parent + W, d_parent + 2 * (size_t)W }, * const cnt[2] = { d_parent + 3 * (size_t)W, d_parent + 4 * (size_t)W };
+		uint32_t* const d_res = d_parent + 5 * (size_t)W;
+		for (uint32_t t = 0; t < K; t++) T[t].res = d_res + 2 * (size_t)t;
+		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTrav ), cudaMemcpyHostToDevice, s ) );
+		CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)W * 4, s ) );
+		CUDA_TRY( cudaMemsetAsync( d_res, 0, (size_t)K * 8, s ) );
+		const uint32_t g = (W + 127) / 128;
+		if (K > 1) k_cw_expand<true><<<g, 128, 0, s>>>( d_T, K, CwTrav{}, W, d_parent );
+		else k_cw_expand<false><<<g, 128, 0, s>>>( 0, 1, T[0], W, d_parent );
+		LAUNCHED();
+		k_cw_jump_init<<<g, 128, 0, s>>>( d_T, K, d_parent, W, anc[0], cnt[0] ); LAUNCHED();
 		int cur = 0;
-		for (uint32_t reach = 1; reach < 2 * count; reach *= 2, cur ^= 1) { k_cw_jump<<<g, 128, 0, s>>>( count, anc[cur], cnt[cur], anc[cur ^ 1], cnt[cur ^ 1] ); LAUNCHED(); }
-		k_cw_pending<<<g, 128, 0, s>>>( count, anc[cur], cnt[cur], d_pending ); LAUNCHED();
-		CUDA_TRY( cudaMemcpyAsync( &pending, d_pending, 4, cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaMemcpyAsync( &range, d_range, 4, cudaMemcpyDeviceToHost, s ) );
+		for (uint32_t reach = 1; reach < 2 * most; reach *= 2, cur ^= 1) { k_cw_jump<<<g, 128, 0, s>>>( W, anc[cur], cnt[cur], anc[cur ^ 1], cnt[cur ^ 1] ); LAUNCHED(); }
+		k_cw_pending<<<g, 128, 0, s>>>( d_T, K, W, anc[cur], cnt[cur] ); LAUNCHED();
+		CUDA_TRY( cudaMemcpyAsync( res.data(), d_res, (size_t)K * 8, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
 	};
 	const int rc = body();
+	cudaStreamSynchronize( s );
 	if (d_parent) cudaFree( d_parent );
-	b->cw_pending = pending;
-	if (rc == TBVH_OK) b->cw_rd_limit = cw_rd_limit_for( range );
+	if (rc == TBVH_OK) for (uint32_t t = 0; t < K; t++) bs[t]->cw_pending = res[2 * (size_t)t + 1], bs[t]->cw_rd_limit = cw_rd_limit_for( res[2 * (size_t)t] );
 	return rc;
 }
 

@@ -1,13 +1,15 @@
-"""Batched builds against a loop of single builds, on the GPU: `python tools/build_batch_perf.py --out DIR [--reps N]`.
+"""Batched builds and conversions against loops of single ones, on the GPU: `python tools/build_batch_perf.py --out DIR [--reps N]`.
 
 Workloads (seeded, procedural):
   a  1,000 meshes, triangle counts log-uniform in [64, 20000]  (a scene of many small BLASses)
   b  16 meshes of 100k..500k triangles + 500 of 100..5,000     (a few big meshes among many small ones)
 For each: a loop of tbvh_build over the meshes and one tbvh_build_batch, alternated, after a warm-up of each - host wall time around the
 complete call(s), device time (sum of info.build_ms for the loop, the batch's build_ms), kernel launches, and a byte comparison of every
-tree.  Then the wall time of the per-handle tbvh_convert( CWBVH ) of the same meshes.  Then the one-tree path against an older build of
-the library (--parent-lib, when given): tbvh_build of the Bistro-sized procedural scene and of
-a 150k-triangle scene, the two libraries alternated on the same card.  The card's name and power limit come from nvidia-smi (read-only).
+tree.  Then the CWBVH conversion of the same meshes' BuildAVX trees (what BVH8_CWBVH builds over): a loop of tbvh_convert( CWBVH ) per
+handle and one tbvh_convert_batch, alternated - wall time (both calls end in a synchronise), launches, and a byte comparison of every
+bvh8Data / bvh8Tris.  Then the one-tree path against an older build of the library (--parent-lib, when given): tbvh_build of the
+Bistro-sized procedural scene and of a 150k-triangle scene, and the wall time of tbvh_convert( CWBVH ) of the Bistro-sized scene's
+Build and BuildHQ trees, the two libraries alternated on the same card.  The card's name and power limit come from nvidia-smi (read-only).
 Writes DIR/build_batch_perf.json and prints it."""
 import argparse
 import ctypes as C
@@ -77,6 +79,13 @@ class Lib:
     def build(self, h, v, flavour=0):
         self.check(self.L.tbvh_build_flavour(h, v.ctypes.data, 16, v.shape[0] // 3, _lib.HOST, 1.0, 1.0, flavour))
 
+    def download_cwbvh(self, h):
+        i = self.info(h)
+        d = np.zeros(i.used_blocks * 4, np.uint32)
+        t = np.zeros(i.cwbvh_tri_count * 12, np.uint32)
+        self.check(self.L.tbvh_download_cwbvh(h, d.ctypes.data, t.ctypes.data, _lib.HOST))
+        return d, t
+
     def download(self, h):
         i = self.info(h)
         nodes = np.zeros(i.used_nodes * 8, np.uint32)
@@ -115,20 +124,40 @@ def run_workload(L, meshes, reps):
     for k in range(n):
         a, b = L.download(loop_h[k]), L.download(batch_h[k])
         same += np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
-    conv = []
-    for _ in range(reps):
-        L.check(L.L.tbvh_build_batch(batch_h, recs, n, _lib.HOST, 1.0, 1.0, _lib.BUILD_AVX))
+    for hs in (loop_h, batch_h):
+        L.check(L.L.tbvh_build_batch(hs, recs, n, _lib.HOST, 1.0, 1.0, _lib.BUILD_AVX))
+    conv = {"loop": {"wall_ms": [], "launches": []}, "batch": {"wall_ms": [], "launches": []}}
+
+    def conv_loop():
         t0 = time.perf_counter()
         for k in range(n):
-            L.check(L.L.tbvh_convert(batch_h[k], _lib.LAYOUT_CWBVH))
-        conv.append((time.perf_counter() - t0) * 1e3)
+            L.check(L.L.tbvh_convert(loop_h[k], _lib.LAYOUT_CWBVH))
+        return (time.perf_counter() - t0) * 1e3
+
+    def conv_batch():
+        t0 = time.perf_counter()
+        L.check(L.L.tbvh_convert_batch(batch_h, n, _lib.LAYOUT_CWBVH))
+        return (time.perf_counter() - t0) * 1e3
+
+    conv_loop(), conv_batch()   # warm-up
+    for _ in range(reps):
+        for name, f in (("loop", conv_loop), ("batch", conv_batch)):
+            n0 = L.L.tbvh_launch_count()
+            conv[name]["wall_ms"].append(f())
+            conv[name]["launches"].append(L.L.tbvh_launch_count() - n0)
+    cw_same = 0
+    for k in range(n):
+        a, b = L.download_cwbvh(loop_h[k]), L.download_cwbvh(batch_h[k])
+        cw_same += np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
     for h in list(loop_h) + list(batch_h):
         L.L.tbvh_bvh_destroy(h)
     out = {"meshes": n, "triangles": int(sum(v.shape[0] // 3 for v in meshes)), "trees_identical": int(same)}
     for name in ("loop", "batch"):
         out[name] = {k: stats(v) for k, v in res[name].items()}
     out["speedup_wall_median"] = out["loop"]["wall_ms"]["median"] / out["batch"]["wall_ms"]["median"]
-    out["convert_cwbvh_per_handle_wall_ms"] = stats(conv)
+    out["convert_cwbvh"] = {name: {k: stats(v) for k, v in conv[name].items()} for name in conv}
+    out["convert_cwbvh"]["cwbvh_identical"] = int(cw_same)
+    out["convert_cwbvh"]["speedup_wall_median"] = out["convert_cwbvh"]["loop"]["wall_ms"]["median"] / out["convert_cwbvh"]["batch"]["wall_ms"]["median"]
     return out
 
 
@@ -151,6 +180,32 @@ def one_tree(libs, reps):
     return out
 
 
+def one_tree_convert(libs, reps):
+    """tbvh_convert( CWBVH ) of one big tree, wall time: the path bench.py reports as cwbvh_convert_ms_wall."""
+    v = scenes.procedural_scene(2837209, 7)
+    out = {}
+    for label, flavour in (("bistro_sized_build", _lib.BUILD_REFERENCE), ("bistro_sized_buildhq", _lib.BUILD_HQ)):
+        hs = {name: L.handles(1) for name, L in libs.items()}
+        ms = {name: [] for name in libs}
+        for name, L in libs.items():
+            L.build(hs[name][0], v, flavour)
+            L.check(L.L.tbvh_convert(hs[name][0], _lib.LAYOUT_CWBVH))   # warm-up
+        for _ in range(reps):
+            for name, L in libs.items():
+                t0 = time.perf_counter()
+                L.check(L.L.tbvh_convert(hs[name][0], _lib.LAYOUT_CWBVH))
+                ms[name].append((time.perf_counter() - t0) * 1e3)
+        cws = [L.download_cwbvh(hs[name][0]) for name, L in libs.items()]
+        out[label] = {name: stats(x) for name, x in ms.items()}
+        # bvh8Tris past the referenced records is uninitialised on an SBVH: compare bvh8Data and the records of the Build tree
+        out[label]["bvh8data_identical"] = all(np.array_equal(c[0], cws[0][0]) for c in cws)
+        if flavour != _lib.BUILD_HQ:
+            out[label]["bvh8tris_identical"] = all(np.array_equal(c[1], cws[0][1]) for c in cws)
+        for name, L in libs.items():
+            L.L.tbvh_bvh_destroy(hs[name][0])
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True, help="directory for build_batch_perf.json")
@@ -168,6 +223,7 @@ def main():
     if args.parent_lib:
         libs = {"parent": Lib(args.parent_lib), "this": L}
     result["one_tree_build_ms"] = one_tree(libs, max(args.reps, 7))
+    result["one_tree_convert_cwbvh_wall_ms"] = one_tree_convert(libs, max(args.reps, 7))
     path = os.path.join(args.out, "build_batch_perf.json")
     with open(path, "w") as f:
         json.dump(result, f, indent=1)
