@@ -17,6 +17,8 @@ void tbvh_set_error( const char* fmt, ... );
 extern unsigned long long g_tbvh_launches;
 #define CUDA_TRY( x ) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { tbvh_set_error( "%s:%d %s -> %s", __FILE__, __LINE__, #x, cudaGetErrorString( e_ ) ); return TBVH_E_CUDA; } } while (0)
 #define LAUNCHED() do { g_tbvh_launches++; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { tbvh_set_error( "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString( e_ ) ); return TBVH_E_CUDA; } } while (0)
+#define ARG_CHECK( c, msg ) do { if (!(c)) { tbvh_set_error( "%s: %s", __func__, msg ); return TBVH_E_ARG; } } while (0)
+#define TRY( x ) do { int r_ = (x); if (r_ != TBVH_OK) return r_; } while (0)
 
 // ---- handles ----------------------------------------------------------------------------------------------
 // one stage buffer set of the host-buffer pipeline (api.cu "host path")
@@ -234,10 +236,12 @@ struct TlasInst { float inv[16]; uint32_t blasIdx, mask, pad0, pad1; };         
 struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root_count; float cw_rd_limit; uint32_t pad1; const float4* cw_nodes; const float4* cw_tris; }; // 48 bytes: BVH-layout arrays, CWBVH traversal nodes + bvh8Tris (0 when absent) and their rD limit
 int make_leaf_tris( tbvh_bvh b, cudaStream_t s );
 int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used_nodes_gpu, cudaStream_t s );
-int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s );
+int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s ); // sets the BVH_GPU bit on success; on failure the handle holds no BVH_GPU
+void drop_bvh_gpu( tbvh_bvh b );                  // the BVH_GPU array, its bit and used_nodes_gpu (no TLAS points at it: the generation stays)
 // BVH8_CWBVH::Build's conversion chain for K handles of one context at once (convert_cwbvh.cu); tbvh_convert is K = 1
 int bvh_to_cwbvh( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
 int cwbvh_refit( tbvh_bvh b, cudaStream_t s );  // tbvh_refit_layouts over b->cw_keep (convert_cwbvh.cu)
-void cw_keep_free( tbvh_bvh b );                // drop b->cw_keep: wherever the CWBVH arrays are replaced or dropped
+// the CWBVH arrays, the kept collapse, the bit, the counts and the traversal limits; a TLAS over the arrays becomes stale
+void drop_cwbvh( tbvh_bvh b );
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)
 int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint32_t n, cudaStream_t s );

@@ -113,19 +113,24 @@ __global__ void k_gpu_emit( const float4* __restrict__ nodes, const uint32_t* __
 	out[(size_t)idx * 4 + 3] = make_float4( r1.x, r1.y, r1.z, __uint_as_float( 0u ) );
 }
 
+void drop_bvh_gpu( tbvh_bvh b )
+{
+	if (b->d_nodes_gpu) cudaFree( b->d_nodes_gpu );
+	b->d_nodes_gpu = 0;
+	b->info.layouts &= ~(1u << TBVH_LAYOUT_BVH_GPU), b->info.used_nodes_gpu = 0;
+}
+
 int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s )
 {
 	const uint32_t used = b->info.used_nodes;
-	if (b->d_nodes_gpu) cudaFree( b->d_nodes_gpu );
-	b->d_nodes_gpu = 0;
-	CUDA_TRY( cudaMalloc( &b->d_nodes_gpu, (size_t)used * 64 ) );
+	drop_bvh_gpu( b );
 	uint32_t* w = 0; // workspace: parent, arrive, sub_int, sub_leaves [used]
 	const size_t words = (size_t)used * 4;
-	CUDA_TRY( cudaMalloc( &w, words * 4 ) );
-	uint32_t* parent = w, * arrive = w + used, * sub_int = arrive + used, * sub_leaves = sub_int + used;
-	int rc = TBVH_OK;
 	auto body = [&]() -> int
 	{
+		CUDA_TRY( cudaMalloc( &b->d_nodes_gpu, (size_t)used * 64 ) );
+		CUDA_TRY( cudaMalloc( &w, words * 4 ) );
+		uint32_t* parent = w, * arrive = w + used, * sub_int = arrive + used, * sub_leaves = sub_int + used;
 		CUDA_TRY( cudaMemsetAsync( w, 0, words * 4, s ) );
 		const uint32_t g = (used + 255) / 256;
 		k_gpu_parents<<<g, 256, 0, s>>>( b->d_nodes, parent, used ); LAUNCHED();
@@ -134,10 +139,11 @@ int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s )
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
 	};
-	rc = body();
+	const int rc = body();
 	cudaStreamSynchronize( s );
 	cudaFree( w );
-	if (rc == TBVH_OK) b->info.used_nodes_gpu = used - 1; // node 1 of the Wald layout is unused
+	if (rc != TBVH_OK) drop_bvh_gpu( b );
+	else b->info.used_nodes_gpu = used - 1, b->info.layouts |= 1u << TBVH_LAYOUT_BVH_GPU; // node 1 of the Wald layout is unused
 	return rc;
 }
 

@@ -64,7 +64,7 @@ struct CwKeep
 	cudaEvent_t e0 = 0, e1 = 0;
 };
 
-void cw_keep_free( tbvh_bvh b )
+static void cw_keep_free( tbvh_bvh b )
 {
 	CwKeep* k = b->cw_keep;
 	if (!k) return;
@@ -502,7 +502,7 @@ static int cw_assign_encode( cudaStream_t s, const float4* ext, const uint32_t* 
 }
 
 // the CWBVH arrays of b and what refers to them go (a TLAS over them becomes stale)
-static void drop_cwbvh( tbvh_bvh b )
+void drop_cwbvh( tbvh_bvh b )
 {
 	if (b->d_cw_trav || b->d_cw_tris) b->generation = tbvh_next_generation(); // a TLAS may hold these addresses (api.cu tlas_check)
 	if (b->d_cw_nodes) cudaFree( b->d_cw_nodes );
@@ -510,6 +510,8 @@ static void drop_cwbvh( tbvh_bvh b )
 	if (b->d_cw_trav) cudaFree( b->d_cw_trav );
 	b->d_cw_nodes = 0, b->d_cw_tris = 0, b->d_cw_trav = 0;
 	cw_keep_free( b );
+	b->info.layouts &= ~(1u << TBVH_LAYOUT_CWBVH), b->info.used_blocks = 0, b->info.cwbvh_tri_count = 0;
+	b->cw_pending = 0, b->cw_rd_limit = -1.0f;
 }
 
 // bs[0 .. K): handles of one context holding BVH-layout trees.  On success each holds the CWBVH a conversion of its own tree gives;
@@ -522,7 +524,6 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 	{
 		const tbvh_bvh b = bs[t];
 		drop_cwbvh( b );
-		b->info.layouts &= ~(1u << TBVH_LAYOUT_CWBVH);
 		T[t] = CwTree{ b->d_nodes, b->d_prim_idx, b->d_verts, 0, 0, 0, N, b->info.used_nodes, cw_seg( b->info.used_nodes ), 0, 0 };
 		N += T[t].seg;
 	}
@@ -661,7 +662,7 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 	#undef CW_ALLOC
 	for (uint32_t t = 0; t < K; t++)
 	{
-		if (rc != TBVH_OK) drop_cwbvh( bs[t] ), bs[t]->info.used_blocks = 0, bs[t]->info.cwbvh_tri_count = 0;
+		if (rc != TBVH_OK) drop_cwbvh( bs[t] );
 		else bs[t]->info.layouts |= 1u << TBVH_LAYOUT_CWBVH;
 	}
 	return rc;

@@ -24,9 +24,6 @@ struct tbvh_group_t
 	std::vector<std::pair<void*, size_t>> host_blocks; // tbvh_group_host_alloc results (mmap + cudaHostRegister)
 };
 
-#define ARG_CHECK( c, msg ) do { if (!(c)) { tbvh_set_error( "%s: %s", __func__, msg ); return TBVH_E_ARG; } } while (0)
-#define TRY( x ) do { int r_ = (x); if (r_ != TBVH_OK) return r_; } while (0)
-
 static void release_replicas( tbvh_group g )
 {
 	for (size_t i = 0; i < g->replica.size(); i++) if (g->replica[i] && g->owned[i]) tbvh_bvh_destroy( g->replica[i] );

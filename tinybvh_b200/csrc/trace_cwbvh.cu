@@ -176,7 +176,6 @@ int cw_make_trav( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 	for (uint32_t t = 0; t < K; t++)
 	{
 		const tbvh_bvh b = bs[t];
-		if (b->d_cw_trav) cudaFree( b->d_cw_trav ), b->d_cw_trav = 0;
 		b->cw_pending = 0xffffffffu, b->cw_rd_limit = -1.0f;
 		const uint32_t count = b->info.used_blocks / 5;
 		if (count == 0) { tbvh_set_error( "cw_make_trav: no CWBVH nodes" ); return TBVH_E_STATE; }
