@@ -200,6 +200,28 @@ int tbvh_refit( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_
  * replicas keep the old boxes until tbvh_group_replicate runs again. */
 int tbvh_refit_layouts( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_count, int space );
 
+/* Many trees refitted in one call, as an animated scene refits its BLASes every frame (tiny_bvh_anim.cpp, tmpl8/game.cpp).
+ * meshes[i] holds the new vertices of bvhs[i] as for tbvh_refit: verts, stride, prim_count; indices must be NULL and vert_count 0
+ * (a refit takes the flat slice).  All meshes are in one `space`; device-space inputs follow the rule above.
+ *  keep_layouts = 0: each bvhs[i] ends up exactly as tbvh_refit of it alone leaves it (BVH_GPU and CWBVH dropped; its generation
+ *  renewed, so a TLAS over it is stale, only where a CWBVH was dropped).
+ *  keep_layouts = 1: each ends up exactly as tbvh_refit_layouts of it alone leaves it: every BVH_GPU and kept CWBVH brought up to
+ *  date in place, the rD limit of each CWBVH recomputed for its own tree, the new root box in its info, and a TLAS over any of them
+ *  stale.  The handles of one batch may hold different subsets of BVH_GPU and CWBVH.
+ * The trees are refitted together by the same kernels, so the fixed cost of a refit (launches, allocations, host round trips) is paid
+ * once per batch instead of once per tree: launches grow with the deepest kept wide tree's level count, not with `count`, and a call
+ * synchronises the host once.  info.build_ms is the device time of the whole batch; the order of `bvhs` and the other trees of the
+ * batch change no tree.
+ *  Refusals come before any handle or vertex array is touched, so every handle keeps its trees and its generation: TBVH_E_ARG for count
+ *  0, a NULL or repeated handle, handles of different contexts, non-NULL indices or a vert_count, an unknown space, or a keep_layouts
+ *  other than 0 or 1; then per handle, in order, tbvh_refit's / tbvh_refit_layouts' own refusals (TBVH_E_STATE for no BVH-layout
+ *  tree, an SBVH, a TLAS, or with keep_layouts a CWBVH that tbvh_convert did not produce; TBVH_E_ARG for another prim_count or a bad
+ *  stride); TBVH_E_LIMIT when the BVH2 nodes, primitive references, or (with keep_layouts) kept split-tree or wide nodes of the batch
+ *  add up to more than TBVH_REFIT_BATCH_MAX_NODES (node indices of the shared index spaces are 32-bit).  A failure after the device
+ *  work started leaves every handle of the batch with its BVH-layout tree, whose boxes are unspecified, and without BVH_GPU or CWBVH. */
+#define TBVH_REFIT_BATCH_MAX_NODES (1u << 31)
+int tbvh_refit_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts );
+
 /* consume a tree built elsewhere, in the reference's own layouts (the public members bvhNode / primIdx /
  * verts of tiny_bvh.h:952-964, BVH_GPU::bvhNode :1124, BVH8_CWBVH::bvh8Data / bvh8Tris :1356-1357) */
 int tbvh_upload_bvh( tbvh_bvh bvh, const void* nodes32, uint32_t used_nodes, const uint32_t* prim_idx, uint32_t idx_count,

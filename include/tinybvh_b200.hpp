@@ -62,6 +62,10 @@ inline void free_pinned( void* p ) { tbvh_host_free( p ); }
 // Refit and Optimize working from the caller's arrays, the public counters.  flavour: TBVH_BUILD_REFERENCE (BVH::Build) or
 // TBVH_BUILD_AVX; by default the builder the class's own Build uses.  BVH_GPU / BVH8_CWBVH objects are converted afterwards.
 template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* const* vertices, const uint32_t* primCounts, uint32_t count, int flavour = -1 );
+// Many refits in one call (tbvh_refit_batch), as an animated scene refits its BLASes every frame: every object refitted from the vertex
+// array it was built from, exactly as its own Refit() would leave it - the tree and the public counters.
+class BVH;
+void RefitBatch( BVH* const* objs, uint32_t count );
 
 class BVHBase
 {
@@ -173,17 +177,12 @@ public:
 	// shim kept the pointer (BVHBase::verts, "we're not copying this data" :2055), the engine receives the new positions
 	void Refit( const uint32_t = 0 )
 	{
-		if (!vertsPtr) { fprintf( stderr, "Fatal error in tinybvh_b200 BVH::Refit: nothing was built from a host vertex array.\n" ); exit( 1 ); }
-		if (!vertIdx) TBVH_FATAL_IF( tbvh_refit( h, vertsPtr, vertsStride, vertsPrims, TBVH_HOST ), "BVH::Refit" );
-		else
-		{
-			// indexed geometry: resolve the indices on the host into the flat order the engine keeps
-			float* flat = (float*)malloc( (size_t)vertsPrims * 3 * 16 );
-			for (size_t i = 0; i < (size_t)vertsPrims * 3; i++) memcpy( flat + i * 4, (const char*)vertsPtr + (size_t)vertIdx[i] * vertsStride, vertsStride < 16 ? vertsStride : 16 );
-			const int rc = tbvh_refit( h, flat, 16, vertsPrims, TBVH_HOST );
-			free( flat );
-			TBVH_FATAL_IF( rc, "BVH::Refit" );
-		}
+		float* flat = 0;
+		uint32_t stride = 0;
+		const void* v = refit_verts( flat, stride, "BVH::Refit" );
+		const int rc = tbvh_refit( h, v, stride, vertsPrims, TBVH_HOST );
+		free( flat );
+		TBVH_FATAL_IF( rc, "BVH::Refit" );
 		sync_info();
 	}
 	// BVH::BuildHQ( const bvhvec4*, uint32_t ) tiny_bvh.h:2623 - SBVH (spatial splits), ends with Compact()
@@ -284,7 +283,20 @@ public:
 #endif
 private:
 	template <class T, class Vec4> friend void BuildBatch( T* const*, const Vec4* const*, const uint32_t*, uint32_t, int );
+	friend void RefitBatch( BVH* const*, uint32_t );
 	void batch_built( const void* v, uint32_t stride, uint32_t prims ) { remember( v, stride, 0, prims ), sync_info(); }
+	// the vertices a refit hands the engine: the caller's array, or - indexed geometry - its triangles resolved on the host into the
+	// flat order the engine keeps (into `flat`, which the caller frees)
+	const void* refit_verts( float*& flat, uint32_t& stride, const char* what ) const
+	{
+		if (!vertsPtr) { fprintf( stderr, "Fatal error in tinybvh_b200 %s: nothing was built from a host vertex array.\n", what ); exit( 1 ); }
+		stride = vertsStride;
+		if (!vertIdx) return vertsPtr;
+		flat = (float*)malloc( (size_t)vertsPrims * 3 * 16 );
+		for (size_t i = 0; i < (size_t)vertsPrims * 3; i++) memcpy( flat + i * 4, (const char*)vertsPtr + (size_t)vertIdx[i] * vertsStride, vertsStride < 16 ? vertsStride : 16 );
+		stride = 16;
+		return flat;
+	}
 	void remember( const void* v, uint32_t stride, const uint32_t* idx, uint32_t prims ) { vertsPtr = v, vertsStride = stride, vertIdx = idx, vertsPrims = prims; }
 	const void* vertsPtr = 0; const uint32_t* vertIdx = 0; // BVHBase::verts / vertIdx (:806-807): pointers to the caller's arrays, for Refit
 	uint32_t vertsStride = 16, vertsPrims = 0;
@@ -424,6 +436,24 @@ template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* cons
 	T::batch_convert( hs, count );
 	free( hs );
 	for (uint32_t k = 0; k < count; k++) objs[k]->batch_built( vertices[k], (uint32_t)sizeof( Vec4 ), primCounts[k] );
+}
+
+inline void RefitBatch( BVH* const* objs, uint32_t count )
+{
+	tbvh_bvh* hs = (tbvh_bvh*)malloc( sizeof( tbvh_bvh ) * (count ? count : 1) );
+	tbvh_mesh* ms = (tbvh_mesh*)calloc( count ? count : 1, sizeof( tbvh_mesh ) );
+	float** flat = (float**)calloc( count ? count : 1, sizeof( float* ) );
+	for (uint32_t k = 0; k < count; k++)
+	{
+		hs[k] = objs[k] ? objs[k]->handle() : 0;
+		if (!objs[k]) continue;
+		ms[k].verts = objs[k]->refit_verts( flat[k], ms[k].stride, "RefitBatch" ), ms[k].prim_count = objs[k]->vertsPrims;
+	}
+	const int rc = tbvh_refit_batch( hs, ms, count, TBVH_HOST, 0 );
+	for (uint32_t k = 0; k < count; k++) free( flat[k] );
+	free( flat ), free( ms ), free( hs );
+	TBVH_FATAL_IF( rc, "RefitBatch" );
+	for (uint32_t k = 0; k < count; k++) objs[k]->sync_info();
 }
 
 } // namespace tinybvh_b200

@@ -27,7 +27,7 @@ class Info(C.Structure):
 
 
 class Mesh(C.Structure):
-    """tbvh_mesh: one mesh of a tbvh_build_batch call"""
+    """tbvh_mesh: one mesh of a tbvh_build_batch or tbvh_refit_batch call"""
     _fields_ = [("verts", C.c_void_p), ("stride", C.c_uint32), ("vert_count", C.c_uint32), ("indices", C.c_void_p), ("prim_count", C.c_uint32)]
 
 
@@ -55,6 +55,7 @@ SYMBOLS = {
     "tbvh_build_tlas": (i32, [vp, vp, u32, u32, vp, u32, f32, f32]),
     "tbvh_refit": (i32, [vp, vp, u32, u32, i32]),
     "tbvh_refit_layouts": (i32, [vp, vp, u32, u32, i32]),
+    "tbvh_refit_batch": (i32, [vp, vp, u32, i32, i32]),
     "tbvh_build_indexed": (i32, [vp, vp, u32, u32, vp, u32, i32, f32, f32, i32]),
     "tbvh_build_batch": (i32, [vp, vp, u32, i32, f32, f32, i32]),
     "tbvh_upload_bvh": (i32, [vp, vp, u32, vp, u32, vp, u32, u32, i32]),

@@ -385,6 +385,33 @@ def convert_batch(objs):
     return objs
 
 
+def refit_batch(objs, meshes, keep_layouts=None):
+    """tbvh_refit_batch: every object refitted to its mesh's new vertices in one call.  `meshes`: numpy vertex arrays, or torch CUDA
+    tensors - one space per call, the same triangles each object was built from.  keep_layouts=None applies the rule of each object's
+    own Refit: BVH objects drop their derived layouts (tbvh_refit, keep_layouts=0), BVH_GPU and BVH8_CWBVH objects keep them up to date
+    (tbvh_refit_layouts, keep_layouts=1); objects of both kinds in one call need an explicit keep_layouts.  A refused call raises
+    TbvhError and leaves every object as it was."""
+    objs, meshes = list(objs), list(meshes)
+    if len(objs) != len(meshes):
+        raise TbvhError("refit_batch: one object per mesh")
+    if len({_is_torch(m) for m in meshes}) > 1:
+        raise TbvhError("refit_batch: host and device meshes in one call")
+    if keep_layouts is None:
+        rule = {b.layout != LAYOUT_BVH for b in objs}
+        if len(rule) > 1:
+            raise TbvhError("refit_batch: BVH objects drop their layouts, BVH_GPU / BVH8_CWBVH objects keep them: pass keep_layouts")
+        keep_layouts = rule.pop() if rule else False
+    recs = (_lib.Mesh * max(len(meshes), 1))()
+    keep, space = [], HOST
+    for r, m in zip(recs, meshes):
+        p, stride, nv, space, k = _verts_arg(m)
+        keep.append(k)
+        r.verts, r.stride, r.vert_count, r.indices, r.prim_count = p.value, stride, 0, None, nv // 3
+    hs = (C.c_void_p * max(len(objs), 1))(*[b.h for b in objs])
+    check(_lib.lib().tbvh_refit_batch(hs, recs, len(meshes), space, int(keep_layouts)))
+    return objs
+
+
 def pinned_empty(n: int, dtype, device: int = None, node: int = None) -> np.ndarray:
     """numpy array in page-locked host memory on the NUMA node of `device` (default: the current CUDA device): full-speed DMA
     for the host path (tbvh_host_alloc / tbvh_host_alloc_near)."""

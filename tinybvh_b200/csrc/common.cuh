@@ -67,6 +67,11 @@ struct tbvh_ctx_t
 	// streams never share one)
 	unsigned long long* d_counters = 0;
 	std::atomic<uint32_t> counter_next{ 0 };
+	// refits (convert_cwbvh.cu refit_trees): tables and scratch of one call, kept and grown, so a steady-state frame allocates nothing
+	std::mutex refit_mutex;
+	void* refit_dev = 0; size_t refit_dev_bytes = 0;   // device: tables, arrival counters, parents, BVH_GPU workspace, results
+	void* refit_host = 0; size_t refit_host_bytes = 0; // page-locked: the tables on their way in, the results on their way out
+	cudaEvent_t refit_e0 = 0, refit_e1 = 0;
 };
 #define TBVH_COUNTERS 256
 
@@ -217,6 +222,33 @@ __device__ __forceinline__ void dfs_rank( const float4* nodes, const uint32_t* p
 	}
 }
 
+// ---- batch tables: the entry of T[0 .. K) whose index range holds g (T[k].*F rises strictly: every entry owns an index)
+template <class E, uint32_t E::*F> __device__ __forceinline__ uint32_t batch_entry( const E* __restrict__ T, const uint32_t K, const uint32_t g )
+{
+	uint32_t lo = 0, hi = K;
+	while (hi - lo > 1) { const uint32_t m = (lo + hi) >> 1; if (T[m].*F <= g) lo = m; else hi = m; }
+	return lo;
+}
+
+// one tree of a refit (refit.cu, convert.cu): BVH::Refit over the batch's node space, the BVH2 traversal records over its primitive
+// reference space.  A single tree passes its entry as a kernel parameter instead of a table.
+struct RfTree
+{
+	float4* nodes;
+	const uint32_t* prim_idx;
+	const float4* verts;
+	float4* leaf_tris;
+	uint32_t* parent;             // the tree's parents by local node number: kept in its CwKeep, or scratch of the call
+	uint32_t nbase, used;         // first node in the batch's node space, BVH2 nodes
+	uint32_t pbase, idx_count;    // first primitive reference in the batch's reference space, references
+	uint32_t fill;                // parent is filled by this call
+};
+// one tree of a BVH_GPU::ConvertFrom pass (convert.cu): its BVH2, its output, and its first node in the pass's node space
+struct GpuTree { const float4* nodes; float4* out; uint32_t nbase, used; };
+// one wide tree of a traversal-node pass (trace_cwbvh.cu): its bvh8Data (src), its traversal nodes (dst), where its results go
+// (res[0]: range, res[1]: pending bound) and its first node in the pass's node index space (wbase)
+struct CwTrav { const uint4* src; uint4* dst; uint32_t* res; uint32_t wbase, count; };
+
 // ---- internal entry points (one per .cu) -------------------------------------------------------------------
 // d_stats: NULL, or two counters the launch ADDS its node visits / triangle tests to (the caller zeroes them once per API call)
 int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
@@ -229,8 +261,21 @@ unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte devi
 // binned-SAH builds of `trees` handles of one context at once (build_sah.cu); a single build is trees = 1
 int build_sah_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, int flavour );
 int build_hq_launch( tbvh_bvh b, float c_trav, float c_int );
-int refit_launch( tbvh_bvh b, cudaStream_t s );
-int refit_enqueue( tbvh_bvh b, cudaStream_t s, uint32_t* parent, uint32_t* arrive, bool fill_parent );
+// BVH::Refit of K trees over one node space of `nodes` nodes; arrive: `nodes` zeroed words; fill: some tree's parents are filled.
+// K = 1 runs the single-tree instances with `one`.
+int refit_enqueue( const RfTree* d_T, uint32_t K, const RfTree& one, uint32_t nodes, uint32_t* arrive, bool fill, cudaStream_t s );
+int refit_roots( const RfTree* d_T, uint32_t K, uint32_t* out, cudaStream_t s ); // each tree's root node (8 words) to out[8 t ..]
+// the leaf-ordered triangle records of K trees over one space of `refs` primitive references (convert.cu); K = 1 as above
+int leaf_tris_enqueue( const RfTree* d_T, uint32_t K, const RfTree& one, uint32_t refs, cudaStream_t s );
+int leaf_tris_alloc( tbvh_bvh b ); // d_leaf_tris sized to idx_count (kept when it is: a TLAS holding its address stays valid)
+// Refit of K handles of one context (tbvh_refit, tbvh_refit_layouts, tbvh_refit_batch): d_verts already hold the new positions.
+// keep_layouts: BVH_GPU and CWBVH brought up to date in place, the generation renewed; else both dropped.  One host synchronisation.
+// On failure every handle holds its BVH-layout tree (boxes unspecified) and neither BVH_GPU nor CWBVH.
+int refit_trees( const tbvh_bvh* bs, uint32_t K, bool keep_layouts, cudaStream_t s );
+void cw_keep_sizes( tbvh_bvh b, uint32_t* total, uint32_t* wide_count ); // split-tree and wide nodes of the kept collapse (0: none)
+// BVH_GPU::ConvertFrom of K trees over one node space of n nodes into their `out` arrays; w: 4 n words of workspace (zeroed here)
+int bvh_gpu_enqueue( const GpuTree* d_T, uint32_t K, const GpuTree& one, uint32_t n, uint32_t* w, cudaStream_t s );
+int cw_expand_batch( const CwTrav* d_T, uint32_t K, uint32_t W, cudaStream_t s ); // k_cw_expand of K trees (W nodes), no pending pass
 int tlas_trace_launch( tbvh_bvh b, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s );
 struct TlasInst { float inv[16]; uint32_t blasIdx, mask, pad0, pad1; };                                  // 80 bytes
 struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root_count; float cw_rd_limit; uint32_t pad1; const float4* cw_nodes; const float4* cw_tris; }; // 48 bytes: BVH-layout arrays, CWBVH traversal nodes + bvh8Tris (0 when absent) and their rD limit
@@ -240,7 +285,6 @@ int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s ); // sets the BVH_GPU bit on suc
 void drop_bvh_gpu( tbvh_bvh b );                  // the BVH_GPU array, its bit and used_nodes_gpu (no TLAS points at it: the generation stays)
 // BVH8_CWBVH::Build's conversion chain for K handles of one context at once (convert_cwbvh.cu); tbvh_convert is K = 1
 int bvh_to_cwbvh( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
-int cwbvh_refit( tbvh_bvh b, cudaStream_t s );  // tbvh_refit_layouts over b->cw_keep (convert_cwbvh.cu)
 // the CWBVH arrays, the kept collapse, the bit, the counts and the traversal limits; a TLAS over the arrays becomes stale
 void drop_cwbvh( tbvh_bvh b );
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)

@@ -12,23 +12,41 @@ uint32_t tbvh_next_generation()
 	return ++counter;
 }
 
-// one thread per primitive reference: 4 B index read + the record (common.cuh leaf_tri_record)
-__global__ void k_make_leaf_tris( const float4* __restrict__ verts, const uint32_t* __restrict__ prim_idx, float4* __restrict__ out, const uint32_t idx_count )
+// one thread per primitive reference: 4 B index read + the record (common.cuh leaf_tri_record).  BATCH: reference g of the batch's
+// reference space, in the tree that owns it (RfTree::pbase); else the one tree `one`
+template <bool BATCH>
+__global__ void k_make_leaf_tris( const RfTree* __restrict__ T, const uint32_t K, const RfTree one, const uint32_t n )
 {
-	const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-	if (p >= idx_count) return;
-	leaf_tri_record( verts, __ldg( prim_idx + p ), out, p );
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	const RfTree& tr = BATCH ? T[batch_entry<RfTree, &RfTree::pbase>( T, K, g )] : one;
+	const uint32_t p = BATCH ? g - tr.pbase : g;
+	leaf_tri_record( tr.verts, __ldg( tr.prim_idx + p ), tr.leaf_tris, p );
 }
 
-int make_leaf_tris( tbvh_bvh b, cudaStream_t s )
+int leaf_tris_enqueue( const RfTree* d_T, const uint32_t K, const RfTree& one, const uint32_t n, cudaStream_t s )
+{
+	if (K == 1) k_make_leaf_tris<false><<<(n + 255) / 256, 256, 0, s>>>( 0, 1, one, n );
+	else k_make_leaf_tris<true><<<(n + 255) / 256, 256, 0, s>>>( d_T, K, RfTree{}, n );
+	LAUNCHED();
+	return TBVH_OK;
+}
+
+int leaf_tris_alloc( tbvh_bvh b )
 {
 	const uint32_t n = b->info.idx_count;
 	// a refit keeps the array (same idx_count): a TLAS holding its address stays valid
 	if (b->d_leaf_tris && b->leaf_tris_count != n) { cudaFree( b->d_leaf_tris ); b->d_leaf_tris = 0; }
 	if (!b->d_leaf_tris) { CUDA_TRY( cudaMalloc( &b->d_leaf_tris, (size_t)n * 48 ) ); b->leaf_tris_count = n; b->generation = tbvh_next_generation(); }
-	k_make_leaf_tris<<<(n + 255) / 256, 256, 0, s>>>( b->d_verts, b->d_prim_idx, b->d_leaf_tris, n );
-	LAUNCHED();
 	return TBVH_OK;
+}
+
+int make_leaf_tris( tbvh_bvh b, cudaStream_t s )
+{
+	TRY( leaf_tris_alloc( b ) );
+	RfTree one = {};
+	one.prim_idx = b->d_prim_idx, one.verts = b->d_verts, one.leaf_tris = b->d_leaf_tris;
+	return leaf_tris_enqueue( 0, 1, one, b->info.idx_count, s );
 }
 
 // one thread per Aila-Laine node i; an interior node writes its children as the pair at slots 2i, 2i+1:
@@ -66,10 +84,26 @@ int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used, cudaStream_t s )
 //     pre(left) = pre(p) + 1,   pre(right) = pre(p) + 1 + size(left)
 // so it depends on the tree's shape alone: neither on the node numbering nor on the order of the leaf ranges in primIdx (a tree
 // after BVH::Optimize, or uploaded from elsewhere, has its leaf ranges out of DFS order).
-__global__ void k_gpu_parents( const float4* __restrict__ nodes, uint32_t* __restrict__ parent, const uint32_t used )
+// BATCH: node g of the pass's node space, in the tree that owns it (GpuTree::nbase); the workspace arrays are the batch's, tree t's
+// from nbase on, and hold local node numbers.  Else the one tree `one`.
+template <bool BATCH> __device__ __forceinline__ const GpuTree& gpu_tree( const GpuTree* __restrict__ T, const uint32_t K, const GpuTree& one, const uint32_t g, uint32_t& x )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= used || x == 1) return;
+	if (!BATCH) { x = g; return one; }
+	const GpuTree& tr = T[batch_entry<GpuTree, &GpuTree::nbase>( T, K, g )];
+	x = g - tr.nbase;
+	return tr;
+}
+
+template <bool BATCH>
+__global__ void k_gpu_parents( const GpuTree* __restrict__ T, const uint32_t K, const GpuTree one, uint32_t* __restrict__ parent, const uint32_t n )
+{
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	uint32_t x;
+	const GpuTree& tr = gpu_tree<BATCH>( T, K, one, g, x );
+	if (x == 1) return;
+	const float4* __restrict__ nodes = tr.nodes;
+	if (BATCH) parent += tr.nbase;
 	if (x == 0) parent[0] = 0xffffffffu;
 	if (__float_as_uint( nodes[(size_t)x * 2 + 1].w ) != 0) return;
 	const uint32_t c = __float_as_uint( nodes[(size_t)x * 2].w );
@@ -77,26 +111,39 @@ __global__ void k_gpu_parents( const float4* __restrict__ nodes, uint32_t* __res
 }
 
 // bottom-up from every leaf: interior nodes and leaves per subtree (every leaf weighs 1)
-__global__ void k_gpu_sizes( const float4* __restrict__ nodes, const uint32_t* __restrict__ parent, uint32_t* arrive, uint32_t* sub_int, uint32_t* sub_leaves,
-	const uint32_t used )
+template <bool BATCH>
+__global__ void k_gpu_sizes( const GpuTree* __restrict__ T, const uint32_t K, const GpuTree one, const uint32_t* __restrict__ parent, uint32_t* arrive,
+	uint32_t* sub_int, uint32_t* sub_leaves, const uint32_t n )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= used || x == 1) return;
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	uint32_t x;
+	const GpuTree& tr = gpu_tree<BATCH>( T, K, one, g, x );
+	if (x == 1) return;
+	const float4* __restrict__ nodes = tr.nodes;
 	if (__float_as_uint( nodes[(size_t)x * 2 + 1].w ) == 0) return; // leaves only
+	if (BATCH) parent += tr.nbase, arrive += tr.nbase, sub_int += tr.nbase, sub_leaves += tr.nbase;
 	dfs_sizes_up( nodes, parent, arrive, sub_int, sub_leaves, x, 1u );
 }
 
 // one thread per node: its preorder index from its path to the root; an interior node's left child follows it, its right child
 // follows the left subtree (sub_int + sub_leaves nodes)
-__global__ void k_gpu_emit( const float4* __restrict__ nodes, const uint32_t* __restrict__ parent, const uint32_t* __restrict__ sub_int,
-	const uint32_t* __restrict__ sub_leaves, float4* __restrict__ out, const uint32_t used )
+template <bool BATCH>
+__global__ void k_gpu_emit( const GpuTree* __restrict__ T, const uint32_t K, const GpuTree one, const uint32_t* __restrict__ parent, const uint32_t* __restrict__ sub_int,
+	const uint32_t* __restrict__ sub_leaves, const uint32_t n )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= used || x == 1) return;
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	uint32_t x;
+	const GpuTree& tr = gpu_tree<BATCH>( T, K, one, g, x );
+	if (x == 1) return;
+	const float4* __restrict__ nodes = tr.nodes;
+	float4* __restrict__ out = tr.out;
+	if (BATCH) parent += tr.nbase, sub_int += tr.nbase, sub_leaves += tr.nbase;
 	const float4 a = nodes[(size_t)x * 2], b = nodes[(size_t)x * 2 + 1];
-	uint32_t K, L, Kp;
-	dfs_rank( nodes, parent, sub_int, sub_leaves, x, K, L, Kp );
-	const uint32_t idx = K + L, cnt = __float_as_uint( b.w );
+	uint32_t Kx, L, Kp;
+	dfs_rank( nodes, parent, sub_int, sub_leaves, x, Kx, L, Kp );
+	const uint32_t idx = Kx + L, cnt = __float_as_uint( b.w );
 	const float4 z = make_float4( 0, 0, 0, 0 );
 	if (cnt)
 	{
@@ -111,6 +158,24 @@ __global__ void k_gpu_emit( const float4* __restrict__ nodes, const uint32_t* __
 	out[(size_t)idx * 4 + 1] = make_float4( l1.x, l1.y, l1.z, __uint_as_float( ridx ) );
 	out[(size_t)idx * 4 + 2] = make_float4( r0.x, r0.y, r0.z, __uint_as_float( 0u ) );
 	out[(size_t)idx * 4 + 3] = make_float4( r1.x, r1.y, r1.z, __uint_as_float( 0u ) );
+}
+
+int bvh_gpu_enqueue( const GpuTree* d_T, const uint32_t K, const GpuTree& one, const uint32_t n, uint32_t* w, cudaStream_t s )
+{
+	uint32_t* parent = w, * arrive = w + n, * sub_int = arrive + n, * sub_leaves = sub_int + n;
+	CUDA_TRY( cudaMemsetAsync( w, 0, (size_t)n * 16, s ) );
+	const uint32_t g = (n + 255) / 256;
+	if (K == 1)
+	{
+		k_gpu_parents<false><<<g, 256, 0, s>>>( 0, 1, one, parent, n ); LAUNCHED();
+		k_gpu_sizes<false><<<g, 256, 0, s>>>( 0, 1, one, parent, arrive, sub_int, sub_leaves, n ); LAUNCHED();
+		k_gpu_emit<false><<<g, 256, 0, s>>>( 0, 1, one, parent, sub_int, sub_leaves, n ); LAUNCHED();
+		return TBVH_OK;
+	}
+	k_gpu_parents<true><<<g, 256, 0, s>>>( d_T, K, GpuTree{}, parent, n ); LAUNCHED();
+	k_gpu_sizes<true><<<g, 256, 0, s>>>( d_T, K, GpuTree{}, parent, arrive, sub_int, sub_leaves, n ); LAUNCHED();
+	k_gpu_emit<true><<<g, 256, 0, s>>>( d_T, K, GpuTree{}, parent, sub_int, sub_leaves, n ); LAUNCHED();
+	return TBVH_OK;
 }
 
 void drop_bvh_gpu( tbvh_bvh b )
@@ -130,12 +195,7 @@ int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s )
 	{
 		CUDA_TRY( cudaMalloc( &b->d_nodes_gpu, (size_t)used * 64 ) );
 		CUDA_TRY( cudaMalloc( &w, words * 4 ) );
-		uint32_t* parent = w, * arrive = w + used, * sub_int = arrive + used, * sub_leaves = sub_int + used;
-		CUDA_TRY( cudaMemsetAsync( w, 0, words * 4, s ) );
-		const uint32_t g = (used + 255) / 256;
-		k_gpu_parents<<<g, 256, 0, s>>>( b->d_nodes, parent, used ); LAUNCHED();
-		k_gpu_sizes<<<g, 256, 0, s>>>( b->d_nodes, parent, arrive, sub_int, sub_leaves, used ); LAUNCHED();
-		k_gpu_emit<<<g, 256, 0, s>>>( b->d_nodes, parent, sub_int, sub_leaves, b->d_nodes_gpu, used ); LAUNCHED();
+		TRY( bvh_gpu_enqueue( 0, 1, GpuTree{ b->d_nodes, b->d_nodes_gpu, 0, used }, used, w, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
 	};

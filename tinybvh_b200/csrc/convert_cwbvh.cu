@@ -15,7 +15,7 @@
 // the reference's without walking the tree sequentially.  tests/test_convert_gpu.py compares bvh8Data / bvh8Tris bytes.
 //
 // On a refittable tree the collapse is kept (CwKeep), and tbvh_refit_layouts runs everything after it again over the refitted boxes
-// (cwbvh_refit): the result is BVH8_CWBVH::ConvertFrom of an MBVH<8> with the collapse of the conversion and the boxes of the
+// (refit_trees): the result is BVH8_CWBVH::ConvertFrom of an MBVH<8> with the collapse of the conversion and the boxes of the
 // refitted tree, which tests/cwbvh_refit_oracle.c restates.
 //
 // Batches (tbvh_convert_batch; a single conversion is K = 1).  K trees share one index space per stage: tree t owns BVH2 nodes
@@ -56,22 +56,18 @@ struct CwKeep
 	uint32_t* list = 0;                           // wide_count: split-tree node of every wide node
 	uint32_t* adopt = 0;                          // wide_count * 8: its children in ADOPTION order (k_assign breaks ties by it)
 	uint32_t* ifirst = 0;                         // wide_count: wide node of its first interior child; the others follow
-	// refit scratch: allocated by the first refit, kept until the CWBVH is dropped
+	// refit scratch: allocated by the first refit, alone or in a batch, and kept until the CWBVH is dropped
 	float4* ext = 0;                              // total * 2: the split tree with the refitted boxes
 	WideNode* wide = 0;                           // wide_count
-	uint32_t* parent = 0, * arrive = 0;           // used each: BVH::Refit's parents (topology only) and arrival counters
-	uint32_t* misc = 0;                           // 16 words: root box (8) + exponent range (1), read back together
-	cudaEvent_t e0 = 0, e1 = 0;
+	uint32_t* parent = 0;                         // used: BVH::Refit's parents (topology only), filled by the first refit
 };
 
 static void cw_keep_free( tbvh_bvh b )
 {
 	CwKeep* k = b->cw_keep;
 	if (!k) return;
-	void* p[] = { k->base, k->ext, k->wide, k->parent, k->arrive, k->misc }; // base also holds list, adopt and ifirst
+	void* p[] = { k->base, k->ext, k->wide, k->parent }; // base also holds list, adopt and ifirst
 	for (void* q : p) if (q) cudaFree( q );
-	if (k->e0) cudaEventDestroy( k->e0 );
-	if (k->e1) cudaEventDestroy( k->e1 );
 	delete k;
 	b->cw_keep = 0;
 }
@@ -89,6 +85,24 @@ struct CwTree
 	uint32_t ext_base;            // first split-tree node (k_tree_bases)
 	uint32_t wide_count;          // wide nodes
 };
+
+// one tree of a refit that keeps its CWBVH (refit_trees): its refitted BVH2, its kept collapse and refit scratch (CwKeep, tree-local
+// numbers), its outputs, and where it sits in the call's BVH2-node and wide-node spaces
+struct CwRefit
+{
+	const float4* nodes;
+	const uint32_t* base, * list, * ifirst;
+	uint32_t* adopt;
+	float4* ext;
+	WideNode* wide;
+	const uint32_t* prim_idx;
+	const float4* verts;
+	float4* cw_nodes, * cw_tris;
+	uint32_t nbase, used;         // first BVH2 node in the call's node space, BVH2 nodes
+	uint32_t wbase, leaf_root;    // first wide node in the call's wide-node space; the wide root wraps a leaf root
+};
+// a batch level is each tree's run of nodes on that level, in batch order: the level's nodes first .. are the tree's nodes lo ..
+struct CwRun { uint32_t first, tree, lo, pad; };
 
 // A tree owns at least two split-tree nodes before its chain nodes: a leaf root is wrapped into node 1 (wrap_leaf_root), which an
 // uploaded one-node tree does not have
@@ -157,11 +171,20 @@ __device__ __forceinline__ void split_emit( float4 a, const float4 b, const uint
 	ext[(size_t)cur * 2 + 1] = make_float4( b.x, b.y, b.z, __uint_as_float( c - (k - 1) * max_prims ) );
 }
 
-// one tree, with the tree's own scan (cwbvh_refit over CwKeep::base)
-__global__ void k_split_emit( const float4* __restrict__ nodes, const uint32_t* __restrict__ base, float4* __restrict__ ext, const uint32_t used, const uint32_t max_prims )
+// a refit: each tree with its own scan (CwKeep::base) into its own split tree.  BATCH: node g of the refit's node space, in the tree
+// of T that owns it; else the one tree of the arguments (n = its used)
+template <bool BATCH>
+__global__ void k_split_emit( const CwRefit* __restrict__ T, const uint32_t K, const float4* __restrict__ nodes, const uint32_t* __restrict__ base,
+	float4* __restrict__ ext, const uint32_t n, const uint32_t max_prims )
 {
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= used) return;
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	uint32_t x = g, used = n;
+	if (BATCH)
+	{
+		const CwRefit& tr = T[batch_entry<CwRefit, &CwRefit::nbase>( T, K, g )];
+		x = g - tr.nbase, used = tr.used, nodes = tr.nodes, base = tr.base, ext = tr.ext;
+	}
 	split_emit( nodes[(size_t)x * 2], nodes[(size_t)x * 2 + 1], x, 0, cw_seg( used ) + base[x], ext, max_prims );
 }
 
@@ -186,6 +209,12 @@ __device__ __forceinline__ void wrap_leaf_root( float4* ext, uint32_t* adopt, co
 	for (int i = 1; i < 8; i++) adopt[(size_t)w * 8 + i] = 0;
 }
 __global__ void k_wrap_leaf_root( float4* ext, uint32_t* adopt ) { wrap_leaf_root( ext, adopt, 0, 0 ); }
+// the leaf roots of a refit's trees, each into its tree's node 1
+__global__ void k_wrap_leaf_roots( const CwRefit* __restrict__ T, const uint32_t K )
+{
+	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t < K && T[t].leaf_root) wrap_leaf_root( T[t].ext, T[t].adopt, 0, 0 );
+}
 
 // ---- MBVH<8>::ConvertFrom collapse for one level of wide nodes (:5010-5033): wide nodes lo .. lo+num-1 of `list`; their interior
 // children are appended to `list` as the next level, each node's contiguously and in adoption order, the nodes in list order.  On
@@ -315,12 +344,21 @@ __global__ void k_keep( const CwTree* __restrict__ T, const uint32_t K, const ui
 	}
 }
 
-// ---- BVH8_CWBVH::ConvertFrom, greedy child -> slot assignment (:5910-5946) and per-node child statistics, one thread per wide node
-__global__ void k_assign( const float4* __restrict__ ext, const uint32_t* __restrict__ list, const uint32_t* __restrict__ adopt, const uint32_t* __restrict__ ifirst,
-	const uint32_t num, const uint32_t roots, WideNode* __restrict__ wide )
+// ---- BVH8_CWBVH::ConvertFrom, greedy child -> slot assignment (:5910-5946) and per-node child statistics, one thread per wide node.
+// BATCH (a refit of several kept collapses): wide node g of the refit's wide-node space, in the tree of T that owns it, whose own
+// arrays it works on with local numbers (its local node 0 is its root); else the arrays of the arguments
+template <bool BATCH>
+__global__ void k_assign( const CwRefit* __restrict__ T, const uint32_t K, const float4* __restrict__ ext, const uint32_t* __restrict__ list,
+	const uint32_t* __restrict__ adopt, const uint32_t* __restrict__ ifirst, const uint32_t num, uint32_t roots, WideNode* __restrict__ wide )
 {
-	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-	if (t >= num) return;
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= num) return;
+	uint32_t t = g;
+	if (BATCH)
+	{
+		const CwRefit& tr = T[batch_entry<CwRefit, &CwRefit::wbase>( T, K, g )];
+		t = g - tr.wbase, ext = tr.ext, list = tr.list, adopt = tr.adopt, ifirst = tr.ifirst, wide = tr.wide, roots = 1;
+	}
 	const uint32_t x = list[t];
 	WideNode w = {};
 	for (int i = 0; i < 8; i++) w.child[i] = adopt[(size_t)t * 8 + i];
@@ -376,12 +414,23 @@ __global__ void k_assign( const float4* __restrict__ ext, const uint32_t* __rest
 	wide[t] = w;
 }
 
+// wide node t of a level: lo + t of `wide`, or (BATCH) the node of the level's run that holds it, in its tree's own array
+template <bool BATCH> __device__ __forceinline__ uint32_t level_node( const CwRefit* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns,
+	const uint32_t lo, const uint32_t t, WideNode* __restrict__& wide )
+{
+	if (!BATCH) return lo + t;
+	const CwRun r = runs[batch_entry<CwRun, &CwRun::first>( runs, nruns, t )];
+	wide = T[r.tree].wide;
+	return r.lo + t - r.first;
+}
+
 // bottom-up: subtree node / triangle counts of wide nodes lo .. lo+num-1 (the next level's are final already)
-__global__ void k_sizes( const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
+template <bool BATCH>
+__global__ void k_sizes( const CwRefit* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= num) return;
-	const uint32_t x = lo + t;
+	const uint32_t x = level_node<BATCH>( T, runs, nruns, lo, t, wide );
 	uint32_t size = 1, tris = wide[x].leaf_tris;
 	for (int s = 0; s < 8; s++)
 	{
@@ -393,11 +442,13 @@ __global__ void k_sizes( const uint32_t lo, const uint32_t num, WideNode* __rest
 }
 
 // top-down: output addresses of the children of wide nodes lo .. lo+num-1 (see the header comment)
-__global__ void k_addresses( const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
+template <bool BATCH>
+__global__ void k_addresses( const CwRefit* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= num) return;
-	const WideNode w = wide[lo + t];
+	const uint32_t x = level_node<BATCH>( T, runs, nruns, lo, t, wide );
+	const WideNode w = wide[x];
 	uint32_t accS = 0, accT = 0, j = w.ichild;
 	for (int s = 7; s >= 0; s--)
 	{
@@ -420,18 +471,10 @@ __device__ __forceinline__ int quant_exponent( const float extent )
 	return (int)(int8_t)(v & 0xff);
 }
 
-// T: the batch's trees, wide node t belongs to tree wtree[t]; T = NULL: every node belongs to `one`
-__global__ void k_encode( const float4* __restrict__ ext, const uint32_t* __restrict__ list, const uint32_t num, const WideNode* __restrict__ wide,
-	const CwTree* __restrict__ T, const uint32_t* __restrict__ wtree, const CwTree one )
+// wide node w over split-tree node x: its 80-byte node at w.addr of out_nodes, its leaf children's triangles from w.tbase of out_tris
+__device__ __forceinline__ void encode_node( const float4* __restrict__ ext, const uint32_t x, const WideNode& w, const uint32_t* __restrict__ prim_idx,
+	const float4* __restrict__ verts, float4* __restrict__ out_nodes, float4* __restrict__ out_tris )
 {
-	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-	if (t >= num) return;
-	const CwTree& io = T ? T[wtree[t]] : one;
-	const uint32_t* __restrict__ prim_idx = io.prim_idx;
-	const float4* __restrict__ verts = io.verts;
-	float4* __restrict__ out_nodes = io.cw_nodes, * __restrict__ out_tris = io.cw_tris;
-	const uint32_t x = list[t];
-	const WideNode w = wide[t];
 	const float4 lo = ext[(size_t)x * 2], hi = ext[(size_t)x * 2 + 1];
 	const int ex = quant_exponent( __fsub_rn( hi.x, lo.x ) ), ey = quant_exponent( __fsub_rn( hi.y, lo.y ) ), ez = quant_exponent( __fsub_rn( hi.z, lo.z ) );
 	const float sx = ldexpf( 1.0f, ex ), sy = ldexpf( 1.0f, ey ), sz = ldexpf( 1.0f, ez ); // powf( 2, e ), exact
@@ -479,6 +522,26 @@ __global__ void k_encode( const float4* __restrict__ ext, const uint32_t* __rest
 	o[4] = make_float4( __uint_as_float( q[8] ), __uint_as_float( q[9] ), __uint_as_float( q[10] ), __uint_as_float( q[11] ) );
 }
 
+// T: the batch's trees, wide node t belongs to tree wtree[t]; T = NULL: every node belongs to `one`
+__global__ void k_encode( const float4* __restrict__ ext, const uint32_t* __restrict__ list, const uint32_t num, const WideNode* __restrict__ wide,
+	const CwTree* __restrict__ T, const uint32_t* __restrict__ wtree, const CwTree one )
+{
+	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= num) return;
+	const CwTree& io = T ? T[wtree[t]] : one;
+	encode_node( ext, list[t], wide[t], io.prim_idx, io.verts, io.cw_nodes, io.cw_tris );
+}
+
+// a refit of several kept collapses: wide node g of the refit's wide-node space, in its tree's own arrays
+__global__ void k_encode_trees( const CwRefit* __restrict__ T, const uint32_t K, const uint32_t num )
+{
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= num) return;
+	const CwRefit& tr = T[batch_entry<CwRefit, &CwRefit::wbase>( T, K, g )];
+	const uint32_t t = g - tr.wbase;
+	encode_node( tr.ext, tr.list[t], tr.wide[t], tr.prim_idx, tr.verts, tr.cw_nodes, tr.cw_tris );
+}
+
 
 // slot assignment, subtree sizes (bottom-up), addresses (top-down), encode: everything after the collapse that depends on boxes.
 // Wide nodes 0 .. roots-1 are roots; T / wtree / one as for k_encode.
@@ -486,16 +549,16 @@ static int cw_assign_encode( cudaStream_t s, const float4* ext, const uint32_t* 
 	const std::vector<uint32_t>& off, WideNode* wide, const uint32_t roots, const CwTree* T, const uint32_t* wtree, const CwTree& one )
 {
 	const uint32_t levels = (uint32_t)off.size() - 1, wide_count = off[levels];
-	k_assign<<<(wide_count + 127) / 128, 128, 0, s>>>( ext, list, adopt, ifirst, wide_count, roots, wide ); LAUNCHED();
+	k_assign<false><<<(wide_count + 127) / 128, 128, 0, s>>>( 0, 0, ext, list, adopt, ifirst, wide_count, roots, wide ); LAUNCHED();
 	for (int l = (int)levels - 1; l >= 0; l--)
 	{
 		const uint32_t num = off[l + 1] - off[l];
-		k_sizes<<<(num + 127) / 128, 128, 0, s>>>( off[l], num, wide ); LAUNCHED();
+		k_sizes<false><<<(num + 127) / 128, 128, 0, s>>>( 0, 0, 0, off[l], num, wide ); LAUNCHED();
 	}
 	for (uint32_t l = 0; l < levels; l++)
 	{
 		const uint32_t num = off[l + 1] - off[l];
-		k_addresses<<<(num + 127) / 128, 128, 0, s>>>( off[l], num, wide ); LAUNCHED();
+		k_addresses<false><<<(num + 127) / 128, 128, 0, s>>>( 0, 0, 0, off[l], num, wide ); LAUNCHED();
 	}
 	k_encode<<<(wide_count + 127) / 128, 128, 0, s>>>( ext, list, wide_count, wide, T, wtree, one ); LAUNCHED();
 	return TBVH_OK;
@@ -668,41 +731,181 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 	return rc;
 }
 
-// tbvh_refit_layouts on a handle that holds a CWBVH from tbvh_convert (b->cw_keep): d_verts already holds the new positions.
-// BVH::Refit, the BVH2 traversal records, then the conversion chain over the KEPT collapse with the refitted boxes - SplitLeafs(3)
-// boxes, leaf-root wrap, slot assignment, addresses, encode, traversal nodes - in place, with one synchronisation at the end.
-int cwbvh_refit( tbvh_bvh b, cudaStream_t s )
+
+void cw_keep_sizes( tbvh_bvh b, uint32_t* total, uint32_t* wide_count )
 {
-	CwKeep* k = b->cw_keep;
-	const bool first = !k->ext;
-	if (first)
+	const CwKeep* k = b->cw_keep;
+	*total = k ? k->total : 0, *wide_count = k ? k->wide_count : 0;
+}
+
+// ---- Refits (tbvh_refit / tbvh_refit_layouts are K = 1 of tbvh_refit_batch).  BVH::Refit over the K trees' node space, the BVH2
+// traversal records, then - keeping the layouts - the conversion chain over each KEPT collapse with the refitted boxes (SplitLeafs(3)
+// boxes, leaf-root wrap, slot assignment, addresses, encode, traversal nodes) and BVH_GPU::ConvertFrom, in place.  The result of a
+// tree is BVH8_CWBVH::ConvertFrom of an MBVH<8> with the collapse of its conversion and its refitted boxes, which
+// tests/cwbvh_refit_oracle.c restates.  The kept collapses are tree-local, so every kernel maps a node through its tree's table
+// entry; a batch level is each tree's run of the level, in batch order.  Tables and scratch come from the context's refit buffers:
+// one upload, one read-back, one host synchronisation.  A step that only one tree of the call takes runs the single-tree instances.
+static int refit_space( tbvh_ctx c, const size_t dev, const size_t host )
+{
+	if (dev > c->refit_dev_bytes)
 	{
-		CUDA_TRY( cudaMalloc( &k->ext, (size_t)k->total * 32 ) );
-		CUDA_TRY( cudaMalloc( &k->wide, (size_t)k->wide_count * sizeof( WideNode ) ) );
-		CUDA_TRY( cudaMalloc( &k->parent, (size_t)k->used * 4 ) );
-		CUDA_TRY( cudaMalloc( &k->arrive, (size_t)k->used * 4 ) );
-		CUDA_TRY( cudaMalloc( &k->misc, 64 ) );
-		CUDA_TRY( cudaEventCreate( &k->e0 ) );
-		CUDA_TRY( cudaEventCreate( &k->e1 ) );
+		if (c->refit_dev) cudaFree( c->refit_dev );
+		c->refit_dev = 0, c->refit_dev_bytes = 0;
+		CUDA_TRY( cudaMalloc( &c->refit_dev, dev + dev / 4 ) );
+		c->refit_dev_bytes = dev + dev / 4;
 	}
-	CUDA_TRY( cudaEventRecord( k->e0, s ) );
-	{ const int r = refit_enqueue( b, s, k->parent, k->arrive, first ); if (r != TBVH_OK) return r; }
-	{ const int r = make_leaf_tris( b, s ); if (r != TBVH_OK) return r; }
-	k_split_emit<<<(k->used + 255) / 256, 256, 0, s>>>( b->d_nodes, k->base, k->ext, k->used, 3 ); LAUNCHED();
-	if (k->leaf_root) { k_wrap_leaf_root<<<1, 1, 0, s>>>( k->ext, k->adopt ); LAUNCHED(); }
-	{ const int r = cw_assign_encode( s, k->ext, k->list, k->adopt, k->ifirst, k->off, k->wide, 1, 0, 0, CwTree{ 0, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris } ); if (r != TBVH_OK) return r; }
-	CUDA_TRY( cudaMemsetAsync( k->misc + 8, 0, 4, s ) );
-	{ const int r = cw_expand_launch( b, s, k->misc + 8 ); if (r != TBVH_OK) return r; }
-	CUDA_TRY( cudaEventRecord( k->e1, s ) );
-	CUDA_TRY( cudaMemcpyAsync( k->misc, b->d_nodes, 32, cudaMemcpyDeviceToDevice, s ) );
-	uint32_t h[9];
-	CUDA_TRY( cudaMemcpyAsync( h, k->misc, 36, cudaMemcpyDeviceToHost, s ) );
-	CUDA_TRY( cudaStreamSynchronize( s ) );
-	float ms = 0;
-	CUDA_TRY( cudaEventElapsedTime( &ms, k->e0, k->e1 ) );
-	b->info.build_ms = ms;
-	memcpy( b->info.aabb_min, h, 12 ), memcpy( b->info.aabb_max, h + 4, 12 );
-	// the exponents and origins moved: a stale limit could send rays with 2^e * rD past the float range down the integer path
-	b->cw_rd_limit = cw_rd_limit_for( h[8] );
+	if (host > c->refit_host_bytes)
+	{
+		if (c->refit_host) cudaFreeHost( c->refit_host );
+		c->refit_host = 0, c->refit_host_bytes = 0;
+		CUDA_TRY( cudaMallocHost( &c->refit_host, host + host / 4 ) );
+		c->refit_host_bytes = host + host / 4;
+	}
+	if (!c->refit_e0) CUDA_TRY( cudaEventCreate( &c->refit_e0 ) );
+	if (!c->refit_e1) CUDA_TRY( cudaEventCreate( &c->refit_e1 ) );
 	return TBVH_OK;
+}
+
+int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, cudaStream_t s )
+{
+	const tbvh_ctx c = bs[0]->ctx;
+	std::lock_guard<std::mutex> lock( c->refit_mutex );
+	// what each tree takes part in; the caller bounds the sums (TBVH_REFIT_BATCH_MAX_NODES)
+	std::vector<uint32_t> cw, gp;
+	uint32_t N = 0, P = 0, NC = 0, WC = 0, NG = 0, levels = 0;
+	for (uint32_t t = 0; t < K; t++)
+	{
+		const tbvh_bvh b = bs[t];
+		if (!keep_layouts) drop_bvh_gpu( b ), drop_cwbvh( b ); // derived layouts describe the old boxes (the reference converts again too)
+		else b->generation = tbvh_next_generation(); // the arrays stay, but a TLAS over this BLAS holds its old root box in its instances
+		const uint32_t used = b->info.used_nodes;
+		if (keep_layouts && b->cw_keep) cw.push_back( t ), NC += used, WC += b->cw_keep->wide_count, levels = std::max( levels, (uint32_t)b->cw_keep->off.size() - 1 );
+		if (keep_layouts && (b->info.layouts & (1u << TBVH_LAYOUT_BVH_GPU))) gp.push_back( t ), NG += used;
+		N += used, P += b->info.idx_count;
+	}
+	const uint32_t KC = (uint32_t)cw.size(), KG = (uint32_t)gp.size();
+	auto body = [&]() -> int
+	{
+		// arrays a tree gets on its first refit: a kept collapse's scratch, and parents that the first refit fills
+		for (uint32_t t = 0; t < K; t++) TRY( leaf_tris_alloc( bs[t] ) );
+		std::vector<bool> fill( K, true );
+		for (const uint32_t t : cw)
+		{
+			CwKeep* k = bs[t]->cw_keep;
+			fill[t] = !k->parent;
+			if (!k->ext) CUDA_TRY( cudaMalloc( &k->ext, (size_t)k->total * 32 ) );
+			if (!k->wide) CUDA_TRY( cudaMalloc( &k->wide, (size_t)k->wide_count * sizeof( WideNode ) ) );
+			if (!k->parent) CUDA_TRY( cudaMalloc( &k->parent, (size_t)k->used * 4 ) );
+		}
+		// the batch levels: each tree's run of every level it reaches
+		std::vector<CwRun> runs;
+		std::vector<uint32_t> rstart( (size_t)levels + 1, 0 ), rnum( levels, 0 );
+		if (KC > 1)
+			for (uint32_t l = 0; l < levels; l++)
+			{
+				rstart[l] = (uint32_t)runs.size();
+				for (uint32_t i = 0; i < KC; i++)
+				{
+					const CwKeep* k = bs[cw[i]]->cw_keep;
+					if (l + 1 < k->off.size()) runs.push_back( CwRun{ rnum[l], i, k->off[l], 0 } ), rnum[l] += k->off[l + 1] - k->off[l];
+				}
+			}
+		rstart[levels] = (uint32_t)runs.size();
+		// device: tables | arrival counters | results (root boxes, exponent ranges) | parents | BVH_GPU workspace;  host: tables | results
+		size_t carve = 0;
+		auto take = [&]( const size_t bytes ) { const size_t o = carve; carve += (bytes + 255) & ~(size_t)255; return o; };
+		const size_t o_rf = take( (size_t)K * sizeof( RfTree ) ), o_cr = take( (size_t)KC * sizeof( CwRefit ) ), o_runs = take( runs.size() * sizeof( CwRun ) );
+		const size_t o_ct = take( (size_t)KC * sizeof( CwTrav ) ), o_gt = take( (size_t)KG * sizeof( GpuTree ) ), tables = carve;
+		const size_t o_arrive = take( (size_t)N * 4 ), res_words = (size_t)K * 8 + KC, o_res = take( res_words * 4 ), zeroed = carve - o_arrive;
+		const size_t o_parent = take( (size_t)N * 4 ), o_gw = take( (size_t)NG * 16 );
+		TRY( refit_space( c, carve, tables + res_words * 4 ) );
+		char* const dev = (char*)c->refit_dev, * const host = (char*)c->refit_host;
+		uint32_t* const res = (uint32_t*)(dev + o_res), * const h_res = (uint32_t*)(host + tables);
+		RfTree* const rf = (RfTree*)(host + o_rf);
+		CwRefit* const cr = (CwRefit*)(host + o_cr);
+		CwTrav* const ct = (CwTrav*)(host + o_ct);
+		GpuTree* const gt = (GpuTree*)(host + o_gt);
+		bool any_fill = false;
+		for (uint32_t t = 0, nb = 0, pb = 0; t < K; t++)
+		{
+			const tbvh_bvh b = bs[t];
+			uint32_t* const parent = b->cw_keep ? b->cw_keep->parent : (uint32_t*)(dev + o_parent) + nb;
+			rf[t] = RfTree{ b->d_nodes, b->d_prim_idx, b->d_verts, b->d_leaf_tris, parent, nb, b->info.used_nodes, pb, b->info.idx_count, fill[t] ? 1u : 0u };
+			any_fill |= fill[t];
+			nb += b->info.used_nodes, pb += b->info.idx_count;
+		}
+		for (uint32_t i = 0, nb = 0, wb = 0; i < KC; i++)
+		{
+			const tbvh_bvh b = bs[cw[i]];
+			CwKeep* k = b->cw_keep;
+			cr[i] = CwRefit{ b->d_nodes, k->base, k->list, k->ifirst, k->adopt, k->ext, k->wide, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris, nb, k->used, wb, k->leaf_root ? 1u : 0u };
+			ct[i] = CwTrav{ (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, res + (size_t)K * 8 + i, wb, k->wide_count };
+			nb += k->used, wb += k->wide_count;
+		}
+		for (uint32_t i = 0, nb = 0; i < KG; i++)
+		{
+			const tbvh_bvh b = bs[gp[i]];
+			gt[i] = GpuTree{ b->d_nodes, b->d_nodes_gpu, nb, b->info.used_nodes };
+			nb += b->info.used_nodes;
+		}
+		if (!runs.empty()) memcpy( host + o_runs, runs.data(), runs.size() * sizeof( CwRun ) );
+		const RfTree* d_rf = (const RfTree*)(dev + o_rf);
+		const CwRefit* d_cr = (const CwRefit*)(dev + o_cr);
+		const CwRun* d_runs = (const CwRun*)(dev + o_runs);
+		CUDA_TRY( cudaMemcpyAsync( dev, host, tables, cudaMemcpyHostToDevice, s ) );
+		CUDA_TRY( cudaEventRecord( c->refit_e0, s ) );
+		CUDA_TRY( cudaMemsetAsync( dev + o_arrive, 0, zeroed, s ) );
+		TRY( refit_enqueue( d_rf, K, rf[0], N, (uint32_t*)(dev + o_arrive), any_fill, s ) );
+		TRY( leaf_tris_enqueue( d_rf, K, rf[0], P, s ) );
+		if (KC == 1)
+		{
+			const tbvh_bvh b = bs[cw[0]];
+			const CwKeep* k = b->cw_keep;
+			k_split_emit<false><<<(k->used + 255) / 256, 256, 0, s>>>( 0, 0, b->d_nodes, k->base, k->ext, k->used, 3 ); LAUNCHED();
+			if (k->leaf_root) { k_wrap_leaf_root<<<1, 1, 0, s>>>( k->ext, k->adopt ); LAUNCHED(); }
+			TRY( cw_assign_encode( s, k->ext, k->list, k->adopt, k->ifirst, k->off, k->wide, 1, 0, 0, CwTree{ 0, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris } ) );
+			TRY( cw_expand_launch( b, s, ct[0].res ) );
+		}
+		else if (KC > 1)
+		{
+			k_split_emit<true><<<(NC + 255) / 256, 256, 0, s>>>( d_cr, KC, 0, 0, 0, NC, 3 ); LAUNCHED();
+			bool any_leaf_root = false;
+			for (uint32_t i = 0; i < KC; i++) any_leaf_root |= cr[i].leaf_root != 0;
+			if (any_leaf_root) { k_wrap_leaf_roots<<<(KC + 127) / 128, 128, 0, s>>>( d_cr, KC ); LAUNCHED(); }
+			k_assign<true><<<(WC + 127) / 128, 128, 0, s>>>( d_cr, KC, 0, 0, 0, 0, WC, 1, 0 ); LAUNCHED();
+			for (int l = (int)levels - 1; l >= 0; l--)
+			{
+				k_sizes<true><<<(rnum[l] + 127) / 128, 128, 0, s>>>( d_cr, d_runs + rstart[l], rstart[l + 1] - rstart[l], 0, rnum[l], 0 ); LAUNCHED();
+			}
+			for (uint32_t l = 0; l < levels; l++)
+			{
+				k_addresses<true><<<(rnum[l] + 127) / 128, 128, 0, s>>>( d_cr, d_runs + rstart[l], rstart[l + 1] - rstart[l], 0, rnum[l], 0 ); LAUNCHED();
+			}
+			k_encode_trees<<<(WC + 127) / 128, 128, 0, s>>>( d_cr, KC, WC ); LAUNCHED();
+			TRY( cw_expand_batch( (const CwTrav*)(dev + o_ct), KC, WC, s ) );
+		}
+		if (KG) TRY( bvh_gpu_enqueue( (const GpuTree*)(dev + o_gt), KG, gt[0], NG, (uint32_t*)(dev + o_gw), s ) );
+		TRY( refit_roots( d_rf, K, res, s ) );
+		CUDA_TRY( cudaEventRecord( c->refit_e1, s ) );
+		CUDA_TRY( cudaMemcpyAsync( h_res, res, res_words * 4, cudaMemcpyDeviceToHost, s ) );
+		CUDA_TRY( cudaStreamSynchronize( s ) );
+		float ms = 0;
+		CUDA_TRY( cudaEventElapsedTime( &ms, c->refit_e0, c->refit_e1 ) );
+		for (uint32_t t = 0; t < K; t++)
+		{
+			tbvh_bvh b = bs[t];
+			b->info.build_ms = ms;
+			memcpy( b->info.aabb_min, h_res + (size_t)t * 8, 12 ), memcpy( b->info.aabb_max, h_res + (size_t)t * 8 + 4, 12 );
+		}
+		// the exponents and origins moved: a stale limit could send rays with 2^e * rD past the float range down the integer path
+		for (uint32_t i = 0; i < KC; i++) bs[cw[i]]->cw_rd_limit = cw_rd_limit_for( h_res[(size_t)K * 8 + i] );
+		return TBVH_OK;
+	};
+	const int rc = body();
+	if (rc != TBVH_OK)
+	{
+		cudaStreamSynchronize( s );
+		for (uint32_t t = 0; t < K; t++) drop_bvh_gpu( bs[t] ), drop_cwbvh( bs[t] );
+	}
+	return rc;
 }

@@ -6,6 +6,11 @@
 // interior node the second arrival (atomic counter) unions the two finished children and carries on, so every node is
 // written exactly once and only after both of its children.  Boxes are min / max of inputs, so the result is the
 // reference's byte for byte.  Node 1 stays untouched, as in the reference (`if (i != 1)`).
+//
+// Batches (tbvh_refit_batch; a single refit is K = 1): the K trees share one node index space, tree t owning nodes nbase .. nbase +
+// used of it, so one launch and one arrival-counter memset cover them all.  A thread finds its tree in a table (RfTree) and works
+// on the tree's own arrays with local node numbers; node 1 is skipped per tree.  K = 1 passes the tree as a kernel parameter.
+// The driver (refit_trees) is in convert_cwbvh.cu, next to the re-encode of the kept CWBVH collapse.
 #include "common.cuh"
 
 namespace
@@ -13,20 +18,35 @@ namespace
 __device__ __forceinline__ float tmin( const float a, const float b ) { return a < b ? a : b; }   // tinybvh_min :432
 __device__ __forceinline__ float tmax( const float a, const float b ) { return a > b ? a : b; }   // tinybvh_max :433
 
-__global__ void k_refit_parents( const float4* __restrict__ nodes, uint32_t* __restrict__ parent, const uint32_t used )
+// node g of the batch: its tree (BATCH) or `one`, and its local number
+template <bool BATCH> __device__ __forceinline__ const RfTree& rf_tree( const RfTree* __restrict__ T, const uint32_t K, const RfTree& one, const uint32_t g, uint32_t& x )
 {
-	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= used || i == 1) return;
+	if (!BATCH) { x = g; return one; }
+	const RfTree& tr = T[batch_entry<RfTree, &RfTree::nbase>( T, K, g )];
+	x = g - tr.nbase;
+	return tr;
+}
+
+template <bool BATCH>
+__global__ void k_refit_parents( const RfTree* __restrict__ T, const uint32_t K, const RfTree one, const uint32_t n )
+{
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	uint32_t i;
+	const RfTree& tr = rf_tree<BATCH>( T, K, one, g, i );
+	if (BATCH && !tr.fill) return;
+	if (i == 1) return;
+	const float4* __restrict__ nodes = tr.nodes;
+	uint32_t* __restrict__ parent = tr.parent;
 	if (i == 0) parent[0] = 0xffffffffu;
 	const float4 a = nodes[(size_t)i * 2], b = nodes[(size_t)i * 2 + 1];
 	if (__float_as_uint( b.w ) == 0) { const uint32_t l = __float_as_uint( a.w ); parent[l] = parent[l + 1] = i; }
 }
 
-__global__ void k_refit( float4* nodes, const uint32_t* __restrict__ prim_idx, const float4* __restrict__ verts, const uint32_t* __restrict__ parent,
-	uint32_t* arrive, const uint32_t used )
+// leaf x of one tree: its box, then the climb (arrive: the tree's counters)
+__device__ __forceinline__ void refit_leaf( float4* nodes, const uint32_t* __restrict__ prim_idx, const float4* __restrict__ verts, const uint32_t* __restrict__ parent,
+	uint32_t* arrive, uint32_t x )
 {
-	uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= used || x == 1) return;
 	const float4 a = nodes[(size_t)x * 2], b = nodes[(size_t)x * 2 + 1];
 	const uint32_t first = __float_as_uint( a.w ), count = __float_as_uint( b.w );
 	if (count == 0) return; // interior nodes are written by whichever child arrives second
@@ -56,47 +76,52 @@ __global__ void k_refit( float4* nodes, const uint32_t* __restrict__ prim_idx, c
 		x = p;
 	}
 }
+
+__global__ void k_refit( float4* nodes, const uint32_t* __restrict__ prim_idx, const float4* __restrict__ verts, const uint32_t* __restrict__ parent,
+	uint32_t* arrive, const uint32_t used )
+{
+	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+	if (x >= used || x == 1) return;
+	refit_leaf( nodes, prim_idx, verts, parent, arrive, x );
+}
+
+// node g of the batch's node space, in the tree that owns it; arrive: the batch's counters, tree t's from nbase on.  A single tree
+// runs k_refit: its pointers read from a table entry cost it registers.
+__global__ void k_refit_batch( const RfTree* __restrict__ T, const uint32_t K, uint32_t* arrive, const uint32_t n )
+{
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	const RfTree& tr = T[batch_entry<RfTree, &RfTree::nbase>( T, K, g )];
+	const uint32_t x = g - tr.nbase;
+	if (x != 1) refit_leaf( tr.nodes, tr.prim_idx, tr.verts, tr.parent, arrive + tr.nbase, x );
+}
+
+// the root node of every tree (its box is the handle's aabb), read back with the call's other results
+__global__ void k_refit_roots( const RfTree* __restrict__ T, const uint32_t K, uint4* __restrict__ out )
+{
+	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= K) return;
+	const uint4* r = (const uint4*)T[t].nodes;
+	out[(size_t)t * 2] = r[0], out[(size_t)t * 2 + 1] = r[1];
+}
 } // namespace
 
-// enqueue BVH::Refit on s (d_verts already holds the new positions).  parent / arrive: `used` words each; parent depends on the
-// topology only, so it is filled only when fill_parent (a caller may keep it between refits)
-int refit_enqueue( tbvh_bvh b, cudaStream_t s, uint32_t* parent, uint32_t* arrive, bool fill_parent )
+int refit_enqueue( const RfTree* d_T, const uint32_t K, const RfTree& one, const uint32_t n, uint32_t* arrive, const bool fill, cudaStream_t s )
 {
-	const uint32_t used = b->info.used_nodes;
-	CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)used * 4, s ) );
-	if (fill_parent) { k_refit_parents<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes, parent, used ); LAUNCHED(); }
-	k_refit<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes, b->d_prim_idx, b->d_verts, parent, arrive, used ); LAUNCHED();
+	const uint32_t g = (n + 255) / 256;
+	if (K == 1)
+	{
+		if (fill) { k_refit_parents<false><<<g, 256, 0, s>>>( 0, 1, one, n ); LAUNCHED(); }
+		k_refit<<<g, 256, 0, s>>>( one.nodes, one.prim_idx, one.verts, one.parent, arrive, n ); LAUNCHED();
+		return TBVH_OK;
+	}
+	if (fill) { k_refit_parents<true><<<g, 256, 0, s>>>( d_T, K, RfTree{}, n ); LAUNCHED(); }
+	k_refit_batch<<<g, 256, 0, s>>>( d_T, K, arrive, n ); LAUNCHED();
 	return TBVH_OK;
 }
 
-// d_verts already holds the new positions
-int refit_launch( tbvh_bvh b, cudaStream_t s )
+int refit_roots( const RfTree* d_T, const uint32_t K, uint32_t* out, cudaStream_t s )
 {
-	const uint32_t used = b->info.used_nodes;
-	uint32_t* d_parent = 0; uint32_t* d_arrive = 0;
-	cudaEvent_t e0 = 0, e1 = 0;
-	auto body = [&]() -> int
-	{
-		CUDA_TRY( cudaMalloc( &d_parent, (size_t)used * 4 ) );
-		CUDA_TRY( cudaMalloc( &d_arrive, (size_t)used * 4 ) );
-		CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) );
-		CUDA_TRY( cudaEventRecord( e0, s ) );
-		{ const int r = refit_enqueue( b, s, d_parent, d_arrive, true ); if (r != TBVH_OK) return r; }
-		CUDA_TRY( cudaEventRecord( e1, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		float ms = 0;
-		CUDA_TRY( cudaEventElapsedTime( &ms, e0, e1 ) );
-		b->info.build_ms = ms;
-		uint32_t rootw[8];
-		CUDA_TRY( cudaMemcpy( rootw, b->d_nodes, 32, cudaMemcpyDeviceToHost ) );
-		memcpy( b->info.aabb_min, rootw, 12 ), memcpy( b->info.aabb_max, rootw + 4, 12 );
-		return TBVH_OK;
-	};
-	const int rc = body();
-	cudaStreamSynchronize( s );
-	if (d_parent) cudaFree( d_parent );
-	if (d_arrive) cudaFree( d_arrive );
-	if (e0) cudaEventDestroy( e0 );
-	if (e1) cudaEventDestroy( e1 );
-	return rc;
+	k_refit_roots<<<(K + 127) / 128, 128, 0, s>>>( d_T, K, (uint4*)out ); LAUNCHED();
+	return TBVH_OK;
 }

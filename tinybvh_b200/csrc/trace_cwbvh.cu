@@ -39,9 +39,7 @@
 // ---- bvh8Data -> traversal nodes ------------------------------------------------------------------------------------
 // One thread per node.  Slot i of the source node: meta byte i (n1.z / n1.w), quantised bounds byte i of the six 8-byte rows at
 // bytes 32..79 (lo.x, lo.y, lo.z, hi.x, hi.y, hi.z) - layout in SURVEY.md 8(a), written by BVH8_CWBVH::ConvertFrom (tiny_bvh.h:5948-6015).
-// One wide tree of a pass: its bvh8Data (src), its traversal nodes (dst), where its results go (res[0]: range, res[1]: pending
-// bound) and its first node in the pass's node index space (wbase).  A batch passes a device table of them, one tree `one`.
-struct CwTrav { const uint4* src; uint4* dst; uint32_t* res; uint32_t wbase, count; };
+// One wide tree of a pass is a CwTrav (common.cuh).  A batch passes a device table of them, one tree `one`.
 
 // the tree that holds node g of a pass (wbase rises strictly: every tree has a node)
 __device__ __forceinline__ uint32_t trav_tree( const CwTrav* __restrict__ T, const uint32_t K, const uint32_t g )
@@ -163,6 +161,13 @@ int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range )
 	const uint32_t count = b->info.used_blocks / 5;
 	const CwTrav one = { (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_range, 0, count };
 	k_cw_expand<false><<<(count + 127) / 128, 128, 0, s>>>( 0, 1, one, count, 0 ); LAUNCHED();
+	return TBVH_OK;
+}
+
+// the nodes of K trees at once, over a device table: a refit re-encodes them in place, so the pending bound stays (parent = NULL)
+int cw_expand_batch( const CwTrav* d_T, const uint32_t K, const uint32_t W, cudaStream_t s )
+{
+	k_cw_expand<true><<<(W + 127) / 128, 128, 0, s>>>( d_T, K, CwTrav{}, W, 0 ); LAUNCHED();
 	return TBVH_OK;
 }
 
