@@ -255,7 +255,9 @@ int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_
 int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
 // traversal nodes, cw_rd_limit and cw_pending of the CWBVH of each of bs[0 .. K), in one pass (trace_cwbvh.cu); synchronises s
 int cw_make_trav( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
-int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range ); // cw_make_trav's node expansion into the existing d_cw_trav
+// cw_make_trav's node expansion of the W nodes of K trees (table d_T; K = 1: `one`) into their d_cw_trav; parent: NULL (a refit)
+// or where the pending pass finds the parents
+int cw_expand( const CwTrav* d_T, uint32_t K, const CwTrav& one, uint32_t W, uint32_t* parent, cudaStream_t s );
 float cw_rd_limit_for( uint32_t range );                               // cw_rd_limit of a tree whose expansion found `range`
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)
 // binned-SAH builds of `trees` handles of one context at once (build_sah.cu); a single build is trees = 1
@@ -275,7 +277,6 @@ int refit_trees( const tbvh_bvh* bs, uint32_t K, bool keep_layouts, cudaStream_t
 void cw_keep_sizes( tbvh_bvh b, uint32_t* total, uint32_t* wide_count ); // split-tree and wide nodes of the kept collapse (0: none)
 // BVH_GPU::ConvertFrom of K trees over one node space of n nodes into their `out` arrays; w: 4 n words of workspace (zeroed here)
 int bvh_gpu_enqueue( const GpuTree* d_T, uint32_t K, const GpuTree& one, uint32_t n, uint32_t* w, cudaStream_t s );
-int cw_expand_batch( const CwTrav* d_T, uint32_t K, uint32_t W, cudaStream_t s ); // k_cw_expand of K trees (W nodes), no pending pass
 int tlas_trace_launch( tbvh_bvh b, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s );
 struct TlasInst { float inv[16]; uint32_t blasIdx, mask, pad0, pad1; };                                  // 80 bytes
 struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root_count; float cw_rd_limit; uint32_t pad1; const float4* cw_nodes; const float4* cw_tris; }; // 48 bytes: BVH-layout arrays, CWBVH traversal nodes + bvh8Tris (0 when absent) and their rD limit

@@ -18,12 +18,14 @@
 // (refit_trees): the result is BVH8_CWBVH::ConvertFrom of an MBVH<8> with the collapse of the conversion and the boxes of the
 // refitted tree, which tests/cwbvh_refit_oracle.c restates.
 //
-// Batches (tbvh_convert_batch; a single conversion is K = 1).  K trees share one index space per stage: tree t owns BVH2 nodes
-// nbase[t] .. nbase[t+1] of the SplitLeafs scan and split-tree nodes ext_base[t] .. ext_base[t+1] of one `ext` array, whose child
-// links are global.  Level 0 of the collapse holds the K roots; a level places every node's interior children by a scan over the
-// level in list order, so each level is grouped by tree in batch order and the lists are deterministic.  Every root gets address 0,
-// so addresses below it are local to its tree; the encode writes through a table of per-tree outputs (CwTree).  The fixed costs -
-// allocations, launches and host round trips - grow with the deepest tree's level count, not with K.
+// Batches (tbvh_convert_batch; a single conversion is K = 1).  Up to the collapse, K trees share one index space per stage: tree t
+// owns BVH2 nodes nbase[t] .. nbase[t+1] of the SplitLeafs scan and split-tree nodes ext_base[t] .. ext_base[t+1] of one `ext`
+// array, whose child links are global.  Level 0 of the collapse holds the K roots; a level places every node's interior children by
+// a scan over the level in list order, so each level is grouped by tree in batch order and the lists are deterministic.
+// Everything after the collapse is one per-tree pipeline, shared with the refit: k_keep makes every tree's collapse tree-local, and
+// cw_assign_encode runs over a table of trees (CwTree) and each tree's runs of the levels (CwRun).  A single tree is its own forest
+// and runs the single-tree instances over its own arrays.  The fixed costs - allocations, launches and host round trips - grow with
+// the deepest tree's level count, not with K.
 #include "common.cuh"
 #include <algorithm>
 #include <new>
@@ -72,49 +74,31 @@ static void cw_keep_free( tbvh_bvh b )
 	b->cw_keep = 0;
 }
 
-// one tree of a conversion: its BVH2, its outputs, and where it sits in the batch's index spaces (device table, indexed by tree)
+// One tree of a conversion or of a refit that keeps its CWBVH (device table, indexed by tree; a step that only one tree takes gets
+// the entry as a kernel parameter instead).  Everything after the collapse works on the tree's own arrays with tree-local numbers.
 struct CwTree
 {
-	const float4* nodes;          // BVH2 nodes (d_nodes)
-	const uint32_t* prim_idx;     // the tree's own primIdx
+	const float4* nodes;                // BVH2 nodes (d_nodes)
+	const uint32_t* prim_idx;           // the tree's own primIdx
 	const float4* verts;
-	float4* cw_nodes, * cw_tris;  // bvh8Data / bvh8Tris of the handle
-	uint32_t* keep;               // refittable: the handle's CwKeep block (base | list | adopt | ifirst), else NULL
-	uint32_t nbase, used;         // first BVH2 node in the batch's node index space, BVH2 nodes
-	uint32_t seg;                 // nodes the tree owns before its chain nodes: cw_seg( used )
-	uint32_t ext_base;            // first split-tree node (k_tree_bases)
-	uint32_t wide_count;          // wide nodes
-};
-
-// one tree of a refit that keeps its CWBVH (refit_trees): its refitted BVH2, its kept collapse and refit scratch (CwKeep, tree-local
-// numbers), its outputs, and where it sits in the call's BVH2-node and wide-node spaces
-struct CwRefit
-{
-	const float4* nodes;
-	const uint32_t* base, * list, * ifirst;
-	uint32_t* adopt;
-	float4* ext;
+	float4* cw_nodes, * cw_tris;        // bvh8Data / bvh8Tris of the handle
+	float4* ext;                        // its split tree, from its node 0
+	const uint32_t* scan;               // its SplitLeafs scan, from its node 0: node x's chain pairs follow scan[x] - scan[0] others
+	uint32_t* list, * adopt, * ifirst;  // its collapse (CwKeep)
 	WideNode* wide;
-	const uint32_t* prim_idx;
-	const float4* verts;
-	float4* cw_nodes, * cw_tris;
-	uint32_t nbase, used;         // first BVH2 node in the call's node space, BVH2 nodes
-	uint32_t wbase, leaf_root;    // first wide node in the call's wide-node space; the wide root wraps a leaf root
+	uint32_t* keep;                     // a conversion's k_keep writes the tree-local collapse here (base | list | adopt | ifirst), else NULL
+	uint32_t shift;                     // added to every child link ext stores: the tree's first node in a conversion's forest (ext_base)
+	uint32_t nbase, used;               // first BVH2 node in the call's node space, BVH2 nodes
+	uint32_t wbase, wide_count;         // first wide node in the call's wide-node space (tree by tree), wide nodes
+	uint32_t leaf_root;                 // the wide root wraps a leaf root
 };
-// a batch level is each tree's run of nodes on that level, in batch order: the level's nodes first .. are the tree's nodes lo ..
+// a batch level is each tree's run of nodes on that level, in batch order: the call's wide nodes first .. (level order) are the
+// tree's nodes lo ..
 struct CwRun { uint32_t first, tree, lo, pad; };
 
 // A tree owns at least two split-tree nodes before its chain nodes: a leaf root is wrapped into node 1 (wrap_leaf_root), which an
 // uploaded one-node tree does not have
 __host__ __device__ __forceinline__ uint32_t cw_seg( const uint32_t used ) { return used < 2 ? 2 : used; }
-
-// the tree that holds BVH2 node g of the batch (nbase rises strictly: every tree has a node)
-__device__ __forceinline__ uint32_t tree_of_node( const CwTree* __restrict__ T, const uint32_t K, const uint32_t g )
-{
-	uint32_t lo = 0, hi = K;
-	while (hi - lo > 1) { const uint32_t m = (lo + hi) >> 1; if (T[m].nbase <= g) lo = m; else hi = m; }
-	return lo;
-}
 
 // BVH::SA (tiny_bvh.h:8477) in the oracle's pairing
 __device__ __forceinline__ float node_sa( const float4 mn, const float4 mx )
@@ -129,28 +113,28 @@ __global__ void k_split_count( const CwTree* __restrict__ T, const uint32_t K, c
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
-	const CwTree& tr = T[tree_of_node( T, K, g )];
+	const CwTree& tr = T[batch_entry<CwTree, &CwTree::nbase>( T, K, g )];
 	const uint32_t x = g - tr.nbase;
 	const uint32_t c = x == 1 || x >= tr.used ? 0 : __float_as_uint( tr.nodes[(size_t)x * 2 + 1].w );
 	extra[g] = c > max_prims ? 2 * ((c + max_prims - 1) / max_prims - 1) : 0;
 }
 
 // first split-tree node of every tree, from the scan of k_split_count: the nodes and chain nodes of the trees before it
-__global__ void k_tree_bases( CwTree* __restrict__ T, const uint32_t K, const uint32_t* __restrict__ base, uint32_t* __restrict__ ext_base )
+__global__ void k_tree_bases( const CwTree* __restrict__ T, const uint32_t K, const uint32_t* __restrict__ base, uint32_t* __restrict__ ext_base )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= K) return;
-	const uint32_t nb = T[t].nbase;
-	T[t].ext_base = ext_base[t] = nb + base[nb];
-	if (t == K - 1) ext_base[K] = nb + T[t].seg + base[nb + T[t].seg];
+	const uint32_t nb = T[t].nbase, seg = cw_seg( T[t].used );
+	ext_base[t] = nb + base[nb];
+	if (t == K - 1) ext_base[K] = nb + seg + base[nb + seg];
 }
 
-// BVH2 node x (a, b) as split-tree node x + shift: a link to its children moves with it, and a long leaf's chain goes to the pairs
-// from `pair` on
+// BVH2 node x (a, b) as node x of the tree's split tree: a link to its children carries `shift`, and a long leaf's chain goes to the
+// pairs from `pair` on
 __device__ __forceinline__ void split_emit( float4 a, const float4 b, const uint32_t x, const uint32_t shift, uint32_t pair, float4* __restrict__ ext, const uint32_t max_prims )
 {
 	const uint32_t c = x == 1 ? 0 : __float_as_uint( b.w ), first = __float_as_uint( a.w );
-	uint32_t cur = x + shift;
+	uint32_t cur = x;
 	if (c <= max_prims)
 	{
 		if (__float_as_uint( b.w ) == 0) a.w = __uint_as_float( first + shift );
@@ -161,7 +145,7 @@ __device__ __forceinline__ void split_emit( float4 a, const float4 b, const uint
 	for (uint32_t j = 0; j + 1 < k; j++, pair += 2)
 	{
 		// `cur` becomes interior over (leaf of max_prims, rest)
-		ext[(size_t)cur * 2] = make_float4( a.x, a.y, a.z, __uint_as_float( pair ) );
+		ext[(size_t)cur * 2] = make_float4( a.x, a.y, a.z, __uint_as_float( pair + shift ) );
 		ext[(size_t)cur * 2 + 1] = make_float4( b.x, b.y, b.z, __uint_as_float( 0u ) );
 		ext[(size_t)pair * 2] = make_float4( a.x, a.y, a.z, __uint_as_float( first + j * max_prims ) );
 		ext[(size_t)pair * 2 + 1] = make_float4( b.x, b.y, b.z, __uint_as_float( max_prims ) );
@@ -171,32 +155,25 @@ __device__ __forceinline__ void split_emit( float4 a, const float4 b, const uint
 	ext[(size_t)cur * 2 + 1] = make_float4( b.x, b.y, b.z, __uint_as_float( c - (k - 1) * max_prims ) );
 }
 
-// a refit: each tree with its own scan (CwKeep::base) into its own split tree.  BATCH: node g of the refit's node space, in the tree
-// of T that owns it; else the one tree of the arguments (n = its used)
+// Every tree's chains follow its own nodes.  A conversion's forest (shift = ext_base, the batch scan from nbase) keeps global child
+// links for k_collapse; a refit's kept split tree (shift = 0, CwKeep::base) is local.  BATCH: node g of the call's node space, in the
+// tree of T that owns it; else node g of `one` (n = its used)
 template <bool BATCH>
-__global__ void k_split_emit( const CwRefit* __restrict__ T, const uint32_t K, const float4* __restrict__ nodes, const uint32_t* __restrict__ base,
-	float4* __restrict__ ext, const uint32_t n, const uint32_t max_prims )
+__global__ void k_split_emit( const CwTree* __restrict__ T, const uint32_t K, const CwTree one, const uint32_t n, const uint32_t max_prims )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
-	uint32_t x = g, used = n;
-	if (BATCH)
-	{
-		const CwRefit& tr = T[batch_entry<CwRefit, &CwRefit::nbase>( T, K, g )];
-		x = g - tr.nbase, used = tr.used, nodes = tr.nodes, base = tr.base, ext = tr.ext;
-	}
-	split_emit( nodes[(size_t)x * 2], nodes[(size_t)x * 2 + 1], x, 0, cw_seg( used ) + base[x], ext, max_prims );
+	const CwTree& tr = BATCH ? T[batch_entry<CwTree, &CwTree::nbase>( T, K, g )] : one;
+	const uint32_t x = BATCH ? g - tr.nbase : g;
+	if (BATCH && x >= tr.used) return; // node 1 of a one-node tree in a conversion: only a leaf-root wrap writes it
+	split_emit( tr.nodes[(size_t)x * 2], tr.nodes[(size_t)x * 2 + 1], x, tr.shift, cw_seg( tr.used ) + tr.scan[x] - tr.scan[0], tr.ext, max_prims );
 }
-
-// every tree of a batch: tree t's chains follow its own nodes, at ext_base + seg + (base[g] - base[nbase]) = nbase + seg + base[g]
-__global__ void k_split_emit_batch( const CwTree* __restrict__ T, const uint32_t K, const uint32_t n, const uint32_t* __restrict__ base, float4* __restrict__ ext, const uint32_t max_prims )
+static int cw_split_emit( const CwTree* d_T, const uint32_t K, const CwTree& one, const uint32_t n, cudaStream_t s )
 {
-	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-	if (g >= n) return;
-	const CwTree& tr = T[tree_of_node( T, K, g )];
-	const uint32_t x = g - tr.nbase;
-	if (x >= tr.used) return; // node 1 of a one-node tree: only a leaf-root wrap writes it
-	split_emit( tr.nodes[(size_t)x * 2], tr.nodes[(size_t)x * 2 + 1], x, tr.ext_base, tr.nbase + tr.seg + base[g], ext, max_prims );
+	if (K > 1) k_split_emit<true><<<(n + 255) / 256, 256, 0, s>>>( d_T, K, CwTree{}, n, 3 );
+	else k_split_emit<false><<<(one.used + 255) / 256, 256, 0, s>>>( 0, 1, one, one.used, 3 );
+	LAUNCHED();
+	return TBVH_OK;
 }
 
 // MBVH<8>::ConvertFrom :5036-5044: a leaf root x is copied to node x + 1 (its tree's unused node 1), and x becomes a one-child
@@ -208,9 +185,8 @@ __device__ __forceinline__ void wrap_leaf_root( float4* ext, uint32_t* adopt, co
 	adopt[(size_t)w * 8] = x + 1;
 	for (int i = 1; i < 8; i++) adopt[(size_t)w * 8 + i] = 0;
 }
-__global__ void k_wrap_leaf_root( float4* ext, uint32_t* adopt ) { wrap_leaf_root( ext, adopt, 0, 0 ); }
 // the leaf roots of a refit's trees, each into its tree's node 1
-__global__ void k_wrap_leaf_roots( const CwRefit* __restrict__ T, const uint32_t K )
+__global__ void k_wrap_leaf_roots( const CwTree* __restrict__ T, const uint32_t K )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t < K && T[t].leaf_root) wrap_leaf_root( T[t].ext, T[t].adopt, 0, 0 );
@@ -303,41 +279,33 @@ __global__ void __launch_bounds__( CW_LEVEL_T ) k_collapse( float4* __restrict__
 	}
 }
 
-// the run of one tree's wide nodes that holds wide node w: runs are sorted by their first node (gfirst) and tile every level
-__device__ __forceinline__ uint32_t run_of( const uint32_t* __restrict__ gfirst, const uint32_t G, const uint32_t w )
-{
-	uint32_t lo = 0, hi = G;
-	while (hi - lo > 1) { const uint32_t m = (lo + hi) >> 1; if (gfirst[m] <= w) lo = m; else hi = m; }
-	return lo;
-}
-
-// the collapse of every refittable tree into its handle's CwKeep block, local to the tree: wide node w of run g is the tree's node
-// w - gfirst[g] + glocal[g], split-tree nodes lose ext_base, and the SplitLeafs scan starts at 0.  Threads 0 .. W-1 take the wide
-// nodes, W .. W+N-1 the BVH2 nodes.
-__global__ void k_keep( const CwTree* __restrict__ T, const uint32_t K, const uint32_t* __restrict__ wtree, const uint32_t* __restrict__ gfirst,
-	const uint32_t* __restrict__ glocal, const uint32_t G, const uint32_t W, const uint32_t* __restrict__ list, const uint32_t* __restrict__ adopt,
-	const uint32_t* __restrict__ ifirst, const uint32_t* __restrict__ base, const uint32_t N )
+// the collapse of a conversion's trees into their keep blocks (every tree of a batch; a single tree when it is refittable), local to
+// the tree: the forest numbers wide nodes in level order, so
+// wide node i of run r (CwRun) is the tree's node r.lo + i - r.first, split-tree nodes lose ext_base, and the SplitLeafs scan starts
+// at 0.  Threads 0 .. W-1 take the wide nodes, W .. W+N-1 the BVH2 nodes.
+__global__ void k_keep( const CwTree* __restrict__ T, const uint32_t K, const CwRun* __restrict__ runs, const uint32_t G, const uint32_t W,
+	const uint32_t* __restrict__ list, const uint32_t* __restrict__ adopt, const uint32_t* __restrict__ ifirst, const uint32_t* __restrict__ base, const uint32_t N )
 {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i < W)
 	{
-		const uint32_t t = wtree[i];
-		const CwTree& tr = T[t];
-		if (!tr.keep) return;
-		const uint32_t g = run_of( gfirst, G, i ), x = i - gfirst[g] + glocal[g];
+		const CwRun r = runs[batch_entry<CwRun, &CwRun::first>( runs, G, i )];
+		const CwTree& tr = T[r.tree];
+		const uint32_t x = r.lo + i - r.first;
 		uint32_t* kl = tr.keep + tr.used + 1, * ka = kl + tr.wide_count, * ki = ka + (size_t)8 * tr.wide_count;
-		kl[x] = list[i] - tr.ext_base;
-		for (int j = 0; j < 8; j++) { const uint32_t a = adopt[(size_t)i * 8 + j]; ka[(size_t)x * 8 + j] = a ? a - tr.ext_base : 0u; }
+		kl[x] = list[i] - tr.shift;
+		for (int j = 0; j < 8; j++) { const uint32_t a = adopt[(size_t)i * 8 + j]; ka[(size_t)x * 8 + j] = a ? a - tr.shift : 0u; }
 		// read only for nodes with interior children, which are the tree's own nodes on the next level
-		const uint32_t c = ifirst[i], gc = c < W ? run_of( gfirst, G, c ) : 0;
-		ki[x] = c < W && wtree[c] == t ? c - gfirst[gc] + glocal[gc] : 0u;
+		const uint32_t c = ifirst[i];
+		const CwRun rc = c < W ? runs[batch_entry<CwRun, &CwRun::first>( runs, G, c )] : CwRun{};
+		ki[x] = c < W && rc.tree == r.tree ? rc.lo + c - rc.first : 0u;
 	}
 	else if (i - W < N)
 	{
 		const uint32_t g = i - W;
-		const CwTree& tr = T[tree_of_node( T, K, g )];
+		const CwTree& tr = T[batch_entry<CwTree, &CwTree::nbase>( T, K, g )];
 		const uint32_t x = g - tr.nbase;
-		if (!tr.keep || x >= tr.used) return;
+		if (x >= tr.used) return;
 		const uint32_t b0 = base[tr.nbase];
 		tr.keep[x] = base[g] - b0;
 		if (x + 1 == tr.used) tr.keep[tr.used] = base[g + 1] - b0;
@@ -345,21 +313,18 @@ __global__ void k_keep( const CwTree* __restrict__ T, const uint32_t K, const ui
 }
 
 // ---- BVH8_CWBVH::ConvertFrom, greedy child -> slot assignment (:5910-5946) and per-node child statistics, one thread per wide node.
-// BATCH (a refit of several kept collapses): wide node g of the refit's wide-node space, in the tree of T that owns it, whose own
-// arrays it works on with local numbers (its local node 0 is its root); else the arrays of the arguments
+// BATCH: wide node g of the call's wide-node space, in the tree of T that owns it; else node g of `one`.  A tree's own arrays, local
+// numbers: its local node 0 is its root.
 template <bool BATCH>
-__global__ void k_assign( const CwRefit* __restrict__ T, const uint32_t K, const float4* __restrict__ ext, const uint32_t* __restrict__ list,
-	const uint32_t* __restrict__ adopt, const uint32_t* __restrict__ ifirst, const uint32_t num, uint32_t roots, WideNode* __restrict__ wide )
+__global__ void k_assign( const CwTree* __restrict__ T, const uint32_t K, const CwTree one, const uint32_t num )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= num) return;
-	uint32_t t = g;
-	if (BATCH)
-	{
-		const CwRefit& tr = T[batch_entry<CwRefit, &CwRefit::wbase>( T, K, g )];
-		t = g - tr.wbase, ext = tr.ext, list = tr.list, adopt = tr.adopt, ifirst = tr.ifirst, wide = tr.wide, roots = 1;
-	}
-	const uint32_t x = list[t];
+	const CwTree& tr = BATCH ? T[batch_entry<CwTree, &CwTree::wbase>( T, K, g )] : one;
+	const uint32_t t = BATCH ? g - tr.wbase : g;
+	const float4* __restrict__ ext = tr.ext;
+	const uint32_t* __restrict__ adopt = tr.adopt;
+	const uint32_t x = tr.list[t];
 	WideNode w = {};
 	for (int i = 0; i < 8; i++) w.child[i] = adopt[(size_t)t * 8 + i];
 	const float4 lo = ext[(size_t)x * 2], hi = ext[(size_t)x * 2 + 1];
@@ -399,7 +364,7 @@ __global__ void k_assign( const CwRefit* __restrict__ T, const uint32_t K, const
 	for (int i = 0; i < 8; i++) if (assignment[i] == -1) for (int s = 0; s < 8; s++) if (slot_empty[s]) { slot_empty[s] = false, assignment[i] = s; break; }
 	// interior children in adoption order are the wide nodes ifirst, ifirst + 1, .. (k_collapse)
 	const uint32_t adopted[8] = { w.child[0], w.child[1], w.child[2], w.child[3], w.child[4], w.child[5], w.child[6], w.child[7] };
-	uint32_t wi = ifirst[t], lt = 0;
+	uint32_t wi = tr.ifirst[t], lt = 0;
 	for (int i = 0; i < 8; i++)
 	{
 		const uint32_t c = adopted[i];
@@ -410,23 +375,23 @@ __global__ void k_assign( const CwRefit* __restrict__ T, const uint32_t K, const
 		if (cnt == 0) w.wchild[s] = wi++, w.ichild++; else lt += cnt;
 	}
 	w.leaf_tris = lt, w.size = 1, w.tris = lt;
-	if (t < roots) w.cbase = 1; // a root (wide nodes 0 .. roots-1): node 0 of its tree, its children from node 1, its triangles from record 0
-	wide[t] = w;
+	if (t == 0) w.cbase = 1; // the root: node 0 of its tree, its children from node 1, its triangles from record 0
+	tr.wide[t] = w;
 }
 
-// wide node t of a level: lo + t of `wide`, or (BATCH) the node of the level's run that holds it, in its tree's own array
-template <bool BATCH> __device__ __forceinline__ uint32_t level_node( const CwRefit* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns,
+// wide node lo + t of the call's level order: of `wide`, or (BATCH) of the level's run that holds it, in its tree's own array
+template <bool BATCH> __device__ __forceinline__ uint32_t level_node( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns,
 	const uint32_t lo, const uint32_t t, WideNode* __restrict__& wide )
 {
 	if (!BATCH) return lo + t;
-	const CwRun r = runs[batch_entry<CwRun, &CwRun::first>( runs, nruns, t )];
+	const CwRun r = runs[batch_entry<CwRun, &CwRun::first>( runs, nruns, lo + t )];
 	wide = T[r.tree].wide;
-	return r.lo + t - r.first;
+	return r.lo + lo + t - r.first;
 }
 
 // bottom-up: subtree node / triangle counts of wide nodes lo .. lo+num-1 (the next level's are final already)
 template <bool BATCH>
-__global__ void k_sizes( const CwRefit* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
+__global__ void k_sizes( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= num) return;
@@ -443,7 +408,7 @@ __global__ void k_sizes( const CwRefit* __restrict__ T, const CwRun* __restrict_
 
 // top-down: output addresses of the children of wide nodes lo .. lo+num-1 (see the header comment)
 template <bool BATCH>
-__global__ void k_addresses( const CwRefit* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
+__global__ void k_addresses( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= num) return;
@@ -522,45 +487,57 @@ __device__ __forceinline__ void encode_node( const float4* __restrict__ ext, con
 	o[4] = make_float4( __uint_as_float( q[8] ), __uint_as_float( q[9] ), __uint_as_float( q[10] ), __uint_as_float( q[11] ) );
 }
 
-// T: the batch's trees, wide node t belongs to tree wtree[t]; T = NULL: every node belongs to `one`
-__global__ void k_encode( const float4* __restrict__ ext, const uint32_t* __restrict__ list, const uint32_t num, const WideNode* __restrict__ wide,
-	const CwTree* __restrict__ T, const uint32_t* __restrict__ wtree, const CwTree one )
-{
-	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-	if (t >= num) return;
-	const CwTree& io = T ? T[wtree[t]] : one;
-	encode_node( ext, list[t], wide[t], io.prim_idx, io.verts, io.cw_nodes, io.cw_tris );
-}
-
-// a refit of several kept collapses: wide node g of the refit's wide-node space, in its tree's own arrays
-__global__ void k_encode_trees( const CwRefit* __restrict__ T, const uint32_t K, const uint32_t num )
+// wide node g: BATCH and one as for k_assign
+template <bool BATCH>
+__global__ void k_encode( const CwTree* __restrict__ T, const uint32_t K, const CwTree one, const uint32_t num )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= num) return;
-	const CwRefit& tr = T[batch_entry<CwRefit, &CwRefit::wbase>( T, K, g )];
-	const uint32_t t = g - tr.wbase;
+	const CwTree& tr = BATCH ? T[batch_entry<CwTree, &CwTree::wbase>( T, K, g )] : one;
+	const uint32_t t = BATCH ? g - tr.wbase : g;
 	encode_node( tr.ext, tr.list[t], tr.wide[t], tr.prim_idx, tr.verts, tr.cw_nodes, tr.cw_tris );
 }
 
-
-// slot assignment, subtree sizes (bottom-up), addresses (top-down), encode: everything after the collapse that depends on boxes.
-// Wide nodes 0 .. roots-1 are roots; T / wtree / one as for k_encode.
-static int cw_assign_encode( cudaStream_t s, const float4* ext, const uint32_t* list, const uint32_t* adopt, const uint32_t* ifirst,
-	const std::vector<uint32_t>& off, WideNode* wide, const uint32_t roots, const CwTree* T, const uint32_t* wtree, const CwTree& one )
+// The levels of K trees in the call's level order: level l is wide nodes off[l] .. off[l+1], each tree's run of it in batch order,
+// runs start[l] .. start[l+1].  tree_off[i]: tree i's own level offsets (CwKeep::off).
+struct CwLevels { std::vector<CwRun> runs; std::vector<uint32_t> off, start; };
+static CwLevels cw_levels( const std::vector<const std::vector<uint32_t>*>& tree_off )
 {
-	const uint32_t levels = (uint32_t)off.size() - 1, wide_count = off[levels];
-	k_assign<false><<<(wide_count + 127) / 128, 128, 0, s>>>( 0, 0, ext, list, adopt, ifirst, wide_count, roots, wide ); LAUNCHED();
-	for (int l = (int)levels - 1; l >= 0; l--)
+	CwLevels lv;
+	size_t levels = 0;
+	for (const auto* o : tree_off) levels = std::max( levels, o->size() - 1 );
+	lv.off.assign( 1, 0 ), lv.start.assign( 1, 0 );
+	for (size_t l = 0; l < levels; l++)
 	{
-		const uint32_t num = off[l + 1] - off[l];
-		k_sizes<false><<<(num + 127) / 128, 128, 0, s>>>( 0, 0, 0, off[l], num, wide ); LAUNCHED();
+		uint32_t at = lv.off.back();
+		for (uint32_t i = 0; i < (uint32_t)tree_off.size(); i++)
+		{
+			const std::vector<uint32_t>& o = *tree_off[i];
+			if (l + 1 < o.size()) lv.runs.push_back( CwRun{ at, i, o[l], 0 } ), at += o[l + 1] - o[l];
+		}
+		lv.off.push_back( at ), lv.start.push_back( (uint32_t)lv.runs.size() );
 	}
-	for (uint32_t l = 0; l < levels; l++)
-	{
-		const uint32_t num = off[l + 1] - off[l];
-		k_addresses<false><<<(num + 127) / 128, 128, 0, s>>>( 0, 0, 0, off[l], num, wide ); LAUNCHED();
-	}
-	k_encode<<<(wide_count + 127) / 128, 128, 0, s>>>( ext, list, wide_count, wide, T, wtree, one ); LAUNCHED();
+	return lv;
+}
+
+// slot assignment, subtree sizes (bottom-up), addresses (top-down), encode: everything after the collapse that depends on boxes, for
+// the K trees of the table d_T whose levels are lv (runs on the device at d_runs).  K = 1 runs the single-tree instances over `one`.
+static int cw_assign_encode( const CwTree* d_T, const uint32_t K, const CwTree& one, const CwLevels& lv, const CwRun* d_runs, cudaStream_t s )
+{
+	const uint32_t levels = (uint32_t)lv.off.size() - 1, W = lv.off[levels];
+	if (K > 1) k_assign<true><<<(W + 127) / 128, 128, 0, s>>>( d_T, K, CwTree{}, W );
+	else k_assign<false><<<(W + 127) / 128, 128, 0, s>>>( 0, 1, one, W );
+	LAUNCHED();
+	#define CW_LEVEL( kernel, l ) do { const uint32_t num_ = lv.off[l + 1] - lv.off[l], g_ = (num_ + 127) / 128; \
+		if (K > 1) kernel<true><<<g_, 128, 0, s>>>( d_T, d_runs + lv.start[l], lv.start[l + 1] - lv.start[l], lv.off[l], num_, 0 ); \
+		else kernel<false><<<g_, 128, 0, s>>>( 0, 0, 0, lv.off[l], num_, one.wide ); \
+		LAUNCHED(); } while (0)
+	for (int l = (int)levels - 1; l >= 0; l--) CW_LEVEL( k_sizes, l );
+	for (uint32_t l = 0; l < levels; l++) CW_LEVEL( k_addresses, l );
+	#undef CW_LEVEL
+	if (K > 1) k_encode<true><<<(W + 127) / 128, 128, 0, s>>>( d_T, K, CwTree{}, W );
+	else k_encode<false><<<(W + 127) / 128, 128, 0, s>>>( 0, 1, one, W );
+	LAUNCHED();
 	return TBVH_OK;
 }
 
@@ -587,8 +564,9 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 	{
 		const tbvh_bvh b = bs[t];
 		drop_cwbvh( b );
-		T[t] = CwTree{ b->d_nodes, b->d_prim_idx, b->d_verts, 0, 0, 0, N, b->info.used_nodes, cw_seg( b->info.used_nodes ), 0, 0 };
-		N += T[t].seg;
+		T[t] = CwTree{};
+		T[t].nodes = b->d_nodes, T[t].prim_idx = b->d_prim_idx, T[t].verts = b->d_verts, T[t].nbase = N, T[t].used = b->info.used_nodes;
+		N += cw_seg( T[t].used );
 	}
 	std::vector<void*> scratch;
 	#define CW_ALLOC( ptr, bytes ) do { CUDA_TRY( cudaMalloc( (void**)&(ptr), (bytes) ) ); scratch.push_back( (void*)(ptr) ); } while (0)
@@ -598,11 +576,10 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 	auto take = [&]( const size_t bytes ) { const size_t o = carve; carve += (bytes + 255) & ~(size_t)255; return o; };
 	CwTree* d_T = 0;
 	uint32_t* extra = 0, * base = 0, * tile = 0, * d_ext = 0, * lists = 0, * wtree = 0, * adopt = 0, * ifirst = 0, * leaf = 0, * tickets = 0, * counts = 0;
-	uint32_t* d_runs = 0, * ngroups = 0;
+	uint32_t* ngroups = 0;
 	uint2* groups = 0;
 	unsigned long long* look = 0;
 	float4* ext = 0;
-	WideNode* wide = 0;
 	auto body = [&]() -> int
 	{
 		// ---- SplitLeafs(3) over every tree, and each tree's first split-tree node
@@ -638,7 +615,9 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 			CUDA_TRY( cudaMemsetAsync( blob + o_leaf, 0, carve - o_leaf, s ) );
 		}
 		ngroups = tickets + CW_MAX_LEVELS;
-		k_split_emit_batch<<<(N + 255) / 256, 256, 0, s>>>( d_T, K, N, base, ext, 3 ); LAUNCHED();
+		for (uint32_t t = 0; t < K; t++) T[t].ext = ext + (size_t)ext_base[t] * 2, T[t].shift = ext_base[t], T[t].scan = base + T[t].nbase;
+		if (K > 1) CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
+		TRY( cw_split_emit( d_T, K, T[0], N, s ) );
 		// ---- collapse to 8-wide, level by level from the K roots
 		std::vector<uint32_t> iota( K );
 		for (uint32_t t = 0; t < K; t++) iota[t] = t;
@@ -663,59 +642,72 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		const uint32_t levels = (uint32_t)off.size() - 1, W = off[levels];
 		// ---- each tree's runs of wide nodes, one per level it reaches: its wide-node count and its own level offsets (a CwKeep's off).
 		// Levels are grouped by tree in batch order, so sorted by first node the runs tile every level and a run ends where the next begins.
-		std::vector<uint32_t> h_leaf( K ), gfirst, glocal;
-		std::vector<uint2> runs;
-		uint32_t G = levels;
+		std::vector<uint32_t> h_leaf( K );
+		std::vector<uint2> groups_h;
+		uint32_t G = 0;
 		if (K > 1) CUDA_TRY( cudaMemcpyAsync( &G, ngroups, 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaMemcpyAsync( h_leaf.data(), leaf, (size_t)K * 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
+		std::vector<std::vector<uint32_t>> toff( K, std::vector<uint32_t>( 1, 0 ) );
 		if (K > 1)
 		{
-			runs.resize( G );
-			CUDA_TRY( cudaMemcpyAsync( runs.data(), groups, (size_t)G * 8, cudaMemcpyDeviceToHost, s ) );
+			groups_h.resize( G );
+			CUDA_TRY( cudaMemcpyAsync( groups_h.data(), groups, (size_t)G * 8, cudaMemcpyDeviceToHost, s ) );
 			CUDA_TRY( cudaStreamSynchronize( s ) );
-			std::sort( runs.begin(), runs.end(), []( const uint2& a, const uint2& b ) { return a.y < b.y; } );
+			std::sort( groups_h.begin(), groups_h.end(), []( const uint2& a, const uint2& b ) { return a.y < b.y; } );
+			for (uint32_t g = 0; g < G; g++)
+			{
+				const uint32_t t = groups_h[g].x, end = g + 1 < G ? groups_h[g + 1].y : W;
+				toff[t].push_back( toff[t].back() + (end - groups_h[g].y) );
+			}
 		}
-		else for (uint32_t l = 0; l < levels; l++) runs.push_back( make_uint2( 0, off[l] ) );
-		std::vector<std::vector<uint32_t>> toff( K, std::vector<uint32_t>( 1, 0 ) );
-		gfirst.resize( G ), glocal.resize( G );
-		for (uint32_t g = 0; g < G; g++)
-		{
-			const uint32_t t = runs[g].x, first = runs[g].y, end = g + 1 < G ? runs[g + 1].y : W;
-			gfirst[g] = first, glocal[g] = toff[t].back();
-			toff[t].push_back( toff[t].back() + (end - first) );
-		}
-		// ---- outputs, per handle
-		bool any_keep = false;
-		for (uint32_t t = 0; t < K; t++)
+		else toff[0] = off;
+		// the same levels again as each tree's runs: the forest's wide nodes are the call's level order
+		std::vector<const std::vector<uint32_t>*> toff_p( K );
+		for (uint32_t t = 0; t < K; t++) toff_p[t] = &toff[t];
+		const CwLevels lv = cw_levels( toff_p );
+		// ---- outputs, per handle; the keep blocks of K > 1 trees that do not keep their collapse are scratch of the call
+		size_t scratch_words = 0;
+		for (uint32_t t = 0, wb = 0; t < K; t++)
 		{
 			const tbvh_bvh b = bs[t];
-			const uint32_t wc = toff[t].back();
+			const uint32_t wc = toff[t].back(), used = b->info.used_nodes;
 			CUDA_TRY( cudaMalloc( &b->d_cw_nodes, (size_t)wc * 80 ) );
 			CUDA_TRY( cudaMalloc( &b->d_cw_tris, (size_t)b->info.idx_count * 48 ) );
-			T[t].cw_nodes = b->d_cw_nodes, T[t].cw_tris = b->d_cw_tris, T[t].ext_base = ext_base[t], T[t].wide_count = wc;
+			T[t].cw_nodes = b->d_cw_nodes, T[t].cw_tris = b->d_cw_tris, T[t].wbase = wb, T[t].wide_count = wc, T[t].leaf_root = h_leaf[t] != 0;
+			wb += wc;
 			b->info.used_blocks = wc * 5, b->info.cwbvh_tri_count = b->info.idx_count;
-			if (!b->refittable) continue;
+			if (!b->refittable) { if (K > 1) scratch_words += (size_t)used + 1 + (size_t)wc * 10; continue; }
 			// keep the collapse for tbvh_refit_layouts, sized to the wide tree
 			CwKeep* k = new (std::nothrow) CwKeep();
 			if (!k) { tbvh_set_error( "CWBVH conversion: out of host memory" ); return TBVH_E_ARG; }
 			b->cw_keep = k;
-			const uint32_t used = b->info.used_nodes;
 			k->used = used, k->total = ext_base[t + 1] - ext_base[t], k->wide_count = wc, k->leaf_root = h_leaf[t] != 0, k->off = toff[t];
 			CUDA_TRY( cudaMalloc( &k->base, ((size_t)used + 1 + (size_t)wc * 10) * 4 ) );
 			k->list = k->base + used + 1, k->adopt = k->list + wc, k->ifirst = k->adopt + (size_t)wc * 8;
-			T[t].keep = k->base, any_keep = true;
+			T[t].keep = k->base;
 		}
-		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
-		CW_ALLOC( wide, (size_t)W * sizeof( WideNode ) );
-		{ const int r = cw_assign_encode( s, ext, lists, adopt, ifirst, off, wide, K, d_T, wtree, CwTree{} ); if (r != TBVH_OK) return r; }
-		if (any_keep)
+		// one allocation: the wide nodes (each tree's slice from its wbase), the runs, the scratch keep blocks
+		carve = 0;
+		const size_t o_wide = take( (size_t)W * sizeof( WideNode ) ), o_runs = take( lv.runs.size() * sizeof( CwRun ) ), o_keep = take( scratch_words * 4 );
+		CW_ALLOC( blob, carve );
+		const CwRun* d_runs = (const CwRun*)(blob + o_runs);
+		uint32_t* spare = (uint32_t*)(blob + o_keep);
+		for (uint32_t t = 0; t < K; t++)
 		{
-			CW_ALLOC( d_runs, (size_t)G * 8 );
-			CUDA_TRY( cudaMemcpyAsync( d_runs, gfirst.data(), (size_t)G * 4, cudaMemcpyHostToDevice, s ) );
-			CUDA_TRY( cudaMemcpyAsync( d_runs + G, glocal.data(), (size_t)G * 4, cudaMemcpyHostToDevice, s ) );
-			k_keep<<<(uint32_t)(((size_t)W + N + 255) / 256), 256, 0, s>>>( d_T, K, wtree, d_runs, d_runs + G, G, W, lists, adopt, ifirst, base, N ); LAUNCHED();
+			CwTree& tr = T[t];
+			tr.wide = (WideNode*)(blob + o_wide) + tr.wbase;
+			if (K == 1) { tr.list = lists, tr.adopt = adopt, tr.ifirst = ifirst; continue; } // its own forest: already tree-local
+			if (!tr.keep) tr.keep = spare, spare += (size_t)tr.used + 1 + (size_t)tr.wide_count * 10;
+			tr.list = tr.keep + tr.used + 1, tr.adopt = tr.list + tr.wide_count, tr.ifirst = tr.adopt + (size_t)tr.wide_count * 8;
 		}
+		if (K > 1 || T[0].keep)
+		{
+			CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
+			CUDA_TRY( cudaMemcpyAsync( (void*)d_runs, lv.runs.data(), lv.runs.size() * sizeof( CwRun ), cudaMemcpyHostToDevice, s ) );
+			k_keep<<<(uint32_t)(((size_t)W + N + 255) / 256), 256, 0, s>>>( d_T, K, d_runs, (uint32_t)lv.runs.size(), W, lists, adopt, ifirst, base, N ); LAUNCHED();
+		}
+		TRY( cw_assign_encode( d_T, K, T[0], lv, d_runs, s ) );
 		// the traversal nodes the kernels read and the pending bound of every wide tree (trace_cwbvh.cu); synchronises the stream
 		return cw_make_trav( bs, K, s );
 	};
@@ -772,14 +764,14 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 	std::lock_guard<std::mutex> lock( c->refit_mutex );
 	// what each tree takes part in; the caller bounds the sums (TBVH_REFIT_BATCH_MAX_NODES)
 	std::vector<uint32_t> cw, gp;
-	uint32_t N = 0, P = 0, NC = 0, WC = 0, NG = 0, levels = 0;
+	uint32_t N = 0, P = 0, NC = 0, NG = 0;
 	for (uint32_t t = 0; t < K; t++)
 	{
 		const tbvh_bvh b = bs[t];
 		if (!keep_layouts) drop_bvh_gpu( b ), drop_cwbvh( b ); // derived layouts describe the old boxes (the reference converts again too)
 		else b->generation = tbvh_next_generation(); // the arrays stay, but a TLAS over this BLAS holds its old root box in its instances
 		const uint32_t used = b->info.used_nodes;
-		if (keep_layouts && b->cw_keep) cw.push_back( t ), NC += used, WC += b->cw_keep->wide_count, levels = std::max( levels, (uint32_t)b->cw_keep->off.size() - 1 );
+		if (keep_layouts && b->cw_keep) cw.push_back( t ), NC += used;
 		if (keep_layouts && (b->info.layouts & (1u << TBVH_LAYOUT_BVH_GPU))) gp.push_back( t ), NG += used;
 		N += used, P += b->info.idx_count;
 	}
@@ -798,23 +790,14 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 			if (!k->parent) CUDA_TRY( cudaMalloc( &k->parent, (size_t)k->used * 4 ) );
 		}
 		// the batch levels: each tree's run of every level it reaches
-		std::vector<CwRun> runs;
-		std::vector<uint32_t> rstart( (size_t)levels + 1, 0 ), rnum( levels, 0 );
-		if (KC > 1)
-			for (uint32_t l = 0; l < levels; l++)
-			{
-				rstart[l] = (uint32_t)runs.size();
-				for (uint32_t i = 0; i < KC; i++)
-				{
-					const CwKeep* k = bs[cw[i]]->cw_keep;
-					if (l + 1 < k->off.size()) runs.push_back( CwRun{ rnum[l], i, k->off[l], 0 } ), rnum[l] += k->off[l + 1] - k->off[l];
-				}
-			}
-		rstart[levels] = (uint32_t)runs.size();
+		std::vector<const std::vector<uint32_t>*> toff( KC );
+		for (uint32_t i = 0; i < KC; i++) toff[i] = &bs[cw[i]]->cw_keep->off;
+		const CwLevels lv = cw_levels( toff );
+		const std::vector<CwRun>& runs = lv.runs;
 		// device: tables | arrival counters | results (root boxes, exponent ranges) | parents | BVH_GPU workspace;  host: tables | results
 		size_t carve = 0;
 		auto take = [&]( const size_t bytes ) { const size_t o = carve; carve += (bytes + 255) & ~(size_t)255; return o; };
-		const size_t o_rf = take( (size_t)K * sizeof( RfTree ) ), o_cr = take( (size_t)KC * sizeof( CwRefit ) ), o_runs = take( runs.size() * sizeof( CwRun ) );
+		const size_t o_rf = take( (size_t)K * sizeof( RfTree ) ), o_cr = take( (size_t)KC * sizeof( CwTree ) ), o_runs = take( runs.size() * sizeof( CwRun ) );
 		const size_t o_ct = take( (size_t)KC * sizeof( CwTrav ) ), o_gt = take( (size_t)KG * sizeof( GpuTree ) ), tables = carve;
 		const size_t o_arrive = take( (size_t)N * 4 ), res_words = (size_t)K * 8 + KC, o_res = take( res_words * 4 ), zeroed = carve - o_arrive;
 		const size_t o_parent = take( (size_t)N * 4 ), o_gw = take( (size_t)NG * 16 );
@@ -822,7 +805,7 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 		char* const dev = (char*)c->refit_dev, * const host = (char*)c->refit_host;
 		uint32_t* const res = (uint32_t*)(dev + o_res), * const h_res = (uint32_t*)(host + tables);
 		RfTree* const rf = (RfTree*)(host + o_rf);
-		CwRefit* const cr = (CwRefit*)(host + o_cr);
+		CwTree* const cr = (CwTree*)(host + o_cr);
 		CwTrav* const ct = (CwTrav*)(host + o_ct);
 		GpuTree* const gt = (GpuTree*)(host + o_gt);
 		bool any_fill = false;
@@ -838,7 +821,8 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 		{
 			const tbvh_bvh b = bs[cw[i]];
 			CwKeep* k = b->cw_keep;
-			cr[i] = CwRefit{ b->d_nodes, k->base, k->list, k->ifirst, k->adopt, k->ext, k->wide, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris, nb, k->used, wb, k->leaf_root ? 1u : 0u };
+			cr[i] = CwTree{ b->d_nodes, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris, k->ext, k->base, k->list, k->adopt, k->ifirst, k->wide, 0, 0,
+				nb, k->used, wb, k->wide_count, k->leaf_root ? 1u : 0u };
 			ct[i] = CwTrav{ (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, res + (size_t)K * 8 + i, wb, k->wide_count };
 			nb += k->used, wb += k->wide_count;
 		}
@@ -850,39 +834,20 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 		}
 		if (!runs.empty()) memcpy( host + o_runs, runs.data(), runs.size() * sizeof( CwRun ) );
 		const RfTree* d_rf = (const RfTree*)(dev + o_rf);
-		const CwRefit* d_cr = (const CwRefit*)(dev + o_cr);
-		const CwRun* d_runs = (const CwRun*)(dev + o_runs);
+		const CwTree* d_cr = (const CwTree*)(dev + o_cr);
 		CUDA_TRY( cudaMemcpyAsync( dev, host, tables, cudaMemcpyHostToDevice, s ) );
 		CUDA_TRY( cudaEventRecord( c->refit_e0, s ) );
 		CUDA_TRY( cudaMemsetAsync( dev + o_arrive, 0, zeroed, s ) );
 		TRY( refit_enqueue( d_rf, K, rf[0], N, (uint32_t*)(dev + o_arrive), any_fill, s ) );
 		TRY( leaf_tris_enqueue( d_rf, K, rf[0], P, s ) );
-		if (KC == 1)
+		if (KC)
 		{
-			const tbvh_bvh b = bs[cw[0]];
-			const CwKeep* k = b->cw_keep;
-			k_split_emit<false><<<(k->used + 255) / 256, 256, 0, s>>>( 0, 0, b->d_nodes, k->base, k->ext, k->used, 3 ); LAUNCHED();
-			if (k->leaf_root) { k_wrap_leaf_root<<<1, 1, 0, s>>>( k->ext, k->adopt ); LAUNCHED(); }
-			TRY( cw_assign_encode( s, k->ext, k->list, k->adopt, k->ifirst, k->off, k->wide, 1, 0, 0, CwTree{ 0, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris } ) );
-			TRY( cw_expand_launch( b, s, ct[0].res ) );
-		}
-		else if (KC > 1)
-		{
-			k_split_emit<true><<<(NC + 255) / 256, 256, 0, s>>>( d_cr, KC, 0, 0, 0, NC, 3 ); LAUNCHED();
+			TRY( cw_split_emit( d_cr, KC, cr[0], NC, s ) );
 			bool any_leaf_root = false;
 			for (uint32_t i = 0; i < KC; i++) any_leaf_root |= cr[i].leaf_root != 0;
 			if (any_leaf_root) { k_wrap_leaf_roots<<<(KC + 127) / 128, 128, 0, s>>>( d_cr, KC ); LAUNCHED(); }
-			k_assign<true><<<(WC + 127) / 128, 128, 0, s>>>( d_cr, KC, 0, 0, 0, 0, WC, 1, 0 ); LAUNCHED();
-			for (int l = (int)levels - 1; l >= 0; l--)
-			{
-				k_sizes<true><<<(rnum[l] + 127) / 128, 128, 0, s>>>( d_cr, d_runs + rstart[l], rstart[l + 1] - rstart[l], 0, rnum[l], 0 ); LAUNCHED();
-			}
-			for (uint32_t l = 0; l < levels; l++)
-			{
-				k_addresses<true><<<(rnum[l] + 127) / 128, 128, 0, s>>>( d_cr, d_runs + rstart[l], rstart[l + 1] - rstart[l], 0, rnum[l], 0 ); LAUNCHED();
-			}
-			k_encode_trees<<<(WC + 127) / 128, 128, 0, s>>>( d_cr, KC, WC ); LAUNCHED();
-			TRY( cw_expand_batch( (const CwTrav*)(dev + o_ct), KC, WC, s ) );
+			TRY( cw_assign_encode( d_cr, KC, cr[0], lv, (const CwRun*)(dev + o_runs), s ) );
+			TRY( cw_expand( (const CwTrav*)(dev + o_ct), KC, ct[0], lv.off.back(), 0, s ) );
 		}
 		if (KG) TRY( bvh_gpu_enqueue( (const GpuTree*)(dev + o_gt), KG, gt[0], NG, (uint32_t*)(dev + o_gw), s ) );
 		TRY( refit_roots( d_rf, K, res, s ) );

@@ -41,14 +41,6 @@
 // bytes 32..79 (lo.x, lo.y, lo.z, hi.x, hi.y, hi.z) - layout in SURVEY.md 8(a), written by BVH8_CWBVH::ConvertFrom (tiny_bvh.h:5948-6015).
 // One wide tree of a pass is a CwTrav (common.cuh).  A batch passes a device table of them, one tree `one`.
 
-// the tree that holds node g of a pass (wbase rises strictly: every tree has a node)
-__device__ __forceinline__ uint32_t trav_tree( const CwTrav* __restrict__ T, const uint32_t K, const uint32_t g )
-{
-	uint32_t lo = 0, hi = K;
-	while (hi - lo > 1) { const uint32_t m = (lo + hi) >> 1; if (T[m].wbase <= g) lo = m; else hi = m; }
-	return lo;
-}
-
 // range: max over a tree's nodes of 128 + the largest exponent byte, or 256 for a node with e = -128 or |p| > 2^126 (cw_ray_fits)
 // BATCH: the trees of the table T; else the one tree `one`, whose pointers stay kernel parameters (read from a table, they make
 // nvcc keep the pair records below in local memory)
@@ -57,7 +49,7 @@ __global__ void k_cw_expand( const CwTrav* __restrict__ T, const uint32_t K, con
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= W) return;
-	const uint32_t tree = BATCH ? trav_tree( T, K, g ) : 0;
+	const uint32_t tree = BATCH ? batch_entry<CwTrav, &CwTrav::wbase>( T, K, g ) : 0;
 	const CwTrav* tr = BATCH ? T + tree : &one;
 	const uint4* __restrict__ src = tr->src;
 	uint4* __restrict__ dst = tr->dst;
@@ -132,7 +124,7 @@ __global__ void k_cw_jump_init( const CwTrav* __restrict__ T, const uint32_t K, 
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= W) return;
-	const uint32_t wb = T[trav_tree( T, K, g )].wbase, p = parent[g];
+	const uint32_t wb = T[batch_entry<CwTrav, &CwTrav::wbase>( T, K, g )].wbase, p = parent[g];
 	// the root steps past itself - unless some node names it as a child, a cycle a walk would never leave: it then stays on itself;
 	// a record no node points at (0xffffffff) gets ancestor W (out of range) and is not counted
 	anc[g] = g == wb ? (p == 0xffffffffu ? CW_ROOT : g) : p == 0xffffffffu ? W : wb + (p & 0x7fffffffu), cnt[g] = (g == wb || p == 0xffffffffu) ? 0u : p >> 31;
@@ -150,24 +142,18 @@ __global__ void k_cw_pending( const CwTrav* __restrict__ T, const uint32_t K, co
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= W) return;
 	const uint32_t a = anc[g];
-	uint32_t* pending = T[trav_tree( T, K, g )].res + 1;
+	uint32_t* pending = T[batch_entry<CwTrav, &CwTrav::wbase>( T, K, g )].res + 1;
 	if (a == CW_ROOT) atomicMax( pending, cnt[g] );
 	else if (a < W) atomicMax( pending, CW_CYCLE );
 }
 
-// k_cw_expand of every node of d_cw_nodes into the allocated d_cw_trav; *d_range (zeroed by the caller) receives the tree's range
-int cw_expand_launch( tbvh_bvh b, cudaStream_t s, uint32_t* d_range )
+// k_cw_expand of the W nodes of the K trees of d_T into their allocated traversal nodes; K = 1 runs the single-tree instance over
+// `one`.  parent: where the pending pass finds every node's parent, or NULL (a refit: the topology and the pending bound stay)
+int cw_expand( const CwTrav* d_T, const uint32_t K, const CwTrav& one, const uint32_t W, uint32_t* parent, cudaStream_t s )
 {
-	const uint32_t count = b->info.used_blocks / 5;
-	const CwTrav one = { (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, d_range, 0, count };
-	k_cw_expand<false><<<(count + 127) / 128, 128, 0, s>>>( 0, 1, one, count, 0 ); LAUNCHED();
-	return TBVH_OK;
-}
-
-// the nodes of K trees at once, over a device table: a refit re-encodes them in place, so the pending bound stays (parent = NULL)
-int cw_expand_batch( const CwTrav* d_T, const uint32_t K, const uint32_t W, cudaStream_t s )
-{
-	k_cw_expand<true><<<(W + 127) / 128, 128, 0, s>>>( d_T, K, CwTrav{}, W, 0 ); LAUNCHED();
+	if (K > 1) k_cw_expand<true><<<(W + 127) / 128, 128, 0, s>>>( d_T, K, CwTrav{}, W, parent );
+	else k_cw_expand<false><<<(W + 127) / 128, 128, 0, s>>>( 0, 1, one, W, parent );
+	LAUNCHED();
 	return TBVH_OK;
 }
 
@@ -207,10 +193,8 @@ int cw_make_trav( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTrav ), cudaMemcpyHostToDevice, s ) );
 		CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)W * 4, s ) );
 		CUDA_TRY( cudaMemsetAsync( d_res, 0, (size_t)K * 8, s ) );
+		TRY( cw_expand( d_T, K, T[0], W, d_parent, s ) );
 		const uint32_t g = (W + 127) / 128;
-		if (K > 1) k_cw_expand<true><<<g, 128, 0, s>>>( d_T, K, CwTrav{}, W, d_parent );
-		else k_cw_expand<false><<<g, 128, 0, s>>>( 0, 1, T[0], W, d_parent );
-		LAUNCHED();
 		k_cw_jump_init<<<g, 128, 0, s>>>( d_T, K, d_parent, W, anc[0], cnt[0] ); LAUNCHED();
 		int cur = 0;
 		for (uint32_t reach = 1; reach < 2 * most; reach *= 2, cur ^= 1) { k_cw_jump<<<g, 128, 0, s>>>( W, anc[cur], cnt[cur], anc[cur ^ 1], cnt[cur ^ 1] ); LAUNCHED(); }

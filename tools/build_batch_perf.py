@@ -9,7 +9,8 @@ tree.  Then the CWBVH conversion of the same meshes' BuildAVX trees (what BVH8_C
 handle and one tbvh_convert_batch, alternated - wall time (both calls end in a synchronise), launches, and a byte comparison of every
 bvh8Data / bvh8Tris.  Then the one-tree path against an older build of the library (--parent-lib, when given): tbvh_build of the
 Bistro-sized procedural scene and of a 150k-triangle scene, and the wall time of tbvh_convert( CWBVH ) of the Bistro-sized scene's
-Build and BuildHQ trees, the two libraries alternated on the same card.  The card's name and power limit come from nvidia-smi (read-only).
+Build and BuildHQ trees, and the wall time of one tbvh_convert_batch( CWBVH ) of workload a's BuildAVX trees and of 200 BuildHQ trees
+with a byte comparison of every handle, the two libraries alternated on the same card.  The card's name and power limit come from nvidia-smi (read-only).
 Writes DIR/build_batch_perf.json and prints it."""
 import argparse
 import ctypes as C
@@ -206,6 +207,39 @@ def one_tree_convert(libs, reps):
     return out
 
 
+def batch_convert(libs, reps):
+    """tbvh_convert_batch( CWBVH ) in one call per library, the libraries alternated: workload a's BuildAVX trees, and 200 BuildHQ trees
+    (SBVHs: a batch of trees that keep no collapse)"""
+    rng = np.random.default_rng(1003)
+    hq = [scenes.procedural_scene(int(n), 20000 + k) for k, n in enumerate(np.exp(rng.uniform(np.log(64), np.log(20000), 200)).astype(int))]
+    out = {}
+    for label, meshes, flavour in (("workload_a_buildavx", workload("a"), _lib.BUILD_AVX), ("buildhq_200", hq, _lib.BUILD_HQ)):
+        n = len(meshes)
+        hs = {name: L.handles(n) for name, L in libs.items()}
+        for name, L in libs.items():
+            for k, v in enumerate(meshes):
+                L.build(hs[name][k], v, flavour)
+        ms = {name: [] for name in libs}
+        for r in range(reps + 1):   # r = 0 warms both up
+            for name, L in libs.items() if r % 2 == 0 else reversed(list(libs.items())):
+                t0 = time.perf_counter()
+                L.check(L.L.tbvh_convert_batch(hs[name], n, _lib.LAYOUT_CWBVH))
+                if r:
+                    ms[name].append((time.perf_counter() - t0) * 1e3)
+        out[label] = {name: stats(x) for name, x in ms.items()}
+        # bvh8Tris past the referenced records is uninitialised on an SBVH: bvh8Data only for BuildHQ
+        same = 0
+        for k in range(n):
+            cws = [L.download_cwbvh(hs[name][k]) for name, L in libs.items()]
+            same += all(np.array_equal(c[0], cws[0][0]) and (flavour == _lib.BUILD_HQ or np.array_equal(c[1], cws[0][1])) for c in cws)
+        out[label]["handles_identical"] = int(same)
+        out[label]["handles"] = n
+        for name, L in libs.items():
+            for h in hs[name]:
+                L.L.tbvh_bvh_destroy(h)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True, help="directory for build_batch_perf.json")
@@ -224,6 +258,7 @@ def main():
         libs = {"parent": Lib(args.parent_lib), "this": L}
     result["one_tree_build_ms"] = one_tree(libs, max(args.reps, 7))
     result["one_tree_convert_cwbvh_wall_ms"] = one_tree_convert(libs, max(args.reps, 7))
+    result["batch_convert_cwbvh_wall_ms"] = batch_convert(libs, max(args.reps, 7))
     path = os.path.join(args.out, "build_batch_perf.json")
     with open(path, "w") as f:
         json.dump(result, f, indent=1)

@@ -7,7 +7,8 @@ ones), BuildAVX trees.  Per frame the vertices are jittered (a new seed each fra
 each from host and from device-resident (torch) vertices.  The two paths alternate; reported: host wall time around the complete call(s)
 (every call ends in a synchronise), kernel launches, device time (the batch's build_ms; the loop's summed build_ms), and a byte
 comparison of every handle after the last frame (BVH2, and bvh8Data / bvh8Tris where held).  With --parent-lib: tools/refit_perf.py's
-frame - tbvh_refit_layouts of one Bistro-sized BVH::Build tree holding its CWBVH - with this library and the older one, alternated.  The
+frame - tbvh_refit_layouts of one Bistro-sized BVH::Build tree holding its CWBVH - and one tbvh_refit_batch( .., keep_layouts = 1 ) of
+workload a's trees per frame, with this library and the older one, alternated.  The
 card's name and power limit come from nvidia-smi (read-only).  Writes DIR/refit_batch_perf.json and prints it."""
 import argparse
 import ctypes as C
@@ -113,6 +114,38 @@ def one_tree(libs, reps):
     return out
 
 
+def batch_refit(libs, reps):
+    """tbvh_refit_batch( .., keep_layouts = 1 ) of workload a's BuildAVX trees holding their CWBVH, host vertices, one call per library
+    and frame, the libraries alternated: wall and device time, and a byte comparison of every handle after the last frame"""
+    meshes = workload("a")
+    n = len(meshes)
+    recs = (_lib.Mesh * n)(*[_lib.Mesh(v.ctypes.data, 16, 0, None, v.shape[0] // 3) for v in meshes])
+    hs = {name: L.handles(n) for name, L in libs.items()}
+    for name, L in libs.items():
+        L.check(L.L.tbvh_build_batch(hs[name], recs, n, _lib.HOST, 1.0, 1.0, _lib.BUILD_AVX))
+        L.check(L.L.tbvh_convert_batch(hs[name], n, _lib.LAYOUT_CWBVH))
+    wall = {name: [] for name in libs}
+    dev = {name: [] for name in libs}
+    for r in range(reps + 1):   # r = 0 warms both up
+        ws = [jitter(v, 7000 + 1000 * r + k) for k, v in enumerate(meshes)]
+        rs = (_lib.Mesh * n)(*[_lib.Mesh(w.ctypes.data, 16, 0, None, w.shape[0] // 3) for w in ws])
+        for name, L in libs.items() if r % 2 == 0 else reversed(list(libs.items())):
+            t0 = time.perf_counter()
+            L.check(L.L.tbvh_refit_batch(hs[name], rs, n, _lib.HOST, 1))
+            if r:
+                wall[name].append((time.perf_counter() - t0) * 1e3), dev[name].append(L.info(hs[name][0]).build_ms)
+    out = {name: {"wall_ms": stats(wall[name]), "device_ms": stats(dev[name])} for name in libs}
+    same = 0
+    for k in range(n):
+        outs = [L.download(hs[name][k]) + L.download_cwbvh(hs[name][k]) for name, L in libs.items()]
+        same += all(all(np.array_equal(a, b) for a, b in zip(o, outs[0])) for o in outs)
+    out["handles_identical"], out["handles"] = int(same), n
+    for name, L in libs.items():
+        for h in hs[name]:
+            L.L.tbvh_bvh_destroy(h)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True, help="directory for refit_batch_perf.json")
@@ -130,7 +163,9 @@ def main():
             for device in (False, True):
                 result[f"workload_{name}_{mode}_{'device' if device else 'host'}"] = run_workload(L, meshes, args.reps, mode, device)
     if args.parent_lib:
-        result["one_tree_refit_layouts"] = one_tree({"parent": Lib(args.parent_lib), "this": L}, max(args.reps, 9))
+        libs = {"parent": Lib(args.parent_lib), "this": L}
+        result["one_tree_refit_layouts"] = one_tree(libs, max(args.reps, 9))
+        result["batch_refit_layouts"] = batch_refit(libs, max(args.reps, 9))
     path = os.path.join(args.out, "refit_batch_perf.json")
     with open(path, "w") as f:
         json.dump(result, f, indent=1)
