@@ -217,6 +217,7 @@ static void split_frag( const hq_t* h, const frag_t* orig, frag_t* left, frag_t*
 
 typedef struct { uint32_t node, sliceStart, sliceEnd, depth; } task_t;
 uint32_t orc_hq_failed_splits = 0; /* diagnostics: low 16 bits = 'spatial split failed' leaves (:2939), high bits = those that read stale idxTmp words */
+uint32_t orc_hq_failed_max = 0;    /* diagnostics: fragment count of the largest node whose spatial split failed */
 
 /* BuildHQTask :2731-3008, non-threaded */
 static void build_hq_task( hq_t* h, uint32_t nodeIdx, uint32_t sliceStart, uint32_t sliceEnd, uint32_t* idxTmp )
@@ -435,6 +436,7 @@ static void build_hq_task( hq_t* h, uint32_t nodeIdx, uint32_t sliceStart, uint3
 			{
 				orc_hq_failed_splits++;
 				if (node->leftFirst != (leftCount ? sliceStart : B)) orc_hq_failed_splits += 1 << 16;
+				if (node->triCount > orc_hq_failed_max) orc_hq_failed_max = node->triCount;
 				for (uint32_t i = 0; i < node->triCount; i++) primIdx[node->leftFirst + i] = fragment[primIdx[node->leftFirst + i]].primIdx;
 				node->minx = fmin_( bestLMin[0], bestRMin[0] ), node->miny = fmin_( bestLMin[1], bestRMin[1] ), node->minz = fmin_( bestLMin[2], bestRMin[2] );
 				node->maxx = fmax_( bestLMax[0], bestRMax[0] ), node->maxy = fmax_( bestLMax[1], bestRMax[1] ), node->maxz = fmax_( bestLMax[2], bestRMax[2] );

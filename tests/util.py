@@ -510,6 +510,24 @@ def translated(v, shift):
     return v
 
 
+def snapped(v, q):
+    """Positions rounded to multiples of 1 / q, with no -0 left (the + 0.0 turns -0 into +0).  Many fragment bounds then sit on
+    the same planes, so BuildHQ's spatial splits often fail (every fragment on one side, tiny_bvh.h:2939), in big nodes too."""
+    v = np.array(v, np.float32).reshape(-1, 4)
+    q = np.float32(q)
+    v[:, :3] = np.round(v[:, :3] * q) / q + np.float32(0.0)
+    return v
+
+
+def lattice_scene(n, seed, k=3):
+    """n triangles whose vertices are seeded points of the integer lattice {0 .. k-1}^3: coincident, collinear and repeated
+    vertices, and bounds on a few shared planes."""
+    rng = np.random.default_rng(seed)
+    v = np.zeros((n * 3, 4), np.float32)
+    v[:, :3] = rng.integers(0, k, (n * 3, 3))
+    return v
+
+
 ONE_TRI = np.array([[0, 0, 0, 0], [1, 0, 0, 0], [0, 1, 0, 0]], np.float32)
 
 

@@ -31,7 +31,17 @@ def context(device: int = 0):
 
 
 def set_option(key: str, value: int, device: int = 0) -> None:
-    """Tuning knob of the engine context (tbvh_set_option): trace_variant, small_t, d2h_mode, h2d_split, host_path."""
+    """Tuning knob of the engine context (tbvh_set_option).  Keys:
+      traversal     trace_variant (BVH2 walk kernel: 0 generic, 3 octant switch, 4 persistent warps),
+                    inst_idx_bits (the host program's INST_IDX_BITS: 32, or 4..31 top bits of hit.prim)
+      Build         small_t (subtrees of at most this many primitives go to the warp kernel, 8..256),
+                    small_mode (warp kernel: bit 0 fragments staged in shared memory, bit 1 aggregated bin updates),
+                    build_mode (0 one persistent launch for the large phase, 1 one launch per stage and level),
+                    build_ctas (CTAs per SM of the persistent large phase, 0 = default, capped at the occupancy and 16)
+      BuildHQ       hq_small (nodes of at most this many fragments go to the warp-per-subtree kernel, clamped to 8..256),
+                    hq_cluster (largest thread-block cluster a node of the level phase may get, clamped to 1..16)
+      host rays     d2h_mode (0..3), h2d_split (1..4), host_path (0, 1, 2), scatter_threads (1..64), chunk_rays (>= 4096)
+    An unknown key raises TbvhError."""
     check(_lib.lib().tbvh_set_option(context(device), key.encode(), int(value)))
 
 

@@ -1154,9 +1154,10 @@ int build_hq_launch( tbvh_bvh b, float c_trav, float c_int )
 		while (num)
 		{
 			CUDA_TRY( cudaMemsetAsync( &A.ctr->next_big, 0, 8, s ) ); // next_big + next_max
-			// cluster size: enough CTAs for the largest node of the level (about 512 fragments per CTA), at most 8 CTAs per SM in flight
+			// cluster size: enough CTAs for the largest node of the level (about 512 fragments per CTA), at most 8 CTAs per SM in flight,
+			// a power of two no larger than max_cluster
 			uint32_t nct = 1;
-			while (nct < max_cluster && (size_t)nct * cta_frags < max_count && (size_t)num * nct * 2 <= (size_t)b->ctx->sm_count * cta_cap) nct <<= 1;
+			while (nct * 2 <= max_cluster && (size_t)nct * cta_frags < max_count && (size_t)num * nct * 2 <= (size_t)b->ctx->sm_count * cta_cap) nct <<= 1;
 			cudaLaunchConfig_t cfg = {};
 			cudaLaunchAttribute attr[1];
 			cfg.gridDim = dim3( num * nct ), cfg.blockDim = dim3( HQ_BIG_THREADS ), cfg.dynamicSmemBytes = 0, cfg.stream = s;
