@@ -179,6 +179,30 @@ int tbvh_instance_update_box( void* instance, const float* blas_aabb_min, const 
 int tbvh_build_tlas( tbvh_bvh tlas, const void* instances, uint32_t inst_stride, uint32_t inst_count, const tbvh_bvh* blasses, uint32_t blas_count,
 	float c_trav, float c_int );
 
+/* BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) tiny_bvh.h:2221 with blasses != 0, the call an animated scene makes every
+ * frame after it refitted its BLASes and wrote the new transforms (tiny_bvh_anim.cpp, tmpl8/game.cpp): every instance is Update()d
+ * (:2245-2250, :8386) and the TLAS is built over the new boxes.  Update runs on the device, one kernel for the whole list, and that
+ * kernel also fills the tables the two-level walk and the builder read: no host loop touches the records.
+ *  instances: inst_count records of the 192-byte BLASInstance, inst_stride bytes apart, in `space`.  Read: transform (byte 0), blasIdx
+ *  (140), mask (156).  Written back in place as Update does: invTransform (64), aabbMin (128), aabbMax (144); no other byte changes.
+ *  TBVH_DEVICE: the pointer and the stride are multiples of 16 and the records follow the rule for device-space inputs above.
+ *  TBVH_HOST: the stride is a multiple of 4 and at least 160; the records go through the device in one strided copy each way.
+ *  The root box of instance i is that of blasses[blasIdx] as tbvh_bvh_info reports it - what tbvh_instance_update uses, and what
+ *  tbvh_refit_batch has just brought up to date.
+ * The result is exactly what tbvh_instance_update on every record followed by tbvh_build_tlas leaves: the same record bytes, TLAS
+ * nodes, primIdx and info (build_ms includes the update kernel), the same rules for the layouts of the BLASses, the same staleness.
+ * (Where the arithmetic itself generates a NaN - a determinant that overflows - both give a NaN; its sign and payload are the processor's.)
+ * Refusals: those of tbvh_build_tlas with the same codes, TBVH_E_STATE for a BLAS without a BVH-layout tree (its root box is not
+ * known: tbvh_instance_update's refusal), TBVH_E_ARG for an unknown space, a bad stride or a misaligned device pointer.  Whatever host
+ * state decides - handles, counts, stride, the state and limits of the BLASses, and for host records blasIdx < blas_count - is checked
+ * before the handle is touched: a refused call leaves a walkable TLAS walkable and the records as they were.  In device records
+ * blasIdx is checked by the kernel, which never dereferences an index past the list: TBVH_E_ARG, the handle left empty as after a
+ * failed build, the records unspecified.
+ * A handle that already is a TLAS over the same inst_count and blas_count keeps its instance boxes, instance and BLAS tables and the
+ * staging of host records; what a frame still allocates is the builder's own (the node and primIdx arrays and its scratch). */
+int tbvh_build_tlas_update( tbvh_bvh tlas, void* instances, uint32_t inst_stride, uint32_t inst_count, int space, const tbvh_bvh* blasses,
+	uint32_t blas_count, float c_trav, float c_int );
+
 /* BVH::Refit (tiny_bvh.h:3055-3093): the triangles moved, the topology stays - leaf boxes from the new vertices, interior
  * boxes bottom-up.  verts as for tbvh_build, same prim_count.  TBVH_E_STATE for an SBVH (the reference's fatal "refitting an
  * SBVH") or when no BVH-layout tree is resident.  Derived layouts on the handle are dropped; tbvh_convert again. */

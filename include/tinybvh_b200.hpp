@@ -218,6 +218,24 @@ public:
 		TBVH_FATAL_IF( rc, "BVH::Build( BLASInstance*, .. )" );
 		sync_info();
 	}
+	// The same Build( BLASInstance*, .. ) for the frame of an animation - RefitBatch( .. ); tlas.BuildUpdated( inst, n, blas, m ); -
+	// through tbvh_build_tlas_update: Update() runs on the device for the whole list and the records come back as above, bit for bit;
+	// rebuilding a TLAS of the same instance and BLAS counts reuses its device tables.
+	template <class Inst> void BuildUpdated( Inst* instances, const uint32_t instCount, BVHBase** blasses, const uint32_t blasCount )
+	{
+		static_assert( sizeof( Inst ) == 192, "tinybvh::BLASInstance is 192 bytes (tiny_bvh.h:1443)" );
+#ifdef INST_IDX_BITS
+		TBVH_FATAL_IF( tbvh_set_option( context(), "inst_idx_bits", INST_IDX_BITS ), "inst_idx_bits" );
+#endif
+		tbvh_bvh* hs = (tbvh_bvh*)malloc( sizeof( tbvh_bvh ) * (blasCount ? blasCount : 1) );
+		bool allWide = blasCount > 0;
+		for (uint32_t k = 0; k < blasCount; k++) hs[k] = blasses[k]->handle(), allWide = allWide && blasses[k]->Layout() == TBVH_LAYOUT_CWBVH;
+		layout = allWide ? TBVH_LAYOUT_CWBVH : TBVH_LAYOUT_BVH;
+		const int rc = tbvh_build_tlas_update( h, instances, (uint32_t)sizeof( Inst ), instCount, TBVH_HOST, hs, blasCount, c_trav, c_int );
+		free( hs );
+		TBVH_FATAL_IF( rc, "BVH::BuildUpdated( BLASInstance*, .. )" );
+		sync_info();
+	}
 	// indexed geometry: BVH::Build / BuildAVX / BuildHQ( vertices, indices, primCount ) tiny_bvh.h:889-900
 	template <class Vec4> void Build( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { build_indexed( vertices, indices, primCount, TBVH_BUILD_REFERENCE, "BVH::Build" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount ), sync_info(); }
 	template <class Vec4> void BuildAVX( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { build_indexed( vertices, indices, primCount, TBVH_BUILD_AVX, "BVH::BuildAVX" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount ), sync_info(); }

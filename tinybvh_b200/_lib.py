@@ -53,6 +53,7 @@ SYMBOLS = {
     "tbvh_instance_update": (i32, [vp, vp]),
     "tbvh_instance_update_box": (i32, [vp, vp, vp]),
     "tbvh_build_tlas": (i32, [vp, vp, u32, u32, vp, u32, f32, f32]),
+    "tbvh_build_tlas_update": (i32, [vp, vp, u32, u32, i32, vp, u32, f32, f32]),
     "tbvh_refit": (i32, [vp, vp, u32, u32, i32]),
     "tbvh_refit_layouts": (i32, [vp, vp, u32, u32, i32]),
     "tbvh_refit_batch": (i32, [vp, vp, u32, i32, i32]),

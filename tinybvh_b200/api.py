@@ -261,6 +261,34 @@ class TLAS(BVH):
         check(_lib.lib().tbvh_build_tlas(self.h, _np_ptr(inst), 192, inst.shape[0], hs, len(self.blasses), self.c_trav, self.c_int))
         return self
 
+    def Rebuild(self, instances, blasses=None, blas_layout: int = None):
+        """The per-frame call of an animated scene (tbvh_build_tlas_update): BLASInstance::Update of every record on the device and the
+        TLAS over the new boxes, in one call.  The records end up as Build( .., update=True ) leaves them, and so does the TLAS.
+        instances: a NumPy array of BLAS_INSTANCE records, or of bytes with shape [n, >= 160] (rows a multiple of 4 bytes apart),
+        updated in place through one copy each way; or a CUDA torch tensor of bytes, shape [n, >= 160] with rows a multiple of 16
+        bytes apart at a 16-byte-aligned address, updated in place on the device - transforms written by a torch kernel never
+        visit the host.
+        blasses / blas_layout: as for Build; by default those of the last Build or Rebuild.  On the handle of a TLAS of the same
+        instance and BLAS counts the device tables are reused."""
+        if blasses is not None:
+            self.blasses = list(blasses)
+        if blas_layout is not None:
+            self.layout = blas_layout
+        if not getattr(self, "blasses", None):
+            raise TbvhError("TLAS.Rebuild: no BLAS list (pass blasses, or Build first)")
+        if _is_torch(instances):
+            import torch
+            assert instances.is_cuda and instances.dim() == 2 and instances.element_size() == 1 and instances.stride(1) == 1 and instances.shape[1] >= 160
+            torch.cuda.current_stream(instances.device).synchronize()   # device-space input: read on the engine's own stream
+            p, stride, n, space = C.c_void_p(instances.data_ptr()), instances.stride(0), instances.shape[0], DEVICE
+        else:
+            assert instances.flags.writeable and (instances.ndim == 1 and instances.dtype.itemsize >= 160 or
+                                                  instances.ndim == 2 and instances.dtype.itemsize == 1 and instances.strides[1] == 1 and instances.shape[1] >= 160)
+            p, stride, n, space = _np_ptr(instances), instances.strides[0], instances.shape[0], HOST
+        hs = (C.c_void_p * len(self.blasses))(*[b.h for b in self.blasses])
+        check(_lib.lib().tbvh_build_tlas_update(self.h, p, stride, n, space, hs, len(self.blasses), self.c_trav, self.c_int))
+        return self
+
 
 def _refit_layouts(obj, vertices):
     p, stride, nv, space, keep = _verts_arg(vertices)

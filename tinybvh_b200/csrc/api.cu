@@ -1,6 +1,7 @@
 // tinybvh_b200/csrc/api.cu - C-ABI entry points (include/tinybvh_b200.h): contexts, handles, uploads, the host-buffer
 // traversal pipeline.  Kernels live in trace_bvh2.cu / trace_cwbvh.cu / build_sah.cu / convert.cu.
 #include "common.cuh"
+#include "instance_update.cuh"
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
@@ -384,10 +385,10 @@ static void free_layouts( tbvh_bvh b )
 	drop_bvh_gpu( b );
 	drop_cwbvh( b );
 	if (b->d_trav && b->d_trav != b->d_nodes) cudaFree( b->d_trav );
-	void* p[] = { b->d_verts, b->d_nodes, b->d_prim_idx, b->d_leaf_tris, b->d_aabbs, b->d_inst, b->d_blas };
+	void* p[] = { b->d_verts, b->d_nodes, b->d_prim_idx, b->d_leaf_tris, b->d_aabbs, b->d_inst, b->d_blas, b->d_inst_stage };
 	for (void* q : p) if (q) cudaFree( q );
 	b->d_verts = 0, b->d_nodes = 0, b->d_prim_idx = 0, b->d_leaf_tris = 0, b->d_trav = 0, b->leaf_tris_count = 0;
-	b->d_aabbs = 0, b->d_inst = 0, b->d_blas = 0, b->inst_count = 0, b->blas_count = 0, b->tlas_blas_layouts = 0;
+	b->d_aabbs = 0, b->d_inst = 0, b->d_blas = 0, b->d_inst_stage = 0, b->blas_table_bytes = 0, b->inst_count = 0, b->blas_count = 0, b->tlas_blas_layouts = 0;
 	b->tlas_deep_blas = 0, b->tlas_deep_depth = 0;
 	b->links.clear();
 	b->generation = tbvh_next_generation(); // a TLAS built over the old arrays must notice (tlas_check)
@@ -708,71 +709,18 @@ int tbvh_sah_cost( tbvh_bvh b, float c_trav, float c_int, float* out )
 	return tbvh_sah_cost_nodes( nodes.data(), b->info.used_nodes, c_trav, c_int, out );
 }
 
-// ---- BLASInstance::Update on the host (the engine's own restatement; host code, so gcc's contraction is switched off for it)
-#define UPD_ATTR __attribute__( (optimize( "fp-contract=off" )) )
-
-/* BLASInstance::InvertTransform (:8402-8428) + Update (:8386-8399).  The frozen reference build vectorises the sixteen cofactor
- * sums, and the lanes of different rows end up with different fused multiply-adds; the shapes below were identified by
- * exhaustive search over every contraction gcc may legally form (3 x 2^4 per cofactor, 12 for the determinant, 6^4 for the
- * corner transform) against BLASInstance::Update on 2,000 random matrices, and are pinned by the tests.  A cofactor is
- * s0*(a0*b0)*c0 + ... + s5*(a5*b5)*c5 with p_k = round( a_k*b_k ):
- *   rows 0,1 : t0 = round( p0*c0 ); acc = fma( +-p1, c1, t0 ); then fma( +-p_k, c_k, acc ) for k = 2..5
- *   row 2    : acc = fma( p0, c0, +-round( p1*c1 ) ); k=2: acc +- round( p2*c2 ); k=3,4: fma; k=5: acc +- round( p5*c5 )
- *   row 3    : acc = fma( p0, c0, +-round( p1*c1 ) ); k=2: fma; k=3,4: acc +- round(..); k=5: fma
- *   det      = fma( T3, c12, fma( T2, c8, fma( T0, c0, round( T1*c4 ) ) ) ); every cell is then multiplied by 1/det
- *   corner   : row = fma( Tz, z, fma( Tx, x, round( Ty*y ) ) ) + Tw, divided by w only when w != 1 */
-typedef struct { signed char s; unsigned char a, b, c; } UPD_TERM;
-static const UPD_TERM UPD_E[16][6] = {
- {{+1,5,10,15},{-1,5,11,14},{-1,9,6,15},{+1,9,7,14},{+1,13,6,11},{-1,13,7,10}}, {{-1,1,10,15},{+1,1,11,14},{+1,9,2,15},{-1,9,3,14},{-1,13,2,11},{+1,13,3,10}},
- {{+1,1,6,15},{-1,1,7,14},{-1,5,2,15},{+1,5,3,14},{+1,13,2,7},{-1,13,3,6}}, {{-1,1,6,11},{+1,1,7,10},{+1,5,2,11},{-1,5,3,10},{-1,9,2,7},{+1,9,3,6}},
- {{-1,4,10,15},{+1,4,11,14},{+1,8,6,15},{-1,8,7,14},{-1,12,6,11},{+1,12,7,10}}, {{+1,0,10,15},{-1,0,11,14},{-1,8,2,15},{+1,8,3,14},{+1,12,2,11},{-1,12,3,10}},
- {{-1,0,6,15},{+1,0,7,14},{+1,4,2,15},{-1,4,3,14},{-1,12,2,7},{+1,12,3,6}}, {{+1,0,6,11},{-1,0,7,10},{-1,4,2,11},{+1,4,3,10},{+1,8,2,7},{-1,8,3,6}},
- {{+1,4,9,15},{-1,4,11,13},{-1,8,5,15},{+1,8,7,13},{+1,12,5,11},{-1,12,7,9}}, {{-1,0,9,15},{+1,0,11,13},{+1,8,1,15},{-1,8,3,13},{-1,12,1,11},{+1,12,3,9}},
- {{+1,0,5,15},{-1,0,7,13},{-1,4,1,15},{+1,4,3,13},{+1,12,1,7},{-1,12,3,5}}, {{-1,0,5,11},{+1,0,7,9},{+1,4,1,11},{-1,4,3,9},{-1,8,1,7},{+1,8,3,5}},
- {{-1,4,9,14},{+1,4,10,13},{+1,8,5,14},{-1,8,6,13},{-1,12,5,10},{+1,12,6,9}}, {{+1,0,9,14},{-1,0,10,13},{-1,8,1,14},{+1,8,2,13},{+1,12,1,10},{-1,12,2,9}},
- {{-1,0,5,14},{+1,0,6,13},{+1,4,1,14},{-1,4,2,13},{-1,12,1,6},{+1,12,2,5}}, {{+1,0,5,10},{-1,0,6,9},{-1,4,1,10},{+1,4,2,9},{+1,8,1,6},{-1,8,2,5}} };
-UPD_ATTR static float upd_cofactor( const float* T, const UPD_TERM* e, const int first_fused_left, const unsigned fused_mask )
+// ---- BLASInstance::Update on the host: the arithmetic of instance_update.cuh, which the device kernel runs too (host code, so gcc's
+// contraction is switched off for the function it is inlined into)
+UPD_HOST_ATTR static void upd_instance_host( const float* T, float* iT, float* aabbMin, float* aabbMax, const float* bmin, const float* bmax )
 {
-	float p[6];
-	for (int k = 0; k < 6; k++) p[k] = T[e[k].a] * T[e[k].b];
-	const float p0 = e[0].s < 0 ? -p[0] : p[0];
-	float acc;
-	if (first_fused_left) { const float t1 = p[1] * T[e[1].c]; acc = fmaf( p0, T[e[0].c], e[1].s > 0 ? t1 : -t1 ); }
-	else { const float t0 = p0 * T[e[0].c]; acc = fmaf( e[1].s > 0 ? p[1] : -p[1], T[e[1].c], t0 ); }
-	for (int k = 2; k < 6; k++)
-	{
-		if (fused_mask & (1u << (k - 2))) acc = fmaf( e[k].s > 0 ? p[k] : -p[k], T[e[k].c], acc );
-		else { const float t = p[k] * T[e[k].c]; acc = e[k].s > 0 ? acc + t : acc - t; }
-	}
-	return acc;
+	upd_instance( T, iT, aabbMin, aabbMax, bmin, bmax );
 }
-UPD_ATTR static void upd_instance( float* T /* transform, 16 */, float* iT /* invTransform, 16 */, float* aabbMin, float* aabbMax, const float* bmin, const float* bmax )
-{
-	float c[16];
-	for (int k = 0; k < 16; k++) c[k] = k < 8 ? upd_cofactor( T, UPD_E[k], 0, 15u ) : k < 12 ? upd_cofactor( T, UPD_E[k], 1, 6u ) : upd_cofactor( T, UPD_E[k], 1, 9u );
-	const float t14 = T[1] * c[4];
-	const float det = fmaf( T[3], c[12], fmaf( T[2], c[8], fmaf( T[0], c[0], t14 ) ) );
-	if (det == 0) { for (int k = 0; k < 16; k++) iT[k] = c[k]; } /* "invert failed": the reference returns with the cofactors stored */
-	else { const float invdet = 1.0f / det; for (int k = 0; k < 16; k++) iT[k] = c[k] * invdet; }
-	for (int k = 0; k < 3; k++) aabbMin[k] = 1e30f, aabbMax[k] = -1e30f;
-	for (int j = 0; j < 8; j++)
-	{
-		const float p[3] = { j & 1 ? bmax[0] : bmin[0], j & 2 ? bmax[1] : bmin[1], j & 4 ? bmax[2] : bmin[2] };
-		float r[3];
-		for (int k = 0; k < 3; k++) { const float ty = T[k * 4 + 1] * p[1]; r[k] = fmaf( T[k * 4 + 2], p[2], fmaf( T[k * 4], p[0], ty ) ) + T[k * 4 + 3]; }
-		const float wy = T[13] * p[1];
-		const float w = fmaf( T[14], p[2], fmaf( T[12], p[0], wy ) ) + T[15];
-		if (!(w == 1)) { const float rw = 1.0f / w; r[0] = r[0] * rw, r[1] = r[1] * rw, r[2] = r[2] * rw; }
-		for (int k = 0; k < 3; k++) aabbMin[k] = aabbMin[k] < r[k] ? aabbMin[k] : r[k], aabbMax[k] = aabbMax[k] > r[k] ? aabbMax[k] : r[k];
-	}
-}
-#undef UPD_ATTR
 int tbvh_instance_update_box( void* instance, const float* bmin, const float* bmax )
 {
 	ARG_CHECK( instance && bmin && bmax, "NULL argument" );
 	float T[16], iT[16], mn[3], mx[3];
 	memcpy( T, instance, 64 );
-	upd_instance( T, iT, mn, mx, bmin, bmax );
+	upd_instance_host( T, iT, mn, mx, bmin, bmax );
 	memcpy( (char*)instance + 64, iT, 64 ), memcpy( (char*)instance + 128, mn, 12 ), memcpy( (char*)instance + 144, mx, 12 );
 	return TBVH_OK;
 }
@@ -783,17 +731,13 @@ int tbvh_instance_update( void* instance, tbvh_bvh blas )
 	return tbvh_instance_update_box( instance, blas->info.aabb_min, blas->info.aabb_max );
 }
 
-// BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) tiny_bvh.h:2221 in its "blasses == 0" mode (:2245): the instances
-// arrive Update()d - inverse transform and world-space box filled in - and the TLAS is the reference builder's tree over the boxes
-int tbvh_build_tlas( tbvh_bvh t, const void* instances, uint32_t inst_stride, uint32_t inst_count, const tbvh_bvh* blasses, uint32_t blas_count, float c_trav, float c_int )
+// the BLAS list of a TLAS build: the device record of every BLAS, the layouts all of them hold, and the first BLAS too deep for the
+// two-level kernel's BVH-layout walk (1 + its number; 0: none).  Reads host state only and touches no handle.
+struct TlasBlasTable { std::vector<BlasRef> refs; uint32_t layouts, deep_blas, deep_depth; };
+static int tlas_blas_table( const tbvh_bvh t, const tbvh_bvh* blasses, const uint32_t blas_count, TlasBlasTable& T )
 {
-	ARG_CHECK( t && instances && blasses && inst_count > 0 && blas_count > 0 && inst_stride >= 160, "bad TLAS arguments" );
-	CUDA_TRY( cudaSetDevice( t->ctx->device ) );
-	free_layouts( t );
-	std::vector<float4> boxes( (size_t)inst_count * 2 );
-	std::vector<TlasInst> inst( inst_count );
-	std::vector<BlasRef> refs( blas_count );
-	uint32_t blas_layouts = (1u << TBVH_LAYOUT_BVH) | (1u << TBVH_LAYOUT_CWBVH);
+	T.refs.assign( blas_count, BlasRef{} );
+	T.layouts = (1u << TBVH_LAYOUT_BVH) | (1u << TBVH_LAYOUT_CWBVH), T.deep_blas = 0, T.deep_depth = 0;
 	for (uint32_t k = 0; k < blas_count; k++)
 	{
 		const tbvh_bvh b = blasses[k];
@@ -807,15 +751,32 @@ int tbvh_build_tlas( tbvh_bvh t, const void* instances, uint32_t inst_stride, ui
 			// the two-level kernel walks a BVH2 BLAS with a TBVH_STACK-entry stack; the CWBVH walk does not use it, so a BLAS that
 			// also holds its CWBVH stays usable through that layout, and a LAYOUT_BVH walk of the TLAS is refused (tlas_check)
 			if (!has_cw) { tbvh_set_error( "TLAS: BLAS %u has depth %u, the two-level kernel walks a BLAS with a %d-entry stack", k, b->info.max_depth, TBVH_STACK ); return TBVH_E_LIMIT; }
-			if (!t->tlas_deep_blas) t->tlas_deep_blas = k + 1, t->tlas_deep_depth = b->info.max_depth;
+			if (!T.deep_blas) T.deep_blas = k + 1, T.deep_depth = b->info.max_depth;
 			has_bvh = false;
 		}
 		if (has_cw && b->cw_pending == 0xffffffffu) { tbvh_set_error( "TLAS: the wide tree of BLAS %u has a cycle in its inner-child links", k ); return TBVH_E_ARG; }
 		if (has_cw && b->cw_pending > 128) { tbvh_set_error( "TLAS: the wide tree of BLAS %u can leave %u node groups pending (128 per ray, tiny_bvh.h:7048)", k, b->cw_pending ); return TBVH_E_LIMIT; }
-		refs[k].trav = has_bvh ? b->d_trav : 0, refs[k].tris = has_bvh ? b->d_leaf_tris : 0, refs[k].root_ref = b->root_ref, refs[k].root_count = b->root_count, refs[k].pad1 = 0;
-		refs[k].cw_nodes = has_cw ? b->d_cw_trav : 0, refs[k].cw_tris = has_cw ? b->d_cw_tris : 0, refs[k].cw_rd_limit = has_cw ? b->cw_rd_limit : -1.0f;
-		blas_layouts &= (has_bvh ? 1u << TBVH_LAYOUT_BVH : 0u) | (has_cw ? 1u << TBVH_LAYOUT_CWBVH : 0u);
+		T.refs[k].trav = has_bvh ? b->d_trav : 0, T.refs[k].tris = has_bvh ? b->d_leaf_tris : 0, T.refs[k].root_ref = b->root_ref, T.refs[k].root_count = b->root_count, T.refs[k].pad1 = 0;
+		T.refs[k].cw_nodes = has_cw ? b->d_cw_trav : 0, T.refs[k].cw_tris = has_cw ? b->d_cw_tris : 0, T.refs[k].cw_rd_limit = has_cw ? b->cw_rd_limit : -1.0f;
+		T.layouts &= (has_bvh ? 1u << TBVH_LAYOUT_BVH : 0u) | (has_cw ? 1u << TBVH_LAYOUT_CWBVH : 0u);
 	}
+	return TBVH_OK;
+}
+
+// BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) tiny_bvh.h:2221 in its "blasses == 0" mode (:2245): the instances
+// arrive Update()d - inverse transform and world-space box filled in - and the TLAS is the reference builder's tree over the boxes
+int tbvh_build_tlas( tbvh_bvh t, const void* instances, uint32_t inst_stride, uint32_t inst_count, const tbvh_bvh* blasses, uint32_t blas_count, float c_trav, float c_int )
+{
+	ARG_CHECK( t && instances && blasses && inst_count > 0 && blas_count > 0 && inst_stride >= 160, "bad TLAS arguments" );
+	CUDA_TRY( cudaSetDevice( t->ctx->device ) );
+	free_layouts( t );
+	std::vector<float4> boxes( (size_t)inst_count * 2 );
+	std::vector<TlasInst> inst( inst_count );
+	TlasBlasTable B;
+	TRY( tlas_blas_table( t, blasses, blas_count, B ) );
+	t->tlas_deep_blas = B.deep_blas, t->tlas_deep_depth = B.deep_depth;
+	const std::vector<BlasRef>& refs = B.refs;
+	const uint32_t blas_layouts = B.layouts;
 	for (uint32_t i = 0; i < inst_count; i++)
 	{
 		// BLASInstance :1443: transform @0, invTransform @64, aabbMin @128, blasIdx @140, aabbMax @144, mask @156
@@ -843,6 +804,85 @@ int tbvh_build_tlas( tbvh_bvh t, const void* instances, uint32_t inst_stride, ui
 	// the device table holds raw addresses of the BLAS arrays: remember which generation of each BLAS they belong to
 	for (uint32_t k = 0; k < blas_count; k++) t->links.push_back( BlasLink{ blasses[k], blasses[k]->generation } );
 	return TBVH_OK;
+}
+
+// BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) tiny_bvh.h:2221 with the BLAS list given: every instance is Update()d
+// (:2245-2250) by k_instance_update, which also writes the TlasInst entries and the builder's boxes, so no host loop walks the records.
+// Everything that can be refused from host state is refused before the handle is touched.
+int tbvh_build_tlas_update( tbvh_bvh t, void* instances, uint32_t inst_stride, uint32_t inst_count, int space, const tbvh_bvh* blasses, uint32_t blas_count,
+	float c_trav, float c_int )
+{
+	ARG_CHECK( t && instances && blasses && inst_count > 0 && blas_count > 0 && inst_stride >= 160, "bad TLAS arguments" );
+	ARG_CHECK( space == TBVH_HOST || space == TBVH_DEVICE, "unknown space" );
+	if (space == TBVH_DEVICE) ARG_CHECK( ((uintptr_t)instances & 15) == 0 && (inst_stride & 15) == 0, "device records: the pointer and the stride must be multiples of 16" );
+	else ARG_CHECK( (inst_stride & 3) == 0, "host records: the stride must be a multiple of 4" );
+	CUDA_TRY( cudaSetDevice( t->ctx->device ) );
+	TlasBlasTable B;
+	TRY( tlas_blas_table( t, blasses, blas_count, B ) );
+	// the device table: BlasRef[blas_count], then the root box of every BLAS (2 float4), then the flag word of the kernel
+	const size_t box_at = (size_t)blas_count * sizeof( BlasRef ), flag_at = box_at + (size_t)blas_count * 32, table_bytes = flag_at + 16;
+	std::vector<char> table( table_bytes, 0 );
+	memcpy( table.data(), B.refs.data(), box_at );
+	for (uint32_t k = 0; k < blas_count; k++)
+	{
+		const tbvh_bvh b = blasses[k];
+		if (!(b->info.layouts & (1u << TBVH_LAYOUT_BVH))) { tbvh_set_error( "TLAS: BLAS %u holds no BVH-layout tree, so its root box is not known (tbvh_instance_update)", k ); return TBVH_E_STATE; }
+		memcpy( table.data() + box_at + (size_t)k * 32, b->info.aabb_min, 12 ), memcpy( table.data() + box_at + (size_t)k * 32 + 16, b->info.aabb_max, 12 );
+	}
+	if (space == TBVH_HOST) for (uint32_t i = 0; i < inst_count; i++)
+	{
+		uint32_t blasIdx;
+		memcpy( &blasIdx, (const char*)instances + (size_t)i * inst_stride + 140, 4 );
+		ARG_CHECK( blasIdx < blas_count, "TLAS: an instance names a BLAS past blas_count" );
+	}
+	// a frame of an animation rebuilds the TLAS it built last frame: same counts, so the instance boxes, the TlasInst and BLAS tables
+	// and the staging of host records are kept; the tree itself is the builder's to allocate
+	const bool reuse = t->d_inst && t->d_aabbs && t->d_blas && t->inst_count == inst_count && t->blas_count == blas_count && t->blas_table_bytes == table_bytes;
+	float4* aabbs = reuse ? t->d_aabbs : 0;
+	void* inst = reuse ? t->d_inst : 0, * blas = reuse ? t->d_blas : 0, * stage = reuse ? t->d_inst_stage : 0;
+	if (reuse) t->d_aabbs = 0, t->d_inst = 0, t->d_blas = 0, t->d_inst_stage = 0;
+	free_layouts( t );
+	t->d_aabbs = aabbs, t->d_inst = inst, t->d_blas = blas, t->d_inst_stage = stage, t->blas_table_bytes = table_bytes;
+	cudaStream_t s = t->ctx->stream;
+	cudaEvent_t e0 = 0, e1 = 0;
+	uint32_t bad_blas = 0;
+	float update_ms = 0;
+	auto body = [&]() -> int
+	{
+		if (!reuse)
+		{
+			CUDA_TRY( cudaMalloc( &t->d_aabbs, (size_t)inst_count * 32 ) );
+			CUDA_TRY( cudaMalloc( &t->d_inst, (size_t)inst_count * sizeof( TlasInst ) ) );
+			CUDA_TRY( cudaMalloc( &t->d_blas, table_bytes ) );
+		}
+		if (space == TBVH_HOST && !t->d_inst_stage) CUDA_TRY( cudaMalloc( &t->d_inst_stage, (size_t)inst_count * 160 ) );
+		CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) );
+		CUDA_TRY( cudaMemcpyAsync( t->d_blas, table.data(), table_bytes, cudaMemcpyHostToDevice, s ) );
+		// host records: bytes 0..159 in, one strided copy; bytes 64..159 (invTransform .. mask) back, one strided copy
+		if (space == TBVH_HOST) CUDA_TRY( cudaMemcpy2DAsync( t->d_inst_stage, 160, instances, inst_stride, 160, inst_count, cudaMemcpyHostToDevice, s ) );
+		CUDA_TRY( cudaEventRecord( e0, s ) );
+		TRY( instance_update_launch( space == TBVH_HOST ? t->d_inst_stage : instances, space == TBVH_HOST ? 160u : inst_stride, inst_count,
+			(const float4*)((char*)t->d_blas + box_at), blas_count, t->d_inst, t->d_aabbs, (uint32_t*)((char*)t->d_blas + flag_at), s ) );
+		CUDA_TRY( cudaEventRecord( e1, s ) );
+		if (space == TBVH_HOST) CUDA_TRY( cudaMemcpy2DAsync( (char*)instances + 64, inst_stride, (char*)t->d_inst_stage + 64, 160, 96, inst_count, cudaMemcpyDeviceToHost, s ) );
+		CUDA_TRY( cudaMemcpyAsync( &bad_blas, (char*)t->d_blas + flag_at, 4, cudaMemcpyDeviceToHost, s ) );
+		CUDA_TRY( cudaStreamSynchronize( s ) ); // the call's one synchronisation outside the builder: `table` and `bad_blas` are on this frame
+		if (bad_blas) { tbvh_set_error( "tbvh_build_tlas_update: an instance names a BLAS past blas_count" ); return TBVH_E_ARG; }
+		CUDA_TRY( cudaEventElapsedTime( &update_ms, e0, e1 ) );
+		t->info.prim_count = inst_count, t->inst_count = inst_count, t->blas_count = blas_count, t->tlas_blas_layouts = B.layouts;
+		t->tlas_deep_blas = B.deep_blas, t->tlas_deep_depth = B.deep_depth;
+		TRY( build_sah_launch( &t, 1, c_trav, c_int, TBVH_BUILD_REFERENCE ) ); // "Build(); // or BuildAVX, for large TLAS." :2258
+		t->info.build_ms += update_ms;
+		t->info.layouts = 1u << TBVH_LAYOUT_BVH, t->refittable = false; // "do not refit a TLAS, use Build(..)" :3060
+		if (t->info.max_depth + 1 > TBVH_STACK) { tbvh_set_error( "TLAS depth %u exceeds the %d-entry stack of IntersectTLAS (tiny_bvh.h:3308)", t->info.max_depth, TBVH_STACK ); return TBVH_E_LIMIT; }
+		for (uint32_t k = 0; k < blas_count; k++) t->links.push_back( BlasLink{ blasses[k], blasses[k]->generation } );
+		return TBVH_OK;
+	};
+	const int rc = body();
+	if (e0) cudaEventDestroy( e0 );
+	if (e1) cudaEventDestroy( e1 );
+	if (rc != TBVH_OK) { cudaStreamSynchronize( s ); free_layouts( t ); cudaGetLastError(); } // as a failed build: the handle is empty, and the error is this call's alone
+	return rc;
 }
 
 // BVH::Refit (tiny_bvh.h:3055): same topology, new vertex positions; derived layouts are dropped (convert_cwbvh.cu refit_trees)

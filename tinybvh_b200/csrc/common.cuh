@@ -106,7 +106,9 @@ struct tbvh_bvh_t
 	// TLAS (BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) :2221): nodes / primIdx over instance boxes + device tables
 	float4* d_aabbs = 0;       // instance boxes the TLAS was built over (2 float4 per instance)
 	void* d_inst = 0;          // TlasInst records (inverse transform, BLAS number, mask)
-	void* d_blas = 0;          // BlasRef records (traversal arrays of every BLAS)
+	void* d_blas = 0;          // BlasRef records (traversal arrays of every BLAS); tbvh_build_tlas_update: then each BLAS's root box and a flag word
+	void* d_inst_stage = 0;    // tbvh_build_tlas_update with host records: bytes 0..159 of every record on their way through the device
+	size_t blas_table_bytes = 0; // bytes of d_blas when tbvh_build_tlas_update made it (0: tbvh_build_tlas's, BlasRef records only)
 	uint32_t inst_count = 0, blas_count = 0;
 	uint32_t tlas_blas_layouts = 0; // TLAS only: layouts EVERY BLAS held at build time (bit TBVH_LAYOUT_BVH / TBVH_LAYOUT_CWBVH)
 	uint32_t tlas_deep_blas = 0, tlas_deep_depth = 0; // TLAS only: 1 + the first BLAS whose BVH2 is too deep for the two-level walk (0: none), and its depth
@@ -280,6 +282,10 @@ int bvh_gpu_enqueue( const GpuTree* d_T, uint32_t K, const GpuTree& one, uint32_
 int tlas_trace_launch( tbvh_bvh b, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s );
 struct TlasInst { float inv[16]; uint32_t blasIdx, mask, pad0, pad1; };                                  // 80 bytes
 struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root_count; float cw_rd_limit; uint32_t pad1; const float4* cw_nodes; const float4* cw_tris; }; // 48 bytes: BVH-layout arrays, CWBVH traversal nodes + bvh8Tris (0 when absent) and their rD limit
+// BLASInstance::Update of n records `stride` bytes apart (instance_update.cu): invTransform and world box into the records, the TlasInst
+// entries and the builder's boxes in one pass; *d_bad_blas is set when a record names a BLAS past blas_count
+int instance_update_launch( void* d_records, uint32_t stride, uint32_t n, const float4* d_blas_box, uint32_t blas_count, void* d_tlas_inst, float4* d_aabbs,
+	uint32_t* d_bad_blas, cudaStream_t s );
 int make_leaf_tris( tbvh_bvh b, cudaStream_t s );
 int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used_nodes_gpu, cudaStream_t s );
 int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s ); // sets the BVH_GPU bit on success; on failure the handle holds no BVH_GPU
