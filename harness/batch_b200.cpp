@@ -1,6 +1,7 @@
 // harness/batch_b200.cpp - many meshes through the shim's BuildBatch: one BVH per mesh (the first step of every instanced scene,
 // one BLAS per mesh as tiny_scene.h builds them), built in one call, then checked against a separate Build of every mesh and
-// walked with a batch of rays.  BVH8_CWBVH objects go through the overload that converts each tree afterwards.  No reference header.
+// walked with a batch of rays.  BVH8_CWBVH objects go through the overload that converts each tree afterwards.  A BuildHQ batch
+// (TBVH_BUILD_HQ) is checked against a separate BuildHQ of every mesh.  No reference header.
 //   g++ -O2 -std=c++17 -Iinclude harness/batch_b200.cpp -Ltinybvh_b200 -ltinybvh_b200 -Wl,-rpath,$PWD/tinybvh_b200 -o batch_b200
 #include "tinybvh_b200.hpp"
 #include <vector>
@@ -59,7 +60,22 @@ int main()
 	for (int i = 0; i < R; i++) hits += rays[i].t < 1e30f, mismatched += (rays[i].t < 1e30f) != (rays[R + i].t < 1e30f) || rays[i].prim != rays[R + i].prim;
 	printf( "batch_b200: %i meshes, %u tris, batch build %.3f ms; %i trees differ from separate builds; mesh 0: %i of %i rays hit, %i differ between layouts, %u CWBVH blocks\n",
 		M, total, batch[0]->buildMs, differ, hits, R, mismatched, wide[0]->usedBlocks );
+	// the SBVH builder: one BuildBatch with TBVH_BUILD_HQ against a separate BuildHQ of every mesh
+	int differHQ = 0;
+	std::vector<tinybvh_b200::BVH*> hq( M ), hqSingle( M );
+	for (int m = 0; m < M; m++) hq[m] = new tinybvh_b200::BVH(), hqSingle[m] = new tinybvh_b200::BVH();
+	tinybvh_b200::BuildBatch( hq.data(), verts.data(), counts.data(), M, TBVH_BUILD_HQ );
+	for (int m = 0; m < M; m++)
+	{
+		hqSingle[m]->BuildHQ( verts[m], counts[m] );
+		const tbvh_info a = hq[m]->Info(), b = hqSingle[m]->Info();
+		std::vector<char> na( (size_t)a.used_nodes * 32 ), nb( (size_t)b.used_nodes * 32 );
+		std::vector<uint32_t> ia( a.idx_count ), ib( b.idx_count );
+		hq[m]->Download( na.data(), ia.data() ), hqSingle[m]->Download( nb.data(), ib.data() );
+		if (hq[m]->usedNodes != hqSingle[m]->usedNodes || hq[m]->idxCount != hqSingle[m]->idxCount || a.max_depth != b.max_depth || na != nb || ia != ib) differHQ++;
+	}
+	printf( "batch_b200: BuildHQ batch %.3f ms; %i HQ trees differ from separate BuildHQ builds\n", hq[0]->buildMs, differHQ );
 	tinybvh_b200::free_pinned( rays );
-	for (int m = 0; m < M; m++) delete batch[m], delete single[m], delete wide[m];
-	return differ == 0 && mismatched == 0 && hits > 0 ? 0 : 1;
+	for (int m = 0; m < M; m++) delete batch[m], delete single[m], delete wide[m], delete hq[m], delete hqSingle[m];
+	return differ == 0 && differHQ == 0 && mismatched == 0 && hits > 0 ? 0 : 1;
 }

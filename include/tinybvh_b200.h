@@ -131,7 +131,7 @@ int tbvh_build_indexed( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32
  * trees are built together by the same kernels, so the fixed cost of a build (allocations, launches, host round trips) is paid once
  * per batch instead of once per mesh; the order of `meshes` changes no tree.  All meshes are in one `space`; device-space inputs
  * follow the rule above.
- *  flavour: TBVH_BUILD_REFERENCE or TBVH_BUILD_AVX; TBVH_BUILD_HQ is TBVH_E_UNSUPPORTED (one SBVH per tbvh_build_flavour call).
+ *  flavour: TBVH_BUILD_REFERENCE or TBVH_BUILD_AVX; TBVH_BUILD_HQ is TBVH_E_UNSUPPORTED (SBVH batches: tbvh_build_batch_hq below).
  *  Refusals come before any handle is touched, so every handle keeps its previous tree: TBVH_E_ARG for count 0, a NULL or repeated
  *  handle, handles of different contexts, prim_count 0, a bad stride, or any index >= vert_count; TBVH_E_LIMIT when the meshes
  *  hold more than TBVH_BATCH_MAX_PRIMS triangles together (positions of one shared index space must fit the builder's 32-bit
@@ -146,6 +146,18 @@ typedef struct tbvh_mesh
 } tbvh_mesh;
 #define TBVH_BATCH_MAX_PRIMS (1u << 30)
 int tbvh_build_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int, int flavour );
+
+/* Many meshes in one SBVH build: BVH::BuildHQ (tiny_bvh.h:2623) per mesh, as a static scene builds its BLASes for the best traversal
+ * quality.  bvhs[i] ends up exactly as tbvh_build_flavour( .., TBVH_BUILD_HQ ) (or, with indices, tbvh_build_indexed) of meshes[i]
+ * alone would leave it: nodes, the whole primIdx (idx_count = prim_count + prim_count / 2, zeros past the leaf entries) and leaf
+ * triangles byte for byte, the same info (build_ms is the device time of the whole batch), layout TBVH_LAYOUT_BVH, not refittable,
+ * and a TLAS built over its old arrays is stale.  The order of `meshes` and their neighbours change no tree.  Launches and host
+ * synchronisations grow with the deepest tree's level count, not with count.
+ *  Refusals are those of tbvh_build_batch, with the same codes, and come before any handle or vertex is touched; besides, TBVH_E_LIMIT
+ *  when the batch's temporary node space, 3 * (total prim_count) + 2 nodes, exceeds TBVH_BATCH_HQ_MAX_NODES (node and position
+ *  numbers of the shared spaces are 32-bit).  A failure after the device work started leaves every handle of the batch empty. */
+#define TBVH_BATCH_HQ_MAX_NODES 0xffffffffu
+int tbvh_build_batch_hq( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int );
 
 /* TLAS: BVH::Build( BLASInstance* instances, instCount, BVHBase** blasses, blasCount ) tiny_bvh.h:2221, traversed by
  * BVH::IntersectTLAS (:3306) / IsOccludedTLAS (:3455) whenever tbvh_intersect / tbvh_occluded (or the _device forms) are

@@ -60,7 +60,8 @@ inline void free_pinned( void* p ) { tbvh_host_free( p ); }
 
 // Many meshes in one call (tbvh_build_batch): objs[i] ends up as if its own Build( vertices[i], primCounts[i] ) had run - the tree,
 // Refit and Optimize working from the caller's arrays, the public counters.  flavour: TBVH_BUILD_REFERENCE (BVH::Build) or
-// TBVH_BUILD_AVX; by default the builder the class's own Build uses.  BVH_GPU / BVH8_CWBVH objects are converted afterwards.
+// TBVH_BUILD_AVX; by default the builder the class's own Build uses.  TBVH_BUILD_HQ: each object as its own BuildHQ( vertices[i],
+// primCounts[i] ) leaves it (tbvh_build_batch_hq).  BVH_GPU / BVH8_CWBVH objects are converted afterwards.
 template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* const* vertices, const uint32_t* primCounts, uint32_t count, int flavour = -1 );
 // Many refits in one call (tbvh_refit_batch), as an animated scene refits its BLASes every frame: every object refitted from the vertex
 // array it was built from, exactly as its own Refit() would leave it - the tree and the public counters.
@@ -446,8 +447,9 @@ template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* cons
 		hs[k] = objs[k] ? objs[k]->handle() : 0;
 		ms[k].verts = vertices[k], ms[k].stride = (uint32_t)sizeof( Vec4 ), ms[k].prim_count = primCounts[k];
 	}
-	const int rc = tbvh_build_batch( hs, ms, count, TBVH_HOST, count && objs[0] ? objs[0]->c_trav : 1.0f, count && objs[0] ? objs[0]->c_int : 1.0f,
-		flavour < 0 ? T::defaultFlavour : flavour );
+	const float ct = count && objs[0] ? objs[0]->c_trav : 1.0f, ci = count && objs[0] ? objs[0]->c_int : 1.0f;
+	const int rc = flavour == TBVH_BUILD_HQ ? tbvh_build_batch_hq( hs, ms, count, TBVH_HOST, ct, ci )
+		: tbvh_build_batch( hs, ms, count, TBVH_HOST, ct, ci, flavour < 0 ? T::defaultFlavour : flavour );
 	free( ms );
 	if (rc != TBVH_OK) free( hs );
 	TBVH_FATAL_IF( rc, "BuildBatch" );

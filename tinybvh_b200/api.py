@@ -371,7 +371,8 @@ class BVH8_CWBVH(_Base):
 
 def build_batch(bvhs, meshes, flavour: int = _lib.BUILD_REFERENCE, indices=None):
     """tbvh_build_batch: one binned-SAH tree per mesh, all built in one call.  bvhs[i] ends up as bvhs[i].Build(meshes[i]) (flavour
-    BUILD_REFERENCE) or .BuildAVX (BUILD_AVX) would leave it.  `meshes`: numpy vertex arrays, or torch CUDA tensors - one space per
+    BUILD_REFERENCE) or .BuildAVX (BUILD_AVX) would leave it; flavour BUILD_HQ builds one SBVH per mesh (tbvh_build_batch_hq), as
+    .BuildHQ would.  `meshes`: numpy vertex arrays, or torch CUDA tensors - one space per
     call; `indices`: None, or one entry per mesh (None for a flat mesh, else its vertex indices in the same space).  BVH_GPU and
     BVH8_CWBVH objects are converted afterwards, as their Build does (the BVH8_CWBVH objects in one convert_batch).  A refused batch
     raises TbvhError and leaves every object as it was."""
@@ -403,7 +404,11 @@ def build_batch(bvhs, meshes, flavour: int = _lib.BUILD_REFERENCE, indices=None)
         r.vert_count, r.prim_count = nv, n // 3
     hs = (C.c_void_p * max(len(bvhs), 1))(*[b.h for b in bvhs]) if bvhs else None
     c0 = bvhs[0] if bvhs else None
-    check(_lib.lib().tbvh_build_batch(hs, recs, len(meshes), space, c0.c_trav if c0 else 1.0, c0.c_int if c0 else 1.0, flavour))
+    c_trav, c_int = (c0.c_trav, c0.c_int) if c0 else (1.0, 1.0)
+    if flavour == _lib.BUILD_HQ:
+        check(_lib.lib().tbvh_build_batch_hq(hs, recs, len(meshes), space, c_trav, c_int))
+    else:
+        check(_lib.lib().tbvh_build_batch(hs, recs, len(meshes), space, c_trav, c_int, flavour))
     cw = [b for b in bvhs if b.layout == LAYOUT_CWBVH]
     if cw:
         convert_batch(cw)

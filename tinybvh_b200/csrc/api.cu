@@ -563,7 +563,7 @@ template <class Upload> static int build_one( const char* fn, tbvh_bvh b, float 
 	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
 	free_layouts( b );
 	TRY( upload( b->ctx->stream ) );
-	if (flavour == TBVH_BUILD_HQ) TRY( build_hq_launch( b, c_trav, c_int ) ); else TRY( build_sah_launch( &b, 1, c_trav, c_int, flavour ) );
+	if (flavour == TBVH_BUILD_HQ) TRY( build_hq_launch( &b, 1, c_trav, c_int ) ); else TRY( build_sah_launch( &b, 1, c_trav, c_int, flavour ) );
 	b->info.layouts = 1u << TBVH_LAYOUT_BVH, b->refittable = flavour != TBVH_BUILD_HQ;
 	return TBVH_OK;
 }
@@ -938,27 +938,31 @@ int tbvh_build_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t
 		[&]( cudaStream_t s ) { return upload_verts_indexed( b, verts, stride, vert_count, indices, prim_count, space, s ); } );
 }
 
-// Many meshes, one build (include/tinybvh_b200.h).  Every refusal comes before any handle is touched, the vertex staging included:
-// each mesh's vertices go into a fresh array first, and only when every index has been found in range do the handles drop their
-// old arrays and adopt the new ones.
-int tbvh_build_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int, int flavour )
+// The shared part of tbvh_build_batch / tbvh_build_batch_hq (include/tinybvh_b200.h) up to the build.  Every refusal comes before any
+// handle is touched, the vertex staging included: each mesh's vertices go into a fresh array first, and only when every index has
+// been found in range do the handles drop their old arrays and adopt the new ones.  The triangle counts are checked against the
+// limits before any index or vertex is read.  hq: the SBVH builder's node space must fit too.
+static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, bool hq )
 {
-	ARG_CHECK( bvhs && meshes && count > 0, "no meshes" );
-	if (flavour == TBVH_BUILD_HQ) { tbvh_set_error( "tbvh_build_batch: BuildHQ (SBVH) builds one tree per call" ); return TBVH_E_UNSUPPORTED; }
-	ARG_CHECK( flavour == TBVH_BUILD_REFERENCE || flavour == TBVH_BUILD_AVX, "unknown builder flavour" );
-	ARG_CHECK( space == TBVH_HOST || space == TBVH_DEVICE, "unknown space" );
-	TRY( check_batch_handles( __func__, bvhs, count ) );
+	if (space != TBVH_HOST && space != TBVH_DEVICE) { tbvh_set_error( "%s: unknown space", fn ); return TBVH_E_ARG; }
+	TRY( check_batch_handles( fn, bvhs, count ) );
 	uint64_t total = 0;
 	for (uint32_t k = 0; k < count; k++)
 	{
 		const tbvh_mesh& m = meshes[k];
-		ARG_CHECK( m.verts && m.stride >= 12 && (m.stride & 3) == 0 && m.prim_count > 0 && (!m.indices || m.vert_count > 0), "bad vertex slice" );
+		if (!(m.verts && m.stride >= 12 && (m.stride & 3) == 0 && m.prim_count > 0 && (!m.indices || m.vert_count > 0))) { tbvh_set_error( "%s: mesh %u: bad vertex slice", fn, k ); return TBVH_E_ARG; }
 		total += m.prim_count;
+	}
+	if (total > TBVH_BATCH_MAX_PRIMS) { tbvh_set_error( "%s: %llu triangles in one batch (at most %u)", fn, (unsigned long long)total, (unsigned)TBVH_BATCH_MAX_PRIMS ); return TBVH_E_LIMIT; }
+	if (hq && 3 * total + 2 > TBVH_BATCH_HQ_MAX_NODES)
+	{ tbvh_set_error( "%s: %llu temporary SBVH nodes in one batch (at most %u)", fn, (unsigned long long)(3 * total + 2), (unsigned)TBVH_BATCH_HQ_MAX_NODES ); return TBVH_E_LIMIT; }
+	for (uint32_t k = 0; k < count; k++)
+	{
+		const tbvh_mesh& m = meshes[k];
 		if (m.indices && space == TBVH_HOST)
 			for (size_t i = 0; i < (size_t)m.prim_count * 3; i++)
-				if (m.indices[i] >= m.vert_count) { tbvh_set_error( "tbvh_build_batch: mesh %u: index %u points past the %u vertices", k, m.indices[i], m.vert_count ); return TBVH_E_ARG; }
+				if (m.indices[i] >= m.vert_count) { tbvh_set_error( "%s: mesh %u: index %u points past the %u vertices", fn, k, m.indices[i], m.vert_count ); return TBVH_E_ARG; }
 	}
-	if (total > TBVH_BATCH_MAX_PRIMS) { tbvh_set_error( "tbvh_build_batch: %llu triangles in one batch (at most %u)", (unsigned long long)total, (unsigned)TBVH_BATCH_MAX_PRIMS ); return TBVH_E_LIMIT; }
 	const tbvh_ctx ctx = bvhs[0]->ctx;
 	CUDA_TRY( cudaSetDevice( ctx->device ) );
 	cudaStream_t s = ctx->stream;
@@ -978,10 +982,10 @@ int tbvh_build_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, i
 		uint32_t bad = 0;
 		CUDA_TRY( cudaMemcpyAsync( &bad, d_bad, 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
-		if (bad) { tbvh_set_error( "tbvh_build_batch: %u indices point past their mesh's vertices", bad ); return TBVH_E_ARG; }
+		if (bad) { tbvh_set_error( "%s: %u indices point past their mesh's vertices", fn, bad ); return TBVH_E_ARG; }
 		return TBVH_OK;
 	};
-	int rc = stage();
+	const int rc = stage();
 	if (d_bad) cudaFree( d_bad );
 	if (rc != TBVH_OK)
 	{
@@ -995,13 +999,36 @@ int tbvh_build_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, i
 		free_layouts( b );
 		b->d_verts = staged[k], b->info.prim_count = meshes[k].prim_count;
 	}
-	rc = build_sah_launch( bvhs, count, c_trav, c_int, flavour );
+	return TBVH_OK;
+}
+
+// after the build of a batch: each handle holds its BVH-layout tree, or, where the build failed, nothing (as a failed build leaves it)
+static int batch_finish( tbvh_bvh* bvhs, uint32_t count, int rc, bool refittable )
+{
 	for (uint32_t k = 0; k < count; k++)
 	{
-		if (rc != TBVH_OK) free_layouts( bvhs[k] ); // as a failed build leaves its handle: empty
-		else bvhs[k]->info.layouts = 1u << TBVH_LAYOUT_BVH, bvhs[k]->refittable = true;
+		if (rc != TBVH_OK) free_layouts( bvhs[k] );
+		else bvhs[k]->info.layouts = 1u << TBVH_LAYOUT_BVH, bvhs[k]->refittable = refittable;
 	}
 	return rc;
+}
+
+// Many meshes, one build (include/tinybvh_b200.h)
+int tbvh_build_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int, int flavour )
+{
+	ARG_CHECK( bvhs && meshes && count > 0, "no meshes" );
+	if (flavour == TBVH_BUILD_HQ) { tbvh_set_error( "tbvh_build_batch: SBVH (BuildHQ) batches are built by tbvh_build_batch_hq" ); return TBVH_E_UNSUPPORTED; }
+	ARG_CHECK( flavour == TBVH_BUILD_REFERENCE || flavour == TBVH_BUILD_AVX, "unknown builder flavour" );
+	TRY( batch_stage( __func__, bvhs, meshes, count, space, false ) );
+	return batch_finish( bvhs, count, build_sah_launch( bvhs, count, c_trav, c_int, flavour ), true );
+}
+
+// Many meshes, one SBVH build (include/tinybvh_b200.h)
+int tbvh_build_batch_hq( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int )
+{
+	ARG_CHECK( bvhs && meshes && count > 0, "no meshes" );
+	TRY( batch_stage( __func__, bvhs, meshes, count, space, true ) );
+	return batch_finish( bvhs, count, build_hq_launch( bvhs, count, c_trav, c_int ), false ); // "can't refit an SBVH" (:3027)
 }
 
 int tbvh_build( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space, float c_trav, float c_int )

@@ -45,34 +45,49 @@ namespace
 struct HQTask { uint32_t node, sliceStart, sliceEnd, depth; };
 struct HQCounters
 {
-	uint32_t node_ptr;       // temp node records allocated (pairs from 2)
-	uint32_t frag_ptr;       // nextFrag
+	uint32_t node_ptr;       // temp node records allocated (pairs from 2 K)
+	uint32_t frag_ptr;       // nextFrag, shared by every tree of a batch
 	uint32_t next_big;       // tasks appended to the next level's list
 	uint32_t next_max;       // largest fragment count among them (sizes the clusters); cleared together with next_big
 	uint32_t small_roots;    // subtree roots for k_hq_subtrees
-	uint32_t max_depth;
 	uint32_t failed_splits;  // ":2939 spatial split failed" leaves
 	uint32_t overflow;       // a task stack / fragment pool ran out (cannot happen within the reference's own bounds)
+	uint32_t negzero;        // some fragment bound is -0
+	unsigned long long prof[32]; // TBVH_HQ_PROFILE=1: leader-thread cycles per phase, [0..15] level phase, [16..31] subtree phase
+};
+
+// One tree of a build: what the reference keeps per BuildHQ call.  A single build is a batch of one.  Tree t owns the positions
+// [ibase, ibase + n + n/2) of the shared primIdx / idxTmp / partition scratch (the reference's idxCount), its original fragments
+// sit at fbase + i, and its root is temporary node 2t (2t + 1 is its unused node 1).
+struct HQTree
+{
+	const float4* verts;
+	float4* out_nodes; uint32_t* out_idx; float4* leaf_tris; // the handle's arrays
+	uint32_t n, ibase, fbase;
 	uint32_t root_key[6];
 	uint32_t root_zpos[6];   // signed zeros (k_hq_root_zero): position word of the last fragment with a zero bound, per root bound
-	uint32_t negzero;        // some fragment bound is -0
 	float root_area;
 	float min_dim[3];
-	unsigned long long prof[32]; // TBVH_HQ_PROFILE=1: leader-thread cycles per phase, [0..15] level phase, [16..31] subtree phase
+	uint32_t max_depth;
+	uint32_t interior, refs; // after Compact: interior nodes, leaf index entries
+	uint32_t root[8];        // after Compact: the output's root node
 };
 
 struct HQArgs
 {
-	const float4* verts;
-	float4* frag_min; float4* frag_max;       // (bmin, primIdx) / (bmax, clipped): the reference's 32-byte Fragment (:792) as two halves
+	const float4* verts;                      // a single build's vertices (tree 0's): kept out of the table where one tree is built
+	HQTree* T; uint32_t trees;
+	float4* frag_min; float4* frag_max;       // (bmin, tree-local primIdx) / (bmax, clipped): the reference's 32-byte Fragment (:792) as two halves
 	uint32_t* prim_idx; uint32_t* idx_tmp;    // both idx_cap words, the reference's primIdx / idxTmp
 	uint32_t* cls; uint32_t* strad; float* spos; // partition scratch, indexed like the slices
 	float4* tmp_nodes; uint32_t* parent; uint32_t* sub_int; uint32_t* sub_prims; uint32_t* arrive;
 	HQTask* lvl[2]; HQTask* small;
 	HQCounters* ctr;
-	uint32_t n, idx_cap, node_cap, lvl_cap, small_t, profile;
+	uint32_t n, idx_cap, node_cap, lvl_cap, small_t, profile; // n, idx_cap, node_cap: summed over the trees
 	float c_trav, c_int;
 };
+__device__ __forceinline__ uint32_t hq_tree_of_pos( const HQArgs& A, const uint32_t pos ) { return A.trees == 1 ? 0u : batch_entry<HQTree, &HQTree::ibase>( A.T, A.trees, pos ); }
+__device__ __forceinline__ uint32_t hq_tree_of_frag( const HQArgs& A, const uint32_t fi ) { return A.trees == 1 ? 0u : batch_entry<HQTree, &HQTree::fbase>( A.T, A.trees, fi ); }
 
 struct GroupSmem
 {
@@ -87,7 +102,11 @@ struct GroupSmem
 	uint32_t nstrad;
 	uint32_t ckey[12];                               // child bounds of a spatial partition: lmin, lmax, rmin, rmax keys
 	uint32_t lc;
+	uint32_t tree;                                   // the node's tree (HQArgs::T)
 };
+// the node's tree, read where it is used rather than held in registers across the node's steps.  The node kernels have a
+// single-tree instance (BATCH = false): tree 0, its vertices from the kernel parameters.
+template <bool BATCH> __device__ __forceinline__ HQTree& hq_tree( const HQArgs& A, const GroupSmem& S0 ) { return A.T[BATCH ? S0.tree : 0u]; }
 
 // ---------------------------------------------------------------------------------------------- shared math
 __device__ __forceinline__ float tmin( const float a, const float b ) { return a < b ? a : b; }   // tinybvh_min :432
@@ -122,10 +141,12 @@ __device__ __forceinline__ void store_frag( const HQArgs& A, const uint32_t fi, 
 	A.frag_min[fi] = make_float4( bmin[0], bmin[1], bmin[2], __uint_as_float( prim ) );
 	A.frag_max[fi] = make_float4( bmax[0], bmax[1], bmax[2], __uint_as_float( 1u ) );
 }
-__device__ __forceinline__ void load_tri( const HQArgs& A, const uint32_t prim, float v[3][3] )
+// prim: the tree-local triangle number a fragment carries, of tree `tree` (a single build: tree 0, vertices from the parameters)
+template <bool BATCH> __device__ __forceinline__ void load_tri( const HQArgs& A, const uint32_t tree, const uint32_t prim, float v[3][3] )
 {
+	const float4* verts = BATCH ? A.T[tree].verts : A.verts;
 	#pragma unroll
-	for (int k = 0; k < 3; k++) { const float4 p = A.verts[(size_t)prim * 3 + k]; v[k][0] = p.x, v[k][1] = p.y, v[k][2] = p.z; }
+	for (int k = 0; k < 3; k++) { const float4 p = verts[(size_t)prim * 3 + k]; v[k][0] = p.x, v[k][1] = p.y, v[k][2] = p.z; }
 }
 // C = v0 + f * (v1 - v0), compiled by the reference build as fma( f, v1 - v0, v0 ) per component
 __device__ __forceinline__ void lerp3( float* C, const float* v0, const float* v1, const float f )
@@ -173,7 +194,7 @@ template <bool CLAMP> __device__ __noinline__ uint32_t clip_slab( float vin[16][
 
 // BVH::ClipFrag :8614-8729: bounds of (fragment's triangle) clipped to box [bmin_in, bmax_in] ^ fragment box.
 // Returns false when nothing is left; nb_min / nb_max receive the new fragment's box either way (as the reference does).
-__device__ __noinline__ bool clip_frag( const HQArgs& A, const Frag& orig, float* nb_min, float* nb_max, const float* bmin_in, const float* bmax_in, const float* minDim, const uint32_t axis )
+template <bool BATCH> __device__ __noinline__ bool clip_frag( const HQArgs& A, const uint32_t tree, const Frag& orig, float* nb_min, float* nb_max, const float* bmin_in, const float* bmax_in, const float* minDim, const uint32_t axis )
 {
 	float bmin[3], bmax[3], extent[3];
 	#pragma unroll
@@ -185,7 +206,7 @@ __device__ __noinline__ bool clip_frag( const HQArgs& A, const Frag& orig, float
 		float vin[16][3], vout[16][3];
 		{
 			float t[3][3];
-			load_tri( A, orig.prim, t );
+			load_tri<BATCH>( A, tree, orig.prim, t );
 			cp3( vin[0], t[0] ), cp3( vin[1], t[1] ), cp3( vin[2], t[2] );
 		}
 		uint32_t Nin = 3;
@@ -211,7 +232,7 @@ __device__ __noinline__ bool clip_frag( const HQArgs& A, const Frag& orig, float
 			const float l = bmin[axis], r = bmax[axis];
 			float vout[4][3], t[3][3], C[3];
 			uint32_t Nout = 0;
-			load_tri( A, orig.prim, t );
+			load_tri<BATCH>( A, tree, orig.prim, t );
 			const bool in0 = t[0][axis] >= l, in1 = t[1][axis] >= l, in2 = t[2][axis] >= l;
 			#pragma unroll
 			for (int e = 0; e < 3; e++)
@@ -254,13 +275,13 @@ __device__ __noinline__ bool clip_frag( const HQArgs& A, const Frag& orig, float
 }
 
 // BVH::SplitFrag :8731-8793: the fragment's polygon cut at splitPos; only the two halves' boxes are kept.
-__device__ __noinline__ void split_frag( const HQArgs& A, const Frag& orig, float* lmin, float* lmax, float* rmin, float* rmax, const float* minDim,
+template <bool BATCH> __device__ __noinline__ void split_frag( const HQArgs& A, const uint32_t tree, const Frag& orig, float* lmin, float* lmax, float* rmin, float* rmax, const float* minDim,
 	const uint32_t splitAxis, const float splitPos, bool& leftOK, bool& rightOK )
 {
 	float vin[16][3], vout[16][3];
 	{
 		float t[3][3];
-		load_tri( A, orig.prim, t );
+		load_tri<BATCH>( A, tree, orig.prim, t );
 		cp3( vin[0], t[0] ), cp3( vin[1], t[1] ), cp3( vin[2], t[2] );
 	}
 	uint32_t Nin = 3, Nleft = 0, Nright = 0;
@@ -465,7 +486,7 @@ __device__ __noinline__ int sweep_select( GroupSmem& S, const bool spatial, cons
 
 // One node, start to finish, by a group of G threads (G = 32: a warp, G = 256: a CTA).  Returns true and the two child
 // tasks when the node was split.
-template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const HQTask t, HQTask& outL, HQTask& outR )
+template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp& g, const HQTask t, HQTask& outL, HQTask& outR )
 {
 	GroupSmem& S = *g.S;            // this CTA's (warp's) tables
 	GroupSmem& S0 = *g.S0;          // the leader's: merged tables, decisions
@@ -478,9 +499,21 @@ template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const H
 	const float4 n0 = A.tmp_nodes[(size_t)t.node * 2], n1 = A.tmp_nodes[(size_t)t.node * 2 + 1];
 	const float nmin3[3] = { n0.x, n0.y, n0.z }, nmax3[3] = { n1.x, n1.y, n1.z };
 	const uint32_t leftFirst = __float_as_uint( n0.w ), count = __float_as_uint( n1.w );
-	const float minDim[3] = { A.ctr->min_dim[0], A.ctr->min_dim[1], A.ctr->min_dim[2] };
+	// the node's tree, found once per node by the leader (its slice lies in the tree's position range) and read by the group
+	// after the next synchronisation
+	if (BATCH && lead && tid == 0) S.tree = hq_tree_of_pos( A, t.sliceStart );
 	const float ext[3] = { __fsub_rn( nmax3[0], nmin3[0] ), __fsub_rn( nmax3[1], nmin3[1] ), __fsub_rn( nmax3[2], nmin3[2] ) };
-	const bool axisOK[3] = { ext[0] > minDim[0], ext[1] > minDim[1], ext[2] > minDim[2] };
+	// the tree's minDim (:2757) and the axes it allows: a single build reads them before the node's first step, a batch after the
+	// synchronisation that publishes the node's tree
+	float minDim[3];
+	bool axisOK[3];
+	auto tree_limits = [&]()
+	{
+		const HQTree& tree = hq_tree<BATCH>( A, S0 );
+		#pragma unroll
+		for (int k = 0; k < 3; k++) minDim[k] = tree.min_dim[k], axisOK[k] = ext[k] > minDim[k];
+	};
+	if (!BATCH) tree_limits();
 	const float rpd3[3] = { __fdiv_rn( (float)HQBINS, ext[0] ), __fdiv_rn( (float)HQBINS, ext[1] ), __fdiv_rn( (float)HQBINS, ext[2] ) };
 	const float rSAV = __fdiv_rn( 1.0f, __fmaf_rn( ext[2], ext[0], __fmaf_rn( ext[1], ext[0], __fmul_rn( ext[1], ext[2] ) ) ) );
 	const float noSplitCost = __fmul_rn( __uint2float_rn( count ), A.c_int );
@@ -490,6 +523,7 @@ template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const H
 	// ---- object split: bins :2758-2775
 	bins_reset( S, tid, G );
 	gsync<G>( g );
+	if (BATCH) tree_limits();
 	// HQ_MLP fragments per thread and trip: the index -> fragment loads of a trip are issued together
 	for (uint32_t i0 = gtid; i0 < count; i0 += GT * HQ_MLP)
 	{
@@ -528,7 +562,7 @@ template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const H
 			{
 				S.bestAxis = best / 7, S.bestPos = best % 7, S.bestIdx = best;
 				// spatialOverlap :2806-2807: half area of (bestLMax - bestRMin) over the root's
-				const float ov = __fdiv_rn( half_area3( __fsub_rn( S.best[3], S.best[6] ), __fsub_rn( S.best[4], S.best[7] ), __fsub_rn( S.best[5], S.best[8] ) ), A.ctr->root_area );
+				const float ov = __fdiv_rn( half_area3( __fsub_rn( S.best[3], S.best[6] ), __fsub_rn( S.best[4], S.best[7] ), __fsub_rn( S.best[5], S.best[8] ) ), hq_tree<BATCH>( A, S0 ).root_area );
 				trySpatial = ov > 1e-4f;
 			}
 			// without an object candidate splitCost == noSplitCost and the reference's second disjunct holds whatever its stale bounds say
@@ -603,7 +637,7 @@ template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const H
 				const float lo_a = __fmaf_rn( __int2float_rn( j ), planeDist, a == 0 ? nmin3[0] : a == 1 ? nmin3[1] : nmin3[2] );
 				const float hi_a = j == HQBINS - 2 ? (a == 0 ? nmax3[0] : a == 1 ? nmax3[1] : nmax3[2]) : __fadd_rn( lo_a, planeDist );
 				if (a == 0) bmin[0] = lo_a, bmax[0] = hi_a; else if (a == 1) bmin[1] = lo_a, bmax[1] = hi_a; else bmin[2] = lo_a, bmax[2] = hi_a;
-				if (!clip_frag( A, f, nbmin, nbmax, bmin, bmax, minDim, a )) continue;
+				if (!clip_frag<BATCH>( A, BATCH ? S0.tree : 0u, f, nbmin, nbmax, bmin, bmax, minDim, a )) continue;
 				bin_grow( S, a, (uint32_t)j, nbmin, nbmax );
 			}
 			lsync<G>();
@@ -632,7 +666,7 @@ template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const H
 	if (S0.splitCost >= noSplitCost)
 	{
 		for (uint32_t i = gtid; i < count; i += GT) { const uint32_t p = leftFirst + i; A.prim_idx[p] = __float_as_uint( A.frag_min[A.prim_idx[p]].w ); }
-		if (lead && tid == 0) atomicMax( &A.ctr->max_depth, t.depth );
+		if (lead && tid == 0) atomicMax( &hq_tree<BATCH>( A, S0 ).max_depth, t.depth );
 		gsync<G>( g ); // nobody reads the leader's tables after it has moved on
 		PH( 9 );
 		return false;
@@ -793,7 +827,7 @@ template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const H
 			const Frag f = load_frag( A, fragIdx );
 			float lmin[3], lmax[3], rmin[3], rmax[3];
 			bool leftOK, rightOK;
-			split_frag( A, f, lmin, lmax, rmin, rmax, minDim, bestAxis, spos[k], leftOK, rightOK );
+			split_frag<BATCH>( A, BATCH ? S0.tree : 0u, f, lmin, lmax, rmin, rmax, minDim, bestAxis, spos[k], leftOK, rightOK );
 			if (leftOK && rightOK)
 			{
 				const uint32_t nf = atomicAdd( &A.ctr->frag_ptr, 1u );
@@ -903,7 +937,7 @@ template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const H
 			const float* b = S.best;
 			A.tmp_nodes[(size_t)t.node * 2] = make_float4( tmin( b[0], b[6] ), tmin( b[1], b[7] ), tmin( b[2], b[8] ), n0.w );
 			A.tmp_nodes[(size_t)t.node * 2 + 1] = make_float4( tmax( b[3], b[9] ), tmax( b[4], b[10] ), tmax( b[5], b[11] ), n1.w );
-			atomicAdd( &A.ctr->failed_splits, 1u ), atomicMax( &A.ctr->max_depth, t.depth );
+			atomicAdd( &A.ctr->failed_splits, 1u ), atomicMax( &hq_tree<BATCH>( A, S0 ).max_depth, t.depth );
 		}
 		gsync<G>( g );
 		return false;
@@ -938,78 +972,113 @@ template <int G> __device__ bool hq_node( const HQArgs& A, const Grp& g, const H
 }
 
 // ---------------------------------------------------------------------------------------------- kernels
+// Where the lanes of a warp may lie in different trees: true when they all lie in lane 0's (one reduction serves the warp),
+// else every lane folds its own value into its tree's word.
+__device__ __forceinline__ bool warp_one_tree( const uint32_t t ) { return __all_sync( 0xffffffffu, t == __shfl_sync( 0xffffffffu, t, 0 ) ); }
+
+// one thread per tree (thread 0 also clears the shared counters)
 __global__ void k_hq_init( HQArgs A )
 {
-	HQCounters* c = A.ctr;
-	c->node_ptr = 2, c->frag_ptr = A.n, c->next_big = 0, c->small_roots = 0, c->max_depth = 0, c->next_max = 0, c->failed_splits = 0, c->overflow = 0;
-	for (int k = 0; k < 3; k++) c->root_key[k] = f2key( BVH_FAR ), c->root_key[3 + k] = f2key( -BVH_FAR );
-	for (int k = 0; k < 6; k++) c->root_zpos[k] = 0;
-	c->negzero = 0;
-	for (int k = 0; k < 32; k++) c->prof[k] = 0;
+	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t == 0)
+	{
+		HQCounters* c = A.ctr;
+		c->node_ptr = 2 * A.trees, c->frag_ptr = A.n, c->next_big = 0, c->small_roots = 0, c->next_max = 0, c->failed_splits = 0, c->overflow = 0;
+		c->negzero = 0;
+		for (int k = 0; k < 32; k++) c->prof[k] = 0;
+	}
+	if (t >= A.trees) return;
+	HQTree& T = A.T[t];
+	for (int k = 0; k < 3; k++) T.root_key[k] = f2key( BVH_FAR ), T.root_key[3 + k] = f2key( -BVH_FAR );
+	for (int k = 0; k < 6; k++) T.root_zpos[k] = 0;
+	T.max_depth = 0, T.interior = 0, T.refs = 0;
 }
 
-// PrepareHQBuild :2677-2686: fragment boxes, identity primIdx, root bounds
+// PrepareHQBuild :2677-2686: fragment boxes, identity primIdx, root bounds.  Fragment i of the batch is triangle i - fbase of its
+// tree, and carries that tree-local number.
 __global__ void k_hq_fragments( HQArgs A )
 {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	const uint32_t t = hq_tree_of_frag( A, min( i, A.n - 1 ) ); // lanes past the end fold neutral bounds into the last tree
 	float mn[3] = { BVH_FAR, BVH_FAR, BVH_FAR }, mx[3] = { -BVH_FAR, -BVH_FAR, -BVH_FAR };
 	if (i < A.n)
 	{
-		const float4 v0 = A.verts[(size_t)i * 3], v1 = A.verts[(size_t)i * 3 + 1], v2 = A.verts[(size_t)i * 3 + 2];
+		const uint32_t p = A.trees == 1 ? i : i - A.T[t].fbase;
+		const float4* verts = A.trees == 1 ? A.verts : A.T[t].verts;
+		const float4 v0 = verts[(size_t)p * 3], v1 = verts[(size_t)p * 3 + 1], v2 = verts[(size_t)p * 3 + 2];
 		mn[0] = tmin( v0.x, tmin( v1.x, v2.x ) ), mn[1] = tmin( v0.y, tmin( v1.y, v2.y ) ), mn[2] = tmin( v0.z, tmin( v1.z, v2.z ) );
 		mx[0] = tmax( v0.x, tmax( v1.x, v2.x ) ), mx[1] = tmax( v0.y, tmax( v1.y, v2.y ) ), mx[2] = tmax( v0.z, tmax( v1.z, v2.z ) );
-		A.frag_min[i] = make_float4( mn[0], mn[1], mn[2], __uint_as_float( i ) );
+		A.frag_min[i] = make_float4( mn[0], mn[1], mn[2], __uint_as_float( p ) );
 		A.frag_max[i] = make_float4( mx[0], mx[1], mx[2], __uint_as_float( 0u ) );
-		A.prim_idx[i] = i;
+		A.prim_idx[(A.trees == 1 ? 0u : A.T[t].ibase) + p] = i;
 	}
 	// a -0 bound anywhere: the root's zero bounds take their sign in k_hq_root_zero (without one the keys are exact)
 	const bool neg = (mn[0] == 0 && signbit( mn[0] )) || (mn[1] == 0 && signbit( mn[1] )) || (mn[2] == 0 && signbit( mn[2] ))
 		|| (mx[0] == 0 && signbit( mx[0] )) || (mx[1] == 0 && signbit( mx[1] )) || (mx[2] == 0 && signbit( mx[2] ));
 	if (__any_sync( 0xffffffffu, neg ) && (threadIdx.x & 31) == 0) A.ctr->negzero = 1;
+	const bool one = warp_one_tree( t );
+	uint32_t* key = A.T[t].root_key;
 	#pragma unroll
 	for (int k = 0; k < 3; k++)
 	{
 		uint32_t a = f2key( mn[k] ), b = f2key( mx[k] );
-		a = __reduce_min_sync( 0xffffffffu, a ), b = __reduce_max_sync( 0xffffffffu, b );
-		if ((threadIdx.x & 31) == 0) atomicMin( &A.ctr->root_key[k], a ), atomicMax( &A.ctr->root_key[3 + k], b );
+		if (one)
+		{
+			a = __reduce_min_sync( 0xffffffffu, a ), b = __reduce_max_sync( 0xffffffffu, b );
+			if ((threadIdx.x & 31) == 0) atomicMin( &key[k], a ), atomicMax( &key[3 + k], b );
+		}
+		else if (i < A.n) atomicMin( &key[k], a ), atomicMax( &key[3 + k], b );
 	}
 }
 
-// With a -0 fragment bound only: each root bound that is a zero takes the sign of the last fragment with a zero there, as
-// PrepareHQBuild's fold gives it (common.cuh zpos_word; build_sah.cu k_root_zero)
+// With a -0 fragment bound only: each root bound that is a zero takes the sign of the last fragment of its tree with a zero there, as
+// PrepareHQBuild's fold gives it (common.cuh zpos_word over the tree-local position; build_sah.cu k_root_zero)
 __global__ void __launch_bounds__( 256 ) k_hq_root_zero( HQArgs A )
 {
 	if (!A.ctr->negzero) return;
-	uint32_t zw[6] = { 0, 0, 0, 0, 0, 0 };
-	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < A.n; i += gridDim.x * blockDim.x)
+	for (uint32_t i0 = blockIdx.x * blockDim.x; i0 < A.n; i0 += gridDim.x * blockDim.x) // uniform per block
 	{
-		const float4 lo = A.frag_min[i], hi = A.frag_max[i];
-		const float f[6] = { lo.x, lo.y, lo.z, hi.x, hi.y, hi.z };
+		const uint32_t i = i0 + threadIdx.x, t = hq_tree_of_frag( A, min( i, A.n - 1 ) );
+		uint32_t zw[6] = { 0, 0, 0, 0, 0, 0 }, any = 0;
+		if (i < A.n)
+		{
+			const uint32_t p = i - A.T[t].fbase;
+			const float4 lo = A.frag_min[i], hi = A.frag_max[i];
+			const float f[6] = { lo.x, lo.y, lo.z, hi.x, hi.y, hi.z };
+			#pragma unroll
+			for (int k = 0; k < 6; k++) if (f[k] == 0) zw[k] = zpos_word( p, f[k] ), any = 1;
+		}
+		if (!__any_sync( 0xffffffffu, any )) continue;
+		const bool one = warp_one_tree( t );
+		uint32_t* zpos = A.T[t].root_zpos;
 		#pragma unroll
-		for (int k = 0; k < 6; k++) if (f[k] == 0) zw[k] = max( zw[k], zpos_word( i, f[k] ) );
-	}
-	#pragma unroll
-	for (int k = 0; k < 6; k++)
-	{
-		const uint32_t w = __reduce_max_sync( 0xffffffffu, zw[k] );
-		if ((threadIdx.x & 31) == 0 && w) atomicMax( &A.ctr->root_zpos[k], w );
+		for (int k = 0; k < 6; k++)
+		{
+			const uint32_t w = one ? __reduce_max_sync( 0xffffffffu, zw[k] ) : zw[k];
+			if ((!one || (threadIdx.x & 31) == 0) && w) atomicMax( &zpos[k], w );
+		}
 	}
 }
 
+// one thread per tree: its root (temporary node 2t over its whole slice), the values its nodes read, and its first task
 __global__ void k_hq_root( HQArgs A )
 {
-	HQCounters* c = A.ctr;
+	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= A.trees) return;
+	HQTree& T = A.T[t];
 	float mn[3], mx[3];
-	for (int k = 0; k < 3; k++) mn[k] = key2f( zero_resolve( c->root_key[k], c->root_zpos[k] ) ), mx[k] = key2f( zero_resolve( c->root_key[3 + k], c->root_zpos[3 + k] ) );
-	A.tmp_nodes[0] = make_float4( mn[0], mn[1], mn[2], __uint_as_float( 0u ) );
-	A.tmp_nodes[1] = make_float4( mx[0], mx[1], mx[2], __uint_as_float( A.n ) );
-	A.tmp_nodes[2] = A.tmp_nodes[3] = make_float4( 0, 0, 0, 0 );
-	A.parent[0] = A.parent[1] = 0xffffffffu;
+	for (int k = 0; k < 3; k++) mn[k] = key2f( zero_resolve( T.root_key[k], T.root_zpos[k] ) ), mx[k] = key2f( zero_resolve( T.root_key[3 + k], T.root_zpos[3 + k] ) );
+	const uint32_t r = 2 * t, n = T.n;
+	A.tmp_nodes[(size_t)r * 2] = make_float4( mn[0], mn[1], mn[2], __uint_as_float( T.ibase ) );
+	A.tmp_nodes[(size_t)r * 2 + 1] = make_float4( mx[0], mx[1], mx[2], __uint_as_float( n ) );
+	A.tmp_nodes[(size_t)r * 2 + 2] = A.tmp_nodes[(size_t)r * 2 + 3] = make_float4( 0, 0, 0, 0 );
+	A.parent[r] = A.parent[r + 1] = 0xffffffffu;
 	const float ex = __fsub_rn( mx[0], mn[0] ), ey = __fsub_rn( mx[1], mn[1] ), ez = __fsub_rn( mx[2], mn[2] );
-	c->root_area = half_area3( ex, ey, ez );
-	c->min_dim[0] = __fmul_rn( ex, 1e-7f ), c->min_dim[1] = __fmul_rn( ey, 1e-7f ), c->min_dim[2] = __fmul_rn( ez, 1e-7f );
-	HQTask t = { 0u, 0u, A.idx_cap, 0u };
-	if (A.n > A.small_t) A.lvl[0][0] = t, c->next_big = 1, c->next_max = A.n; else A.small[0] = t, c->small_roots = 1;
+	T.root_area = half_area3( ex, ey, ez );
+	T.min_dim[0] = __fmul_rn( ex, 1e-7f ), T.min_dim[1] = __fmul_rn( ey, 1e-7f ), T.min_dim[2] = __fmul_rn( ez, 1e-7f );
+	const HQTask task = { r, T.ibase, T.ibase + n + (n >> 1), 0u };
+	if (n > A.small_t) A.lvl[0][atomicAdd( &A.ctr->next_big, 1u )] = task, atomicMax( &A.ctr->next_max, n );
+	else A.small[atomicAdd( &A.ctr->small_roots, 1u )] = task;
 }
 
 __device__ __forceinline__ void hq_enqueue( const HQArgs& A, HQTask* next, const HQTask c )
@@ -1025,7 +1094,7 @@ __device__ __forceinline__ void hq_enqueue( const HQArgs& A, HQTask* next, const
 }
 
 // level-synchronous phase: one cluster of nct CTAs (run-time cluster dimension, 1..16) per node
-__global__ void __launch_bounds__( HQ_BIG_THREADS, 3 ) k_hq_level( HQArgs A, const HQTask* cur, HQTask* next, const uint32_t nct )
+template <bool BATCH> __global__ void __launch_bounds__( HQ_BIG_THREADS, 3 ) k_hq_level( HQArgs A, const HQTask* cur, HQTask* next, const uint32_t nct )
 {
 	__shared__ GroupSmem S;
 	__shared__ uint32_t job[3 * HQ_MLP * HQ_BIG_THREADS];
@@ -1038,11 +1107,11 @@ __global__ void __launch_bounds__( HQ_BIG_THREADS, 3 ) k_hq_level( HQArgs A, con
 	}
 	g.gtid = (int)(g.rank * HQ_BIG_THREADS + threadIdx.x), g.GT = (int)(nct * HQ_BIG_THREADS);
 	HQTask l, r;
-	const bool split = hq_node<HQ_BIG_THREADS>( A, g, cur[blockIdx.x / nct], l, r );
+	const bool split = hq_node<HQ_BIG_THREADS, BATCH>( A, g, cur[blockIdx.x / nct], l, r );
 	if (split && g.rank == 0 && threadIdx.x == 0) hq_enqueue( A, next, l ), hq_enqueue( A, next, r );
 }
 
-__global__ void __launch_bounds__( HQ_SMALL_WARPS * 32, 6 ) k_hq_subtrees( HQArgs A, const uint32_t roots )
+template <bool BATCH> __global__ void __launch_bounds__( HQ_SMALL_WARPS * 32, 6 ) k_hq_subtrees( HQArgs A, const uint32_t roots )
 {
 	__shared__ GroupSmem Ss[HQ_SMALL_WARPS];
 	__shared__ HQTask stack[HQ_SMALL_WARPS][HQ_STACK];
@@ -1056,7 +1125,7 @@ __global__ void __launch_bounds__( HQ_SMALL_WARPS * 32, 6 ) k_hq_subtrees( HQArg
 	for (;;)
 	{
 		HQTask l, r;
-		if (hq_node<32>( A, g, t, l, r ))
+		if (hq_node<32, BATCH>( A, g, t, l, r ))
 		{
 			// continue with the child that holds fewer fragments, park the other: the stack stays logarithmic
 			const uint32_t cl = __float_as_uint( A.tmp_nodes[(size_t)l.node * 2 + 1].w ), cr = __float_as_uint( A.tmp_nodes[(size_t)r.node * 2 + 1].w );
@@ -1073,91 +1142,139 @@ __global__ void __launch_bounds__( HQ_SMALL_WARPS * 32, 6 ) k_hq_subtrees( HQArg
 	}
 }
 
-// ---- Compact() :3733-3770 as a parallel relayout
-// bottom-up: number of interior nodes / of leaf index entries per subtree (second arrival at a parent carries on)
+// ---- Compact() :3733-3770 as a parallel relayout, every tree of the batch at once over the shared temporary node space
+// bottom-up: number of interior nodes / of leaf index entries per subtree (second arrival at a parent carries on; a root's parent
+// is 0xffffffff, so no walk leaves its tree)
 __global__ void k_hq_up( HQArgs A, const uint32_t tmp_count )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= tmp_count || x == 1) return;
+	if (x >= tmp_count || (x < 2 * A.trees && (x & 1u))) return; // a tree's unused node 1
 	const uint32_t cnt = __float_as_uint( A.tmp_nodes[(size_t)x * 2 + 1].w );
 	if (cnt == 0) return; // interior
 	dfs_sizes_up( A.tmp_nodes, A.parent, A.arrive, A.sub_int, A.sub_prims, x, cnt );
 }
-// top-down by walking to the root: K = interior nodes before x in DFS preorder, O = leaf index entries before x
-__global__ void k_hq_down( HQArgs A, const uint32_t tmp_count, float4* out_nodes, uint32_t* out_idx )
+// top-down by walking to the tree's root: K = interior nodes before x in DFS preorder, O = leaf index entries before x, both
+// local to the tree; the node goes into its handle's arrays
+__global__ void k_hq_down( HQArgs A, const uint32_t tmp_count )
 {
 	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
 	if (x >= tmp_count) return;
-	if (x == 1) { out_nodes[2] = out_nodes[3] = make_float4( 0, 0, 0, 0 ); return; }
+	if (x < 2 * A.trees && (x & 1u)) { float4* o = A.T[x >> 1].out_nodes; o[2] = o[3] = make_float4( 0, 0, 0, 0 ); return; }
 	uint32_t K, O, Kparent; // K(parent) = K(x) - Kparent
-	dfs_rank( A.tmp_nodes, A.parent, A.sub_int, A.sub_prims, x, K, O, Kparent );
-	const uint32_t dst = x == 0 ? 0u : 2u + 2u * (K - Kparent) + ((x & 1u) ? 1u : 0u); // pairs start at even temp indices: odd = right child
+	const uint32_t root = dfs_rank( A.tmp_nodes, A.parent, A.sub_int, A.sub_prims, x, K, O, Kparent );
+	HQTree& T = A.T[root >> 1];
+	const uint32_t dst = x == root ? 0u : 2u + 2u * (K - Kparent) + ((x & 1u) ? 1u : 0u); // pairs start at even temp indices: odd = right child
 	const float4 a = A.tmp_nodes[(size_t)x * 2], b = A.tmp_nodes[(size_t)x * 2 + 1];
 	const uint32_t cnt = __float_as_uint( b.w );
-	if (cnt == 0) out_nodes[(size_t)dst * 2] = make_float4( a.x, a.y, a.z, __uint_as_float( 2u + 2u * K ) ), out_nodes[(size_t)dst * 2 + 1] = b;
-	else
+	const float4 o = make_float4( a.x, a.y, a.z, __uint_as_float( cnt == 0 ? 2u + 2u * K : O ) );
+	T.out_nodes[(size_t)dst * 2] = o, T.out_nodes[(size_t)dst * 2 + 1] = b;
+	if (cnt)
 	{
-		out_nodes[(size_t)dst * 2] = make_float4( a.x, a.y, a.z, __uint_as_float( O ) ), out_nodes[(size_t)dst * 2 + 1] = b;
 		const uint32_t first = __float_as_uint( a.w );
-		for (uint32_t i = 0; i < cnt; i++) out_idx[O + i] = A.prim_idx[first + i];
+		for (uint32_t i = 0; i < cnt; i++) T.out_idx[O + i] = A.prim_idx[first + i];
 	}
+	if (x == root)
+	{
+		T.interior = A.sub_int[x], T.refs = A.sub_prims[x];
+		const float w[8] = { o.x, o.y, o.z, o.w, b.x, b.y, b.z, b.w };
+		for (int k = 0; k < 8; k++) T.root[k] = __float_as_uint( w[k] );
+	}
+}
+// one thread per position of the batch: the tail of each handle's primIdx (past its leaf entries) zeroed, as the reference leaves
+// it, and the leaf-ordered triangle records of every tree (make_leaf_tris)
+__global__ void __launch_bounds__( 256 ) k_hq_outputs( HQArgs A )
+{
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= A.idx_cap) return;
+	const HQTree& T = A.T[hq_tree_of_pos( A, g )];
+	const uint32_t p = g - T.ibase;
+	uint32_t pi = 0;
+	if (p < T.refs) pi = T.out_idx[p]; else T.out_idx[p] = 0;
+	leaf_tri_record( T.verts, pi, T.leaf_tris, p );
 }
 } // namespace
 
 #define DEV_ALLOC( p, bytes ) do { void* q_ = 0; CUDA_TRY( cudaMalloc( &q_, (bytes) ) ); scratch.push_back( q_ ); (p) = (decltype( p ))q_; } while (0)
 
-int build_hq_launch( tbvh_bvh b, float c_trav, float c_int )
+// bs[0 .. K): handles of one context holding their triangles (d_verts, info.prim_count); on success each holds its SBVH as a
+// build of its own would leave it.  On failure the caller empties them.
+int build_hq_launch( const tbvh_bvh* bs, const uint32_t K, float c_trav, float c_int )
 {
-	const uint32_t n = b->info.prim_count, slack = n >> 1;
-	cudaStream_t s = b->ctx->stream;
+	const tbvh_ctx ctx = bs[0]->ctx;
+	cudaStream_t s = ctx->stream;
 	std::vector<void*> scratch;
 	HQArgs A = {};
-	A.verts = b->d_verts, A.n = n, A.c_trav = c_trav, A.c_int = c_int;
-	A.idx_cap = n + slack, A.node_cap = 3 * n + 2;
+	A.verts = bs[0]->d_verts, A.trees = K, A.c_trav = c_trav, A.c_int = c_int;
 	{
-		const int t = b->ctx->hq_small;
+		const int t = ctx->hq_small;
 		A.small_t = (uint32_t)(t < 8 ? 8 : t > HQ_SMALL_MAX ? HQ_SMALL_MAX : t);
 	}
-	A.lvl_cap = A.idx_cap / A.small_t + 2;
+	// the shared index spaces (the caller has checked that 3 n + 2 fits 32 bits), and the trees that start in the level phase
+	std::vector<HQTree> T( K );
+	uint32_t n = 0, idx = 0, num = 0, max_count = 0;
+	for (uint32_t t = 0; t < K; t++)
+	{
+		const tbvh_bvh b = bs[t];
+		const uint32_t nt = b->info.prim_count;
+		T[t] = HQTree{};
+		T[t].verts = b->d_verts, T[t].n = nt, T[t].ibase = idx, T[t].fbase = n;
+		n += nt, idx += nt + (nt >> 1);
+		if (nt > A.small_t) num++, max_count = std::max( max_count, nt );
+	}
+	A.n = n, A.idx_cap = idx, A.node_cap = 3 * n + 2;
+	A.lvl_cap = A.idx_cap / A.small_t + K + 2;
 	{ const char* e = getenv( "TBVH_HQ_PROFILE" ); A.profile = e ? (uint32_t)atoi( e ) : 0u; }
+	// outputs (kept by the handles)
+	for (uint32_t t = 0; t < K; t++)
+	{
+		const tbvh_bvh b = bs[t];
+		const uint32_t nt = T[t].n, it = nt + (nt >> 1);
+		CUDA_TRY( cudaMalloc( &b->d_nodes, ((size_t)3 * nt + 2) * 32 ) );
+		CUDA_TRY( cudaMalloc( &b->d_prim_idx, (size_t)it * 4 ) );
+		CUDA_TRY( cudaMalloc( &b->d_leaf_tris, (size_t)it * 48 ) ); b->leaf_tris_count = it;
+		T[t].out_nodes = b->d_nodes, T[t].out_idx = b->d_prim_idx, T[t].leaf_tris = b->d_leaf_tris;
+	}
 	HQCounters* h_ctr = 0;
 	cudaEvent_t e0 = 0, e1 = 0;
-	CUDA_TRY( cudaMalloc( &b->d_nodes, (size_t)A.node_cap * 32 ) );
-	CUDA_TRY( cudaMalloc( &b->d_prim_idx, (size_t)A.idx_cap * 4 ) );
 	auto body = [&]() -> int
 	{
+		DEV_ALLOC( A.T, (size_t)K * sizeof( HQTree ) );
 		DEV_ALLOC( A.frag_min, (size_t)A.idx_cap * 16 ); DEV_ALLOC( A.frag_max, (size_t)A.idx_cap * 16 );
 		DEV_ALLOC( A.prim_idx, (size_t)A.idx_cap * 4 ); DEV_ALLOC( A.idx_tmp, (size_t)A.idx_cap * 4 );
 		DEV_ALLOC( A.cls, (size_t)A.idx_cap * 4 ); DEV_ALLOC( A.strad, (size_t)A.idx_cap * 4 ); DEV_ALLOC( A.spos, (size_t)A.idx_cap * 4 );
 		DEV_ALLOC( A.tmp_nodes, (size_t)A.node_cap * 32 ); DEV_ALLOC( A.parent, (size_t)A.node_cap * 4 );
 		DEV_ALLOC( A.sub_int, (size_t)A.node_cap * 4 ); DEV_ALLOC( A.sub_prims, (size_t)A.node_cap * 4 ); DEV_ALLOC( A.arrive, (size_t)A.node_cap * 4 );
 		DEV_ALLOC( A.lvl[0], (size_t)A.lvl_cap * sizeof( HQTask ) ); DEV_ALLOC( A.lvl[1], (size_t)A.lvl_cap * sizeof( HQTask ) );
-		DEV_ALLOC( A.small, ((size_t)A.idx_cap + 1) * sizeof( HQTask ) );
+		DEV_ALLOC( A.small, ((size_t)A.idx_cap + K) * sizeof( HQTask ) );
 		DEV_ALLOC( A.ctr, sizeof( HQCounters ) );
 		CUDA_TRY( cudaMallocHost( &h_ctr, sizeof( HQCounters ) ) );
 		CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) );
+		CUDA_TRY( cudaMemcpyAsync( A.T, T.data(), (size_t)K * sizeof( HQTree ), cudaMemcpyHostToDevice, s ) );
 		CUDA_TRY( cudaEventRecord( e0, s ) );
-		// the reference clears primIdx beyond triCount (:2700) and all of idxTmp (:3008)
+		// the reference clears primIdx beyond triCount (:2700) and all of idxTmp (:3008): a never-written idxTmp word is fragment 0,
+		// whose tree-local triangle number is 0 in every tree
 		CUDA_TRY( cudaMemsetAsync( A.prim_idx, 0, (size_t)A.idx_cap * 4, s ) );
 		CUDA_TRY( cudaMemsetAsync( A.idx_tmp, 0, (size_t)A.idx_cap * 4, s ) );
 		CUDA_TRY( cudaMemsetAsync( A.arrive, 0, (size_t)A.node_cap * 4, s ) );
-		k_hq_init<<<1, 1, 0, s>>>( A ); LAUNCHED();
+		k_hq_init<<<(K + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
 		k_hq_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
-		k_hq_root_zero<<<b->ctx->sm_count, 256, 0, s>>>( A ); LAUNCHED();
-		k_hq_root<<<1, 1, 0, s>>>( A ); LAUNCHED();
-		uint32_t num = n > A.small_t ? 1 : 0, level = 0, max_count = n;
-		uint32_t max_cluster = (uint32_t)(b->ctx->hq_cluster < 1 ? 1 : b->ctx->hq_cluster > HQ_MAX_CLUSTER ? HQ_MAX_CLUSTER : b->ctx->hq_cluster);
+		k_hq_root_zero<<<ctx->sm_count, 256, 0, s>>>( A ); LAUNCHED();
+		k_hq_root<<<(K + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+		uint32_t level = 0;
+		uint32_t max_cluster = (uint32_t)(ctx->hq_cluster < 1 ? 1 : ctx->hq_cluster > HQ_MAX_CLUSTER ? HQ_MAX_CLUSTER : ctx->hq_cluster);
 		// tuning knobs of the cluster sizing rule, read from the environment: fragments per CTA, CTAs per SM in flight
 		const char* env_cf = getenv( "TBVH_HQ_CTA_FRAGS" ); const char* env_cc = getenv( "TBVH_HQ_CTA_CAP" );
 		const size_t cta_frags = env_cf && atoi( env_cf ) > 0 ? (size_t)atoi( env_cf ) : 512, cta_cap = env_cc && atoi( env_cc ) > 0 ? (size_t)atoi( env_cc ) : 16;
-		if (max_cluster > 8) CUDA_TRY( cudaFuncSetAttribute( k_hq_level, cudaFuncAttributeNonPortableClusterSizeAllowed, 1 ) );
+		void (*level_kernel)( HQArgs, const HQTask*, HQTask*, uint32_t ) = K > 1 ? k_hq_level<true> : k_hq_level<false>;
+		if (max_cluster > 8) CUDA_TRY( cudaFuncSetAttribute( level_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1 ) );
+		// one level list for every tree: the cluster size follows the level's largest node, whichever tree holds it
 		while (num)
 		{
 			CUDA_TRY( cudaMemsetAsync( &A.ctr->next_big, 0, 8, s ) ); // next_big + next_max
 			// cluster size: enough CTAs for the largest node of the level (about 512 fragments per CTA), at most 8 CTAs per SM in flight,
 			// a power of two no larger than max_cluster
 			uint32_t nct = 1;
-			while (nct * 2 <= max_cluster && (size_t)nct * cta_frags < max_count && (size_t)num * nct * 2 <= (size_t)b->ctx->sm_count * cta_cap) nct <<= 1;
+			while (nct * 2 <= max_cluster && (size_t)nct * cta_frags < max_count && (size_t)num * nct * 2 <= (size_t)ctx->sm_count * cta_cap) nct <<= 1;
 			cudaLaunchConfig_t cfg = {};
 			cudaLaunchAttribute attr[1];
 			cfg.gridDim = dim3( num * nct ), cfg.blockDim = dim3( HQ_BIG_THREADS ), cfg.dynamicSmemBytes = 0, cfg.stream = s;
@@ -1166,7 +1283,7 @@ int build_hq_launch( tbvh_bvh b, float c_trav, float c_int )
 			{
 				// a cluster shape the device cannot co-schedule (MIG slices, fewer SMs per GPC) fails at launch: nothing has run, so
 				// fall back to the next smaller shape
-				const cudaError_t le = cudaLaunchKernelEx( &cfg, k_hq_level, A, (const HQTask*)A.lvl[level & 1], A.lvl[(level + 1) & 1], nct );
+				const cudaError_t le = cudaLaunchKernelEx( &cfg, level_kernel, A, (const HQTask*)A.lvl[level & 1], A.lvl[(level + 1) & 1], nct );
 				if (le != cudaSuccess && nct > 1) { cudaGetLastError(); max_cluster = nct >> 1; continue; }
 				CUDA_TRY( le ); LAUNCHED();
 			}
@@ -1186,8 +1303,14 @@ int build_hq_launch( tbvh_bvh b, float c_trav, float c_int )
 		}
 		CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( HQCounters ), cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
+		// one launch for the warp subtrees of every tree
 		const uint32_t roots = h_ctr->small_roots;
-		if (roots) { k_hq_subtrees<<<(roots + HQ_SMALL_WARPS - 1) / HQ_SMALL_WARPS, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots ); LAUNCHED(); }
+		if (roots)
+		{
+			const uint32_t grid = (roots + HQ_SMALL_WARPS - 1) / HQ_SMALL_WARPS;
+			if (K > 1) k_hq_subtrees<true><<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots ); else k_hq_subtrees<false><<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots );
+			LAUNCHED();
+		}
 		CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( HQCounters ), cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		if (h_ctr->overflow) { tbvh_set_error( "BuildHQ: pool overflow in the subtree phase" ); return TBVH_E_LIMIT; }
@@ -1198,30 +1321,27 @@ int build_hq_launch( tbvh_bvh b, float c_trav, float c_int )
 			for (int k = 0; k < 12; k++) fprintf( stderr, "hq-profile %-10s level %10.3f Mcyc   subtree %10.3f Mcyc\n", nm[k], h_ctr->prof[k] * 1e-6, h_ctr->prof[16 + k] * 1e-6 );
 			fprintf( stderr, "hq-profile failed_splits %u small_roots %u\n", h_ctr->failed_splits, h_ctr->small_roots );
 		}
-		// Compact(): DFS-preorder numbering, leaf index ranges packed in DFS order; the tail of the index array is zeroed
-		CUDA_TRY( cudaMemsetAsync( b->d_prim_idx, 0, (size_t)A.idx_cap * 4, s ) );
-		if (tmp_count > 2)
-		{
-			k_hq_up<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count ); LAUNCHED();
-			k_hq_down<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count, b->d_nodes, b->d_prim_idx ); LAUNCHED();
-		}
-		else
-		{
-			CUDA_TRY( cudaMemcpyAsync( b->d_nodes, A.tmp_nodes, 64, cudaMemcpyDeviceToDevice, s ) );
-			CUDA_TRY( cudaMemcpyAsync( b->d_prim_idx, A.prim_idx, (size_t)A.idx_cap * 4, cudaMemcpyDeviceToDevice, s ) );
-		}
+		// Compact(): DFS-preorder numbering, leaf index ranges packed in DFS order, per tree
+		k_hq_up<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count ); LAUNCHED();
+		k_hq_down<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count ); LAUNCHED();
 		CUDA_TRY( cudaEventRecord( e1, s ) );
+		k_hq_outputs<<<(A.idx_cap + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+		CUDA_TRY( cudaMemcpyAsync( T.data(), A.T, (size_t)K * sizeof( HQTree ), cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		float ms = 0;
 		CUDA_TRY( cudaEventElapsedTime( &ms, e0, e1 ) );
-		b->info.build_ms = ms;
-		b->info.used_nodes = tmp_count, b->info.idx_count = A.idx_cap, b->info.max_depth = h_ctr->max_depth;
-		uint32_t rootw[8];
-		CUDA_TRY( cudaMemcpy( rootw, b->d_nodes, 32, cudaMemcpyDeviceToHost ) );
-		memcpy( b->info.aabb_min, rootw, 12 ), memcpy( b->info.aabb_max, rootw + 4, 12 );
-		b->root_ref = rootw[3], b->root_count = rootw[7];
-		b->d_trav = b->d_nodes;
-		return make_leaf_tris( b, s );
+		for (uint32_t t = 0; t < K; t++)
+		{
+			const tbvh_bvh b = bs[t];
+			const uint32_t* rootw = T[t].root;
+			b->info.build_ms = ms;
+			b->info.used_nodes = 2 + 2 * T[t].interior, b->info.idx_count = T[t].n + (T[t].n >> 1), b->info.max_depth = T[t].max_depth;
+			memcpy( b->info.aabb_min, rootw, 12 ), memcpy( b->info.aabb_max, rootw + 4, 12 );
+			b->root_ref = rootw[3], b->root_count = rootw[7];
+			b->d_trav = b->d_nodes;
+			b->generation = tbvh_next_generation(); // new arrays: a TLAS built over the old ones must notice (tlas_check)
+		}
+		return TBVH_OK;
 	};
 	const int rc = body();
 	cudaStreamSynchronize( s );

@@ -210,18 +210,22 @@ __device__ __forceinline__ void dfs_sizes_up( const float4* nodes, const uint32_
 }
 // Top-down by walking x's path to the root: K = interior nodes before x in DFS preorder, O = leaf weights before x, Kp = the part of
 // K that x's own step added (K of x's parent is K - Kp).  With every leaf weighing 1, x's preorder index is K + O.
-__device__ __forceinline__ void dfs_rank( const float4* nodes, const uint32_t* parent, const uint32_t* sub_int, const uint32_t* sub_w,
+// The walk ends at node 0 or at a node whose parent is 0xffffffff, and returns that root: the trees of a BuildHQ batch share one
+// node space, tree t rooted at node 2t.
+__device__ __forceinline__ uint32_t dfs_rank( const float4* nodes, const uint32_t* parent, const uint32_t* sub_int, const uint32_t* sub_w,
 	const uint32_t x, uint32_t& K, uint32_t& O, uint32_t& Kp )
 {
 	K = 0, O = 0, Kp = 0;
-	for (uint32_t c = x; c != 0;)
+	uint32_t c = x;
+	for (uint32_t p; c != 0 && (p = parent[c]) != 0xffffffffu; c = p)
 	{
-		const uint32_t p = parent[c], lc = __float_as_uint( nodes[(size_t)p * 2].w );
+		const uint32_t lc = __float_as_uint( nodes[(size_t)p * 2].w );
 		uint32_t add = 1;
 		if (c == lc + 1) add += sub_int[lc], O += sub_w[lc];
 		if (c == x) Kp = add;
-		K += add, c = p;
+		K += add;
 	}
+	return c;
 }
 
 // ---- batch tables: the entry of T[0 .. K) whose index range holds g (T[k].*F rises strictly: every entry owns an index)
@@ -264,7 +268,8 @@ float cw_rd_limit_for( uint32_t range );                               // cw_rd_
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)
 // binned-SAH builds of `trees` handles of one context at once (build_sah.cu); a single build is trees = 1
 int build_sah_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, int flavour );
-int build_hq_launch( tbvh_bvh b, float c_trav, float c_int );
+// SBVH builds (BuildHQ) of K handles of one context at once (build_hq.cu); a single build is K = 1
+int build_hq_launch( const tbvh_bvh* bs, uint32_t K, float c_trav, float c_int );
 // BVH::Refit of K trees over one node space of `nodes` nodes; arrive: `nodes` zeroed words; fill: some tree's parents are filled.
 // K = 1 runs the single-tree instances with `one`.
 int refit_enqueue( const RfTree* d_T, uint32_t K, const RfTree& one, uint32_t nodes, uint32_t* arrive, bool fill, cudaStream_t s );

@@ -11,6 +11,10 @@ bvh8Data / bvh8Tris.  Then the one-tree path against an older build of the libra
 Bistro-sized procedural scene and of a 150k-triangle scene, and the wall time of tbvh_convert( CWBVH ) of the Bistro-sized scene's
 Build and BuildHQ trees, and the wall time of one tbvh_convert_batch( CWBVH ) of workload a's BuildAVX trees and of 200 BuildHQ trees
 with a byte comparison of every handle, the two libraries alternated on the same card.  The card's name and power limit come from nvidia-smi (read-only).
+The HQ arm (--arms hq, or all): on workloads a and b, a loop of tbvh_build_flavour( BuildHQ ) over the meshes against one
+tbvh_build_batch_hq, alternated after a warm-up of each - wall time, device time, launches and a byte comparison of every handle's nodes
+and primIdx - and, with --parent-lib, a single BuildHQ of the Bistro-sized procedural scene (the build bench.py times) in both
+libraries, alternated.
 Writes DIR/build_batch_perf.json and prints it."""
 import argparse
 import ctypes as C
@@ -162,6 +166,68 @@ def run_workload(L, meshes, reps):
     return out
 
 
+def run_hq_workload(L, meshes, reps):
+    """a loop of BuildHQ over the meshes against one tbvh_build_batch_hq"""
+    n = len(meshes)
+    loop_h, batch_h = L.handles(n), L.handles(n)
+    recs = (_lib.Mesh * n)(*[_lib.Mesh(v.ctypes.data, 16, 0, None, v.shape[0] // 3) for v in meshes])
+    res = {"loop": {"wall_ms": [], "device_ms": [], "launches": []}, "batch": {"wall_ms": [], "device_ms": [], "launches": []}}
+
+    def loop():
+        n0 = L.L.tbvh_launch_count()
+        t0 = time.perf_counter()
+        for k, v in enumerate(meshes):
+            L.build(loop_h[k], v, _lib.BUILD_HQ)
+        wall = (time.perf_counter() - t0) * 1e3
+        return wall, sum(L.info(loop_h[k]).build_ms for k in range(n)), L.L.tbvh_launch_count() - n0
+
+    def batch():
+        n0 = L.L.tbvh_launch_count()
+        t0 = time.perf_counter()
+        L.check(L.L.tbvh_build_batch_hq(batch_h, recs, n, _lib.HOST, 1.0, 1.0))
+        wall = (time.perf_counter() - t0) * 1e3
+        return wall, L.info(batch_h[0]).build_ms, L.L.tbvh_launch_count() - n0
+
+    loop(), batch()   # warm-up
+    for _ in range(reps):
+        for name, f in (("loop", loop), ("batch", batch)):
+            w, d, l = f()
+            res[name]["wall_ms"].append(w), res[name]["device_ms"].append(d), res[name]["launches"].append(l)
+    same = 0
+    for k in range(n):
+        a, b = L.download(loop_h[k]), L.download(batch_h[k])
+        ia, ib = L.info(loop_h[k]), L.info(batch_h[k])
+        same += np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]) and bytes(ia)[:_lib.Info.build_ms.offset] == bytes(ib)[:_lib.Info.build_ms.offset]
+    for h in list(loop_h) + list(batch_h):
+        L.L.tbvh_bvh_destroy(h)
+    out = {"meshes": n, "triangles": int(sum(v.shape[0] // 3 for v in meshes)), "handles_identical": int(same)}
+    for name in ("loop", "batch"):
+        out[name] = {k: stats(v) for k, v in res[name].items()}
+    out["speedup_wall_median"] = out["loop"]["wall_ms"]["median"] / out["batch"]["wall_ms"]["median"]
+    return out
+
+
+def one_tree_hq(libs, reps):
+    """BuildHQ of the Bistro-sized procedural scene (bench.py's tree) in every library, alternated: device and wall time"""
+    v = scenes.procedural_scene(2837209, 7)
+    hs = {name: L.handles(1) for name, L in libs.items()}
+    dev, wall = {name: [] for name in libs}, {name: [] for name in libs}
+    for name, L in libs.items():
+        L.build(hs[name][0], v, _lib.BUILD_HQ)   # warm-up
+    for r in range(reps):
+        for name, L in libs.items() if r % 2 == 0 else reversed(list(libs.items())):
+            t0 = time.perf_counter()
+            L.build(hs[name][0], v, _lib.BUILD_HQ)
+            wall[name].append((time.perf_counter() - t0) * 1e3)
+            dev[name].append(L.info(hs[name][0]).build_ms)
+    trees = [L.download(hs[name][0]) for name, L in libs.items()]
+    out = {"device_ms": {name: stats(x) for name, x in dev.items()}, "wall_ms": {name: stats(x) for name, x in wall.items()}}
+    out["trees_identical"] = all(np.array_equal(t[0], trees[0][0]) and np.array_equal(t[1], trees[0][1]) for t in trees)
+    for name, L in libs.items():
+        L.L.tbvh_bvh_destroy(hs[name][0])
+    return out
+
+
 def one_tree(libs, reps):
     out = {}
     for label, v in (("bistro_sized_2837209", scenes.procedural_scene(2837209, 7)), ("tris_150k", scenes.procedural_scene(150000, 8))):
@@ -245,20 +311,27 @@ def main():
     ap.add_argument("--out", required=True, help="directory for build_batch_perf.json")
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--parent-lib", default=None, help="libtinybvh_b200.so of an older build to compare the one-tree path with")
+    ap.add_argument("--arms", choices=("all", "sah", "hq"), default="all", help="sah: the binned-SAH builds and conversions; hq: BuildHQ")
     args = ap.parse_args()
     if api.device_count() < 1:
         raise SystemExit("build_batch_perf: needs a CUDA device")
     os.makedirs(args.out, exist_ok=True)
     L = Lib(_lib.SO)
     result = {"card": gpu_card(), "reps": args.reps}
-    for name in ("a", "b"):
-        result[f"workload_{name}"] = run_workload(L, workload(name), args.reps)
     libs = {"this": L}
     if args.parent_lib:
         libs = {"parent": Lib(args.parent_lib), "this": L}
-    result["one_tree_build_ms"] = one_tree(libs, max(args.reps, 7))
-    result["one_tree_convert_cwbvh_wall_ms"] = one_tree_convert(libs, max(args.reps, 7))
-    result["batch_convert_cwbvh_wall_ms"] = batch_convert(libs, max(args.reps, 7))
+    if args.arms in ("all", "sah"):
+        for name in ("a", "b"):
+            result[f"workload_{name}"] = run_workload(L, workload(name), args.reps)
+        result["one_tree_build_ms"] = one_tree(libs, max(args.reps, 7))
+        result["one_tree_convert_cwbvh_wall_ms"] = one_tree_convert(libs, max(args.reps, 7))
+        result["batch_convert_cwbvh_wall_ms"] = batch_convert(libs, max(args.reps, 7))
+    if args.arms in ("all", "hq"):
+        for name in ("a", "b"):
+            result[f"hq_workload_{name}"] = run_hq_workload(L, workload(name), args.reps)
+        if args.parent_lib:
+            result["one_tree_buildhq"] = one_tree_hq(libs, max(args.reps, 10))
     path = os.path.join(args.out, "build_batch_perf.json")
     with open(path, "w") as f:
         json.dump(result, f, indent=1)
