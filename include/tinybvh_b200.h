@@ -258,6 +258,26 @@ int tbvh_refit_layouts( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32
 #define TBVH_REFIT_BATCH_MAX_NODES (1u << 31)
 int tbvh_refit_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts );
 
+/* Refit of indexed meshes: BVH::Refit (tiny_bvh.h:3055-3093) of a tree built with vertIdx set reads the moved vertices through the
+ * indices (BVHBase::vertIdx, :806-807), so the caller moves vert_count vertices, not 3 * prim_count.  A refittable indexed build -
+ * tbvh_build_indexed with TBVH_BUILD_REFERENCE or TBVH_BUILD_AVX, or a mesh with indices of tbvh_build_batch - keeps a device copy of
+ * its indices and its vert_count on the handle for this call: 12 bytes of device memory per triangle.  SBVH builds and flat builds keep
+ * none.  Every build, tbvh_upload_bvh / tbvh_upload_bvh_gpu and TLAS build on the handle, and a failed batch build, drop them; refits
+ * and conversions leave them.  Group replicas do not carry them.
+ *  meshes[i].vert_count > 0: verts holds the new positions of the vert_count vertices bvhs[i] was built from (the build's vert_count),
+ *  `stride` bytes apart; indices must be NULL (the kept ones are used); prim_count and stride as for tbvh_refit.
+ *  meshes[i].vert_count == 0: a flat slice, as for tbvh_refit_batch; the flat and indexed meshes of a scene refit in one call.
+ * Each handle ends up exactly as tbvh_refit (keep_layouts = 0) or tbvh_refit_layouts (keep_layouts = 1) of the flat slice
+ * verts[indices[j]], j < 3 * prim_count, at the same stride leaves it: BVH2 nodes, primIdx, BVH_GPU, bvh8Data / bvh8Tris, leaf
+ * triangles, info, traversal limits, generation and the staleness of a TLAS over it.  As in tbvh_refit, below stride 16 the w lanes are
+ * not replaced.  The vertex rows of the indexed meshes are staged at a 16-byte pitch on the device (host and device space alike) and
+ * one kernel writes every indexed handle's vertices through its indices; then the refit runs as in tbvh_refit_batch, with one host
+ * synchronisation.  count = 1 refits a single handle.
+ *  Refusals come before any handle or vertex array is touched: those of tbvh_refit_batch with the same codes, except that a mesh may
+ *  carry a vert_count; besides, TBVH_E_ARG for non-NULL indices or a vert_count other than the build's, TBVH_E_STATE for a vert_count on
+ *  a handle that keeps no indices, and TBVH_E_LIMIT also when the indexed meshes hold more than TBVH_REFIT_BATCH_MAX_NODES indices. */
+int tbvh_refit_batch_indexed( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts );
+
 /* consume a tree built elsewhere, in the reference's own layouts (the public members bvhNode / primIdx /
  * verts of tiny_bvh.h:952-964, BVH_GPU::bvhNode :1124, BVH8_CWBVH::bvh8Data / bvh8Tris :1356-1357) */
 int tbvh_upload_bvh( tbvh_bvh bvh, const void* nodes32, uint32_t used_nodes, const uint32_t* prim_idx, uint32_t idx_count,

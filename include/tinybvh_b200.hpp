@@ -140,12 +140,13 @@ protected:
 		memcpy( aabbMin, i.aabb_min, 12 ), memcpy( aabbMax, i.aabb_max, 12 );
 	}
 	// the ( vertices, indices, primCount ) overloads (tiny_bvh.h:889-900, 1111-1117, 1145-1150): the reference takes no vertex
-	// count there, so it is derived from the largest index
-	template <class Vec4> void build_indexed( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount, const int flavour, const char* what )
+	// count there, so it is derived from the largest index; returns that count
+	template <class Vec4> uint32_t build_indexed( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount, const int flavour, const char* what )
 	{
 		uint32_t vmax = 0;
 		for (size_t i = 0; i < (size_t)primCount * 3; i++) vmax = indices[i] > vmax ? indices[i] : vmax;
 		TBVH_FATAL_IF( tbvh_build_indexed( h, vertices, (uint32_t)sizeof( Vec4 ), vmax + 1, indices, primCount, TBVH_HOST, c_trav, c_int, flavour ), what );
+		return vmax + 1;
 	}
 	static void batch_convert( tbvh_bvh*, uint32_t ) {} // BuildBatch: layouts converted for the whole batch at once (BVH8_CWBVH)
 	void adopt( const BVHBase& o ) { if (own) tbvh_bvh_destroy( h ); h = o.h, own = false; } // "both must be kept alive" (README.md:99)
@@ -175,15 +176,13 @@ public:
 		remember( vertices, (uint32_t)sizeof( Vec4 ), 0, primCount ), sync_info();
 	}
 	// BVH::Refit( nodeIdx = 0 ) tiny_bvh.h:3055 - the caller moved the vertices in the array it built from; like the reference the
-	// shim kept the pointer (BVHBase::verts, "we're not copying this data" :2055), the engine receives the new positions
+	// shim kept the pointer (BVHBase::verts, "we're not copying this data" :2055), the engine receives the new positions.  Indexed
+	// geometry: the vertex array itself, read on the device through the indices the engine kept from the build (vertIdx, :806-807)
 	void Refit( const uint32_t = 0 )
 	{
-		float* flat = 0;
-		uint32_t stride = 0;
-		const void* v = refit_verts( flat, stride, "BVH::Refit" );
-		const int rc = tbvh_refit( h, v, stride, vertsPrims, TBVH_HOST );
-		free( flat );
-		TBVH_FATAL_IF( rc, "BVH::Refit" );
+		const tbvh_mesh m = refit_mesh( "BVH::Refit" );
+		tbvh_bvh hb = h;
+		TBVH_FATAL_IF( m.vert_count ? tbvh_refit_batch_indexed( &hb, &m, 1, TBVH_HOST, 0 ) : tbvh_refit( h, m.verts, m.stride, m.prim_count, TBVH_HOST ), "BVH::Refit" );
 		sync_info();
 	}
 	// BVH::BuildHQ( const bvhvec4*, uint32_t ) tiny_bvh.h:2623 - SBVH (spatial splits), ends with Compact()
@@ -238,8 +237,8 @@ public:
 		sync_info();
 	}
 	// indexed geometry: BVH::Build / BuildAVX / BuildHQ( vertices, indices, primCount ) tiny_bvh.h:889-900
-	template <class Vec4> void Build( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { build_indexed( vertices, indices, primCount, TBVH_BUILD_REFERENCE, "BVH::Build" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount ), sync_info(); }
-	template <class Vec4> void BuildAVX( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { build_indexed( vertices, indices, primCount, TBVH_BUILD_AVX, "BVH::BuildAVX" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount ), sync_info(); }
+	template <class Vec4> void Build( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { const uint32_t n = build_indexed( vertices, indices, primCount, TBVH_BUILD_REFERENCE, "BVH::Build" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount, n ), sync_info(); }
+	template <class Vec4> void BuildAVX( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { const uint32_t n = build_indexed( vertices, indices, primCount, TBVH_BUILD_AVX, "BVH::BuildAVX" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount, n ), sync_info(); }
 	template <class Vec4> void BuildHQ( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { build_indexed( vertices, indices, primCount, TBVH_BUILD_HQ, "BVH::BuildHQ" ); sync_info(); }
 	// BVH::SAHCost( nodeIdx = 0 ) tiny_bvh.h:1889 - the reference's value, bit for bit
 	float SAHCost( const uint32_t = 0 ) const { float c = 0; TBVH_FATAL_IF( tbvh_sah_cost( h, c_trav, c_int, &c ), "BVH::SAHCost" ); return c; }
@@ -304,21 +303,18 @@ private:
 	template <class T, class Vec4> friend void BuildBatch( T* const*, const Vec4* const*, const uint32_t*, uint32_t, int );
 	friend void RefitBatch( BVH* const*, uint32_t );
 	void batch_built( const void* v, uint32_t stride, uint32_t prims ) { remember( v, stride, 0, prims ), sync_info(); }
-	// the vertices a refit hands the engine: the caller's array, or - indexed geometry - its triangles resolved on the host into the
-	// flat order the engine keeps (into `flat`, which the caller frees)
-	const void* refit_verts( float*& flat, uint32_t& stride, const char* what ) const
+	// the mesh a refit hands the engine (tbvh_refit_batch_indexed): the caller's array the object was built from - a flat triangle
+	// soup, or the vertices of indexed geometry with their count, which the engine reads through the indices it kept
+	tbvh_mesh refit_mesh( const char* what ) const
 	{
 		if (!vertsPtr) { fprintf( stderr, "Fatal error in tinybvh_b200 %s: nothing was built from a host vertex array.\n", what ); exit( 1 ); }
-		stride = vertsStride;
-		if (!vertIdx) return vertsPtr;
-		flat = (float*)malloc( (size_t)vertsPrims * 3 * 16 );
-		for (size_t i = 0; i < (size_t)vertsPrims * 3; i++) memcpy( flat + i * 4, (const char*)vertsPtr + (size_t)vertIdx[i] * vertsStride, vertsStride < 16 ? vertsStride : 16 );
-		stride = 16;
-		return flat;
+		tbvh_mesh m = {};
+		m.verts = vertsPtr, m.stride = vertsStride, m.vert_count = vertIdx ? vertsCount : 0, m.prim_count = vertsPrims;
+		return m;
 	}
-	void remember( const void* v, uint32_t stride, const uint32_t* idx, uint32_t prims ) { vertsPtr = v, vertsStride = stride, vertIdx = idx, vertsPrims = prims; }
+	void remember( const void* v, uint32_t stride, const uint32_t* idx, uint32_t prims, uint32_t nverts = 0 ) { vertsPtr = v, vertsStride = stride, vertIdx = idx, vertsPrims = prims, vertsCount = nverts; }
 	const void* vertsPtr = 0; const uint32_t* vertIdx = 0; // BVHBase::verts / vertIdx (:806-807): pointers to the caller's arrays, for Refit
-	uint32_t vertsStride = 16, vertsPrims = 0;
+	uint32_t vertsStride = 16, vertsPrims = 0, vertsCount = 0; // vertsCount: vertices of an indexed build (the largest index + 1)
 };
 
 class BVH_GPU : public BVHBase
@@ -462,16 +458,13 @@ inline void RefitBatch( BVH* const* objs, uint32_t count )
 {
 	tbvh_bvh* hs = (tbvh_bvh*)malloc( sizeof( tbvh_bvh ) * (count ? count : 1) );
 	tbvh_mesh* ms = (tbvh_mesh*)calloc( count ? count : 1, sizeof( tbvh_mesh ) );
-	float** flat = (float**)calloc( count ? count : 1, sizeof( float* ) );
 	for (uint32_t k = 0; k < count; k++)
 	{
 		hs[k] = objs[k] ? objs[k]->handle() : 0;
-		if (!objs[k]) continue;
-		ms[k].verts = objs[k]->refit_verts( flat[k], ms[k].stride, "RefitBatch" ), ms[k].prim_count = objs[k]->vertsPrims;
+		if (objs[k]) ms[k] = objs[k]->refit_mesh( "RefitBatch" );
 	}
-	const int rc = tbvh_refit_batch( hs, ms, count, TBVH_HOST, 0 );
-	for (uint32_t k = 0; k < count; k++) free( flat[k] );
-	free( flat ), free( ms ), free( hs );
+	const int rc = tbvh_refit_batch_indexed( hs, ms, count, TBVH_HOST, 0 );
+	free( ms ), free( hs );
 	TBVH_FATAL_IF( rc, "RefitBatch" );
 	for (uint32_t k = 0; k < count; k++) objs[k]->sync_info();
 }

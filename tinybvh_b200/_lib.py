@@ -57,6 +57,7 @@ SYMBOLS = {
     "tbvh_refit": (i32, [vp, vp, u32, u32, i32]),
     "tbvh_refit_layouts": (i32, [vp, vp, u32, u32, i32]),
     "tbvh_refit_batch": (i32, [vp, vp, u32, i32, i32]),
+    "tbvh_refit_batch_indexed": (i32, [vp, vp, u32, i32, i32]),
     "tbvh_build_indexed": (i32, [vp, vp, u32, u32, vp, u32, i32, f32, f32, i32]),
     "tbvh_build_batch": (i32, [vp, vp, u32, i32, f32, f32, i32]),
     "tbvh_build_batch_hq": (i32, [vp, vp, u32, i32, f32, f32]),

@@ -93,10 +93,12 @@ class _Base:
         self.h = C.c_void_p()
         check(_lib.lib().tbvh_bvh_create(self.ctx, C.byref(self.h)))
         self.c_trav, self.c_int = 1.0, 1.0  # BVHBase::c_trav / c_int (:819-820)
+        self.vert_count = 0                 # vertices of the last build when it was indexed (refit_batch_indexed), else 0
 
     def _build(self, vertices, primCount, flavour, indices=None):
         """tbvh_build_flavour, or tbvh_build_indexed for the (vertices, indices, primCount) overloads (tiny_bvh.h:889-900)."""
         p, stride, nv, space, keep = _verts_arg(vertices)
+        self.vert_count = 0
         if indices is None:
             check(_lib.lib().tbvh_build_flavour(self.h, p, stride, primCount or nv // 3, space, self.c_trav, self.c_int, flavour))
             return
@@ -108,6 +110,7 @@ class _Base:
             indices = np.ascontiguousarray(indices, np.uint32).reshape(-1)
             ip, ni = _np_ptr(indices), indices.shape[0]
         check(_lib.lib().tbvh_build_indexed(self.h, p, stride, nv, ip, primCount or ni // 3, space, self.c_trav, self.c_int, flavour))
+        self.vert_count = nv
 
     def __del__(self):
         try:
@@ -222,6 +225,7 @@ class BVH(_Base):
         nodes = np.ascontiguousarray(nodes)
         primIdx = np.ascontiguousarray(primIdx, np.uint32)
         assert nodes.dtype.itemsize == 32
+        self.vert_count = 0
         check(_lib.lib().tbvh_upload_bvh(self.h, _np_ptr(nodes), nodes.shape[0], _np_ptr(primIdx), primIdx.shape[0], p, stride, nv // 3, space))
         return self
 
@@ -258,6 +262,7 @@ class TLAS(BVH):
             for i in range(inst.shape[0]):
                 check(_lib.lib().tbvh_instance_update(C.c_void_p(inst[i:i + 1].ctypes.data), self.blasses[int(inst["blasIdx"][i])].h))
         hs = (C.c_void_p * len(self.blasses))(*[b.h for b in self.blasses])
+        self.vert_count = 0
         check(_lib.lib().tbvh_build_tlas(self.h, _np_ptr(inst), 192, inst.shape[0], hs, len(self.blasses), self.c_trav, self.c_int))
         return self
 
@@ -286,6 +291,7 @@ class TLAS(BVH):
                                                   instances.ndim == 2 and instances.dtype.itemsize == 1 and instances.strides[1] == 1 and instances.shape[1] >= 160)
             p, stride, n, space = _np_ptr(instances), instances.strides[0], instances.shape[0], HOST
         hs = (C.c_void_p * len(self.blasses))(*[b.h for b in self.blasses])
+        self.vert_count = 0
         check(_lib.lib().tbvh_build_tlas_update(self.h, p, stride, n, space, hs, len(self.blasses), self.c_trav, self.c_int))
         return self
 
@@ -322,6 +328,7 @@ class BVH_GPU(_Base):
         nodes = np.ascontiguousarray(nodes)
         primIdx = np.ascontiguousarray(primIdx, np.uint32)
         assert nodes.dtype.itemsize == 64
+        self.vert_count = 0
         check(_lib.lib().tbvh_upload_bvh_gpu(self.h, _np_ptr(nodes), nodes.shape[0], _np_ptr(primIdx), primIdx.shape[0], p, stride, nv // 3, space))
         return self
 
@@ -409,6 +416,8 @@ def build_batch(bvhs, meshes, flavour: int = _lib.BUILD_REFERENCE, indices=None)
         check(_lib.lib().tbvh_build_batch_hq(hs, recs, len(meshes), space, c_trav, c_int))
     else:
         check(_lib.lib().tbvh_build_batch(hs, recs, len(meshes), space, c_trav, c_int, flavour))
+    for b, r in zip(bvhs, recs):
+        b.vert_count = r.vert_count
     cw = [b for b in bvhs if b.layout == LAYOUT_CWBVH]
     if cw:
         convert_batch(cw)
@@ -434,24 +443,42 @@ def refit_batch(objs, meshes, keep_layouts=None):
     own Refit: BVH objects drop their derived layouts (tbvh_refit, keep_layouts=0), BVH_GPU and BVH8_CWBVH objects keep them up to date
     (tbvh_refit_layouts, keep_layouts=1); objects of both kinds in one call need an explicit keep_layouts.  A refused call raises
     TbvhError and leaves every object as it was."""
+    return _refit_batch("refit_batch", objs, meshes, keep_layouts, False)
+
+
+def refit_batch_indexed(objs, meshes, keep_layouts=None):
+    """tbvh_refit_batch_indexed: refit_batch for a scene with indexed meshes.  For an object whose last build was indexed
+    (Build( vertices, indices=.. ), build_batch with indices) its mesh holds the new positions of the vertices it was built from - the
+    same number of rows -, which the engine reads through the indices it kept from the build; for any other object its mesh is the flat
+    triangle soup, as in refit_batch.  Each object ends up as its refit from vertices[indices] would leave it.  `meshes`: numpy arrays
+    or torch CUDA tensors, one space per call; keep_layouts as for refit_batch.  A refused call raises TbvhError and leaves every
+    object as it was."""
+    return _refit_batch("refit_batch_indexed", objs, meshes, keep_layouts, True)
+
+
+def _refit_batch(fn, objs, meshes, keep_layouts, indexed):
     objs, meshes = list(objs), list(meshes)
     if len(objs) != len(meshes):
-        raise TbvhError("refit_batch: one object per mesh")
+        raise TbvhError(f"{fn}: one object per mesh")
     if len({_is_torch(m) for m in meshes}) > 1:
-        raise TbvhError("refit_batch: host and device meshes in one call")
+        raise TbvhError(f"{fn}: host and device meshes in one call")
     if keep_layouts is None:
         rule = {b.layout != LAYOUT_BVH for b in objs}
         if len(rule) > 1:
-            raise TbvhError("refit_batch: BVH objects drop their layouts, BVH_GPU / BVH8_CWBVH objects keep them: pass keep_layouts")
+            raise TbvhError(f"{fn}: BVH objects drop their layouts, BVH_GPU / BVH8_CWBVH objects keep them: pass keep_layouts")
         keep_layouts = rule.pop() if rule else False
     recs = (_lib.Mesh * max(len(meshes), 1))()
     keep, space = [], HOST
-    for r, m in zip(recs, meshes):
+    for r, m, b in zip(recs, meshes, objs):
         p, stride, nv, space, k = _verts_arg(m)
         keep.append(k)
-        r.verts, r.stride, r.vert_count, r.indices, r.prim_count = p.value, stride, 0, None, nv // 3
+        if indexed and b.vert_count:
+            r.verts, r.stride, r.vert_count, r.indices, r.prim_count = p.value, stride, nv, None, b.triCount
+        else:
+            r.verts, r.stride, r.vert_count, r.indices, r.prim_count = p.value, stride, 0, None, nv // 3
     hs = (C.c_void_p * max(len(objs), 1))(*[b.h for b in objs])
-    check(_lib.lib().tbvh_refit_batch(hs, recs, len(meshes), space, int(keep_layouts)))
+    entry = _lib.lib().tbvh_refit_batch_indexed if indexed else _lib.lib().tbvh_refit_batch
+    check(entry(hs, recs, len(meshes), space, int(keep_layouts)))
     return objs
 
 

@@ -256,6 +256,7 @@ int tbvh_ctx_destroy( tbvh_ctx c )
 	if (c->refit_host) cudaFreeHost( c->refit_host );
 	if (c->refit_e0) cudaEventDestroy( c->refit_e0 );
 	if (c->refit_e1) cudaEventDestroy( c->refit_e1 );
+	if (c->ix_dev) cudaFree( c->ix_dev );
 	delete c->pool;
 	delete c;
 	return TBVH_OK;
@@ -385,9 +386,9 @@ static void free_layouts( tbvh_bvh b )
 	drop_bvh_gpu( b );
 	drop_cwbvh( b );
 	if (b->d_trav && b->d_trav != b->d_nodes) cudaFree( b->d_trav );
-	void* p[] = { b->d_verts, b->d_nodes, b->d_prim_idx, b->d_leaf_tris, b->d_aabbs, b->d_inst, b->d_blas, b->d_inst_stage };
+	void* p[] = { b->d_verts, b->d_vert_idx, b->d_nodes, b->d_prim_idx, b->d_leaf_tris, b->d_aabbs, b->d_inst, b->d_blas, b->d_inst_stage };
 	for (void* q : p) if (q) cudaFree( q );
-	b->d_verts = 0, b->d_nodes = 0, b->d_prim_idx = 0, b->d_leaf_tris = 0, b->d_trav = 0, b->leaf_tris_count = 0;
+	b->d_verts = 0, b->d_vert_idx = 0, b->vert_count = 0, b->d_nodes = 0, b->d_prim_idx = 0, b->d_leaf_tris = 0, b->d_trav = 0, b->leaf_tris_count = 0;
 	b->d_aabbs = 0, b->d_inst = 0, b->d_blas = 0, b->d_inst_stage = 0, b->blas_table_bytes = 0, b->inst_count = 0, b->blas_count = 0, b->tlas_blas_layouts = 0;
 	b->tlas_deep_blas = 0, b->tlas_deep_depth = 0;
 	b->links.clear();
@@ -433,17 +434,20 @@ int tbvh_get_stats_ex( tbvh_bvh b, uint64_t out[4] )
 
 // ---- uploads ------------------------------------------------------------------------------------------------
 
-// vertices -> engine-owned float4 array (xyz of each vertex, w copied when the stride holds it)
-static int copy_verts( float4* dst, const void* verts, uint32_t stride, size_t nv, int space, cudaStream_t s )
+// nv vertices `stride` bytes apart -> rows of a 16-byte-pitch array: the first min( stride, 16 ) bytes of each, so below stride 16
+// the w lane of dst is left as it was
+static int copy_rows( float4* dst, const void* verts, uint32_t stride, size_t nv, int space, cudaStream_t s )
 {
 	const cudaMemcpyKind kind = space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
 	if (stride == 16) CUDA_TRY( cudaMemcpyAsync( dst, verts, nv * 16, kind, s ) );
-	else
-	{
-		CUDA_TRY( cudaMemsetAsync( dst, 0, nv * 16, s ) );
-		CUDA_TRY( cudaMemcpy2DAsync( dst, 16, verts, stride, stride < 16 ? stride : 16, nv, kind, s ) );
-	}
+	else CUDA_TRY( cudaMemcpy2DAsync( dst, 16, verts, stride, stride < 16 ? stride : 16, nv, kind, s ) );
 	return TBVH_OK;
+}
+// vertices -> engine-owned float4 array (xyz of each vertex, w copied when the stride holds it)
+static int copy_verts( float4* dst, const void* verts, uint32_t stride, size_t nv, int space, cudaStream_t s )
+{
+	if (stride != 16) CUDA_TRY( cudaMemsetAsync( dst, 0, nv * 16, s ) );
+	return copy_rows( dst, verts, stride, nv, space, s );
 }
 static int upload_verts( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space, cudaStream_t s )
 {
@@ -466,8 +470,26 @@ __global__ void k_gather_verts( const float4* __restrict__ src, const uint32_t* 
 	if (v >= vert_count) { atomicAdd( bad, 1u ); dst[i] = make_float4( 0, 0, 0, 0 ); return; }
 	dst[i] = src[v];
 }
-// the gather into dst; indices past vert_count are counted into d_bad.  Synchronises the stream.
-static int gather_verts( float4* dst, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space, cudaStream_t s, uint32_t* d_bad )
+// An indexed refit (tbvh_refit_batch_indexed) reads the moved vertices through the indices kept from the build, as BVH::Refit reads
+// them through vertIdx (tiny_bvh.h:3055): one thread per kept index of every indexed mesh of the call.  The indices were checked at
+// build time and the vertex count is the build's, so there is no bounds check.  One mesh: its staged new vertices (16-byte pitch),
+// its kept indices, the handle's d_verts, its first index in the call's index space, and full = the stride holds w (>= 16), when
+// all four lanes are written; below stride 16 w of d_verts stays, as refit_copy leaves it (k_encode writes v.w differences).
+struct IxMesh { const float4* src; const uint32_t* idx; float4* dst; uint32_t base, full; };
+__global__ void k_refit_gather( const IxMesh* __restrict__ T, const uint32_t K, const uint32_t n )
+{
+	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+	if (g >= n) return;
+	const IxMesh& m = T[batch_entry<IxMesh, &IxMesh::base>( T, K, g )];
+	const uint32_t i = g - m.base;
+	const float4 v = m.src[m.idx[i]];
+	if (m.full) m.dst[i] = v;
+	else m.dst[i] = make_float4( v.x, v.y, v.z, m.dst[i].w );
+}
+// the gather into dst; indices past vert_count are counted into d_bad.  Synchronises the stream.  keep_idx: NULL, or where the
+// device copy of the indices is handed to the caller (who frees it) instead of being freed here
+static int gather_verts( float4* dst, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space, cudaStream_t s, uint32_t* d_bad,
+	uint32_t** keep_idx )
 {
 	const size_t nv = (size_t)prim_count * 3;
 	const cudaMemcpyKind kind = space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
@@ -483,10 +505,13 @@ static int gather_verts( float4* dst, const void* verts, uint32_t stride, uint32
 	};
 	const int rc = body();
 	cudaStreamSynchronize( s );
-	cudaFree( d_src ), cudaFree( d_idx );
+	cudaFree( d_src );
+	if (rc == TBVH_OK && keep_idx) *keep_idx = d_idx; else cudaFree( d_idx );
 	return rc;
 }
-static int upload_verts_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space, cudaStream_t s )
+// keep: the handle keeps the indices and vert_count for tbvh_refit_batch_indexed (a refittable build)
+static int upload_verts_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space, cudaStream_t s,
+	bool keep )
 {
 	ARG_CHECK( verts && indices && stride >= 12 && (stride & 3) == 0 && prim_count > 0 && vert_count > 0, "bad indexed vertex slice" );
 	const size_t nv = (size_t)prim_count * 3;
@@ -497,7 +522,7 @@ static int upload_verts_indexed( tbvh_bvh b, const void* verts, uint32_t stride,
 		CUDA_TRY( cudaMalloc( &d_bad, 4 ) );
 		CUDA_TRY( cudaMalloc( &b->d_verts, nv * 16 ) );
 		CUDA_TRY( cudaMemsetAsync( d_bad, 0, 4, s ) );
-		TRY( gather_verts( b->d_verts, verts, stride, vert_count, indices, prim_count, space, s, d_bad ) );
+		TRY( gather_verts( b->d_verts, verts, stride, vert_count, indices, prim_count, space, s, d_bad, keep ? &b->d_vert_idx : 0 ) );
 		uint32_t bad = 0;
 		CUDA_TRY( cudaMemcpy( &bad, d_bad, 4, cudaMemcpyDeviceToHost ) );
 		if (bad) { tbvh_set_error( "indexed build: %u indices point past the %u vertices", bad, vert_count ); return TBVH_E_ARG; }
@@ -505,6 +530,8 @@ static int upload_verts_indexed( tbvh_bvh b, const void* verts, uint32_t stride,
 	};
 	rc = body();
 	cudaFree( d_bad );
+	if (rc != TBVH_OK && b->d_vert_idx) cudaFree( b->d_vert_idx ), b->d_vert_idx = 0;
+	b->vert_count = b->d_vert_idx ? vert_count : 0;
 	b->info.prim_count = prim_count;
 	return rc;
 }
@@ -584,11 +611,39 @@ static int refit_check( const char* fn, tbvh_bvh b, const void* verts, uint32_t 
 // the new vertices of a refit.  Unlike copy_verts the copy leaves w alone below stride 16 (k_encode writes v.w differences into bvh8Tris)
 static int refit_copy( tbvh_bvh b, const void* verts, uint32_t stride, int space )
 {
-	cudaStream_t s = b->ctx->stream;
-	const size_t nv = (size_t)b->info.prim_count * 3;
-	const cudaMemcpyKind kind = space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-	if (stride == 16) CUDA_TRY( cudaMemcpyAsync( b->d_verts, verts, nv * 16, kind, s ) );
-	else CUDA_TRY( cudaMemcpy2DAsync( b->d_verts, 16, verts, stride, stride < 16 ? stride : 16, nv, kind, s ) );
+	return copy_rows( b->d_verts, verts, stride, (size_t)b->info.prim_count * 3, space, b->ctx->stream );
+}
+
+// the new vertices of the indexed meshes of a refit (meshes[k].vert_count > 0, n kept indices in all): each mesh's vert_count rows
+// staged at a 16-byte pitch into the context's buffer, then one k_refit_gather for all of them.  The caller holds c->ix_mutex until
+// the stream has run the gather.
+static int refit_gather( tbvh_ctx c, const tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, uint64_t n )
+{
+	cudaStream_t s = c->stream;
+	std::vector<IxMesh> T;
+	size_t rows = 0;
+	for (uint32_t k = 0, base = 0; k < count; k++) if (meshes[k].vert_count)
+	{
+		T.push_back( IxMesh{ 0, bvhs[k]->d_vert_idx, bvhs[k]->d_verts, base, meshes[k].stride >= 16 ? 1u : 0u } );
+		rows += meshes[k].vert_count, base += meshes[k].prim_count * 3;
+	}
+	const size_t o_rows = (T.size() * sizeof( IxMesh ) + 255) & ~(size_t)255, bytes = o_rows + rows * 16;
+	if (bytes > c->ix_dev_bytes)
+	{
+		if (c->ix_dev) cudaFree( c->ix_dev );
+		c->ix_dev = 0, c->ix_dev_bytes = 0;
+		CUDA_TRY( cudaMalloc( &c->ix_dev, bytes + bytes / 4 ) );
+		c->ix_dev_bytes = bytes + bytes / 4;
+	}
+	float4* at = (float4*)((char*)c->ix_dev + o_rows);
+	for (uint32_t k = 0, i = 0; k < count; k++) if (meshes[k].vert_count)
+	{
+		T[i++].src = at;
+		TRY( copy_rows( at, meshes[k].verts, meshes[k].stride, meshes[k].vert_count, space, s ) );
+		at += meshes[k].vert_count;
+	}
+	CUDA_TRY( cudaMemcpyAsync( c->ix_dev, T.data(), T.size() * sizeof( IxMesh ), cudaMemcpyHostToDevice, s ) );
+	k_refit_gather<<<(unsigned)((n + 255) / 256), 256, 0, s>>>( (const IxMesh*)c->ix_dev, (uint32_t)T.size(), (uint32_t)n ); LAUNCHED();
 	return TBVH_OK;
 }
 
@@ -897,45 +952,70 @@ int tbvh_refit_layouts( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t
 	return refit_one( __func__, b, verts, stride, prim_count, space, true );
 }
 
-// Many trees, one refit (include/tinybvh_b200.h).  Refit validation is host-side only: every refusal comes before any handle or
-// vertex array is touched, then the vertices are copied and the trees refitted together.
-int tbvh_refit_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts )
+// Many trees, one refit (include/tinybvh_b200.h): tbvh_refit_batch, and with `indexed` tbvh_refit_batch_indexed, whose meshes with a
+// vert_count are the moved vertices of an indexed build.  Refit validation is host-side only: every refusal comes before any handle
+// or vertex array is touched, then the vertices are copied (indexed meshes: gathered) and the trees refitted together.
+static int refit_batch( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts, bool indexed )
 {
-	ARG_CHECK( bvhs && meshes && count > 0, "no meshes" );
-	ARG_CHECK( space == TBVH_HOST || space == TBVH_DEVICE, "unknown space" );
-	ARG_CHECK( keep_layouts == 0 || keep_layouts == 1, "keep_layouts is 0 or 1" );
-	TRY( check_batch_handles( __func__, bvhs, count ) );
-	uint64_t nodes = 0, refs = 0, split = 0, wide = 0;
+	if (!(bvhs && meshes && count > 0)) { tbvh_set_error( "%s: no meshes", fn ); return TBVH_E_ARG; }
+	if (space != TBVH_HOST && space != TBVH_DEVICE) { tbvh_set_error( "%s: unknown space", fn ); return TBVH_E_ARG; }
+	if (keep_layouts != 0 && keep_layouts != 1) { tbvh_set_error( "%s: keep_layouts is 0 or 1", fn ); return TBVH_E_ARG; }
+	TRY( check_batch_handles( fn, bvhs, count ) );
+	uint64_t nodes = 0, refs = 0, split = 0, wide = 0, ix = 0;
 	for (uint32_t k = 0; k < count; k++)
 	{
 		const tbvh_mesh& m = meshes[k];
-		if (m.indices || m.vert_count) { tbvh_set_error( "tbvh_refit_batch: mesh %u: a refit takes a flat vertex slice (indices NULL, vert_count 0)", k ); return TBVH_E_ARG; }
-		TRY( refit_check( __func__, bvhs[k], m.verts, m.stride, m.prim_count, keep_layouts != 0 ) );
+		if (!indexed && (m.indices || m.vert_count)) { tbvh_set_error( "%s: mesh %u: a refit takes a flat vertex slice (indices NULL, vert_count 0)", fn, k ); return TBVH_E_ARG; }
+		if (m.indices) { tbvh_set_error( "%s: mesh %u: an indexed refit reads the indices kept from the build (indices NULL)", fn, k ); return TBVH_E_ARG; }
+		TRY( refit_check( fn, bvhs[k], m.verts, m.stride, m.prim_count, keep_layouts != 0 ) );
+		if (m.vert_count)
+		{
+			const tbvh_bvh b = bvhs[k];
+			if (!b->d_vert_idx) { tbvh_set_error( "%s: mesh %u: the tree was not built from indexed geometry by a refittable builder, so it keeps no indices", fn, k ); return TBVH_E_STATE; }
+			if (m.vert_count != b->vert_count) { tbvh_set_error( "%s: mesh %u: %u vertices, the tree was built from %u", fn, k, m.vert_count, b->vert_count ); return TBVH_E_ARG; }
+			ix += (uint64_t)m.prim_count * 3;
+		}
 		uint32_t t = 0, w = 0;
 		if (keep_layouts) cw_keep_sizes( bvhs[k], &t, &w );
 		nodes += bvhs[k]->info.used_nodes, refs += bvhs[k]->info.idx_count, split += t, wide += w;
 	}
-	if (std::max( std::max( nodes, refs ), std::max( split, wide ) ) > TBVH_REFIT_BATCH_MAX_NODES)
+	if (std::max( std::max( std::max( nodes, refs ), std::max( split, wide ) ), ix ) > TBVH_REFIT_BATCH_MAX_NODES)
 	{
-		tbvh_set_error( "tbvh_refit_batch: %llu BVH2 nodes, %llu primitive references, %llu split-tree and %llu wide nodes in one batch (at most %u each)",
-			(unsigned long long)nodes, (unsigned long long)refs, (unsigned long long)split, (unsigned long long)wide, (unsigned)TBVH_REFIT_BATCH_MAX_NODES );
+		tbvh_set_error( "%s: %llu BVH2 nodes, %llu primitive references, %llu split-tree and %llu wide nodes, %llu vertex indices in one batch (at most %u each)", fn,
+			(unsigned long long)nodes, (unsigned long long)refs, (unsigned long long)split, (unsigned long long)wide, (unsigned long long)ix, (unsigned)TBVH_REFIT_BATCH_MAX_NODES );
 		return TBVH_E_LIMIT;
 	}
 	const tbvh_ctx ctx = bvhs[0]->ctx;
 	CUDA_TRY( cudaSetDevice( ctx->device ) );
-	for (uint32_t k = 0; k < count; k++)
+	std::unique_lock<std::mutex> staging( ctx->ix_mutex, std::defer_lock );
+	if (ix) staging.lock(); // released after refit_trees has synchronised the stream, so the gather has read the staged vertices
+	auto copies = [&]() -> int
 	{
-		const int rc = refit_copy( bvhs[k], meshes[k].verts, meshes[k].stride, space );
-		if (rc != TBVH_OK) { cudaStreamSynchronize( ctx->stream ); for (uint32_t j = 0; j < count; j++) drop_bvh_gpu( bvhs[j] ), drop_cwbvh( bvhs[j] ); return rc; }
-	}
+		for (uint32_t k = 0; k < count; k++) if (!meshes[k].vert_count) TRY( refit_copy( bvhs[k], meshes[k].verts, meshes[k].stride, space ) );
+		if (ix) TRY( refit_gather( ctx, bvhs, meshes, count, space, ix ) );
+		return TBVH_OK;
+	};
+	const int rc = copies();
+	if (rc != TBVH_OK) { cudaStreamSynchronize( ctx->stream ); for (uint32_t j = 0; j < count; j++) drop_bvh_gpu( bvhs[j] ), drop_cwbvh( bvhs[j] ); return rc; }
 	return refit_trees( bvhs, count, keep_layouts != 0, ctx->stream );
+}
+
+int tbvh_refit_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts )
+{
+	return refit_batch( __func__, bvhs, meshes, count, space, keep_layouts, false );
+}
+
+// Many trees, one refit, indexed meshes through their kept indices (include/tinybvh_b200.h)
+int tbvh_refit_batch_indexed( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts )
+{
+	return refit_batch( __func__, bvhs, meshes, count, space, keep_layouts, true );
 }
 
 int tbvh_build_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space,
 	float c_trav, float c_int, int flavour )
 {
 	return build_one( __func__, b, c_trav, c_int, flavour,
-		[&]( cudaStream_t s ) { return upload_verts_indexed( b, verts, stride, vert_count, indices, prim_count, space, s ); } );
+		[&]( cudaStream_t s ) { return upload_verts_indexed( b, verts, stride, vert_count, indices, prim_count, space, s, flavour != TBVH_BUILD_HQ ); } );
 }
 
 // The shared part of tbvh_build_batch / tbvh_build_batch_hq (include/tinybvh_b200.h) up to the build.  Every refusal comes before any
@@ -967,6 +1047,7 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 	CUDA_TRY( cudaSetDevice( ctx->device ) );
 	cudaStream_t s = ctx->stream;
 	std::vector<float4*> staged( count, (float4*)0 );
+	std::vector<uint32_t*> staged_idx( count, (uint32_t*)0 ); // indexed meshes of a refittable batch: the indices the handle keeps
 	uint32_t* d_bad = 0;
 	auto stage = [&]() -> int
 	{
@@ -976,7 +1057,7 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 		{
 			const tbvh_mesh& m = meshes[k];
 			CUDA_TRY( cudaMalloc( &staged[k], (size_t)m.prim_count * 3 * 16 ) );
-			if (m.indices) TRY( gather_verts( staged[k], m.verts, m.stride, m.vert_count, m.indices, m.prim_count, space, s, d_bad ) );
+			if (m.indices) TRY( gather_verts( staged[k], m.verts, m.stride, m.vert_count, m.indices, m.prim_count, space, s, d_bad, hq ? 0 : &staged_idx[k] ) );
 			else TRY( copy_verts( staged[k], m.verts, m.stride, (size_t)m.prim_count * 3, space, s ) );
 		}
 		uint32_t bad = 0;
@@ -991,6 +1072,7 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 	{
 		cudaStreamSynchronize( s );
 		for (float4* p : staged) if (p) cudaFree( p );
+		for (uint32_t* p : staged_idx) if (p) cudaFree( p );
 		return rc;
 	}
 	for (uint32_t k = 0; k < count; k++)
@@ -998,6 +1080,7 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 		const tbvh_bvh b = bvhs[k];
 		free_layouts( b );
 		b->d_verts = staged[k], b->info.prim_count = meshes[k].prim_count;
+		b->d_vert_idx = staged_idx[k], b->vert_count = staged_idx[k] ? meshes[k].vert_count : 0;
 	}
 	return TBVH_OK;
 }

@@ -72,6 +72,10 @@ struct tbvh_ctx_t
 	void* refit_dev = 0; size_t refit_dev_bytes = 0;   // device: tables, arrival counters, parents, BVH_GPU workspace, results
 	void* refit_host = 0; size_t refit_host_bytes = 0; // page-locked: the tables on their way in, the results on their way out
 	cudaEvent_t refit_e0 = 0, refit_e1 = 0;
+	// indexed refits (api.cu tbvh_refit_batch_indexed): the new vertices of the call's indexed meshes at a 16-byte pitch and the gather
+	// table, kept and grown; the mutex is held for the whole call (the refit inside it takes refit_mutex)
+	std::mutex ix_mutex;
+	void* ix_dev = 0; size_t ix_dev_bytes = 0;
 };
 #define TBVH_COUNTERS 256
 
@@ -84,6 +88,10 @@ struct tbvh_bvh_t
 	tbvh_info info = {};
 	// geometry (engine-owned copy, float4 per vertex)
 	float4* d_verts = 0;
+	// indexed, refittable builds: the 3 * prim_count vertex indices and the vertex count (BVHBase::vertIdx, tiny_bvh.h:806-807), through
+	// which tbvh_refit_batch_indexed writes d_verts from the new positions.  Dropped with the tree (free_layouts); 0 otherwise.
+	uint32_t* d_vert_idx = 0;
+	uint32_t vert_count = 0;
 	// LAYOUT_BVH: reference node array; children of an interior node are the 64-byte pair at nodes[leftFirst]
 	float4* d_nodes = 0;       // 2 float4 per node
 	uint32_t* d_prim_idx = 0;
