@@ -333,6 +333,43 @@ int tbvh_occluded( tbvh_bvh bvh, int layout, const void* rays, uint32_t stride, 
 int tbvh_intersect_device( tbvh_bvh bvh, int layout, void* d_rays, uint32_t stride, void* d_hits, uint64_t n, void* stream );
 int tbvh_occluded_device( tbvh_bvh bvh, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, void* stream );
 
+/* Traversal from the caller's own kernels (include/tinybvh_b200_device.cuh): the traversal functions of the reference's GPU code
+ * (traverse_cwbvh / isoccluded_cwbvh, traverse_ailalaine, traverse_tlas / isoccluded_tlas, SURVEY.md 2.3) as device functions over a
+ * view of a resident tree.  A view holds what the matching tbvh_intersect_device / tbvh_occluded_device launch passes its kernel:
+ * plain device pointers, the root, and the walk's limits.  It is passed to a kernel by value (64 bytes).
+ *  tbvh_device_view  the view of `bvh` for `layout`, which means what it means in tbvh_intersect_device: TBVH_LAYOUT_BVH or
+ *                    TBVH_LAYOUT_BVH_GPU -> kind TBVH_VIEW_BVH (the BVH2 walk), TBVH_LAYOUT_CWBVH -> TBVH_VIEW_CWBVH; on a TLAS the
+ *                    layout its BLASses are walked in -> TBVH_VIEW_TLAS_BVH / TBVH_VIEW_TLAS_CWBVH.
+ *  Refusals are exactly those of tbvh_intersect_device / tbvh_occluded_device for the same handle and layout (n > 0), with the same
+ *  codes: TBVH_E_STATE when the layout is not resident or a TLAS is stale; TBVH_E_LIMIT for a BVH2 of depth 256 or more, a CWBVH
+ *  that can leave more than CW_STACK node groups pending, or a TLAS walked in TBVH_LAYOUT_BVH over a BLAS too deep for it;
+ *  TBVH_E_ARG for a wide tree whose links form a cycle, an unknown layout, or NULL arguments.  A refused call leaves *out of kind 0,
+ *  which every device function ignores.
+ *  Taking a view is host work only: no launch, no copy, no synchronisation.
+ *  Lifetime: a view is valid as long as the batch call on the same handle would walk the same arrays.  A rebuild, an upload, a
+ *  (re)conversion, a tbvh_refit or refit batch that drops layouts, and tbvh_bvh_destroy end it; so does, for a TLAS, anything that
+ *  makes the TLAS stale (a BLAS rebuilt, re-uploaded, re-converted, refitted or destroyed), any rebuild of the TLAS itself, and
+ *  tbvh_set_option( inst_idx_bits ), whose value a TLAS view holds (inst_shift) where the batch call reads it at each launch.  Take
+ *  a new view per frame: a stale view is a dangling pointer, which no device function can detect. */
+#define TBVH_VIEW_BVH 1          /* tbvh::intersect_bvh / isoccluded_bvh */
+#define TBVH_VIEW_CWBVH 10       /* tbvh::intersect_cwbvh / isoccluded_cwbvh */
+#define TBVH_VIEW_TLAS_BVH 101   /* tbvh::intersect_tlas< TBVH_LAYOUT_BVH > / isoccluded_tlas< TBVH_LAYOUT_BVH > */
+#define TBVH_VIEW_TLAS_CWBVH 110 /* tbvh::intersect_tlas< TBVH_LAYOUT_CWBVH > / isoccluded_tlas< TBVH_LAYOUT_CWBVH > */
+typedef struct tbvh_view
+{
+	int32_t kind;                  /* TBVH_VIEW_*, 0 = no tree */
+	uint32_t root_ref, root_count; /* BVH2, TLAS: the root as a child record (count 0: child-pair index, else leaf range) */
+	uint32_t stack;                /* BVH2: traversal stack entries, 64 for a tree of depth below 64, else 256 */
+	const void* nodes;             /* BVH2: child-pair nodes; CWBVH: traversal nodes; TLAS: the TLAS's child-pair nodes */
+	const void* tris;              /* BVH2: leaf-ordered triangle records; CWBVH: bvh8Tris */
+	const void* prim_idx;          /* TLAS: primIdx (instance numbers) */
+	const void* inst;              /* TLAS: instance table (inverse transform, BLAS number, mask) */
+	const void* blas;              /* TLAS: BLAS table (each BLAS's traversal arrays) */
+	float cw_rd_limit;             /* CWBVH: rays with |rD| up to this (and |O| <= 2^126) may take the integer-ordered slab test */
+	uint32_t inst_shift;           /* TLAS: 32 - INST_IDX_BITS (tbvh_set_option inst_idx_bits), 0 = the instance goes to hit.inst */
+} tbvh_view;
+int tbvh_device_view( tbvh_bvh bvh, int layout, tbvh_view* out );
+
 /* counters of the last device traversal on this handle when statistics are enabled (debug aid; the reference
  * returns the per-ray cost from Intersect, tiny_bvh.h:3303): steps = nodes visited, tris = triangle tests. */
 int tbvh_set_stats( tbvh_bvh bvh, int enable );

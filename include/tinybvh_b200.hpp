@@ -113,6 +113,8 @@ public:
 		Sync();
 		return d;
 	}
+	// the view a kernel of the caller's passes to tbvh::intersect_* / isoccluded_* (include/tinybvh_b200_device.cuh); take a new one per frame
+	tbvh_view DeviceView() const { tbvh_view v; TBVH_FATAL_IF( tbvh_device_view( h, layout, &v ), "DeviceView" ); return v; }
 	void IntersectDevice( void* d_rays64, uint64_t n ) const { TBVH_FATAL_IF( tbvh_intersect_device( h, layout, d_rays64, 64, 0, n, 0 ), "IntersectDevice" ); }
 	void IsOccludedDevice( const void* d_rays64, uint64_t n, uint32_t* d_bits ) const { TBVH_FATAL_IF( tbvh_occluded_device( h, layout, d_rays64, 64, d_bits, n, 0 ), "IsOccludedDevice" ); }
 	// t,u,v,prim of n device records back into host Ray records

@@ -31,6 +31,17 @@ class Mesh(C.Structure):
     _fields_ = [("verts", C.c_void_p), ("stride", C.c_uint32), ("vert_count", C.c_uint32), ("indices", C.c_void_p), ("prim_count", C.c_uint32)]
 
 
+class DeviceView(C.Structure):
+    """tbvh_view: what tbvh_device_view hands a kernel that calls the device functions of include/tinybvh_b200_device.cuh (64 bytes,
+    passed by value or as bytes(view))"""
+    _fields_ = [("kind", C.c_int32), ("root_ref", C.c_uint32), ("root_count", C.c_uint32), ("stack", C.c_uint32),
+                ("nodes", C.c_void_p), ("tris", C.c_void_p), ("prim_idx", C.c_void_p), ("inst", C.c_void_p), ("blas", C.c_void_p),
+                ("cw_rd_limit", C.c_float), ("inst_shift", C.c_uint32)]
+
+
+VIEW_BVH, VIEW_CWBVH, VIEW_TLAS_BVH, VIEW_TLAS_CWBVH = 1, 10, 101, 110
+
+
 # every symbol include/tinybvh_b200.h declares: name -> (restype, argtypes)
 vp, u32, u64, i32, f32, sz = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int, C.c_float, C.c_size_t
 SYMBOLS = {
@@ -74,6 +85,7 @@ SYMBOLS = {
     "tbvh_occluded": (i32, [vp, i32, vp, u32, u64, vp]),
     "tbvh_intersect_device": (i32, [vp, i32, vp, u32, vp, u64, vp]),
     "tbvh_occluded_device": (i32, [vp, i32, vp, u32, vp, u64, vp]),
+    "tbvh_device_view": (i32, [vp, i32, C.POINTER(DeviceView)]),
     "tbvh_set_stats": (i32, [vp, i32]),
     "tbvh_get_stats": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),
     "tbvh_launch_count": (u64, []),

@@ -177,6 +177,13 @@ class _Base:
         check(L.tbvh_occluded(self.h, self.layout, _np_ptr(rays), rays.dtype.itemsize, n, _np_ptr(bits)))
         return bits
 
+    def device_view(self, layout: int = None) -> _lib.DeviceView:
+        """tbvh_device_view: the view a kernel of the caller's passes to the device functions of include/tinybvh_b200_device.cuh, for
+        `layout` (default: the layout Intersect walks).  Host work only; valid until the handle's arrays change (include/tinybvh_b200.h)."""
+        v = _lib.DeviceView()
+        check(_lib.lib().tbvh_device_view(self.h, self.layout if layout is None else layout, C.byref(v)))
+        return v
+
     def set_stats(self, enable: bool):
         check(_lib.lib().tbvh_set_stats(self.h, int(enable)))
 

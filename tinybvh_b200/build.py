@@ -10,6 +10,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
 SO = os.path.join(HERE, "libtinybvh_b200.so")
+DEVICE_HEADER = os.path.join(REPO, "include", "tinybvh_b200_device.cuh")  # the walks, shared with callers' kernels
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "--use_fast_math=false"]
 NVCC_FLAGS = [f for f in NVCC_FLAGS if f != "--use_fast_math=false"]  # never fast-math: parity is bit-exact
@@ -23,7 +24,8 @@ def stale() -> bool:
     if not os.path.isfile(SO):
         return True
     t = os.path.getmtime(SO)
-    deps = sources() + glob.glob(os.path.join(HERE, "csrc", "*.cuh")) + [os.path.join(REPO, "include", "tinybvh_b200.h")]
+    deps = (sources() + glob.glob(os.path.join(HERE, "csrc", "*.cuh")) + [os.path.join(REPO, "include", "tinybvh_b200.h"), DEVICE_HEADER]
+            + glob.glob(os.path.join(REPO, "include", "tinybvh_b200_device", "*.cuh")))
     return any(os.path.getmtime(d) > t for d in deps)
 
 

@@ -1250,6 +1250,36 @@ int tbvh_occluded_device( tbvh_bvh b, int layout, const void* d_rays, uint32_t s
 	return trace_dispatch( b, layout, d_rays, stride, 0, 0, d_bits, n, true, (cudaStream_t)stream );
 }
 
+// what the batch launch of the same handle and layout passes its kernel, after the same refusals (host only)
+int tbvh_device_view( tbvh_bvh b, int layout, tbvh_view* out )
+{
+	ARG_CHECK( b && out, "NULL argument" );
+	*out = tbvh_view{};
+	tbvh_view v{};
+	if (b->d_inst)
+	{
+		TRY( tlas_check( b, layout ) );
+		TRY( tlas_trace_check( b, layout ) );
+		v.kind = layout == TBVH_LAYOUT_CWBVH ? TBVH_VIEW_TLAS_CWBVH : TBVH_VIEW_TLAS_BVH;
+		v.nodes = b->d_nodes, v.prim_idx = b->d_prim_idx, v.inst = b->d_inst, v.blas = b->d_blas;
+		v.root_ref = b->root_ref, v.root_count = b->root_count, v.inst_shift = tlas_inst_shift( b );
+	}
+	else if (layout == TBVH_LAYOUT_BVH || layout == TBVH_LAYOUT_BVH_GPU)
+	{
+		TRY( bvh2_trace_check( b, 1 ) );
+		v.kind = TBVH_VIEW_BVH, v.nodes = b->d_trav, v.tris = b->d_leaf_tris, v.root_ref = b->root_ref, v.root_count = b->root_count;
+		v.stack = b->info.max_depth + 1 > TBVH_STACK ? TBVH_STACK_DEEP : TBVH_STACK;
+	}
+	else if (layout == TBVH_LAYOUT_CWBVH)
+	{
+		TRY( cwbvh_trace_check( b, 1 ) );
+		v.kind = TBVH_VIEW_CWBVH, v.nodes = b->d_cw_trav, v.tris = b->d_cw_tris, v.cw_rd_limit = b->cw_rd_limit;
+	}
+	else { tbvh_set_error( "unknown layout %d", layout ); return TBVH_E_ARG; }
+	*out = v;
+	return TBVH_OK;
+}
+
 // plain device memory for callers of the *_device entry points that do not link the CUDA runtime themselves
 int tbvh_device_alloc( tbvh_ctx c, size_t bytes, void** out )
 {

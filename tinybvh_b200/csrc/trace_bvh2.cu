@@ -2,8 +2,10 @@
 //
 // Replaces BVH::Intersect<posX,posY,posZ> (tiny_bvh.h:3247-3304), BVH::IsOccluded<...> (:3407-3453) and the OpenCL
 // kernels traverse_ailalaine / isoccluded_ailalaine (traverse_bvh2.cl:80,147) for whole ray batches.  The walk itself - node
-// layout, slab test, descent order, leaf loop - is bvh2_walk.cuh, shared with the two-level kernel (trace_tlas.cu).
-#include "bvh2_walk.cuh"
+// layout, slab test, descent order, leaf loop - is include/tinybvh_b200_device/bvh2_walk.cuh, and the per-ray body is
+// tbvh::bvh2_trace, shared with the two-level kernel (trace_tlas.cu) and the device functions callers' kernels use.
+#include "common.cuh"
+#include "../../include/tinybvh_b200_device.cuh"
 #include <stdlib.h>
 
 // 128 threads with at least 10 resident CTAs per SM (40 warps / SM without spills; 12 and 16 were measured slower).
@@ -30,16 +32,8 @@ __global__ void __launch_bounds__( 128, 10 ) k_trace_bvh2( const float4* __restr
 	}
 	if (valid)
 	{
-		float tmax = rh4.x, hu = rh4.y, hv = rh4.z;
-		uint32_t hprim = __float_as_uint( rh4.w );
 		uint2 stack[STACKN];
-		occluded = bvh2_walk<ANYHIT, STATS>( nodes, tris, root_ref, root_count, ro4.x, ro4.y, ro4.z, rd4.x, rd4.y, rd4.z,
-			rr4.x, rr4.y, rr4.z, uni, tmax, hu, hv, hprim, stack, stats );
-		if (!ANYHIT)
-		{
-			float4* hp = (float4*)(hits + i * hit_stride);
-			*hp = make_float4( tmax, hu, hv, __uint_as_float( hprim ) );
-		}
+		occluded = tbvh::bvh2_trace<ANYHIT, STATS>( nodes, tris, root_ref, root_count, ro4, rd4, rr4, rh4, (float4*)(hits + i * hit_stride), uni, stack, stats );
 	}
 	if (ANYHIT) store_occlusion_word( bits, i, n, occluded );
 }
@@ -96,9 +90,9 @@ __global__ void __launch_bounds__( 128, 10 ) k_trace_bvh2_persist( const float4*
 			{
 				if (cnt == 0)
 				{
-					if (bvh2_pair_step( nodes, ref, cnt, stack, sp, posX, posY, posZ, false, rdx, rdy, rdz, nrox, nroy, nroz, tmax )) continue;
+					if (tbvh::bvh2_pair_step( nodes, ref, cnt, stack, sp, posX, posY, posZ, false, rdx, rdy, rdz, nrox, nroy, nroz, tmax )) continue;
 				}
-				else if (bvh2_leaf<ANYHIT, false>( tris, ref, cnt, ox, oy, oz, dx, dy, dz, tmax, hu, hv, hprim, nullptr ) && ANYHIT) { occluded = done = true; break; }
+				else if (tbvh::bvh2_leaf<ANYHIT, false>( tris, ref, cnt, ox, oy, oz, dx, dy, dz, tmax, hu, hv, hprim, nullptr ) && ANYHIT) { occluded = done = true; break; }
 				if (sp == 0) { done = true; break; }
 				const uint2 e = stack[--sp];
 				ref = e.x, cnt = e.y;
@@ -115,12 +109,19 @@ __global__ void __launch_bounds__( 128, 10 ) k_trace_bvh2_persist( const float4*
 
 unsigned long long* ctx_next_counter( tbvh_ctx c ) { return c->d_counters + (c->counter_next.fetch_add( 1 ) % TBVH_COUNTERS); }
 
-int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits,
-	uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats )
+int bvh2_trace_check( tbvh_bvh b, uint64_t n )
 {
 	if (!b->d_trav || !b->d_leaf_tris) { tbvh_set_error( "BVH2 layout not resident" ); return TBVH_E_STATE; }
 	if (n == 0) return TBVH_OK;
 	if (b->info.max_depth + 1 > TBVH_STACK_DEEP) { tbvh_set_error( "BVH depth %u exceeds the %d-entry traversal stack (the reference's own, tiny_bvh.h:3249)", b->info.max_depth, TBVH_STACK_DEEP ); return TBVH_E_LIMIT; }
+	return TBVH_OK;
+}
+
+int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits,
+	uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats )
+{
+	TRY( bvh2_trace_check( b, n ) );
+	if (n == 0) return TBVH_OK;
 	const bool deep = b->info.max_depth + 1 > TBVH_STACK;
 	const uint32_t root_ref = b->root_ref, root_count = b->root_count;
 	const uint32_t block = 128;

@@ -6,7 +6,8 @@
 // a child is hit iff  max( tnear_x, tnear_y, tnear_z, 0 ) <= min( tfar_x, tfar_y, tfar_z, t )  with
 // t_plane = fma( q, 2^e * rD, ( p - O ) * rD ),  triangles run through the oracle's Moeller-Trumbore (common.cuh mt_test).
 // This file builds the traversal nodes (cw_make_trav) and holds the single-level kernel (k_trace_wide); the walk over them
-// (node_hits, cw_trace) is cw_walk.cuh, shared with the two-level kernel (trace_tlas.cu).
+// (node_hits, cw_trace) is include/tinybvh_b200_device/cw_walk.cuh and the per-ray body tbvh::cw_trace_ray, shared with the
+// two-level kernel (trace_tlas.cu) and the device functions callers' kernels use.
 //
 // What is different from the reference kernels (traverse_cwbvh.cl) is everything the format does not dictate:
 //
@@ -33,7 +34,8 @@
 //  * The per-axis scales 2^e are stored as the top halves of their float patterns: one shift or mask each instead of a byte decode.
 //
 // Triangles are the reference's 48-byte records (e2, e1, v0 | primIdx) read straight from bvh8Tris.
-#include "cw_walk.cuh"
+#include "common.cuh"
+#include "../../include/tinybvh_b200_device.cuh"
 #include <vector>
 
 // ---- bvh8Data -> traversal nodes ------------------------------------------------------------------------------------
@@ -238,49 +240,30 @@ __global__ void __launch_bounds__( 128 ) k_trace_wide( const float4* __restrict_
 		const uint32_t oct0 = __shfl_sync( 0xffffffffu, oct, vm ? __ffs( vm ) - 1 : 0 );
 		uni = __all_sync( 0xffffffffu, !valid || (oct == oct0 && o == 7u - oct) );
 	}
-	const bool iord = __all_sync( 0xffffffffu, !valid || cw_ray_fits( ox, oy, oz, rdx, rdy, rdz, rd_limit ) );
+	const bool iord = __all_sync( 0xffffffffu, !valid || tbvh::cw_ray_fits( ox, oy, oz, rdx, rdy, rdz, rd_limit ) );
 	if (valid)
 	{
-		float t = rh4.x, hu = rh4.y, hv = rh4.z;
-		uint32_t hprim = __float_as_uint( rh4.w );
 		uint2 pending[CW_STACK];
-		#define TRACE( O, I ) occluded = cw_trace<ANYHIT, STATS, O, I>( nodes, tris, ox, oy, oz, dx, dy, dz, rdx, rdy, rdz, o, negx, negy, negz, t, hu, hv, hprim, pending, stats )
-		if (OCTSW && uni && iord)
-		{
-			switch (oct)
-			{
-			case 0: TRACE( 0, true ); break;
-			case 1: TRACE( 1, true ); break;
-			case 2: TRACE( 2, true ); break;
-			case 3: TRACE( 3, true ); break;
-			case 4: TRACE( 4, true ); break;
-			case 5: TRACE( 5, true ); break;
-			case 6: TRACE( 6, true ); break;
-			default: TRACE( 7, true ); break;
-			}
-		}
-		else if (iord) TRACE( -1, true );
-		else TRACE( -1, false );
-		#undef TRACE
-		if (!ANYHIT)
-		{
-			// the reference stores t, but u, v and prim only when t < BVH_FAR (end of :7046-7154): a NaN or infinite distance (Moeller-Trumbore
-			// overflowing on huge coordinates) leaves the ray's own u, v, prim
-			if (!(t < BVH_FAR)) hu = rh4.y, hv = rh4.z, hprim = __float_as_uint( rh4.w );
-			float4* hp = (float4*)(hits + i * hit_stride);
-			*hp = make_float4( t, hu, hv, __uint_as_float( hprim ) );
-		}
+		occluded = tbvh::cw_trace_ray<ANYHIT, STATS>( nodes, tris, ox, oy, oz, dx, dy, dz, rdx, rdy, rdz, rh4, (float4*)(hits + i * hit_stride), o, oct, negx,
+			negy, negz, OCTSW && uni && iord, iord, pending, stats );
 	}
 	if (ANYHIT) store_occlusion_word( bits, i, n, occluded );
 }
 
-int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits,
-	uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats )
+int cwbvh_trace_check( tbvh_bvh b, uint64_t n )
 {
 	if (!b->d_cw_trav || !b->d_cw_tris) { tbvh_set_error( "CWBVH layout not resident" ); return TBVH_E_STATE; }
 	if (n == 0) return TBVH_OK;
 	if (b->cw_pending == CW_CYCLE) { tbvh_set_error( "the wide tree's inner-child links form a cycle" ); return TBVH_E_ARG; }
 	if (b->cw_pending > CW_STACK) { tbvh_set_error( "the wide tree can leave %u node groups pending, more than the %d a ray can hold (the reference's own limit)", b->cw_pending, CW_STACK ); return TBVH_E_LIMIT; }
+	return TBVH_OK;
+}
+
+int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits,
+	uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats )
+{
+	TRY( cwbvh_trace_check( b, n ) );
+	if (n == 0) return TBVH_OK;
 	const uint32_t block = 128;
 	const uint64_t grid = (n + block - 1) / block;
 	if (grid > 0x7fffffffull) { tbvh_set_error( "ray batch too large for one launch" ); return TBVH_E_ARG; }
