@@ -391,7 +391,23 @@ int tbvh_copy_from_device( void* host, const void* d_src, size_t bytes );
  * during traversal).  The reference has no counterpart: its GPU path drives one OpenCL device (tiny_bvh_speedtest.cpp:1092-1241).
  *  tbvh_group_create     devices[count] (NULL / 0 = all devices), one engine context each, peer access enabled where possible
  *  tbvh_group_replicate  copy the traversal arrays of a built / uploaded / converted BVH to every device of the group (peer copies
- *                        over NVLink); ms_out = device time of the copies.  Call again after the source changed.
+ *                        over NVLink); ms_out = device time of the copies.  Call again after the source changed.  A plain BVH's
+ *                        replicas are released and made again on every call.
+ *                        A TLAS (an instanced scene): every device whose context is not the source's gets one replica BLAS per
+ *                        distinct BLAS handle the TLAS links to, holding only what the two-level walk reads in the layouts the
+ *                        source can be walked in (the BVH2 pair array and leaf triangles, the CWBVH traversal nodes and bvh8Tris),
+ *                        and one replica TLAS (nodes, primIdx, instances; its BLAS table made over the replica BLASes).  The
+ *                        replica TLAS refuses exactly what the source refuses, with the same codes.  Called once per frame, after
+ *                        the refits and tbvh_build_tlas_update, it refreshes in place: BLASes whose handle and generation did not
+ *                        change are not copied, changed ones of unchanged sizes are copied into their arrays, unlinked ones are
+ *                        released, and every byte bound for one device goes in one copy launch (one cudaMemcpyPeerAsync per array
+ *                        where that device cannot read the source's).  Refused before any replica is touched: a stale source TLAS,
+ *                        a TLAS whose BLASes share no walkable layout, and a group context whose inst_idx_bits differs from the
+ *                        source context's (TBVH_E_STATE).  A failure after the copies began releases every replica.  A plain BVH
+ *                        replicated after a TLAS releases the scene's replicas, and the other way round.
+ *  tbvh_group_replica    replica i: the source itself where its context is device i's, else the group's copy (for a TLAS, the
+ *                        replica TLAS).  It and tbvh_device_view of it stay valid until the next tbvh_group_replicate or
+ *                        tbvh_group_destroy; a view of replica i reads device i's own arrays.
  *  tbvh_group_intersect / _occluded  tbvh_intersect / tbvh_occluded on a HOST batch, rays [first, first+count) of
  *                        tbvh_shard_range( n, g, size ) going to device g from a worker thread bound to that device's NUMA node
  *  tbvh_group_host_alloc page-locked buffer of n records whose index ranges live on the NUMA node of the device that reads them

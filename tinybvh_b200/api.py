@@ -540,8 +540,9 @@ def shard_range(n: int, part: int, parts: int):
 
 
 class Group:
-    """Several GPUs of one process (tbvh_group_*): `replicate(bvh)` copies a BVH to every device over NVLink, `Intersect` /
-    `IsOccluded` shard a host ray batch by index over the devices.  `layout` follows the replicated object."""
+    """Several GPUs of one process (tbvh_group_*): `replicate(bvh)` copies a BVH, or a TLAS with its BLASes, to every device over
+    NVLink, `Intersect` / `IsOccluded` shard a host ray batch by index over the devices.  `layout` follows the replicated object.
+    An animated scene calls `replicate(tlas)` once per frame: the replicas are refreshed in place."""
 
     def __init__(self, devices=None):
         self.h = C.c_void_p()
@@ -561,6 +562,16 @@ class Group:
         check(_lib.lib().tbvh_group_replicate(self.h, bvh.h, C.byref(ms)))
         self.src, self.layout = bvh, bvh.layout
         return ms.value
+
+    def device_view(self, i: int, layout: int = None) -> _lib.DeviceView:
+        """tbvh_device_view of device i's replica, over that device's own arrays (default layout: the replicated object's).  Valid
+        until the next replicate() or close()."""
+        h = _lib.lib().tbvh_group_replica(self.h, i)
+        if not h:
+            raise TbvhError("Group.device_view: no replica %d (replicate first)" % i)
+        v = _lib.DeviceView()
+        check(_lib.lib().tbvh_device_view(C.c_void_p(h), self.layout if layout is None else layout, C.byref(v)))
+        return v
 
     def empty_rays(self, n: int, dtype) -> np.ndarray:
         """page-locked array whose index ranges sit on the NUMA node of the device that will read them (tbvh_group_host_alloc)"""

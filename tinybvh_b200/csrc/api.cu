@@ -786,10 +786,7 @@ int tbvh_instance_update( void* instance, tbvh_bvh blas )
 	return tbvh_instance_update_box( instance, blas->info.aabb_min, blas->info.aabb_max );
 }
 
-// the BLAS list of a TLAS build: the device record of every BLAS, the layouts all of them hold, and the first BLAS too deep for the
-// two-level kernel's BVH-layout walk (1 + its number; 0: none).  Reads host state only and touches no handle.
-struct TlasBlasTable { std::vector<BlasRef> refs; uint32_t layouts, deep_blas, deep_depth; };
-static int tlas_blas_table( const tbvh_bvh t, const tbvh_bvh* blasses, const uint32_t blas_count, TlasBlasTable& T )
+extern "C++" int tlas_blas_table( const tbvh_bvh t, const tbvh_bvh* blasses, const uint32_t blas_count, TlasBlasTable& T )
 {
 	T.refs.assign( blas_count, BlasRef{} );
 	T.layouts = (1u << TBVH_LAYOUT_BVH) | (1u << TBVH_LAYOUT_CWBVH), T.deep_blas = 0, T.deep_depth = 0;
@@ -1204,6 +1201,11 @@ static int tlas_check( tbvh_bvh t, int layout )
 	{ tbvh_set_error( "TLAS: BLAS %u has depth %u, the two-level kernel walks a BVH-layout BLAS with a %d-entry stack (walk its CWBVH layout)", t->tlas_deep_blas - 1, t->tlas_deep_depth, TBVH_STACK ); return TBVH_E_LIMIT; }
 	if (!(t->tlas_blas_layouts & want))
 	{ tbvh_set_error( "TLAS: not every BLAS held its %s layout when the TLAS was built", layout == TBVH_LAYOUT_CWBVH ? "CWBVH" : "BVH" ); return TBVH_E_STATE; }
+	return tlas_stale_check( t );
+}
+
+extern "C++" int tlas_stale_check( tbvh_bvh t )
+{
 	std::lock_guard<std::mutex> lk( g_live_mutex );
 	for (const BlasLink& l : t->links)
 	{

@@ -115,6 +115,8 @@ struct tbvh_bvh_t
 	uint32_t cw_pending = 0;   // most node groups a walk of the wide tree can leave pending (trace_cwbvh.cu k_cw_pending)
 	float cw_rd_limit = -1.0f; // rays with |rD| up to this (and |O| <= 2^126) take the integer-ordered slab test (cw_walk.cuh cw_ray_fits); < 0: none
 	uint32_t generation = 0;   // renewed (tbvh_next_generation) whenever the arrays a TLAS may point at are replaced (build, upload, refit, convert)
+	uint32_t revision = 0;     // counts refits: a refit that drops no layout rewrites the BVH2 arrays in place under the same generation, and a
+	                           // group's scene replicas (multi.cu) must notice that too
 	// TLAS (BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) :2221): nodes / primIdx over instance boxes + device tables
 	float4* d_aabbs = 0;       // instance boxes the TLAS was built over (2 float4 per instance)
 	void* d_inst = 0;          // TlasInst records (inverse transform, BLAS number, mask)
@@ -268,6 +270,11 @@ int bvh2_trace_check( tbvh_bvh b, uint64_t n );
 int cwbvh_trace_check( tbvh_bvh b, uint64_t n );
 int tlas_trace_check( tbvh_bvh b, int layout );
 uint32_t tlas_inst_shift( tbvh_bvh b ); // 32 - INST_IDX_BITS of the context's inst_idx_bits, 0 for 32 (hit.inst)
+// the BLAS list of a TLAS build (api.cu): the device record of every BLAS, the layouts all of them hold, and the first BLAS too deep for
+// the two-level kernel's BVH-layout walk (1 + its number; 0: none).  Reads host state only and touches no handle.
+struct TlasBlasTable { std::vector<BlasRef> refs; uint32_t layouts, deep_blas, deep_depth; };
+int tlas_blas_table( const tbvh_bvh t, const tbvh_bvh* blasses, const uint32_t blas_count, TlasBlasTable& T );
+int tlas_stale_check( tbvh_bvh t ); // TBVH_E_STATE once a BLAS the TLAS was built over has been rebuilt, re-uploaded or destroyed
 // BLASInstance::Update of n records `stride` bytes apart (instance_update.cu): invTransform and world box into the records, the TlasInst
 // entries and the builder's boxes in one pass; *d_bad_blas is set when a record names a BLAS past blas_count
 int instance_update_launch( void* d_records, uint32_t stride, uint32_t n, const float4* d_blas_box, uint32_t blas_count, void* d_tlas_inst, float4* d_aabbs,

@@ -770,6 +770,7 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 		const tbvh_bvh b = bs[t];
 		if (!keep_layouts) drop_bvh_gpu( b ), drop_cwbvh( b ); // derived layouts describe the old boxes (the reference converts again too)
 		else b->generation = tbvh_next_generation(); // the arrays stay, but a TLAS over this BLAS holds its old root box in its instances
+		b->revision++;
 		const uint32_t used = b->info.used_nodes;
 		if (keep_layouts && b->cw_keep) cw.push_back( t ), NC += used;
 		if (keep_layouts && (b->info.layouts & (1u << TBVH_LAYOUT_BVH_GPU))) gp.push_back( t ), NG += used;
