@@ -182,6 +182,30 @@ int tbvh_build_batch_hq( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count
 int tbvh_sah_cost( tbvh_bvh bvh, float c_trav, float c_int, float* out );
 int tbvh_sah_cost_nodes( const void* nodes32, uint32_t used_nodes, float c_trav, float c_int, float* out );
 
+/* Lower the SAH cost of a resident tree on the device: rounds of parallel subtree reinsertion (Meister & Bittner 2018).  The
+ * reference's optimiser, BVH::Optimize tiny_bvh.h:3043 over BVH_Verbose::Optimize :4338, reinserts one subtree at a time; this is
+ * a different algorithm and its tree is NOT the reference's.  Each round every node searches the round's tree for its cheapest
+ * place, the non-conflicting moves are applied together and interior boxes refolded; the round is kept when SAHCost( c_trav,
+ * c_int ) falls strictly and the depth stays <= max( max_depth, 63 ), else it is retried with the better half of its moves, down
+ * to one; the call ends after max_rounds kept rounds or at the first round nothing is kept.  Rules: DESIGN.md §4.7.
+ *  Input: any handle holding a BVH-layout tree: builds of every flavour, indexed or flat, batch builds, and tbvh_upload_bvh trees
+ *  whose node slots but node 1 all belong to the tree (as every builder leaves them).  A tbvh_upload_bvh_gpu upload holds no
+ *  BVH-layout tree (tbvh_sah_cost and tbvh_refit refuse it too).  Leaves keep firstTri, triCount and their box bits; primIdx,
+ *  idx_count and prim_count stay as they are; only the interior structure moves.
+ *  Output: the handle ends up as tbvh_upload_bvh( .., TBVH_DEVICE ) of the new nodes would leave it (traversal arrays, root,
+ *  max_depth, stack choice, aabb_min / aabb_max), keeping its primIdx, vertices, kept indices and refittability.  The nodes are
+ *  numbered as BVH::ConvertFrom( BVH_Verbose ) numbers a tree: DFS preorder, the k-th interior node's children at 2 + 2k and
+ *  3 + 2k, interior boxes the fold of their children; used_nodes = 2 + 2 x interior nodes.  BVH_GPU and CWBVH are dropped (as
+ *  tbvh_refit drops them), the generation is renewed (a TLAS over the handle is stale), device views end; info.build_ms is the
+ *  device time of the call.  When no round is kept (always for a tree of one or two leaves) the handle is left exactly as it was.
+ *  *rounds: rounds kept (<= max_rounds); *sah: the final SAHCost, bit for bit tbvh_sah_cost of the result; either may be NULL.
+ *  Refusals come before anything is touched: TBVH_E_ARG for a NULL handle, max_rounds 0, or c_trav / c_int not finite and > 0;
+ *  TBVH_E_STATE for a TLAS, a handle without a BVH-layout tree (an empty handle, a tbvh_upload_bvh_gpu or CWBVH-only upload), or a
+ *  tbvh_upload_bvh tree with slots outside it (a slot other than node 1 unreached, or node 1, a slot past used_nodes or one slot
+ *  twice reached from the root); TBVH_E_LIMIT for a tree deeper than 255 (the search's stack).
+ *  A failure after the device work began leaves the handle empty, as a failed build does. */
+int tbvh_optimize( tbvh_bvh bvh, uint32_t max_rounds, float c_trav, float c_int, uint32_t* rounds, float* sah );
+
 /* BLASInstance::Update( BVHBase* blas ) tiny_bvh.h:8386 on one 192-byte record: invTransform = inverse of transform
  * (InvertTransform :8402), aabbMin / aabbMax = box of the eight transformed corners of the BLAS's root box.  Host arithmetic in
  * the reference build's own operation order: the record comes out bit-identical to the reference's.  _box takes the root box

@@ -78,6 +78,17 @@ public:
 	tbvh_bvh handle() const { return h; }
 	int Layout() const { return layout; }  // TBVH_LAYOUT_*: the layout Intersect / IsOccluded walk (BVHBase::layout, tiny_bvh.h:795-805)
 	tbvh_info Info() const { tbvh_info i; TBVH_FATAL_IF( tbvh_bvh_info( h, &i ), "Info" ); return i; }
+	// tbvh_optimize: rounds of parallel subtree reinsertion on the device that lower the resident tree's SAH cost - indexed and
+	// device-resident builds included.  Not the reference's BVH::Optimize (tiny_bvh.h:3043), which BVH::Optimize below still runs
+	// on the host.  A BVH_GPU or BVH8_CWBVH converts the optimised tree again, as its Build does.  Returns the rounds kept.
+	uint32_t OptimizeOnDevice( const uint32_t maxRounds = 8 )
+	{
+		uint32_t rounds = 0;
+		TBVH_FATAL_IF( tbvh_optimize( h, maxRounds, c_trav, c_int, &rounds, 0 ), "OptimizeOnDevice" );
+		if (rounds && layout != TBVH_LAYOUT_BVH) TBVH_FATAL_IF( tbvh_convert( h, layout ), "OptimizeOnDevice" );
+		sync_info();
+		return rounds;
+	}
 	// batch traversal: the calls the patched harness makes instead of its per-ray loops
 	// Return value: 0, or - with collectCost set - the sum over the batch of what the reference's per-ray Intersect returns,
 	// (int32_t)( c_trav * nodes visited + c_int * triangles tested ) (tiny_bvh.h:3303; the speedtest adds these up into rayCost,

@@ -61,6 +61,7 @@ SYMBOLS = {
     "tbvh_build_flavour": (i32, [vp, vp, u32, u32, i32, f32, f32, i32]),
     "tbvh_sah_cost": (i32, [vp, f32, f32, vp]),
     "tbvh_sah_cost_nodes": (i32, [vp, u32, f32, f32, vp]),
+    "tbvh_optimize": (i32, [vp, u32, f32, f32, vp, vp]),
     "tbvh_instance_update": (i32, [vp, vp]),
     "tbvh_instance_update_box": (i32, [vp, vp, vp]),
     "tbvh_build_tlas": (i32, [vp, vp, u32, u32, vp, u32, f32, f32]),

@@ -219,6 +219,11 @@ class BVH(_Base):
         check(_lib.lib().tbvh_sah_cost(self.h, self.c_trav, self.c_int, C.byref(out)))
         return float(out.value)
 
+    def optimize(self, max_rounds: int, c_trav: float = 1.0, c_int: float = 1.0):
+        """tbvh_optimize: rounds of parallel subtree reinsertion on the device that lower the tree's SAH cost; not the reference's
+        BVH::Optimize (tiny_bvh.h:3043), which reinserts one subtree at a time.  -> (rounds kept, final SAHCost)."""
+        return _optimize(self, max_rounds, c_trav, c_int)
+
     def Refit(self, vertices):
         """BVH::Refit (tiny_bvh.h:3055): same triangles, new positions.  The reference re-reads the caller's vertex array through
         the pointer it kept; the engine holds its own copy, so the array is passed again."""
@@ -303,6 +308,14 @@ class TLAS(BVH):
         return self
 
 
+def _optimize(obj, max_rounds, c_trav, c_int, layout=LAYOUT_BVH):
+    rounds, sah = C.c_uint32(), C.c_float()
+    check(_lib.lib().tbvh_optimize(obj.h, max_rounds, c_trav, c_int, C.byref(rounds), C.byref(sah)))
+    if rounds.value and layout != LAYOUT_BVH:
+        check(_lib.lib().tbvh_convert(obj.h, layout))   # the optimised BVH2 converted again, as Build converts the built one
+    return int(rounds.value), float(sah.value)
+
+
 def _refit_layouts(obj, vertices):
     p, stride, nv, space, keep = _verts_arg(vertices)
     check(_lib.lib().tbvh_refit_layouts(obj.h, p, stride, nv // 3, space))
@@ -324,6 +337,10 @@ class BVH_GPU(_Base):
         self._build(vertices, primCount, _lib.BUILD_HQ, indices)
         check(_lib.lib().tbvh_convert(self.h, LAYOUT_BVH_GPU))
         return self
+
+    def optimize(self, max_rounds: int, c_trav: float = 1.0, c_int: float = 1.0):
+        """BVH.optimize of the underlying tree, then ConvertFrom again on the device.  -> (rounds kept, final SAHCost)."""
+        return _optimize(self, max_rounds, c_trav, c_int, LAYOUT_BVH_GPU)
 
     def Refit(self, vertices):
         """BVH::Refit of the underlying tree, then ConvertFrom again on the device (tbvh_refit_layouts): same triangles, new
@@ -361,6 +378,10 @@ class BVH8_CWBVH(_Base):
         self._build(vertices, primCount, _lib.BUILD_HQ, indices)
         check(_lib.lib().tbvh_convert(self.h, LAYOUT_CWBVH))
         return self
+
+    def optimize(self, max_rounds: int, c_trav: float = 1.0, c_int: float = 1.0):
+        """BVH.optimize of the underlying tree, then the CWBVH conversion chain again.  -> (rounds kept, final SAHCost)."""
+        return _optimize(self, max_rounds, c_trav, c_int, LAYOUT_CWBVH)
 
     def Refit(self, vertices):
         """Refit without a new collapse (tbvh_refit_layouts): BVH::Refit of the underlying tree, then BVH8_CWBVH::ConvertFrom of the

@@ -6,6 +6,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <cmath>
 #include <vector>
 #include <thread>
 #include <atomic>
@@ -394,7 +395,7 @@ static void free_layouts( tbvh_bvh b )
 	b->links.clear();
 	b->generation = tbvh_next_generation(); // a TLAS built over the old arrays must notice (tlas_check)
 	memset( &b->info, 0, sizeof( b->info ) );
-	b->refittable = true;
+	b->refittable = true, b->stray_slots = false;
 }
 
 int tbvh_bvh_destroy( tbvh_bvh b )
@@ -554,6 +555,25 @@ template <class Children> static uint32_t tree_depth( const uint32_t* nodes, con
 	return maxd;
 }
 
+// true when the 32-byte node array is one tree over every slot but node 1: walked from the root, no child pointer leaves
+// [0, used_nodes), node 1 is never reached, no slot is reached twice, and every other slot is reached
+static bool slots_form_tree( const uint32_t* nodes, const uint32_t used_nodes )
+{
+	std::vector<uint8_t> seen( used_nodes, 0 );
+	std::vector<uint32_t> st( 1, 0u );
+	uint32_t reached = 0;
+	while (!st.empty())
+	{
+		const uint32_t x = st.back();
+		st.pop_back();
+		if (x >= used_nodes || x == 1 || seen[x]) return false;
+		seen[x] = 1, reached++;
+		const uint32_t* n = nodes + (size_t)x * 8;
+		if (n[7] == 0) st.push_back( n[3] + 1 ), st.push_back( n[3] );
+	}
+	return reached == used_nodes - (used_nodes > 1 ? 1 : 0);
+}
+
 // the shared part of tbvh_upload_bvh / tbvh_upload_bvh_gpu after the argument check: the handle emptied, the vertices, `used_nodes`
 // nodes of `node_bytes` each into *d_nodes (room for at least min_nodes) and primIdx copied in.  *hn: the nodes as the host reads
 // them (for device-space input, a copy in `host`)
@@ -684,6 +704,7 @@ int tbvh_upload_bvh( tbvh_bvh b, const void* nodes32, uint32_t used_nodes, const
 	TRY( make_leaf_tris( b, s ) );
 	CUDA_TRY( cudaStreamSynchronize( s ) );
 	b->info.layouts = 1u << TBVH_LAYOUT_BVH;
+	b->stray_slots = !slots_form_tree( hn, used_nodes );
 	return TBVH_OK;
 }
 
@@ -762,6 +783,51 @@ int tbvh_sah_cost( tbvh_bvh b, float c_trav, float c_int, float* out )
 	std::vector<float> nodes( (size_t)b->info.used_nodes * 8 );
 	CUDA_TRY( cudaMemcpy( nodes.data(), b->d_nodes, nodes.size() * 4, cudaMemcpyDeviceToHost ) );
 	return tbvh_sah_cost_nodes( nodes.data(), b->info.used_nodes, c_trav, c_int, out );
+}
+
+// ---- tbvh_optimize: the checks and the handle's bookkeeping around optimize.cu's rounds
+int tbvh_optimize( tbvh_bvh b, uint32_t max_rounds, float c_trav, float c_int, uint32_t* rounds, float* sah )
+{
+	ARG_CHECK( b, "NULL handle" );
+	ARG_CHECK( max_rounds > 0, "max_rounds must be at least 1" );
+	ARG_CHECK( std::isfinite( c_trav ) && std::isfinite( c_int ) && c_trav > 0.0f && c_int > 0.0f, "c_trav and c_int must be finite and > 0" );
+	if (b->d_inst) { tbvh_set_error( "tbvh_optimize: a TLAS is rebuilt per frame, not optimised" ); return TBVH_E_STATE; }
+	if (!(b->info.layouts & (1u << TBVH_LAYOUT_BVH)) || !b->d_nodes) { tbvh_set_error( "tbvh_optimize: no BVH-layout tree on this handle" ); return TBVH_E_STATE; }
+	if (b->stray_slots) { tbvh_set_error( "tbvh_optimize: the uploaded node array holds slots outside the tree (every slot but node 1 must belong to it)" ); return TBVH_E_STATE; }
+	if (b->info.max_depth > 255) { tbvh_set_error( "tbvh_optimize: depth %u exceeds the search's 255 levels", b->info.max_depth ); return TBVH_E_LIMIT; }
+	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
+	uint32_t kept = 0, used = 0, depth = 0;
+	float cost = 0.0f, ms = 0.0f;
+	float4* out = 0;
+	if (b->info.used_nodes >= 5 && b->root_count == 0) // a leaf root, or a root over two leaves, offers no move
+	{
+		const int rc = optimize_tree( b, max_rounds, c_trav, c_int, &out, &used, &depth, &kept, &cost, &ms );
+		if (rc != TBVH_OK) { cudaStreamSynchronize( b->ctx->stream ); free_layouts( b ); cudaGetLastError(); return rc; }
+	}
+	if (kept == 0)
+	{
+		if (rounds) *rounds = 0;
+		return sah ? tbvh_sah_cost( b, c_trav, c_int, sah ) : TBVH_OK;
+	}
+	float root[8];
+	if (cudaMemcpy( root, out, 32, cudaMemcpyDeviceToHost ) != cudaSuccess)
+	{
+		tbvh_set_error( "tbvh_optimize: %s", cudaGetErrorString( cudaGetLastError() ) );
+		cudaFree( out ), free_layouts( b );
+		return TBVH_E_CUDA;
+	}
+	drop_bvh_gpu( b );
+	drop_cwbvh( b );
+	if (b->d_trav && b->d_trav != b->d_nodes) cudaFree( b->d_trav );
+	cudaFree( b->d_nodes );
+	b->d_nodes = b->d_trav = out;
+	memcpy( &b->root_ref, root + 3, 4 ), memcpy( &b->root_count, root + 7, 4 );
+	memcpy( b->info.aabb_min, root, 12 ), memcpy( b->info.aabb_max, root + 4, 12 );
+	b->info.used_nodes = used, b->info.max_depth = depth, b->info.layouts = 1u << TBVH_LAYOUT_BVH, b->info.build_ms = ms;
+	b->generation = tbvh_next_generation(); // d_leaf_tris depends on primIdx and the vertices alone: it stays
+	if (rounds) *rounds = kept;
+	if (sah) *sah = cost;
+	return TBVH_OK;
 }
 
 // ---- BLASInstance::Update on the host: the arithmetic of instance_update.cuh, which the device kernel runs too (host code, so gcc's

@@ -128,6 +128,8 @@ struct tbvh_bvh_t
 	uint32_t tlas_deep_blas = 0, tlas_deep_depth = 0; // TLAS only: 1 + the first BLAS whose BVH2 is too deep for the two-level walk (0: none), and its depth
 	std::vector<BlasLink> links; // TLAS only: the BLAS handles it points into, with the generation they had at build time
 	bool refittable = true;    // BVHBase::refittable (:811): false after BuildHQ ("can't refit an SBVH", :3027)
+	bool stray_slots = false;  // tbvh_upload_bvh: a slot other than node 1 is outside the tree, or the tree reaches node 1 or a slot past
+	                           // used_nodes, or reaches a slot twice (builders never leave such a tree; tbvh_optimize refuses it)
 	struct CwKeep* cw_keep = 0; // refittable trees: the 8-wide collapse of the last tbvh_convert to CWBVH (convert_cwbvh.cu), for tbvh_refit_layouts
 	// statistics
 	int stats = 0;
@@ -287,5 +289,8 @@ void drop_bvh_gpu( tbvh_bvh b );                  // the BVH_GPU array, its bit 
 int bvh_to_cwbvh( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
 // the CWBVH arrays, the kept collapse, the bit, the counts and the traversal limits; a TLAS over the arrays becomes stale
 void drop_cwbvh( tbvh_bvh b );
+// tbvh_optimize's rounds over b's BVH-layout tree (optimize.cu).  Writes nothing when *rounds ends 0; else *out is a new allocation
+// holding the renumbered tree (*used nodes, depth *depth), *sah its SAHCost and *ms the device time of the call.
+int optimize_tree( tbvh_bvh b, uint32_t max_rounds, float c_trav, float c_int, float4** out, uint32_t* used, uint32_t* depth, uint32_t* rounds, float* sah, float* ms );
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)
 int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint32_t n, cudaStream_t s );
