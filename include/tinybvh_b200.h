@@ -120,7 +120,14 @@ int tbvh_build_flavour( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32
 /* Indexed geometry: BVH::Build / BuildAVX / BuildHQ( const bvhvec4* vertices, const uint32_t* indices, primCount ) and their
  * bvhvec4slice forms (tiny_bvh.h:889-900; PrepareBuild reads verts[vertIdx[3 i + k]], :2290-2297).  verts: vert_count
  * vertices `stride` bytes apart; indices: 3 * prim_count entries.  primIdx numbers triangles exactly as the reference does
- * (triangle i = indices[3 i .. 3 i + 2]); an index >= vert_count is TBVH_E_ARG (the reference reads out of bounds). */
+ * (triangle i = indices[3 i .. 3 i + 2]); an index >= vert_count is TBVH_E_ARG (the reference reads out of bounds).
+ * tbvh_build, tbvh_build_flavour and tbvh_build_indexed are one-mesh calls of tbvh_build_batch / tbvh_build_batch_hq below, with their
+ * refusals, codes and limits.  Every refusal comes before the handle is touched, so a refused build leaves the handle and a TLAS over
+ * it as they were: TBVH_E_ARG for a NULL handle or verts, an unknown flavour or space, prim_count 0, a bad stride, NULL indices,
+ * vert_count 0, or an index >= vert_count (host indices are checked on the CPU before anything is read on the device); TBVH_E_LIMIT
+ * for more than TBVH_BATCH_MAX_PRIMS triangles, before any vertex is read.  The new vertices are staged before the old arrays are
+ * released, so a rebuild of a handle briefly holds both (48 bytes per triangle on top of the old tree).  A failure after the device
+ * work started leaves the handle empty. */
 int tbvh_build_indexed( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space,
 	float c_trav, float c_int, int flavour );
 
@@ -240,8 +247,11 @@ int tbvh_build_tlas_update( tbvh_bvh tlas, void* instances, uint32_t inst_stride
 	uint32_t blas_count, float c_trav, float c_int );
 
 /* BVH::Refit (tiny_bvh.h:3055-3093): the triangles moved, the topology stays - leaf boxes from the new vertices, interior
- * boxes bottom-up.  verts as for tbvh_build, same prim_count.  TBVH_E_STATE for an SBVH (the reference's fatal "refitting an
- * SBVH") or when no BVH-layout tree is resident.  Derived layouts on the handle are dropped; tbvh_convert again. */
+ * boxes bottom-up.  verts as for tbvh_build, same prim_count.  Derived layouts on the handle are dropped; tbvh_convert again.
+ * tbvh_refit and tbvh_refit_layouts are one-mesh calls of tbvh_refit_batch below (keep_layouts 0 and 1), with its refusals, codes and
+ * limit, all before the handle is touched: TBVH_E_ARG for a NULL handle or verts, an unknown space, another prim_count or a bad
+ * stride; TBVH_E_STATE for an SBVH (the reference's fatal "refitting an SBVH"), a TLAS, or when no BVH-layout tree is resident;
+ * TBVH_E_LIMIT past TBVH_REFIT_BATCH_MAX_NODES. */
 int tbvh_refit( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_count, int space );
 
 /* Refit that keeps the derived layouts: tbvh_refit's BVH::Refit, then every layout the handle holds brought up to date in place
@@ -255,7 +265,8 @@ int tbvh_refit( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_
  *    of its first frame: call tbvh_convert again to collapse anew.
  *  - info.build_ms is the device time of the call, aabb_min / aabb_max the new root box.
  * Refusals leave the handle unmodified: TBVH_E_STATE for an SBVH, a TLAS, no BVH-layout tree, or a CWBVH that tbvh_convert did not
- * produce from the resident tree (tbvh_upload_cwbvh, a group replica); TBVH_E_ARG for another prim_count.
+ * produce from the resident tree (tbvh_upload_cwbvh, a group replica); TBVH_E_ARG for another prim_count, a bad stride or an
+ * unknown space; TBVH_E_LIMIT as for tbvh_refit.
  * As after every refit, a TLAS over this BLAS is stale (its instance boxes are) until tbvh_build_tlas runs again, and group
  * replicas keep the old boxes until tbvh_group_replicate runs again. */
 int tbvh_refit_layouts( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_count, int space );
@@ -311,9 +322,11 @@ int tbvh_upload_bvh_gpu( tbvh_bvh bvh, const void* nodes64, uint32_t used_nodes,
 int tbvh_upload_cwbvh( tbvh_bvh bvh, const void* bvh8_data, uint32_t used_blocks, const void* bvh8_tris, uint32_t tri_count, int space );
 
 /* layout conversion on the device: BVH_GPU::ConvertFrom tiny_bvh.h:4612; BVH8_CWBVH::Build's chain
- * Compact :3733 + SplitLeafs(3) :1988 + MBVH<8>::ConvertFrom :4975 + BVH8_CWBVH::ConvertFrom :5884.  A TLAS handle has no
- * CWBVH (its leaves are instances, not triangles): TBVH_E_STATE.  A conversion to CWBVH that fails on the device leaves the
- * handle without a CWBVH. */
+ * Compact :3733 + SplitLeafs(3) :1988 + MBVH<8>::ConvertFrom :4975 + BVH8_CWBVH::ConvertFrom :5884.  A handle without a
+ * BVH-layout tree is TBVH_E_STATE whatever the target; another target than the two is TBVH_E_UNSUPPORTED.  To CWBVH the call is a
+ * one-handle tbvh_convert_batch below, with its refusals, codes and limit, all before the handle is touched: TBVH_E_STATE for a TLAS
+ * (its leaves are instances, not triangles); TBVH_E_LIMIT when the split tree could hold more than TBVH_CONVERT_BATCH_MAX_NODES
+ * nodes.  A conversion to CWBVH that fails on the device leaves the handle without a CWBVH. */
 int tbvh_convert( tbvh_bvh bvh, int to_layout );
 
 /* Many trees converted to CWBVH in one call, as a scene converts every BLAS before a TLAS walks them in TBVH_LAYOUT_CWBVH.

@@ -103,13 +103,18 @@ def upload_cwbvh(c, b, dev, used_blocks=None):
     return L().tbvh_upload_cwbvh(b.h, p(a[0]), used_blocks or c.d8.shape[0], p(a[1]), c.t8.shape[0] // 3, int(dev))
 
 
-def build(c, b, flavour):
-    return L().tbvh_build_flavour(b.h, p(c.v2), 16, c.v2.shape[0] // 3, api.HOST, 1.0, 1.0, flavour)
+def build(c, b, flavour, stride=16):
+    return L().tbvh_build_flavour(b.h, p(c.v2), stride, c.v2.shape[0] // 3, api.HOST, 1.0, 1.0, flavour)
 
 
-def build_indexed(c, b):
+def build_indexed(c, b, bad=False, dev=False):
+    """bad: one index points past vert_count; dev: vertices and indices in device memory"""
     idx = np.arange(c.v2.shape[0], dtype=np.uint32)
-    return L().tbvh_build_indexed(b.h, p(c.v2), 16, c.v2.shape[0], p(idx), c.v2.shape[0] // 3, api.HOST, 1.0, 1.0, _lib.BUILD_REFERENCE)
+    if bad:
+        idx[7] = c.v2.shape[0]
+    a = [c.v2, idx]
+    a = [on_device(x) for x in a] if dev else a
+    return L().tbvh_build_indexed(b.h, p(a[0]), 16, c.v2.shape[0], p(a[1]), c.v2.shape[0] // 3, int(dev), 1.0, 1.0, _lib.BUILD_REFERENCE)
 
 
 def build_batch(c, b, handles=None):
@@ -127,8 +132,8 @@ def convert_batch(c, b, layout=CW):
     return L().tbvh_convert_batch((C.c_void_p * 2)(b.h.value, c.keep.h.value), 2, layout)
 
 
-def refit(c, b, fn, prim_count=None):
-    return fn(b.h, p(c.moved), 16, prim_count or c.moved.shape[0] // 3, api.HOST)
+def refit(c, b, fn, prim_count=None, space=api.HOST):
+    return fn(b.h, p(c.moved), 16, prim_count or c.moved.shape[0] // 3, space)
 
 
 STALE = (STATE, STATE)
@@ -158,6 +163,9 @@ CASES = {
     "refit_layouts without CWBVH": (False, lambda c, b: refit(c, b, L().tbvh_refit_layouts), OK, NO_CW, STALE),
     # refusals leave the handle and the TLAS over it as they were
     "refused build": (True, lambda c, b: build(c, b, 7), _lib.E_ARG, FULL, (OK, OK)),
+    "refused build stride": (True, lambda c, b: build(c, b, _lib.BUILD_REFERENCE, stride=14), _lib.E_ARG, FULL, (OK, OK)),
+    "refused indexed build host": (True, lambda c, b: build_indexed(c, b, bad=True), _lib.E_ARG, FULL, (OK, OK)),
+    "refused indexed build device": (True, lambda c, b: build_indexed(c, b, bad=True, dev=True), _lib.E_ARG, FULL, (OK, OK)),
     "refused build_batch": (True, lambda c, b: build_batch(c, b, [b.h.value, b.h.value]), _lib.E_ARG, FULL, (OK, OK)),
     "refused upload_bvh": (True, lambda c, b: L().tbvh_upload_bvh(b.h, p(c.nodes32), 0, p(c.idx), c.idx.shape[0], p(c.v2), 16, c.v2.shape[0] // 3, api.HOST),
                            _lib.E_ARG, FULL, (OK, OK)),
@@ -168,6 +176,7 @@ CASES = {
     "refused convert_batch": (True, lambda c, b: convert_batch(c, b, GPU), _lib.E_UNSUPPORTED, FULL, (OK, OK)),
     "refused refit": (True, lambda c, b: refit(c, b, L().tbvh_refit, c.moved.shape[0] // 3 - 1), _lib.E_ARG, FULL, (OK, OK)),
     "refused refit_layouts": (True, lambda c, b: refit(c, b, L().tbvh_refit_layouts, c.moved.shape[0] // 3 - 1), _lib.E_ARG, FULL, (OK, OK)),
+    "refused refit space": (True, lambda c, b: refit(c, b, L().tbvh_refit, space=5), _lib.E_ARG, FULL, (OK, OK)),
 }
 
 

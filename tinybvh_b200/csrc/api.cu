@@ -510,32 +510,6 @@ static int gather_verts( float4* dst, const void* verts, uint32_t stride, uint32
 	if (rc == TBVH_OK && keep_idx) *keep_idx = d_idx; else cudaFree( d_idx );
 	return rc;
 }
-// keep: the handle keeps the indices and vert_count for tbvh_refit_batch_indexed (a refittable build)
-static int upload_verts_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space, cudaStream_t s,
-	bool keep )
-{
-	ARG_CHECK( verts && indices && stride >= 12 && (stride & 3) == 0 && prim_count > 0 && vert_count > 0, "bad indexed vertex slice" );
-	const size_t nv = (size_t)prim_count * 3;
-	uint32_t* d_bad = 0;
-	int rc = TBVH_OK;
-	auto body = [&]() -> int
-	{
-		CUDA_TRY( cudaMalloc( &d_bad, 4 ) );
-		CUDA_TRY( cudaMalloc( &b->d_verts, nv * 16 ) );
-		CUDA_TRY( cudaMemsetAsync( d_bad, 0, 4, s ) );
-		TRY( gather_verts( b->d_verts, verts, stride, vert_count, indices, prim_count, space, s, d_bad, keep ? &b->d_vert_idx : 0 ) );
-		uint32_t bad = 0;
-		CUDA_TRY( cudaMemcpy( &bad, d_bad, 4, cudaMemcpyDeviceToHost ) );
-		if (bad) { tbvh_set_error( "indexed build: %u indices point past the %u vertices", bad, vert_count ); return TBVH_E_ARG; }
-		return TBVH_OK;
-	};
-	rc = body();
-	cudaFree( d_bad );
-	if (rc != TBVH_OK && b->d_vert_idx) cudaFree( b->d_vert_idx ), b->d_vert_idx = 0;
-	b->vert_count = b->d_vert_idx ? vert_count : 0;
-	b->info.prim_count = prim_count;
-	return rc;
-}
 
 // depth of the deepest node (root = 0) of a tree of `words`-word nodes, by iterative DFS; children( n, c ) writes the two children of
 // node n to c and says whether the walk descends into them
@@ -602,19 +576,6 @@ static int upload_tree( tbvh_bvh b, float4** d_nodes, const void* nodes, uint32_
 	return TBVH_OK;
 }
 
-// the shared part of tbvh_build_flavour / tbvh_build_indexed: upload( stream ) puts the vertices into the emptied handle
-template <class Upload> static int build_one( const char* fn, tbvh_bvh b, float c_trav, float c_int, int flavour, Upload upload )
-{
-	if (!b) { tbvh_set_error( "%s: NULL handle", fn ); return TBVH_E_ARG; }
-	if (flavour != TBVH_BUILD_REFERENCE && flavour != TBVH_BUILD_AVX && flavour != TBVH_BUILD_HQ) { tbvh_set_error( "%s: unknown builder flavour", fn ); return TBVH_E_ARG; }
-	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
-	free_layouts( b );
-	TRY( upload( b->ctx->stream ) );
-	if (flavour == TBVH_BUILD_HQ) TRY( build_hq_launch( &b, 1, c_trav, c_int ) ); else TRY( build_sah_launch( &b, 1, c_trav, c_int, flavour ) );
-	b->info.layouts = 1u << TBVH_LAYOUT_BVH, b->refittable = flavour != TBVH_BUILD_HQ;
-	return TBVH_OK;
-}
-
 // the refusals of tbvh_refit / tbvh_refit_layouts / tbvh_refit_batch, in this order
 static int refit_check( const char* fn, tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, bool keep_layouts )
 {
@@ -665,14 +626,6 @@ static int refit_gather( tbvh_ctx c, const tbvh_bvh* bvhs, const tbvh_mesh* mesh
 	CUDA_TRY( cudaMemcpyAsync( c->ix_dev, T.data(), T.size() * sizeof( IxMesh ), cudaMemcpyHostToDevice, s ) );
 	k_refit_gather<<<(unsigned)((n + 255) / 256), 256, 0, s>>>( (const IxMesh*)c->ix_dev, (uint32_t)T.size(), (uint32_t)n ); LAUNCHED();
 	return TBVH_OK;
-}
-
-static int refit_one( const char* fn, tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space, bool keep_layouts )
-{
-	// every refusal comes before the vertex copy: a refused call leaves the handle as it was
-	TRY( refit_check( fn, b, verts, stride, prim_count, keep_layouts ) );
-	TRY( refit_copy( b, verts, stride, space ) );
-	return refit_trees( &b, 1, keep_layouts, b->ctx->stream );
 }
 
 // the handle list of a batch call: no NULL handle, one context, no handle twice
@@ -748,11 +701,6 @@ int tbvh_upload_cwbvh( tbvh_bvh b, const void* bvh8_data, uint32_t used_blocks, 
 	if (rc != TBVH_OK) drop_cwbvh( b );
 	else b->info.layouts |= 1u << TBVH_LAYOUT_CWBVH;
 	return rc;
-}
-
-int tbvh_build_flavour( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space, float c_trav, float c_int, int flavour )
-{
-	return build_one( __func__, b, c_trav, c_int, flavour, [&]( cudaStream_t s ) { return upload_verts( b, verts, stride, prim_count, space, s ); } );
 }
 
 // ---- BVH::SAHCost (tiny_bvh.h:1889-1897) over a downloaded node array: host recursion in the reference's own order
@@ -1003,21 +951,10 @@ int tbvh_build_tlas_update( tbvh_bvh t, void* instances, uint32_t inst_stride, u
 	return rc;
 }
 
-// BVH::Refit (tiny_bvh.h:3055): same topology, new vertex positions; derived layouts are dropped (convert_cwbvh.cu refit_trees)
-int tbvh_refit( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space )
-{
-	return refit_one( __func__, b, verts, stride, prim_count, space, false );
-}
-
-// BVH::Refit, then every derived layout brought up to date in place (include/tinybvh_b200.h)
-int tbvh_refit_layouts( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space )
-{
-	return refit_one( __func__, b, verts, stride, prim_count, space, true );
-}
-
 // Many trees, one refit (include/tinybvh_b200.h): tbvh_refit_batch, and with `indexed` tbvh_refit_batch_indexed, whose meshes with a
-// vert_count are the moved vertices of an indexed build.  Refit validation is host-side only: every refusal comes before any handle
-// or vertex array is touched, then the vertices are copied (indexed meshes: gathered) and the trees refitted together.
+// vert_count are the moved vertices of an indexed build; tbvh_refit and tbvh_refit_layouts are count = 1.  Refit validation is host-side
+// only: every refusal comes before any handle or vertex array is touched, then the vertices are copied (indexed meshes: gathered) and
+// the trees refitted together.
 static int refit_batch( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts, bool indexed )
 {
 	if (!(bvhs && meshes && count > 0)) { tbvh_set_error( "%s: no meshes", fn ); return TBVH_E_ARG; }
@@ -1063,6 +1000,20 @@ static int refit_batch( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 	return refit_trees( bvhs, count, keep_layouts != 0, ctx->stream );
 }
 
+// BVH::Refit (tiny_bvh.h:3055): same topology, new vertex positions; derived layouts are dropped (convert_cwbvh.cu refit_trees)
+int tbvh_refit( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space )
+{
+	const tbvh_mesh m{ verts, stride, 0, 0, prim_count };
+	return refit_batch( __func__, &b, &m, 1, space, 0, false );
+}
+
+// BVH::Refit, then every derived layout brought up to date in place (include/tinybvh_b200.h)
+int tbvh_refit_layouts( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space )
+{
+	const tbvh_mesh m{ verts, stride, 0, 0, prim_count };
+	return refit_batch( __func__, &b, &m, 1, space, 1, false );
+}
+
 int tbvh_refit_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, int keep_layouts )
 {
 	return refit_batch( __func__, bvhs, meshes, count, space, keep_layouts, false );
@@ -1074,17 +1025,10 @@ int tbvh_refit_batch_indexed( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t 
 	return refit_batch( __func__, bvhs, meshes, count, space, keep_layouts, true );
 }
 
-int tbvh_build_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space,
-	float c_trav, float c_int, int flavour )
-{
-	return build_one( __func__, b, c_trav, c_int, flavour,
-		[&]( cudaStream_t s ) { return upload_verts_indexed( b, verts, stride, vert_count, indices, prim_count, space, s, flavour != TBVH_BUILD_HQ ); } );
-}
-
-// The shared part of tbvh_build_batch / tbvh_build_batch_hq (include/tinybvh_b200.h) up to the build.  Every refusal comes before any
-// handle is touched, the vertex staging included: each mesh's vertices go into a fresh array first, and only when every index has
-// been found in range do the handles drop their old arrays and adopt the new ones.  The triangle counts are checked against the
-// limits before any index or vertex is read.  hq: the SBVH builder's node space must fit too.
+// The part of build_batch up to the build.  Every refusal comes before any handle is touched, the vertex staging included: each
+// mesh's vertices go into a fresh array first, and only when every index has been found in range do the handles drop their old arrays
+// and adopt the new ones.  The triangle counts are checked against the limits before any index or vertex is read.  hq: the SBVH
+// builder's node space must fit too.  Only a call with indexed meshes waits for the device here: flat ones are copied and no more.
 static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, bool hq )
 {
 	if (space != TBVH_HOST && space != TBVH_DEVICE) { tbvh_set_error( "%s: unknown space", fn ); return TBVH_E_ARG; }
@@ -1099,9 +1043,11 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 	if (total > TBVH_BATCH_MAX_PRIMS) { tbvh_set_error( "%s: %llu triangles in one batch (at most %u)", fn, (unsigned long long)total, (unsigned)TBVH_BATCH_MAX_PRIMS ); return TBVH_E_LIMIT; }
 	if (hq && 3 * total + 2 > TBVH_BATCH_HQ_MAX_NODES)
 	{ tbvh_set_error( "%s: %llu temporary SBVH nodes in one batch (at most %u)", fn, (unsigned long long)(3 * total + 2), (unsigned)TBVH_BATCH_HQ_MAX_NODES ); return TBVH_E_LIMIT; }
+	bool indexed = false;
 	for (uint32_t k = 0; k < count; k++)
 	{
 		const tbvh_mesh& m = meshes[k];
+		indexed |= m.indices != 0;
 		if (m.indices && space == TBVH_HOST)
 			for (size_t i = 0; i < (size_t)m.prim_count * 3; i++)
 				if (m.indices[i] >= m.vert_count) { tbvh_set_error( "%s: mesh %u: index %u points past the %u vertices", fn, k, m.indices[i], m.vert_count ); return TBVH_E_ARG; }
@@ -1114,8 +1060,11 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 	uint32_t* d_bad = 0;
 	auto stage = [&]() -> int
 	{
-		CUDA_TRY( cudaMalloc( &d_bad, 4 ) );
-		CUDA_TRY( cudaMemsetAsync( d_bad, 0, 4, s ) );
+		if (indexed)
+		{
+			CUDA_TRY( cudaMalloc( &d_bad, 4 ) );
+			CUDA_TRY( cudaMemsetAsync( d_bad, 0, 4, s ) );
+		}
 		for (uint32_t k = 0; k < count; k++)
 		{
 			const tbvh_mesh& m = meshes[k];
@@ -1123,6 +1072,7 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 			if (m.indices) TRY( gather_verts( staged[k], m.verts, m.stride, m.vert_count, m.indices, m.prim_count, space, s, d_bad, hq ? 0 : &staged_idx[k] ) );
 			else TRY( copy_verts( staged[k], m.verts, m.stride, (size_t)m.prim_count * 3, space, s ) );
 		}
+		if (!indexed) return TBVH_OK;
 		uint32_t bad = 0;
 		CUDA_TRY( cudaMemcpyAsync( &bad, d_bad, 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
@@ -1148,38 +1098,73 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 	return TBVH_OK;
 }
 
-// after the build of a batch: each handle holds its BVH-layout tree, or, where the build failed, nothing (as a failed build leaves it)
-static int batch_finish( tbvh_bvh* bvhs, uint32_t count, int rc, bool refittable )
+// Many meshes, one build (include/tinybvh_b200.h): tbvh_build_batch and tbvh_build_batch_hq; tbvh_build_flavour and tbvh_build_indexed
+// are count = 1.  fn: the entry point the error texts name.  A failed build leaves each handle of the call empty.
+static int build_batch( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int, int flavour )
 {
+	if (!(bvhs && meshes && count > 0)) { tbvh_set_error( "%s: no meshes", fn ); return TBVH_E_ARG; }
+	if (flavour != TBVH_BUILD_REFERENCE && flavour != TBVH_BUILD_AVX && flavour != TBVH_BUILD_HQ) { tbvh_set_error( "%s: unknown builder flavour", fn ); return TBVH_E_ARG; }
+	const bool hq = flavour == TBVH_BUILD_HQ;
+	TRY( batch_stage( fn, bvhs, meshes, count, space, hq ) );
+	const int rc = hq ? build_hq_launch( bvhs, count, c_trav, c_int ) : build_sah_launch( bvhs, count, c_trav, c_int, flavour );
 	for (uint32_t k = 0; k < count; k++)
 	{
 		if (rc != TBVH_OK) free_layouts( bvhs[k] );
-		else bvhs[k]->info.layouts = 1u << TBVH_LAYOUT_BVH, bvhs[k]->refittable = refittable;
+		else bvhs[k]->info.layouts = 1u << TBVH_LAYOUT_BVH, bvhs[k]->refittable = !hq; // "can't refit an SBVH" (:3027)
 	}
 	return rc;
 }
 
-// Many meshes, one build (include/tinybvh_b200.h)
 int tbvh_build_batch( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int, int flavour )
 {
 	ARG_CHECK( bvhs && meshes && count > 0, "no meshes" );
 	if (flavour == TBVH_BUILD_HQ) { tbvh_set_error( "tbvh_build_batch: SBVH (BuildHQ) batches are built by tbvh_build_batch_hq" ); return TBVH_E_UNSUPPORTED; }
-	ARG_CHECK( flavour == TBVH_BUILD_REFERENCE || flavour == TBVH_BUILD_AVX, "unknown builder flavour" );
-	TRY( batch_stage( __func__, bvhs, meshes, count, space, false ) );
-	return batch_finish( bvhs, count, build_sah_launch( bvhs, count, c_trav, c_int, flavour ), true );
+	return build_batch( __func__, bvhs, meshes, count, space, c_trav, c_int, flavour );
 }
 
-// Many meshes, one SBVH build (include/tinybvh_b200.h)
 int tbvh_build_batch_hq( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int )
 {
-	ARG_CHECK( bvhs && meshes && count > 0, "no meshes" );
-	TRY( batch_stage( __func__, bvhs, meshes, count, space, true ) );
-	return batch_finish( bvhs, count, build_hq_launch( bvhs, count, c_trav, c_int ), false ); // "can't refit an SBVH" (:3027)
+	return build_batch( __func__, bvhs, meshes, count, space, c_trav, c_int, TBVH_BUILD_HQ );
+}
+
+int tbvh_build_flavour( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space, float c_trav, float c_int, int flavour )
+{
+	const tbvh_mesh m{ verts, stride, 0, 0, prim_count };
+	return build_batch( __func__, &b, &m, 1, space, c_trav, c_int, flavour );
+}
+
+int tbvh_build_indexed( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t vert_count, const uint32_t* indices, uint32_t prim_count, int space,
+	float c_trav, float c_int, int flavour )
+{
+	ARG_CHECK( indices, "indices == NULL" ); // a mesh record without indices is a flat one
+	const tbvh_mesh m{ verts, stride, vert_count, indices, prim_count };
+	return build_batch( __func__, &b, &m, 1, space, c_trav, c_int, flavour );
 }
 
 int tbvh_build( tbvh_bvh b, const void* verts, uint32_t stride, uint32_t prim_count, int space, float c_trav, float c_int )
 {
 	return tbvh_build_flavour( b, verts, stride, prim_count, space, c_trav, c_int, TBVH_BUILD_REFERENCE );
+}
+
+// Many trees, one conversion (include/tinybvh_b200.h): tbvh_convert_batch; tbvh_convert( .., TBVH_LAYOUT_CWBVH ) is count = 1.  Every
+// refusal comes before any handle is touched.
+static int convert_batch( const char* fn, tbvh_bvh* bvhs, uint32_t count, int to_layout )
+{
+	if (!(bvhs && count > 0)) { tbvh_set_error( "%s: no handles", fn ); return TBVH_E_ARG; }
+	TRY( check_batch_handles( fn, bvhs, count ) );
+	uint64_t nodes = 0;
+	for (uint32_t k = 0; k < count; k++)
+	{
+		const tbvh_bvh b = bvhs[k];
+		if (!(b->info.layouts & (1u << TBVH_LAYOUT_BVH))) { tbvh_set_error( "%s: handle %u holds no BVH-layout tree", fn, k ); return TBVH_E_STATE; }
+		if (b->d_inst) { tbvh_set_error( "%s: handle %u is a TLAS, which has no CWBVH layout", fn, k ); return TBVH_E_STATE; }
+		// at least two nodes per tree (a leaf root is wrapped into node 1); SplitLeafs(3) adds at most 2 nodes per 3 primitives
+		nodes += (uint64_t)std::max( b->info.used_nodes, 2u ) + 2 * (((uint64_t)b->info.idx_count + 2) / 3);
+	}
+	if (to_layout != TBVH_LAYOUT_CWBVH) { tbvh_set_error( "%s: target layout %d (only TBVH_LAYOUT_CWBVH converts in batches)", fn, to_layout ); return TBVH_E_UNSUPPORTED; }
+	if (nodes > TBVH_CONVERT_BATCH_MAX_NODES) { tbvh_set_error( "%s: up to %llu split-tree nodes in one batch (at most %u)", fn, (unsigned long long)nodes, (unsigned)TBVH_CONVERT_BATCH_MAX_NODES ); return TBVH_E_LIMIT; }
+	CUDA_TRY( cudaSetDevice( bvhs[0]->ctx->device ) );
+	return bvh_to_cwbvh( bvhs, count, bvhs[0]->ctx->stream );
 }
 
 int tbvh_convert( tbvh_bvh b, int to_layout )
@@ -1188,34 +1173,14 @@ int tbvh_convert( tbvh_bvh b, int to_layout )
 	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
 	if (!(b->info.layouts & (1u << TBVH_LAYOUT_BVH))) { tbvh_set_error( "tbvh_convert: source layout BVH not resident" ); return TBVH_E_STATE; }
 	if (to_layout == TBVH_LAYOUT_BVH_GPU) return bvh_to_bvh_gpu( b, b->ctx->stream );
-	if (to_layout == TBVH_LAYOUT_CWBVH)
-	{
-		// a TLAS's leaves are instances: there are no triangles to encode (its handle holds no vertices)
-		if (b->d_inst) { tbvh_set_error( "tbvh_convert: a TLAS has no CWBVH layout (convert its BLASses)" ); return TBVH_E_STATE; }
-		return bvh_to_cwbvh( &b, 1, b->ctx->stream );
-	}
+	if (to_layout == TBVH_LAYOUT_CWBVH) return convert_batch( __func__, &b, 1, to_layout );
 	tbvh_set_error( "tbvh_convert: unsupported target layout %d", to_layout );
 	return TBVH_E_UNSUPPORTED;
 }
 
-// Many trees, one conversion (include/tinybvh_b200.h).  Every refusal comes before any handle is touched.
 int tbvh_convert_batch( tbvh_bvh* bvhs, uint32_t count, int to_layout )
 {
-	ARG_CHECK( bvhs && count > 0, "no handles" );
-	TRY( check_batch_handles( __func__, bvhs, count ) );
-	uint64_t nodes = 0;
-	for (uint32_t k = 0; k < count; k++)
-	{
-		const tbvh_bvh b = bvhs[k];
-		if (!(b->info.layouts & (1u << TBVH_LAYOUT_BVH))) { tbvh_set_error( "tbvh_convert_batch: handle %u holds no BVH-layout tree", k ); return TBVH_E_STATE; }
-		if (b->d_inst) { tbvh_set_error( "tbvh_convert_batch: handle %u is a TLAS, which has no CWBVH layout", k ); return TBVH_E_STATE; }
-		// at least two nodes per tree (a leaf root is wrapped into node 1); SplitLeafs(3) adds at most 2 nodes per 3 primitives
-		nodes += (uint64_t)std::max( b->info.used_nodes, 2u ) + 2 * (((uint64_t)b->info.idx_count + 2) / 3);
-	}
-	if (to_layout != TBVH_LAYOUT_CWBVH) { tbvh_set_error( "tbvh_convert_batch: target layout %d (only TBVH_LAYOUT_CWBVH converts in batches)", to_layout ); return TBVH_E_UNSUPPORTED; }
-	if (nodes > TBVH_CONVERT_BATCH_MAX_NODES) { tbvh_set_error( "tbvh_convert_batch: up to %llu split-tree nodes in one batch (at most %u)", (unsigned long long)nodes, (unsigned)TBVH_CONVERT_BATCH_MAX_NODES ); return TBVH_E_LIMIT; }
-	CUDA_TRY( cudaSetDevice( bvhs[0]->ctx->device ) );
-	return bvh_to_cwbvh( bvhs, count, bvhs[0]->ctx->stream );
+	return convert_batch( __func__, bvhs, count, to_layout );
 }
 
 static cudaMemcpyKind out_kind( int space ) { return space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost; }
