@@ -218,7 +218,7 @@ template <class E, uint32_t E::*F> __device__ __forceinline__ uint32_t batch_ent
 }
 
 // one tree of a refit (refit.cu, convert.cu): BVH::Refit over the batch's node space, the BVH2 traversal records over its primitive
-// reference space.  A single tree passes its entry as a kernel parameter instead of a table.
+// reference space.  A single tree is a one-entry table.
 struct RfTree
 {
 	float4* nodes;
@@ -242,21 +242,20 @@ int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_
 int cwbvh_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_hits, uint32_t hit_stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s, unsigned long long* d_stats );
 // traversal nodes, cw_rd_limit and cw_pending of the CWBVH of each of bs[0 .. K), in one pass (trace_cwbvh.cu); synchronises s
 int cw_make_trav( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
-// cw_make_trav's node expansion of the W nodes of K trees (table d_T; K = 1: `one`) into their d_cw_trav; parent: NULL (a refit)
-// or where the pending pass finds the parents
-int cw_expand( const CwTrav* d_T, uint32_t K, const CwTrav& one, uint32_t W, uint32_t* parent, cudaStream_t s );
+// cw_make_trav's node expansion of the W nodes of K trees (table d_T) into their d_cw_trav; parent: NULL (a refit) or where the
+// pending pass finds the parents
+int cw_expand( const CwTrav* d_T, uint32_t K, uint32_t W, uint32_t* parent, cudaStream_t s );
 float cw_rd_limit_for( uint32_t range );                               // cw_rd_limit of a tree whose expansion found `range`
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)
 // binned-SAH builds of `trees` handles of one context at once (build_sah.cu); a single build is trees = 1
 int build_sah_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, int flavour );
 // SBVH builds (BuildHQ) of K handles of one context at once (build_hq.cu); a single build is K = 1
 int build_hq_launch( const tbvh_bvh* bs, uint32_t K, float c_trav, float c_int );
-// BVH::Refit of K trees over one node space of `nodes` nodes; arrive: `nodes` zeroed words; fill: some tree's parents are filled.
-// K = 1 runs the single-tree instances with `one`.
-int refit_enqueue( const RfTree* d_T, uint32_t K, const RfTree& one, uint32_t nodes, uint32_t* arrive, bool fill, cudaStream_t s );
+// BVH::Refit of K trees over one node space of `nodes` nodes; arrive: `nodes` zeroed words; fill: some tree's parents are filled
+int refit_enqueue( const RfTree* d_T, uint32_t K, uint32_t nodes, uint32_t* arrive, bool fill, cudaStream_t s );
 int refit_roots( const RfTree* d_T, uint32_t K, uint32_t* out, cudaStream_t s ); // each tree's root node (8 words) to out[8 t ..]
-// the leaf-ordered triangle records of K trees over one space of `refs` primitive references (convert.cu); K = 1 as above
-int leaf_tris_enqueue( const RfTree* d_T, uint32_t K, const RfTree& one, uint32_t refs, cudaStream_t s );
+// the leaf-ordered triangle records of K trees over one space of `refs` primitive references (convert.cu)
+int leaf_tris_enqueue( const RfTree* d_T, uint32_t K, uint32_t refs, cudaStream_t s );
 int leaf_tris_alloc( tbvh_bvh b ); // d_leaf_tris sized to idx_count (kept when it is: a TLAS holding its address stays valid)
 // Refit of K handles of one context (tbvh_refit, tbvh_refit_layouts, tbvh_refit_batch): d_verts already hold the new positions.
 // keep_layouts: BVH_GPU and CWBVH brought up to date in place, the generation renewed; else both dropped.  One host synchronisation.
@@ -264,7 +263,7 @@ int leaf_tris_alloc( tbvh_bvh b ); // d_leaf_tris sized to idx_count (kept when 
 int refit_trees( const tbvh_bvh* bs, uint32_t K, bool keep_layouts, cudaStream_t s );
 void cw_keep_sizes( tbvh_bvh b, uint32_t* total, uint32_t* wide_count ); // split-tree and wide nodes of the kept collapse (0: none)
 // BVH_GPU::ConvertFrom of K trees over one node space of n nodes into their `out` arrays; w: 4 n words of workspace (zeroed here)
-int bvh_gpu_enqueue( const GpuTree* d_T, uint32_t K, const GpuTree& one, uint32_t n, uint32_t* w, cudaStream_t s );
+int bvh_gpu_enqueue( const GpuTree* d_T, uint32_t K, uint32_t n, uint32_t* w, cudaStream_t s );
 int tlas_trace_launch( tbvh_bvh b, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, bool anyhit, cudaStream_t s );
 // the refusals of a launch of n rays before any work (n = 0 refuses only what precedes the launches' own `n == 0` exit); the device
 // views (api.cu tbvh_device_view) make the same checks for n > 0

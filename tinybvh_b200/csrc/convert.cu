@@ -12,22 +12,20 @@ uint32_t tbvh_next_generation()
 	return ++counter;
 }
 
-// one thread per primitive reference: 4 B index read + the record (common.cuh leaf_tri_record).  BATCH: reference g of the batch's
-// reference space, in the tree that owns it (RfTree::pbase); else the one tree `one`
-template <bool BATCH>
-__global__ void k_make_leaf_tris( const RfTree* __restrict__ T, const uint32_t K, const RfTree one, const uint32_t n )
+// one thread per primitive reference: 4 B index read + the record (common.cuh leaf_tri_record).  Reference g of the batch's
+// reference space, in the tree that owns it (RfTree::pbase)
+__global__ void k_make_leaf_tris( const RfTree* __restrict__ T, const uint32_t K, const uint32_t n )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
-	const RfTree& tr = BATCH ? T[batch_entry<RfTree, &RfTree::pbase>( T, K, g )] : one;
-	const uint32_t p = BATCH ? g - tr.pbase : g;
+	const RfTree& tr = T[batch_entry<RfTree, &RfTree::pbase>( T, K, g )];
+	const uint32_t p = g - tr.pbase;
 	leaf_tri_record( tr.verts, __ldg( tr.prim_idx + p ), tr.leaf_tris, p );
 }
 
-int leaf_tris_enqueue( const RfTree* d_T, const uint32_t K, const RfTree& one, const uint32_t n, cudaStream_t s )
+int leaf_tris_enqueue( const RfTree* d_T, const uint32_t K, const uint32_t n, cudaStream_t s )
 {
-	if (K == 1) k_make_leaf_tris<false><<<(n + 255) / 256, 256, 0, s>>>( 0, 1, one, n );
-	else k_make_leaf_tris<true><<<(n + 255) / 256, 256, 0, s>>>( d_T, K, RfTree{}, n );
+	k_make_leaf_tris<<<(n + 255) / 256, 256, 0, s>>>( d_T, K, n );
 	LAUNCHED();
 	return TBVH_OK;
 }
@@ -44,9 +42,22 @@ int leaf_tris_alloc( tbvh_bvh b )
 int make_leaf_tris( tbvh_bvh b, cudaStream_t s )
 {
 	TRY( leaf_tris_alloc( b ) );
-	RfTree one = {};
-	one.prim_idx = b->d_prim_idx, one.verts = b->d_verts, one.leaf_tris = b->d_leaf_tris;
-	return leaf_tris_enqueue( 0, 1, one, b->info.idx_count, s );
+	// the tree as a one-entry table; an upload synchronises right after, so the table lives for the call only
+	RfTree entry = {};
+	entry.prim_idx = b->d_prim_idx, entry.verts = b->d_verts, entry.leaf_tris = b->d_leaf_tris;
+	RfTree* d_T = 0;
+	CUDA_TRY( cudaMalloc( &d_T, sizeof( RfTree ) ) );
+	auto body = [&]() -> int
+	{
+		CUDA_TRY( cudaMemcpyAsync( d_T, &entry, sizeof( RfTree ), cudaMemcpyHostToDevice, s ) );
+		TRY( leaf_tris_enqueue( d_T, 1, b->info.idx_count, s ) );
+		CUDA_TRY( cudaStreamSynchronize( s ) );
+		return TBVH_OK;
+	};
+	const int rc = body();
+	cudaStreamSynchronize( s );
+	cudaFree( d_T );
+	return rc;
 }
 
 // one thread per Aila-Laine node i; an interior node writes its children as the pair at slots 2i, 2i+1:
@@ -84,26 +95,17 @@ int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used, cudaStream_t s )
 //     pre(left) = pre(p) + 1,   pre(right) = pre(p) + 1 + size(left)
 // so it depends on the tree's shape alone: neither on the node numbering nor on the order of the leaf ranges in primIdx (a tree
 // after BVH::Optimize, or uploaded from elsewhere, has its leaf ranges out of DFS order).
-// BATCH: node g of the pass's node space, in the tree that owns it (GpuTree::nbase); the workspace arrays are the batch's, tree t's
-// from nbase on, and hold local node numbers.  Else the one tree `one`.
-template <bool BATCH> __device__ __forceinline__ const GpuTree& gpu_tree( const GpuTree* __restrict__ T, const uint32_t K, const GpuTree& one, const uint32_t g, uint32_t& x )
-{
-	if (!BATCH) { x = g; return one; }
-	const GpuTree& tr = T[batch_entry<GpuTree, &GpuTree::nbase>( T, K, g )];
-	x = g - tr.nbase;
-	return tr;
-}
-
-template <bool BATCH>
-__global__ void k_gpu_parents( const GpuTree* __restrict__ T, const uint32_t K, const GpuTree one, uint32_t* __restrict__ parent, const uint32_t n )
+// Node g of the pass's node space, in the tree that owns it (GpuTree::nbase); the workspace arrays are the pass's, tree t's from nbase
+// on, and hold local node numbers.
+__global__ void k_gpu_parents( const GpuTree* __restrict__ T, const uint32_t K, uint32_t* __restrict__ parent, const uint32_t n )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
-	uint32_t x;
-	const GpuTree& tr = gpu_tree<BATCH>( T, K, one, g, x );
+	const GpuTree& tr = T[batch_entry<GpuTree, &GpuTree::nbase>( T, K, g )];
+	const uint32_t x = g - tr.nbase;
 	if (x == 1) return;
 	const float4* __restrict__ nodes = tr.nodes;
-	if (BATCH) parent += tr.nbase;
+	parent += tr.nbase;
 	if (x == 0) parent[0] = 0xffffffffu;
 	if (__float_as_uint( nodes[(size_t)x * 2 + 1].w ) != 0) return;
 	const uint32_t c = __float_as_uint( nodes[(size_t)x * 2].w );
@@ -111,35 +113,33 @@ __global__ void k_gpu_parents( const GpuTree* __restrict__ T, const uint32_t K, 
 }
 
 // bottom-up from every leaf: interior nodes and leaves per subtree (every leaf weighs 1)
-template <bool BATCH>
-__global__ void k_gpu_sizes( const GpuTree* __restrict__ T, const uint32_t K, const GpuTree one, const uint32_t* __restrict__ parent, uint32_t* arrive,
-	uint32_t* sub_int, uint32_t* sub_leaves, const uint32_t n )
+__global__ void k_gpu_sizes( const GpuTree* __restrict__ T, const uint32_t K, const uint32_t* __restrict__ parent, uint32_t* arrive, uint32_t* sub_int,
+	uint32_t* sub_leaves, const uint32_t n )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
-	uint32_t x;
-	const GpuTree& tr = gpu_tree<BATCH>( T, K, one, g, x );
+	const GpuTree& tr = T[batch_entry<GpuTree, &GpuTree::nbase>( T, K, g )];
+	const uint32_t x = g - tr.nbase;
 	if (x == 1) return;
 	const float4* __restrict__ nodes = tr.nodes;
 	if (__float_as_uint( nodes[(size_t)x * 2 + 1].w ) == 0) return; // leaves only
-	if (BATCH) parent += tr.nbase, arrive += tr.nbase, sub_int += tr.nbase, sub_leaves += tr.nbase;
+	parent += tr.nbase, arrive += tr.nbase, sub_int += tr.nbase, sub_leaves += tr.nbase;
 	dfs_sizes_up( nodes, parent, arrive, sub_int, sub_leaves, x, 1u );
 }
 
 // one thread per node: its preorder index from its path to the root; an interior node's left child follows it, its right child
 // follows the left subtree (sub_int + sub_leaves nodes)
-template <bool BATCH>
-__global__ void k_gpu_emit( const GpuTree* __restrict__ T, const uint32_t K, const GpuTree one, const uint32_t* __restrict__ parent, const uint32_t* __restrict__ sub_int,
+__global__ void k_gpu_emit( const GpuTree* __restrict__ T, const uint32_t K, const uint32_t* __restrict__ parent, const uint32_t* __restrict__ sub_int,
 	const uint32_t* __restrict__ sub_leaves, const uint32_t n )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
-	uint32_t x;
-	const GpuTree& tr = gpu_tree<BATCH>( T, K, one, g, x );
+	const GpuTree& tr = T[batch_entry<GpuTree, &GpuTree::nbase>( T, K, g )];
+	const uint32_t x = g - tr.nbase;
 	if (x == 1) return;
 	const float4* __restrict__ nodes = tr.nodes;
 	float4* __restrict__ out = tr.out;
-	if (BATCH) parent += tr.nbase, sub_int += tr.nbase, sub_leaves += tr.nbase;
+	parent += tr.nbase, sub_int += tr.nbase, sub_leaves += tr.nbase;
 	const float4 a = nodes[(size_t)x * 2], b = nodes[(size_t)x * 2 + 1];
 	uint32_t Kx, L, Kp;
 	dfs_rank( nodes, parent, sub_int, sub_leaves, x, Kx, L, Kp );
@@ -160,21 +160,14 @@ __global__ void k_gpu_emit( const GpuTree* __restrict__ T, const uint32_t K, con
 	out[(size_t)idx * 4 + 3] = make_float4( r1.x, r1.y, r1.z, __uint_as_float( 0u ) );
 }
 
-int bvh_gpu_enqueue( const GpuTree* d_T, const uint32_t K, const GpuTree& one, const uint32_t n, uint32_t* w, cudaStream_t s )
+int bvh_gpu_enqueue( const GpuTree* d_T, const uint32_t K, const uint32_t n, uint32_t* w, cudaStream_t s )
 {
 	uint32_t* parent = w, * arrive = w + n, * sub_int = arrive + n, * sub_leaves = sub_int + n;
 	CUDA_TRY( cudaMemsetAsync( w, 0, (size_t)n * 16, s ) );
 	const uint32_t g = (n + 255) / 256;
-	if (K == 1)
-	{
-		k_gpu_parents<false><<<g, 256, 0, s>>>( 0, 1, one, parent, n ); LAUNCHED();
-		k_gpu_sizes<false><<<g, 256, 0, s>>>( 0, 1, one, parent, arrive, sub_int, sub_leaves, n ); LAUNCHED();
-		k_gpu_emit<false><<<g, 256, 0, s>>>( 0, 1, one, parent, sub_int, sub_leaves, n ); LAUNCHED();
-		return TBVH_OK;
-	}
-	k_gpu_parents<true><<<g, 256, 0, s>>>( d_T, K, GpuTree{}, parent, n ); LAUNCHED();
-	k_gpu_sizes<true><<<g, 256, 0, s>>>( d_T, K, GpuTree{}, parent, arrive, sub_int, sub_leaves, n ); LAUNCHED();
-	k_gpu_emit<true><<<g, 256, 0, s>>>( d_T, K, GpuTree{}, parent, sub_int, sub_leaves, n ); LAUNCHED();
+	k_gpu_parents<<<g, 256, 0, s>>>( d_T, K, parent, n ); LAUNCHED();
+	k_gpu_sizes<<<g, 256, 0, s>>>( d_T, K, parent, arrive, sub_int, sub_leaves, n ); LAUNCHED();
+	k_gpu_emit<<<g, 256, 0, s>>>( d_T, K, parent, sub_int, sub_leaves, n ); LAUNCHED();
 	return TBVH_OK;
 }
 
@@ -189,13 +182,16 @@ int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s )
 {
 	const uint32_t used = b->info.used_nodes;
 	drop_bvh_gpu( b );
-	uint32_t* w = 0; // workspace: parent, arrive, sub_int, sub_leaves [used]
+	uint32_t* w = 0; // workspace: parent, arrive, sub_int, sub_leaves [used], then the tree as a one-entry table
 	const size_t words = (size_t)used * 4;
 	auto body = [&]() -> int
 	{
 		CUDA_TRY( cudaMalloc( &b->d_nodes_gpu, (size_t)used * 64 ) );
-		CUDA_TRY( cudaMalloc( &w, words * 4 ) );
-		TRY( bvh_gpu_enqueue( 0, 1, GpuTree{ b->d_nodes, b->d_nodes_gpu, 0, used }, used, w, s ) );
+		CUDA_TRY( cudaMalloc( &w, words * 4 + sizeof( GpuTree ) ) );
+		const GpuTree entry{ b->d_nodes, b->d_nodes_gpu, 0, used };
+		GpuTree* const d_T = (GpuTree*)(w + words);
+		CUDA_TRY( cudaMemcpyAsync( d_T, &entry, sizeof( GpuTree ), cudaMemcpyHostToDevice, s ) );
+		TRY( bvh_gpu_enqueue( d_T, 1, used, w, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
 	};

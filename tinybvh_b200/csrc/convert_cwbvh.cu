@@ -23,9 +23,9 @@
 // array, whose child links are global.  Level 0 of the collapse holds the K roots; a level places every node's interior children by
 // a scan over the level in list order, so each level is grouped by tree in batch order and the lists are deterministic.
 // Everything after the collapse is one per-tree pipeline, shared with the refit: k_keep makes every tree's collapse tree-local, and
-// cw_assign_encode runs over a table of trees (CwTree) and each tree's runs of the levels (CwRun).  A single tree is its own forest
-// and runs the single-tree instances over its own arrays.  The fixed costs - allocations, launches and host round trips - grow with
-// the deepest tree's level count, not with K.
+// cw_assign_encode runs over a table of trees (CwTree) and each tree's runs of the levels (CwRun).  A single tree is a one-entry
+// table; its forest is already tree-local, so unless it keeps its collapse the table points into the forest and k_keep does not run.
+// The fixed costs - allocations, launches and host round trips - grow with the deepest tree's level count, not with K.
 #include "common.cuh"
 #include <algorithm>
 #include <new>
@@ -74,8 +74,8 @@ static void cw_keep_free( tbvh_bvh b )
 	b->cw_keep = 0;
 }
 
-// One tree of a conversion or of a refit that keeps its CWBVH (device table, indexed by tree; a step that only one tree takes gets
-// the entry as a kernel parameter instead).  Everything after the collapse works on the tree's own arrays with tree-local numbers.
+// One tree of a conversion or of a refit that keeps its CWBVH (device table, indexed by tree).  Everything after the collapse works on
+// the tree's own arrays with tree-local numbers.
 struct CwTree
 {
 	const float4* nodes;                // BVH2 nodes (d_nodes)
@@ -156,22 +156,20 @@ __device__ __forceinline__ void split_emit( float4 a, const float4 b, const uint
 }
 
 // Every tree's chains follow its own nodes.  A conversion's forest (shift = ext_base, the batch scan from nbase) keeps global child
-// links for k_collapse; a refit's kept split tree (shift = 0, CwKeep::base) is local.  BATCH: node g of the call's node space, in the
-// tree of T that owns it; else node g of `one` (n = its used)
-template <bool BATCH>
-__global__ void k_split_emit( const CwTree* __restrict__ T, const uint32_t K, const CwTree one, const uint32_t n, const uint32_t max_prims )
+// links for k_collapse; a refit's kept split tree (shift = 0, CwKeep::base) is local.  Node g of the call's node space, in the tree
+// of T that owns it.
+__global__ void k_split_emit( const CwTree* __restrict__ T, const uint32_t K, const uint32_t n, const uint32_t max_prims )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
-	const CwTree& tr = BATCH ? T[batch_entry<CwTree, &CwTree::nbase>( T, K, g )] : one;
-	const uint32_t x = BATCH ? g - tr.nbase : g;
-	if (BATCH && x >= tr.used) return; // node 1 of a one-node tree in a conversion: only a leaf-root wrap writes it
+	const CwTree& tr = T[batch_entry<CwTree, &CwTree::nbase>( T, K, g )];
+	const uint32_t x = g - tr.nbase;
+	if (x >= tr.used) return; // node 1 of a one-node tree in a conversion: only a leaf-root wrap writes it
 	split_emit( tr.nodes[(size_t)x * 2], tr.nodes[(size_t)x * 2 + 1], x, tr.shift, cw_seg( tr.used ) + tr.scan[x] - tr.scan[0], tr.ext, max_prims );
 }
-static int cw_split_emit( const CwTree* d_T, const uint32_t K, const CwTree& one, const uint32_t n, cudaStream_t s )
+static int cw_split_emit( const CwTree* d_T, const uint32_t K, const uint32_t n, cudaStream_t s )
 {
-	if (K > 1) k_split_emit<true><<<(n + 255) / 256, 256, 0, s>>>( d_T, K, CwTree{}, n, 3 );
-	else k_split_emit<false><<<(one.used + 255) / 256, 256, 0, s>>>( 0, 1, one, one.used, 3 );
+	k_split_emit<<<(n + 255) / 256, 256, 0, s>>>( d_T, K, n, 3 );
 	LAUNCHED();
 	return TBVH_OK;
 }
@@ -313,15 +311,14 @@ __global__ void k_keep( const CwTree* __restrict__ T, const uint32_t K, const Cw
 }
 
 // ---- BVH8_CWBVH::ConvertFrom, greedy child -> slot assignment (:5910-5946) and per-node child statistics, one thread per wide node.
-// BATCH: wide node g of the call's wide-node space, in the tree of T that owns it; else node g of `one`.  A tree's own arrays, local
-// numbers: its local node 0 is its root.
-template <bool BATCH>
-__global__ void k_assign( const CwTree* __restrict__ T, const uint32_t K, const CwTree one, const uint32_t num )
+// Wide node g of the call's wide-node space, in the tree of T that owns it.  A tree's own arrays, local numbers: its local node 0 is
+// its root.
+__global__ void k_assign( const CwTree* __restrict__ T, const uint32_t K, const uint32_t num )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= num) return;
-	const CwTree& tr = BATCH ? T[batch_entry<CwTree, &CwTree::wbase>( T, K, g )] : one;
-	const uint32_t t = BATCH ? g - tr.wbase : g;
+	const CwTree& tr = T[batch_entry<CwTree, &CwTree::wbase>( T, K, g )];
+	const uint32_t t = g - tr.wbase;
 	const float4* __restrict__ ext = tr.ext;
 	const uint32_t* __restrict__ adopt = tr.adopt;
 	const uint32_t x = tr.list[t];
@@ -379,23 +376,22 @@ __global__ void k_assign( const CwTree* __restrict__ T, const uint32_t K, const 
 	tr.wide[t] = w;
 }
 
-// wide node lo + t of the call's level order: of `wide`, or (BATCH) of the level's run that holds it, in its tree's own array
-template <bool BATCH> __device__ __forceinline__ uint32_t level_node( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns,
-	const uint32_t lo, const uint32_t t, WideNode* __restrict__& wide )
+// wide node lo + t of the call's level order: of the level's run that holds it, in its tree's own array
+__device__ __forceinline__ uint32_t level_node( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo,
+	const uint32_t t, WideNode* __restrict__& wide )
 {
-	if (!BATCH) return lo + t;
 	const CwRun r = runs[batch_entry<CwRun, &CwRun::first>( runs, nruns, lo + t )];
 	wide = T[r.tree].wide;
 	return r.lo + lo + t - r.first;
 }
 
 // bottom-up: subtree node / triangle counts of wide nodes lo .. lo+num-1 (the next level's are final already)
-template <bool BATCH>
-__global__ void k_sizes( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
+__global__ void k_sizes( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= num) return;
-	const uint32_t x = level_node<BATCH>( T, runs, nruns, lo, t, wide );
+	WideNode* wide;
+	const uint32_t x = level_node( T, runs, nruns, lo, t, wide );
 	uint32_t size = 1, tris = wide[x].leaf_tris;
 	for (int s = 0; s < 8; s++)
 	{
@@ -407,12 +403,12 @@ __global__ void k_sizes( const CwTree* __restrict__ T, const CwRun* __restrict__
 }
 
 // top-down: output addresses of the children of wide nodes lo .. lo+num-1 (see the header comment)
-template <bool BATCH>
-__global__ void k_addresses( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num, WideNode* __restrict__ wide )
+__global__ void k_addresses( const CwTree* __restrict__ T, const CwRun* __restrict__ runs, const uint32_t nruns, const uint32_t lo, const uint32_t num )
 {
 	const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
 	if (t >= num) return;
-	const uint32_t x = level_node<BATCH>( T, runs, nruns, lo, t, wide );
+	WideNode* wide;
+	const uint32_t x = level_node( T, runs, nruns, lo, t, wide );
 	const WideNode w = wide[x];
 	uint32_t accS = 0, accT = 0, j = w.ichild;
 	for (int s = 7; s >= 0; s--)
@@ -487,14 +483,13 @@ __device__ __forceinline__ void encode_node( const float4* __restrict__ ext, con
 	o[4] = make_float4( __uint_as_float( q[8] ), __uint_as_float( q[9] ), __uint_as_float( q[10] ), __uint_as_float( q[11] ) );
 }
 
-// wide node g: BATCH and one as for k_assign
-template <bool BATCH>
-__global__ void k_encode( const CwTree* __restrict__ T, const uint32_t K, const CwTree one, const uint32_t num )
+// wide node g, as for k_assign
+__global__ void k_encode( const CwTree* __restrict__ T, const uint32_t K, const uint32_t num )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= num) return;
-	const CwTree& tr = BATCH ? T[batch_entry<CwTree, &CwTree::wbase>( T, K, g )] : one;
-	const uint32_t t = BATCH ? g - tr.wbase : g;
+	const CwTree& tr = T[batch_entry<CwTree, &CwTree::wbase>( T, K, g )];
+	const uint32_t t = g - tr.wbase;
 	encode_node( tr.ext, tr.list[t], tr.wide[t], tr.prim_idx, tr.verts, tr.cw_nodes, tr.cw_tris );
 }
 
@@ -521,23 +516,17 @@ static CwLevels cw_levels( const std::vector<const std::vector<uint32_t>*>& tree
 }
 
 // slot assignment, subtree sizes (bottom-up), addresses (top-down), encode: everything after the collapse that depends on boxes, for
-// the K trees of the table d_T whose levels are lv (runs on the device at d_runs).  K = 1 runs the single-tree instances over `one`.
-static int cw_assign_encode( const CwTree* d_T, const uint32_t K, const CwTree& one, const CwLevels& lv, const CwRun* d_runs, cudaStream_t s )
+// the K trees of the table d_T whose levels are lv (runs on the device at d_runs)
+static int cw_assign_encode( const CwTree* d_T, const uint32_t K, const CwLevels& lv, const CwRun* d_runs, cudaStream_t s )
 {
 	const uint32_t levels = (uint32_t)lv.off.size() - 1, W = lv.off[levels];
-	if (K > 1) k_assign<true><<<(W + 127) / 128, 128, 0, s>>>( d_T, K, CwTree{}, W );
-	else k_assign<false><<<(W + 127) / 128, 128, 0, s>>>( 0, 1, one, W );
-	LAUNCHED();
-	#define CW_LEVEL( kernel, l ) do { const uint32_t num_ = lv.off[l + 1] - lv.off[l], g_ = (num_ + 127) / 128; \
-		if (K > 1) kernel<true><<<g_, 128, 0, s>>>( d_T, d_runs + lv.start[l], lv.start[l + 1] - lv.start[l], lv.off[l], num_, 0 ); \
-		else kernel<false><<<g_, 128, 0, s>>>( 0, 0, 0, lv.off[l], num_, one.wide ); \
-		LAUNCHED(); } while (0)
+	k_assign<<<(W + 127) / 128, 128, 0, s>>>( d_T, K, W ); LAUNCHED();
+	#define CW_LEVEL( kernel, l ) do { const uint32_t num_ = lv.off[l + 1] - lv.off[l]; \
+		kernel<<<(num_ + 127) / 128, 128, 0, s>>>( d_T, d_runs + lv.start[l], lv.start[l + 1] - lv.start[l], lv.off[l], num_ ); LAUNCHED(); } while (0)
 	for (int l = (int)levels - 1; l >= 0; l--) CW_LEVEL( k_sizes, l );
 	for (uint32_t l = 0; l < levels; l++) CW_LEVEL( k_addresses, l );
 	#undef CW_LEVEL
-	if (K > 1) k_encode<true><<<(W + 127) / 128, 128, 0, s>>>( d_T, K, CwTree{}, W );
-	else k_encode<false><<<(W + 127) / 128, 128, 0, s>>>( 0, 1, one, W );
-	LAUNCHED();
+	k_encode<<<(W + 127) / 128, 128, 0, s>>>( d_T, K, W ); LAUNCHED();
 	return TBVH_OK;
 }
 
@@ -616,8 +605,8 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		}
 		ngroups = tickets + CW_MAX_LEVELS;
 		for (uint32_t t = 0; t < K; t++) T[t].ext = ext + (size_t)ext_base[t] * 2, T[t].shift = ext_base[t], T[t].scan = base + T[t].nbase;
-		if (K > 1) CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
-		TRY( cw_split_emit( d_T, K, T[0], N, s ) );
+		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
+		TRY( cw_split_emit( d_T, K, N, s ) );
 		// ---- collapse to 8-wide, level by level from the K roots
 		std::vector<uint32_t> iota( K );
 		for (uint32_t t = 0; t < K; t++) iota[t] = t;
@@ -697,17 +686,16 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		{
 			CwTree& tr = T[t];
 			tr.wide = (WideNode*)(blob + o_wide) + tr.wbase;
-			if (K == 1) { tr.list = lists, tr.adopt = adopt, tr.ifirst = ifirst; continue; } // its own forest: already tree-local
+			// a single tree's forest is already tree-local: its table entry points into it, which spares a tree that keeps no collapse
+			// (tbvh_convert of an SBVH) the k_keep pass and a copy of 10 words per wide node
+			if (K == 1) { tr.list = lists, tr.adopt = adopt, tr.ifirst = ifirst; continue; }
 			if (!tr.keep) tr.keep = spare, spare += (size_t)tr.used + 1 + (size_t)tr.wide_count * 10;
 			tr.list = tr.keep + tr.used + 1, tr.adopt = tr.list + tr.wide_count, tr.ifirst = tr.adopt + (size_t)tr.wide_count * 8;
 		}
-		if (K > 1 || T[0].keep)
-		{
-			CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
-			CUDA_TRY( cudaMemcpyAsync( (void*)d_runs, lv.runs.data(), lv.runs.size() * sizeof( CwRun ), cudaMemcpyHostToDevice, s ) );
-			k_keep<<<(uint32_t)(((size_t)W + N + 255) / 256), 256, 0, s>>>( d_T, K, d_runs, (uint32_t)lv.runs.size(), W, lists, adopt, ifirst, base, N ); LAUNCHED();
-		}
-		TRY( cw_assign_encode( d_T, K, T[0], lv, d_runs, s ) );
+		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTree ), cudaMemcpyHostToDevice, s ) );
+		CUDA_TRY( cudaMemcpyAsync( (void*)d_runs, lv.runs.data(), lv.runs.size() * sizeof( CwRun ), cudaMemcpyHostToDevice, s ) );
+		if (K > 1 || T[0].keep) { k_keep<<<(uint32_t)(((size_t)W + N + 255) / 256), 256, 0, s>>>( d_T, K, d_runs, (uint32_t)lv.runs.size(), W, lists, adopt, ifirst, base, N ); LAUNCHED(); }
+		TRY( cw_assign_encode( d_T, K, lv, d_runs, s ) );
 		// the traversal nodes the kernels read and the pending bound of every wide tree (trace_cwbvh.cu); synchronises the stream
 		return cw_make_trav( bs, K, s );
 	};
@@ -736,7 +724,7 @@ void cw_keep_sizes( tbvh_bvh b, uint32_t* total, uint32_t* wide_count )
 // tree is BVH8_CWBVH::ConvertFrom of an MBVH<8> with the collapse of its conversion and its refitted boxes, which
 // tests/cwbvh_refit_oracle.c restates.  The kept collapses are tree-local, so every kernel maps a node through its tree's table
 // entry; a batch level is each tree's run of the level, in batch order.  Tables and scratch come from the context's refit buffers:
-// one upload, one read-back, one host synchronisation.  A step that only one tree of the call takes runs the single-tree instances.
+// one upload, one read-back, one host synchronisation.
 static int refit_space( tbvh_ctx c, const size_t dev, const size_t host )
 {
 	if (dev > c->refit_dev_bytes)
@@ -839,18 +827,18 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 		CUDA_TRY( cudaMemcpyAsync( dev, host, tables, cudaMemcpyHostToDevice, s ) );
 		CUDA_TRY( cudaEventRecord( c->refit_e0, s ) );
 		CUDA_TRY( cudaMemsetAsync( dev + o_arrive, 0, zeroed, s ) );
-		TRY( refit_enqueue( d_rf, K, rf[0], N, (uint32_t*)(dev + o_arrive), any_fill, s ) );
-		TRY( leaf_tris_enqueue( d_rf, K, rf[0], P, s ) );
+		TRY( refit_enqueue( d_rf, K, N, (uint32_t*)(dev + o_arrive), any_fill, s ) );
+		TRY( leaf_tris_enqueue( d_rf, K, P, s ) );
 		if (KC)
 		{
-			TRY( cw_split_emit( d_cr, KC, cr[0], NC, s ) );
+			TRY( cw_split_emit( d_cr, KC, NC, s ) );
 			bool any_leaf_root = false;
 			for (uint32_t i = 0; i < KC; i++) any_leaf_root |= cr[i].leaf_root != 0;
 			if (any_leaf_root) { k_wrap_leaf_roots<<<(KC + 127) / 128, 128, 0, s>>>( d_cr, KC ); LAUNCHED(); }
-			TRY( cw_assign_encode( d_cr, KC, cr[0], lv, (const CwRun*)(dev + o_runs), s ) );
-			TRY( cw_expand( (const CwTrav*)(dev + o_ct), KC, ct[0], lv.off.back(), 0, s ) );
+			TRY( cw_assign_encode( d_cr, KC, lv, (const CwRun*)(dev + o_runs), s ) );
+			TRY( cw_expand( (const CwTrav*)(dev + o_ct), KC, lv.off.back(), 0, s ) );
 		}
-		if (KG) TRY( bvh_gpu_enqueue( (const GpuTree*)(dev + o_gt), KG, gt[0], NG, (uint32_t*)(dev + o_gw), s ) );
+		if (KG) TRY( bvh_gpu_enqueue( (const GpuTree*)(dev + o_gt), KG, NG, (uint32_t*)(dev + o_gw), s ) );
 		TRY( refit_roots( d_rf, K, res, s ) );
 		CUDA_TRY( cudaEventRecord( c->refit_e1, s ) );
 		CUDA_TRY( cudaMemcpyAsync( h_res, res, res_words * 4, cudaMemcpyDeviceToHost, s ) );

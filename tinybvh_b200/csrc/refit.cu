@@ -9,7 +9,7 @@
 //
 // Batches (tbvh_refit_batch; a single refit is K = 1): the K trees share one node index space, tree t owning nodes nbase .. nbase +
 // used of it, so one launch and one arrival-counter memset cover them all.  A thread finds its tree in a table (RfTree) and works
-// on the tree's own arrays with local node numbers; node 1 is skipped per tree.  K = 1 passes the tree as a kernel parameter.
+// on the tree's own arrays with local node numbers; node 1 is skipped per tree.  A single tree is a one-entry table.
 // The driver (refit_trees) is in convert_cwbvh.cu, next to the re-encode of the kept CWBVH collapse.
 #include "common.cuh"
 
@@ -18,24 +18,13 @@ namespace
 __device__ __forceinline__ float tmin( const float a, const float b ) { return a < b ? a : b; }   // tinybvh_min :432
 __device__ __forceinline__ float tmax( const float a, const float b ) { return a > b ? a : b; }   // tinybvh_max :433
 
-// node g of the batch: its tree (BATCH) or `one`, and its local number
-template <bool BATCH> __device__ __forceinline__ const RfTree& rf_tree( const RfTree* __restrict__ T, const uint32_t K, const RfTree& one, const uint32_t g, uint32_t& x )
-{
-	if (!BATCH) { x = g; return one; }
-	const RfTree& tr = T[batch_entry<RfTree, &RfTree::nbase>( T, K, g )];
-	x = g - tr.nbase;
-	return tr;
-}
-
-template <bool BATCH>
-__global__ void k_refit_parents( const RfTree* __restrict__ T, const uint32_t K, const RfTree one, const uint32_t n )
+__global__ void k_refit_parents( const RfTree* __restrict__ T, const uint32_t K, const uint32_t n )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
-	uint32_t i;
-	const RfTree& tr = rf_tree<BATCH>( T, K, one, g, i );
-	if (BATCH && !tr.fill) return;
-	if (i == 1) return;
+	const RfTree& tr = T[batch_entry<RfTree, &RfTree::nbase>( T, K, g )];
+	const uint32_t i = g - tr.nbase;
+	if (!tr.fill || i == 1) return;
 	const float4* __restrict__ nodes = tr.nodes;
 	uint32_t* __restrict__ parent = tr.parent;
 	if (i == 0) parent[0] = 0xffffffffu;
@@ -77,17 +66,8 @@ __device__ __forceinline__ void refit_leaf( float4* nodes, const uint32_t* __res
 	}
 }
 
-__global__ void k_refit( float4* nodes, const uint32_t* __restrict__ prim_idx, const float4* __restrict__ verts, const uint32_t* __restrict__ parent,
-	uint32_t* arrive, const uint32_t used )
-{
-	const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-	if (x >= used || x == 1) return;
-	refit_leaf( nodes, prim_idx, verts, parent, arrive, x );
-}
-
-// node g of the batch's node space, in the tree that owns it; arrive: the batch's counters, tree t's from nbase on.  A single tree
-// runs k_refit: its pointers read from a table entry cost it registers.
-__global__ void k_refit_batch( const RfTree* __restrict__ T, const uint32_t K, uint32_t* arrive, const uint32_t n )
+// node g of the batch's node space, in the tree that owns it; arrive: the batch's counters, tree t's from nbase on
+__global__ void k_refit( const RfTree* __restrict__ T, const uint32_t K, uint32_t* arrive, const uint32_t n )
 {
 	const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
 	if (g >= n) return;
@@ -106,17 +86,11 @@ __global__ void k_refit_roots( const RfTree* __restrict__ T, const uint32_t K, u
 }
 } // namespace
 
-int refit_enqueue( const RfTree* d_T, const uint32_t K, const RfTree& one, const uint32_t n, uint32_t* arrive, const bool fill, cudaStream_t s )
+int refit_enqueue( const RfTree* d_T, const uint32_t K, const uint32_t n, uint32_t* arrive, const bool fill, cudaStream_t s )
 {
 	const uint32_t g = (n + 255) / 256;
-	if (K == 1)
-	{
-		if (fill) { k_refit_parents<false><<<g, 256, 0, s>>>( 0, 1, one, n ); LAUNCHED(); }
-		k_refit<<<g, 256, 0, s>>>( one.nodes, one.prim_idx, one.verts, one.parent, arrive, n ); LAUNCHED();
-		return TBVH_OK;
-	}
-	if (fill) { k_refit_parents<true><<<g, 256, 0, s>>>( d_T, K, RfTree{}, n ); LAUNCHED(); }
-	k_refit_batch<<<g, 256, 0, s>>>( d_T, K, arrive, n ); LAUNCHED();
+	if (fill) { k_refit_parents<<<g, 256, 0, s>>>( d_T, K, n ); LAUNCHED(); }
+	k_refit<<<g, 256, 0, s>>>( d_T, K, arrive, n ); LAUNCHED();
 	return TBVH_OK;
 }
 
