@@ -115,6 +115,16 @@ int tbvh_build( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_
  * and unsplitting, followed by Compact() (:3733).  idx_count becomes prim_count + prim_count/2 as in the reference (the
  * leaves reference the first sum(triCount) entries; the rest is zero), used_nodes up to 3 * prim_count. */
 #define TBVH_BUILD_HQ 2          /* BVH::BuildHQ */
+/* Not a reference builder: parallel locally-ordered clustering (Meister & Bittner 2018), a bottom-up build for meshes rebuilt every
+ * few frames (skinned, deforming, breaking).  Triangles are put in Morton order (21 bits per axis of the box centroid in the root
+ * box), neighbouring clusters within 16 places that are each other's cheapest union merge until one remains, and subtrees of at most
+ * 4 triangles whose SAH leaf cost (c_int) is not above their interior cost (c_trav) become one leaf.  DESIGN.md §4.8 states every
+ * rule; the tree is the same alone or in any batch (not promised for vertices with a NaN coordinate).  The nodes are numbered as BVH::ConvertFrom( BVH_Verbose ) numbers them (DFS
+ * preorder, node 1 unused) and every box is the one BVH::Refit computes, so the handle is what tbvh_upload_bvh of the same arrays
+ * leaves, plus refittable, kept indices and build_ms; idx_count = prim_count.  Its SAHCost is close to, but not, that of
+ * BVH::Build's tree.  Refusals, limits and failures are those of TBVH_BUILD_REFERENCE.  Device scratch: about 330 bytes per
+ * triangle during the build. */
+#define TBVH_BUILD_PLOC 3        /* parallel locally-ordered clustering */
 int tbvh_build_flavour( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32_t prim_count, int space, float c_trav, float c_int, int flavour );
 
 /* Indexed geometry: BVH::Build / BuildAVX / BuildHQ( const bvhvec4* vertices, const uint32_t* indices, primCount ) and their
@@ -138,7 +148,7 @@ int tbvh_build_indexed( tbvh_bvh bvh, const void* verts, uint32_t stride, uint32
  * trees are built together by the same kernels, so the fixed cost of a build (allocations, launches, host round trips) is paid once
  * per batch instead of once per mesh; the order of `meshes` changes no tree.  All meshes are in one `space`; device-space inputs
  * follow the rule above.
- *  flavour: TBVH_BUILD_REFERENCE or TBVH_BUILD_AVX; TBVH_BUILD_HQ is TBVH_E_UNSUPPORTED (SBVH batches: tbvh_build_batch_hq below).
+ *  flavour: TBVH_BUILD_REFERENCE, TBVH_BUILD_AVX or TBVH_BUILD_PLOC; TBVH_BUILD_HQ is TBVH_E_UNSUPPORTED (SBVH batches: tbvh_build_batch_hq below).
  *  Refusals come before any handle is touched, so every handle keeps its previous tree: TBVH_E_ARG for count 0, a NULL or repeated
  *  handle, handles of different contexts, prim_count 0, a bad stride, or any index >= vert_count; TBVH_E_LIMIT when the meshes
  *  hold more than TBVH_BATCH_MAX_PRIMS triangles together (positions of one shared index space must fit the builder's 32-bit

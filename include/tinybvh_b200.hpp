@@ -59,8 +59,8 @@ inline void* malloc_pinned( size_t bytes ) { void* p = 0; TBVH_FATAL_IF( tbvh_ho
 inline void free_pinned( void* p ) { tbvh_host_free( p ); }
 
 // Many meshes in one call (tbvh_build_batch): objs[i] ends up as if its own Build( vertices[i], primCounts[i] ) had run - the tree,
-// Refit and Optimize working from the caller's arrays, the public counters.  flavour: TBVH_BUILD_REFERENCE (BVH::Build) or
-// TBVH_BUILD_AVX; by default the builder the class's own Build uses.  TBVH_BUILD_HQ: each object as its own BuildHQ( vertices[i],
+// Refit and Optimize working from the caller's arrays, the public counters.  flavour: TBVH_BUILD_REFERENCE (BVH::Build),
+// TBVH_BUILD_AVX or TBVH_BUILD_PLOC (BuildPLOC, not in the reference); by default the builder the class's own Build uses.  TBVH_BUILD_HQ: each object as its own BuildHQ( vertices[i],
 // primCounts[i] ) leaves it (tbvh_build_batch_hq).  BVH_GPU / BVH8_CWBVH objects are converted afterwards.
 template <class T, class Vec4> void BuildBatch( T* const* objs, const Vec4* const* vertices, const uint32_t* primCounts, uint32_t count, int flavour = -1 );
 // Many refits in one call (tbvh_refit_batch), as an animated scene refits its BLASes every frame: every object refitted from the vertex
@@ -253,6 +253,13 @@ public:
 	template <class Vec4> void Build( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { const uint32_t n = build_indexed( vertices, indices, primCount, TBVH_BUILD_REFERENCE, "BVH::Build" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount, n ), sync_info(); }
 	template <class Vec4> void BuildAVX( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { const uint32_t n = build_indexed( vertices, indices, primCount, TBVH_BUILD_AVX, "BVH::BuildAVX" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount, n ), sync_info(); }
 	template <class Vec4> void BuildHQ( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { build_indexed( vertices, indices, primCount, TBVH_BUILD_HQ, "BVH::BuildHQ" ); sync_info(); }
+	// not in the reference: the PLOC build (TBVH_BUILD_PLOC), a refittable tree for meshes rebuilt every few frames
+	template <class Vec4> void BuildPLOC( const Vec4* vertices, const uint32_t primCount )
+	{
+		TBVH_FATAL_IF( tbvh_build_flavour( h, vertices, (uint32_t)sizeof( Vec4 ), primCount, TBVH_HOST, c_trav, c_int, TBVH_BUILD_PLOC ), "BVH::BuildPLOC" );
+		remember( vertices, (uint32_t)sizeof( Vec4 ), 0, primCount ), sync_info();
+	}
+	template <class Vec4> void BuildPLOC( const Vec4* vertices, const uint32_t* indices, const uint32_t primCount ) { const uint32_t n = build_indexed( vertices, indices, primCount, TBVH_BUILD_PLOC, "BVH::BuildPLOC" ); remember( vertices, (uint32_t)sizeof( Vec4 ), indices, primCount, n ), sync_info(); }
 	// BVH::SAHCost( nodeIdx = 0 ) tiny_bvh.h:1889 - the reference's value, bit for bit
 	float SAHCost( const uint32_t = 0 ) const { float c = 0; TBVH_FATAL_IF( tbvh_sah_cost( h, c_trav, c_int, &c ), "BVH::SAHCost" ); return c; }
 	// consume / produce the reference's public arrays (bvhNode, primIdx: tiny_bvh.h:952-964)
@@ -354,6 +361,13 @@ public:
 		TBVH_FATAL_IF( tbvh_convert( h, TBVH_LAYOUT_BVH_GPU ), "BVH_GPU::BuildHQ" );
 		sync_info();
 	}
+	// not in the reference: the PLOC build (TBVH_BUILD_PLOC), then the conversion
+	template <class Vec4> void BuildPLOC( const Vec4* vertices, const uint32_t primCount )
+	{
+		TBVH_FATAL_IF( tbvh_build_flavour( h, vertices, (uint32_t)sizeof( Vec4 ), primCount, TBVH_HOST, c_trav, c_int, TBVH_BUILD_PLOC ), "BVH_GPU::BuildPLOC" );
+		TBVH_FATAL_IF( tbvh_convert( h, TBVH_LAYOUT_BVH_GPU ), "BVH_GPU::BuildPLOC" );
+		sync_info();
+	}
 	// BVH_GPU::BuildHQ tiny_bvh.h:4588: bvh.BuildHQ, then ConvertFrom
 	template <class Vec4> void BuildHQ( const Vec4* vertices, const uint32_t primCount )
 	{
@@ -391,6 +405,13 @@ public:
 	{
 		build_indexed( vertices, indices, primCount, TBVH_BUILD_AVX, "BVH8_CWBVH::Build" );
 		TBVH_FATAL_IF( tbvh_convert( h, TBVH_LAYOUT_CWBVH ), "BVH8_CWBVH::Build" );
+		sync_info(), usedBlocks = Info().used_blocks;
+	}
+	// not in the reference: the PLOC build (TBVH_BUILD_PLOC), then the conversion
+	template <class Vec4> void BuildPLOC( const Vec4* vertices, const uint32_t primCount )
+	{
+		TBVH_FATAL_IF( tbvh_build_flavour( h, vertices, (uint32_t)sizeof( Vec4 ), primCount, TBVH_HOST, c_trav, c_int, TBVH_BUILD_PLOC ), "BVH8_CWBVH::BuildPLOC" );
+		TBVH_FATAL_IF( tbvh_convert( h, TBVH_LAYOUT_CWBVH ), "BVH8_CWBVH::BuildPLOC" );
 		sync_info(), usedBlocks = Info().used_blocks;
 	}
 	// BVH8_CWBVH::BuildHQ tiny_bvh.h:5859: bvh.BuildHQ, SplitLeafs(3), MBVH<8> collapse, CWBVH encode

@@ -12,7 +12,7 @@ SO = os.path.join(HERE, "libtinybvh_b200.so")
 OK, HOST, DEVICE = 0, 0, 1
 E_CUDA, E_ARG, E_STATE, E_LIMIT, E_UNSUPPORTED = -1, -2, -3, -4, -5
 LAYOUT_BVH, LAYOUT_BVH_GPU, LAYOUT_CWBVH = 1, 5, 10
-BUILD_REFERENCE, BUILD_AVX, BUILD_HQ = 0, 1, 2
+BUILD_REFERENCE, BUILD_AVX, BUILD_HQ, BUILD_PLOC = 0, 1, 2, 3
 
 
 class TbvhError(RuntimeError):

@@ -12,7 +12,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import LAYOUT_BVH, LAYOUT_BVH_GPU, LAYOUT_CWBVH, HOST, DEVICE, TbvhError, check
+from ._lib import LAYOUT_BVH, LAYOUT_BVH_GPU, LAYOUT_CWBVH, HOST, DEVICE, BUILD_PLOC, TbvhError, check
 
 NODE32 = np.dtype([("aabbMin", "3f4"), ("leftFirst", "u4"), ("aabbMax", "3f4"), ("triCount", "u4")])
 NODE64 = np.dtype([("lmin", "3f4"), ("left", "u4"), ("lmax", "3f4"), ("right", "u4"),
@@ -213,6 +213,11 @@ class BVH(_Base):
         self._build(vertices, primCount, _lib.BUILD_HQ, indices)
         return self
 
+    def BuildPLOC(self, vertices, primCount: int = 0, indices=None):
+        """Not in the reference: the bottom-up PLOC build (TBVH_BUILD_PLOC, DESIGN.md §4.8), a refittable tree for per-frame rebuilds."""
+        self._build(vertices, primCount, _lib.BUILD_PLOC, indices)
+        return self
+
     def SAHCost(self) -> float:
         """BVH::SAHCost( 0 ) (tiny_bvh.h:1889): host recursion over the downloaded nodes, the reference's value bit for bit."""
         out = C.c_float()
@@ -407,7 +412,7 @@ class BVH8_CWBVH(_Base):
 def build_batch(bvhs, meshes, flavour: int = _lib.BUILD_REFERENCE, indices=None):
     """tbvh_build_batch: one binned-SAH tree per mesh, all built in one call.  bvhs[i] ends up as bvhs[i].Build(meshes[i]) (flavour
     BUILD_REFERENCE) or .BuildAVX (BUILD_AVX) would leave it; flavour BUILD_HQ builds one SBVH per mesh (tbvh_build_batch_hq), as
-    .BuildHQ would.  `meshes`: numpy vertex arrays, or torch CUDA tensors - one space per
+    .BuildHQ would, and BUILD_PLOC one PLOC tree per mesh, as .BuildPLOC would.  `meshes`: numpy vertex arrays, or torch CUDA tensors - one space per
     call; `indices`: None, or one entry per mesh (None for a flat mesh, else its vertex indices in the same space).  BVH_GPU and
     BVH8_CWBVH objects are converted afterwards, as their Build does (the BVH8_CWBVH objects in one convert_batch).  A refused batch
     raises TbvhError and leaves every object as it was."""

@@ -1103,10 +1103,11 @@ static int batch_stage( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes,
 static int build_batch( const char* fn, tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count, int space, float c_trav, float c_int, int flavour )
 {
 	if (!(bvhs && meshes && count > 0)) { tbvh_set_error( "%s: no meshes", fn ); return TBVH_E_ARG; }
-	if (flavour != TBVH_BUILD_REFERENCE && flavour != TBVH_BUILD_AVX && flavour != TBVH_BUILD_HQ) { tbvh_set_error( "%s: unknown builder flavour", fn ); return TBVH_E_ARG; }
+	if (flavour != TBVH_BUILD_REFERENCE && flavour != TBVH_BUILD_AVX && flavour != TBVH_BUILD_HQ && flavour != TBVH_BUILD_PLOC) { tbvh_set_error( "%s: unknown builder flavour", fn ); return TBVH_E_ARG; }
 	const bool hq = flavour == TBVH_BUILD_HQ;
 	TRY( batch_stage( fn, bvhs, meshes, count, space, hq ) );
-	const int rc = hq ? build_hq_launch( bvhs, count, c_trav, c_int ) : build_sah_launch( bvhs, count, c_trav, c_int, flavour );
+	const int rc = hq ? build_hq_launch( bvhs, count, c_trav, c_int )
+		: flavour == TBVH_BUILD_PLOC ? build_ploc_launch( bvhs, count, c_trav, c_int ) : build_sah_launch( bvhs, count, c_trav, c_int, flavour );
 	for (uint32_t k = 0; k < count; k++)
 	{
 		if (rc != TBVH_OK) free_layouts( bvhs[k] );

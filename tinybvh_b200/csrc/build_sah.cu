@@ -1247,6 +1247,25 @@ int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint3
 
 #define DEV_ALLOC( ptr, bytes ) do { CUDA_TRY( cudaMalloc( (void**)&(ptr), (bytes) ) ); scratch.push_back( (void*)(ptr) ); } while (0)
 
+int fragments_launch( const tbvh_bvh* bs, const uint32_t trees, const uint32_t* d_base, const uint32_t n, float4* frag_min, float4* frag_max,
+	const uint32_t** keys, uint32_t* key_stride, std::vector<void*>& scratch, cudaStream_t s )
+{
+	BuildArgs A = {};
+	A.trees = trees, A.tree_base = d_base, A.n = n, A.frag_min = frag_min, A.frag_max = frag_max;
+	std::vector<TreeIO> io( trees );
+	for (uint32_t t = 0; t < trees; t++) io[t] = TreeIO{ bs[t]->d_verts, 0, 0, 0 };
+	TreeIO* d_io = 0;
+	DEV_ALLOC( d_io, io.size() * sizeof( TreeIO ) ); DEV_ALLOC( A.ts, (size_t)trees * sizeof( TreeState ) ); DEV_ALLOC( A.ctr, sizeof( Counters ) );
+	DEV_ALLOC( A.idx[0], (size_t)n * 4 );
+	A.io = d_io;
+	CUDA_TRY( cudaMemcpyAsync( d_io, io.data(), io.size() * sizeof( TreeIO ), cudaMemcpyHostToDevice, s ) );
+	k_init_counters<<<(trees + 255) / 256, 256, 0, s>>>( A, 0 ); LAUNCHED();
+	k_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+	static_assert( offsetof( TreeState, key ) == 0 && sizeof( TreeState ) % 4 == 0, "keys at the front of TreeState" );
+	*keys = (const uint32_t*)A.ts, *key_stride = (uint32_t)(sizeof( TreeState ) / 4);
+	return TBVH_OK;
+}
+
 // bs[0 .. trees): handles of one context holding their primitives (d_verts, or d_aabbs for a TLAS, which is built alone) and
 // info.prim_count; on success each holds its tree as a build of its own would leave it.  On failure the caller empties them.
 int build_sah_launch( const tbvh_bvh* bs, const uint32_t trees, float c_trav, float c_int, int flavour )

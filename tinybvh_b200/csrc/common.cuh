@@ -249,6 +249,13 @@ float cw_rd_limit_for( uint32_t range );                               // cw_rd_
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)
 // binned-SAH builds of `trees` handles of one context at once (build_sah.cu); a single build is trees = 1
 int build_sah_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, int flavour );
+// the fragment pass of the binned builder (k_fragments) for the PLOC builder: every triangle's box into frag_min / frag_max at its
+// position of the batch's index space (tree t from d_base[t] on), every tree's root box as six ordered keys (min xyz, max xyz) at
+// (*keys)[key_stride * t ..]; allocations go to scratch
+int fragments_launch( const tbvh_bvh* bs, uint32_t trees, const uint32_t* d_base, uint32_t n, float4* frag_min, float4* frag_max,
+	const uint32_t** keys, uint32_t* key_stride, std::vector<void*>& scratch, cudaStream_t s );
+// PLOC builds (TBVH_BUILD_PLOC) of `trees` handles of one context at once (build_ploc.cu); a single build is trees = 1
+int build_ploc_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int );
 // SBVH builds (BuildHQ) of K handles of one context at once (build_hq.cu); a single build is K = 1
 int build_hq_launch( const tbvh_bvh* bs, uint32_t K, float c_trav, float c_int );
 // BVH::Refit of K trees over one node space of `nodes` nodes; arrive: `nodes` zeroed words; fill: some tree's parents are filled
