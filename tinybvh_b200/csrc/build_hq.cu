@@ -1194,15 +1194,10 @@ __global__ void __launch_bounds__( 256 ) k_hq_outputs( HQArgs A )
 }
 } // namespace
 
-#define DEV_ALLOC( p, bytes ) do { void* q_ = 0; CUDA_TRY( cudaMalloc( &q_, (bytes) ) ); scratch.push_back( q_ ); (p) = (decltype( p ))q_; } while (0)
-
-// bs[0 .. K): handles of one context holding their triangles (d_verts, info.prim_count); on success each holds its SBVH as a
-// build of its own would leave it.  On failure the caller empties them.
-int build_hq_launch( const tbvh_bvh* bs, const uint32_t K, float c_trav, float c_int )
+int build_hq_launch( const tbvh_bvh* bs, const uint32_t K, float c_trav, float c_int, BuiltTree* out, float* ms )
 {
 	const tbvh_ctx ctx = bs[0]->ctx;
 	cudaStream_t s = ctx->stream;
-	std::vector<void*> scratch;
 	HQArgs A = {};
 	A.verts = bs[0]->d_verts, A.trees = K, A.c_trav = c_trav, A.c_int = c_int;
 	{
@@ -1234,120 +1229,103 @@ int build_hq_launch( const tbvh_bvh* bs, const uint32_t K, float c_trav, float c
 		CUDA_TRY( cudaMalloc( &b->d_leaf_tris, (size_t)it * 48 ) ); b->leaf_tris_count = it;
 		T[t].out_nodes = b->d_nodes, T[t].out_idx = b->d_prim_idx, T[t].leaf_tris = b->d_leaf_tris;
 	}
+	Scratch sc( s );
 	HQCounters* h_ctr = 0;
-	cudaEvent_t e0 = 0, e1 = 0;
-	auto body = [&]() -> int
+	TRY( sc.alloc( A.T, (size_t)K * sizeof( HQTree ) ) );
+	TRY( sc.alloc( A.frag_min, (size_t)A.idx_cap * 16 ) ); TRY( sc.alloc( A.frag_max, (size_t)A.idx_cap * 16 ) );
+	TRY( sc.alloc( A.prim_idx, (size_t)A.idx_cap * 4 ) ); TRY( sc.alloc( A.idx_tmp, (size_t)A.idx_cap * 4 ) );
+	TRY( sc.alloc( A.cls, (size_t)A.idx_cap * 4 ) ); TRY( sc.alloc( A.strad, (size_t)A.idx_cap * 4 ) ); TRY( sc.alloc( A.spos, (size_t)A.idx_cap * 4 ) );
+	TRY( sc.alloc( A.tmp_nodes, (size_t)A.node_cap * 32 ) ); TRY( sc.alloc( A.parent, (size_t)A.node_cap * 4 ) );
+	TRY( sc.alloc( A.sub_int, (size_t)A.node_cap * 4 ) ); TRY( sc.alloc( A.sub_prims, (size_t)A.node_cap * 4 ) ); TRY( sc.alloc( A.arrive, (size_t)A.node_cap * 4 ) );
+	TRY( sc.alloc( A.lvl[0], (size_t)A.lvl_cap * sizeof( HQTask ) ) ); TRY( sc.alloc( A.lvl[1], (size_t)A.lvl_cap * sizeof( HQTask ) ) );
+	TRY( sc.alloc( A.small, ((size_t)A.idx_cap + K) * sizeof( HQTask ) ) );
+	TRY( sc.alloc( A.ctr, sizeof( HQCounters ) ) );
+	TRY( sc.alloc_host( h_ctr, sizeof( HQCounters ) ) );
+	TRY( sc.events() );
+	CUDA_TRY( cudaMemcpyAsync( A.T, T.data(), (size_t)K * sizeof( HQTree ), cudaMemcpyHostToDevice, s ) );
+	CUDA_TRY( cudaEventRecord( sc.e0, s ) );
+	// the reference clears primIdx beyond triCount (:2700) and all of idxTmp (:3008): a never-written idxTmp word is fragment 0,
+	// whose tree-local triangle number is 0 in every tree
+	CUDA_TRY( cudaMemsetAsync( A.prim_idx, 0, (size_t)A.idx_cap * 4, s ) );
+	CUDA_TRY( cudaMemsetAsync( A.idx_tmp, 0, (size_t)A.idx_cap * 4, s ) );
+	CUDA_TRY( cudaMemsetAsync( A.arrive, 0, (size_t)A.node_cap * 4, s ) );
+	k_hq_init<<<(K + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+	k_hq_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+	k_hq_root_zero<<<ctx->sm_count, 256, 0, s>>>( A ); LAUNCHED();
+	k_hq_root<<<(K + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+	uint32_t level = 0;
+	uint32_t max_cluster = (uint32_t)(ctx->hq_cluster < 1 ? 1 : ctx->hq_cluster > HQ_MAX_CLUSTER ? HQ_MAX_CLUSTER : ctx->hq_cluster);
+	// tuning knobs of the cluster sizing rule, read from the environment: fragments per CTA, CTAs per SM in flight
+	const char* env_cf = getenv( "TBVH_HQ_CTA_FRAGS" ); const char* env_cc = getenv( "TBVH_HQ_CTA_CAP" );
+	const size_t cta_frags = env_cf && atoi( env_cf ) > 0 ? (size_t)atoi( env_cf ) : 512, cta_cap = env_cc && atoi( env_cc ) > 0 ? (size_t)atoi( env_cc ) : 16;
+	void (*level_kernel)( HQArgs, const HQTask*, HQTask*, uint32_t ) = K > 1 ? k_hq_level<true> : k_hq_level<false>;
+	if (max_cluster > 8) CUDA_TRY( cudaFuncSetAttribute( level_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1 ) );
+	// one level list for every tree: the cluster size follows the level's largest node, whichever tree holds it
+	while (num)
 	{
-		DEV_ALLOC( A.T, (size_t)K * sizeof( HQTree ) );
-		DEV_ALLOC( A.frag_min, (size_t)A.idx_cap * 16 ); DEV_ALLOC( A.frag_max, (size_t)A.idx_cap * 16 );
-		DEV_ALLOC( A.prim_idx, (size_t)A.idx_cap * 4 ); DEV_ALLOC( A.idx_tmp, (size_t)A.idx_cap * 4 );
-		DEV_ALLOC( A.cls, (size_t)A.idx_cap * 4 ); DEV_ALLOC( A.strad, (size_t)A.idx_cap * 4 ); DEV_ALLOC( A.spos, (size_t)A.idx_cap * 4 );
-		DEV_ALLOC( A.tmp_nodes, (size_t)A.node_cap * 32 ); DEV_ALLOC( A.parent, (size_t)A.node_cap * 4 );
-		DEV_ALLOC( A.sub_int, (size_t)A.node_cap * 4 ); DEV_ALLOC( A.sub_prims, (size_t)A.node_cap * 4 ); DEV_ALLOC( A.arrive, (size_t)A.node_cap * 4 );
-		DEV_ALLOC( A.lvl[0], (size_t)A.lvl_cap * sizeof( HQTask ) ); DEV_ALLOC( A.lvl[1], (size_t)A.lvl_cap * sizeof( HQTask ) );
-		DEV_ALLOC( A.small, ((size_t)A.idx_cap + K) * sizeof( HQTask ) );
-		DEV_ALLOC( A.ctr, sizeof( HQCounters ) );
-		CUDA_TRY( cudaMallocHost( &h_ctr, sizeof( HQCounters ) ) );
-		CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) );
-		CUDA_TRY( cudaMemcpyAsync( A.T, T.data(), (size_t)K * sizeof( HQTree ), cudaMemcpyHostToDevice, s ) );
-		CUDA_TRY( cudaEventRecord( e0, s ) );
-		// the reference clears primIdx beyond triCount (:2700) and all of idxTmp (:3008): a never-written idxTmp word is fragment 0,
-		// whose tree-local triangle number is 0 in every tree
-		CUDA_TRY( cudaMemsetAsync( A.prim_idx, 0, (size_t)A.idx_cap * 4, s ) );
-		CUDA_TRY( cudaMemsetAsync( A.idx_tmp, 0, (size_t)A.idx_cap * 4, s ) );
-		CUDA_TRY( cudaMemsetAsync( A.arrive, 0, (size_t)A.node_cap * 4, s ) );
-		k_hq_init<<<(K + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
-		k_hq_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
-		k_hq_root_zero<<<ctx->sm_count, 256, 0, s>>>( A ); LAUNCHED();
-		k_hq_root<<<(K + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
-		uint32_t level = 0;
-		uint32_t max_cluster = (uint32_t)(ctx->hq_cluster < 1 ? 1 : ctx->hq_cluster > HQ_MAX_CLUSTER ? HQ_MAX_CLUSTER : ctx->hq_cluster);
-		// tuning knobs of the cluster sizing rule, read from the environment: fragments per CTA, CTAs per SM in flight
-		const char* env_cf = getenv( "TBVH_HQ_CTA_FRAGS" ); const char* env_cc = getenv( "TBVH_HQ_CTA_CAP" );
-		const size_t cta_frags = env_cf && atoi( env_cf ) > 0 ? (size_t)atoi( env_cf ) : 512, cta_cap = env_cc && atoi( env_cc ) > 0 ? (size_t)atoi( env_cc ) : 16;
-		void (*level_kernel)( HQArgs, const HQTask*, HQTask*, uint32_t ) = K > 1 ? k_hq_level<true> : k_hq_level<false>;
-		if (max_cluster > 8) CUDA_TRY( cudaFuncSetAttribute( level_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1 ) );
-		// one level list for every tree: the cluster size follows the level's largest node, whichever tree holds it
-		while (num)
+		CUDA_TRY( cudaMemsetAsync( &A.ctr->next_big, 0, 8, s ) ); // next_big + next_max
+		// cluster size: enough CTAs for the largest node of the level (about 512 fragments per CTA), at most 8 CTAs per SM in flight,
+		// a power of two no larger than max_cluster
+		uint32_t nct = 1;
+		while (nct * 2 <= max_cluster && (size_t)nct * cta_frags < max_count && (size_t)num * nct * 2 <= (size_t)ctx->sm_count * cta_cap) nct <<= 1;
+		cudaLaunchConfig_t cfg = {};
+		cudaLaunchAttribute attr[1];
+		cfg.gridDim = dim3( num * nct ), cfg.blockDim = dim3( HQ_BIG_THREADS ), cfg.dynamicSmemBytes = 0, cfg.stream = s;
+		attr[0].id = cudaLaunchAttributeClusterDimension, attr[0].val.clusterDim.x = nct, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;
+		cfg.attrs = attr, cfg.numAttrs = 1;
 		{
-			CUDA_TRY( cudaMemsetAsync( &A.ctr->next_big, 0, 8, s ) ); // next_big + next_max
-			// cluster size: enough CTAs for the largest node of the level (about 512 fragments per CTA), at most 8 CTAs per SM in flight,
-			// a power of two no larger than max_cluster
-			uint32_t nct = 1;
-			while (nct * 2 <= max_cluster && (size_t)nct * cta_frags < max_count && (size_t)num * nct * 2 <= (size_t)ctx->sm_count * cta_cap) nct <<= 1;
-			cudaLaunchConfig_t cfg = {};
-			cudaLaunchAttribute attr[1];
-			cfg.gridDim = dim3( num * nct ), cfg.blockDim = dim3( HQ_BIG_THREADS ), cfg.dynamicSmemBytes = 0, cfg.stream = s;
-			attr[0].id = cudaLaunchAttributeClusterDimension, attr[0].val.clusterDim.x = nct, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;
-			cfg.attrs = attr, cfg.numAttrs = 1;
-			{
-				// a cluster shape the device cannot co-schedule (MIG slices, fewer SMs per GPC) fails at launch: nothing has run, so
-				// fall back to the next smaller shape
-				const cudaError_t le = cudaLaunchKernelEx( &cfg, level_kernel, A, (const HQTask*)A.lvl[level & 1], A.lvl[(level + 1) & 1], nct );
-				if (le != cudaSuccess && nct > 1) { cudaGetLastError(); max_cluster = nct >> 1; continue; }
-				CUDA_TRY( le ); LAUNCHED();
-			}
-			CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( HQCounters ), cudaMemcpyDeviceToHost, s ) );
-			CUDA_TRY( cudaStreamSynchronize( s ) );
-			if (A.profile > 1)
-			{
-				static unsigned long long prev[12];
-				if (level == 0) memset( prev, 0, sizeof( prev ) );
-				fprintf( stderr, "hq-level %2u nodes %5u nct %2u max %7u:", level, num, nct, max_count );
-				for (int k = 0; k < 12; k++) { fprintf( stderr, " %7.1f", (h_ctr->prof[k] - prev[k]) * 1e-3 / num ); prev[k] = h_ctr->prof[k]; }
-				fprintf( stderr, "  kcyc/node\n" );
-			}
-			num = h_ctr->next_big, max_count = h_ctr->next_max;
-			if (h_ctr->overflow) { tbvh_set_error( "BuildHQ: pool overflow in the level phase" ); return TBVH_E_LIMIT; }
-			if (++level > 4096) { tbvh_set_error( "BuildHQ: runaway level count" ); return TBVH_E_LIMIT; }
+			// a cluster shape the device cannot co-schedule (MIG slices, fewer SMs per GPC) fails at launch: nothing has run, so
+			// fall back to the next smaller shape
+			const cudaError_t le = cudaLaunchKernelEx( &cfg, level_kernel, A, (const HQTask*)A.lvl[level & 1], A.lvl[(level + 1) & 1], nct );
+			if (le != cudaSuccess && nct > 1) { cudaGetLastError(); max_cluster = nct >> 1; continue; }
+			CUDA_TRY( le ); LAUNCHED();
 		}
 		CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( HQCounters ), cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
-		// one launch for the warp subtrees of every tree
-		const uint32_t roots = h_ctr->small_roots;
-		if (roots)
+		if (A.profile > 1)
 		{
-			const uint32_t grid = (roots + HQ_SMALL_WARPS - 1) / HQ_SMALL_WARPS;
-			if (K > 1) k_hq_subtrees<true><<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots ); else k_hq_subtrees<false><<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots );
-			LAUNCHED();
+			static unsigned long long prev[12];
+			if (level == 0) memset( prev, 0, sizeof( prev ) );
+			fprintf( stderr, "hq-level %2u nodes %5u nct %2u max %7u:", level, num, nct, max_count );
+			for (int k = 0; k < 12; k++) { fprintf( stderr, " %7.1f", (h_ctr->prof[k] - prev[k]) * 1e-3 / num ); prev[k] = h_ctr->prof[k]; }
+			fprintf( stderr, "  kcyc/node\n" );
 		}
-		CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( HQCounters ), cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		if (h_ctr->overflow) { tbvh_set_error( "BuildHQ: pool overflow in the subtree phase" ); return TBVH_E_LIMIT; }
-		const uint32_t tmp_count = h_ctr->node_ptr;
-		if (A.profile)
-		{
-			static const char* nm[12] = { "obj-bin", "obj-sweep", "spat-bin", "spat-sweep", "part-obj", "part-p1", "chain", "split", "p4+bounds", "leaf", "copyback", "emit" };
-			for (int k = 0; k < 12; k++) fprintf( stderr, "hq-profile %-10s level %10.3f Mcyc   subtree %10.3f Mcyc\n", nm[k], h_ctr->prof[k] * 1e-6, h_ctr->prof[16 + k] * 1e-6 );
-			fprintf( stderr, "hq-profile failed_splits %u small_roots %u\n", h_ctr->failed_splits, h_ctr->small_roots );
-		}
-		// Compact(): DFS-preorder numbering, leaf index ranges packed in DFS order, per tree
-		k_hq_up<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count ); LAUNCHED();
-		k_hq_down<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count ); LAUNCHED();
-		CUDA_TRY( cudaEventRecord( e1, s ) );
-		k_hq_outputs<<<(A.idx_cap + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
-		CUDA_TRY( cudaMemcpyAsync( T.data(), A.T, (size_t)K * sizeof( HQTree ), cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		float ms = 0;
-		CUDA_TRY( cudaEventElapsedTime( &ms, e0, e1 ) );
-		for (uint32_t t = 0; t < K; t++)
-		{
-			const tbvh_bvh b = bs[t];
-			const uint32_t* rootw = T[t].root;
-			b->info.build_ms = ms;
-			b->info.used_nodes = 2 + 2 * T[t].interior, b->info.idx_count = T[t].n + (T[t].n >> 1), b->info.max_depth = T[t].max_depth;
-			memcpy( b->info.aabb_min, rootw, 12 ), memcpy( b->info.aabb_max, rootw + 4, 12 );
-			b->root_ref = rootw[3], b->root_count = rootw[7];
-			b->d_trav = b->d_nodes;
-			b->generation = tbvh_next_generation(); // new arrays: a TLAS built over the old ones must notice (tlas_check)
-		}
-		return TBVH_OK;
-	};
-	const int rc = body();
-	cudaStreamSynchronize( s );
-	for (void* p : scratch) cudaFree( p );
-	if (h_ctr) cudaFreeHost( h_ctr );
-	if (e0) cudaEventDestroy( e0 );
-	if (e1) cudaEventDestroy( e1 );
-	return rc;
+		num = h_ctr->next_big, max_count = h_ctr->next_max;
+		if (h_ctr->overflow) { tbvh_set_error( "BuildHQ: pool overflow in the level phase" ); return TBVH_E_LIMIT; }
+		if (++level > 4096) { tbvh_set_error( "BuildHQ: runaway level count" ); return TBVH_E_LIMIT; }
+	}
+	CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( HQCounters ), cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	// one launch for the warp subtrees of every tree
+	const uint32_t roots = h_ctr->small_roots;
+	if (roots)
+	{
+		const uint32_t grid = (roots + HQ_SMALL_WARPS - 1) / HQ_SMALL_WARPS;
+		if (K > 1) k_hq_subtrees<true><<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots ); else k_hq_subtrees<false><<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots );
+		LAUNCHED();
+	}
+	CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( HQCounters ), cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	if (h_ctr->overflow) { tbvh_set_error( "BuildHQ: pool overflow in the subtree phase" ); return TBVH_E_LIMIT; }
+	const uint32_t tmp_count = h_ctr->node_ptr;
+	if (A.profile)
+	{
+		static const char* nm[12] = { "obj-bin", "obj-sweep", "spat-bin", "spat-sweep", "part-obj", "part-p1", "chain", "split", "p4+bounds", "leaf", "copyback", "emit" };
+		for (int k = 0; k < 12; k++) fprintf( stderr, "hq-profile %-10s level %10.3f Mcyc   subtree %10.3f Mcyc\n", nm[k], h_ctr->prof[k] * 1e-6, h_ctr->prof[16 + k] * 1e-6 );
+		fprintf( stderr, "hq-profile failed_splits %u small_roots %u\n", h_ctr->failed_splits, h_ctr->small_roots );
+	}
+	// Compact(): DFS-preorder numbering, leaf index ranges packed in DFS order, per tree
+	k_hq_up<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count ); LAUNCHED();
+	k_hq_down<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count ); LAUNCHED();
+	CUDA_TRY( cudaEventRecord( sc.e1, s ) );
+	k_hq_outputs<<<(A.idx_cap + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+	CUDA_TRY( cudaMemcpyAsync( T.data(), A.T, (size_t)K * sizeof( HQTree ), cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	CUDA_TRY( cudaEventElapsedTime( ms, sc.e0, sc.e1 ) );
+	for (uint32_t t = 0; t < K; t++)
+	{
+		memcpy( out[t].root, T[t].root, 32 );
+		out[t].used_nodes = 2 + 2 * T[t].interior, out[t].idx_count = T[t].n + (T[t].n >> 1), out[t].max_depth = T[t].max_depth;
+	}
+	return TBVH_OK;
 }

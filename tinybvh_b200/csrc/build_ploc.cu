@@ -276,18 +276,13 @@ template <class Sort> static int sort_enqueue( cudaStream_t s, Sort sort )
 	return TBVH_OK;
 }
 
-#define DEV_ALLOC( ptr, bytes ) do { CUDA_TRY( cudaMalloc( (void**)&(ptr), (bytes) ) ); scratch.push_back( (void*)(ptr) ); } while (0)
-
-int build_ploc_launch( const tbvh_bvh* bs, const uint32_t trees, const float c_trav, const float c_int )
+int build_ploc_launch( const tbvh_bvh* bs, const uint32_t trees, const float c_trav, const float c_int, BuiltTree* out, float* ms )
 {
 	const tbvh_ctx ctx = bs[0]->ctx;
 	cudaStream_t s = ctx->stream;
-	std::vector<void*> scratch;
 	std::vector<uint32_t> base( (size_t)trees + 1, 0 );
 	for (uint32_t t = 0; t < trees; t++) base[t + 1] = base[t] + bs[t]->info.prim_count;
 	const uint32_t n = base[trees], slots = 2 * n;
-	uint32_t* h_res = 0;
-	cudaEvent_t e0 = 0, e1 = 0;
 	for (uint32_t t = 0; t < trees; t++)
 	{
 		const tbvh_bvh b = bs[t];
@@ -297,125 +292,107 @@ int build_ploc_launch( const tbvh_bvh* bs, const uint32_t trees, const float c_t
 		CUDA_TRY( cudaMalloc( &b->d_leaf_tris, nt * 48 ) );
 		b->leaf_tris_count = (uint32_t)nt;
 	}
-	auto body = [&]() -> int
+	Scratch sc( s );
+	uint32_t* h_res = 0;
+	uint32_t* d_base = 0, * seg[2] = {}, * nn = 0, * flags = 0, * scan = 0, * tile = 0, * pairs = 0, * parent = 0, * arrive = 0, * cnt = 0, * coll = 0, * sub_int = 0, * sub_w = 0, * depth = 0;
+	uint32_t* val[2] = {}, * tkey[2] = {};
+	uint64_t* code[2] = {};
+	float4* fmin_ = 0, * fmax_ = 0, * cl[2] = {}, * pool = 0;
+	float* cost = 0;
+	PlocOut* d_io = 0;
+	TRY( sc.alloc( d_base, base.size() * 4 ) );
+	TRY( sc.alloc( fmin_, (size_t)n * 16 ) ); TRY( sc.alloc( fmax_, (size_t)n * 16 ) );
+	for (int k = 0; k < 2; k++) { TRY( sc.alloc( code[k], (size_t)n * 8 ) ); TRY( sc.alloc( val[k], (size_t)n * 4 ) ); TRY( sc.alloc( cl[k], (size_t)n * 32 ) ); TRY( sc.alloc( seg[k], ((size_t)trees + 1) * 4 ) ); }
+	if (trees > 1) for (int k = 0; k < 2; k++) TRY( sc.alloc( tkey[k], (size_t)n * 4 ) );
+	TRY( sc.alloc( nn, (size_t)n * 4 ) ); TRY( sc.alloc( flags, ((size_t)n + 1) * 4 ) ); TRY( sc.alloc( scan, ((size_t)n + 1) * 4 ) ); TRY( sc.alloc( tile, ((size_t)n / 2048 + 2) * 4 ) );
+	TRY( sc.alloc( pairs, 4 ) ); TRY( sc.alloc( pool, (size_t)slots * 32 ) ); TRY( sc.alloc( parent, (size_t)slots * 4 ) ); TRY( sc.alloc( arrive, (size_t)slots * 4 ) );
+	TRY( sc.alloc( cnt, (size_t)slots * 4 ) ); TRY( sc.alloc( coll, (size_t)slots * 4 ) ); TRY( sc.alloc( cost, (size_t)slots * 4 ) );
+	TRY( sc.alloc( sub_int, (size_t)slots * 4 ) ); TRY( sc.alloc( sub_w, (size_t)slots * 4 ) ); TRY( sc.alloc( depth, (size_t)trees * 4 ) ); TRY( sc.alloc( d_io, (size_t)trees * sizeof( PlocOut ) ) );
+	TRY( sc.alloc_host( h_res, ((size_t)trees * 2 + 2) * 4 ) );
+	TRY( sc.events() );
+	std::vector<PlocOut> io( trees );
+	for (uint32_t t = 0; t < trees; t++) io[t] = PlocOut{ bs[t]->d_nodes, bs[t]->d_prim_idx, base[t] };
+	CUDA_TRY( cudaEventRecord( sc.e0, s ) );
+	CUDA_TRY( cudaMemcpyAsync( d_base, base.data(), base.size() * 4, cudaMemcpyHostToDevice, s ) );
+	CUDA_TRY( cudaMemcpyAsync( d_io, io.data(), io.size() * sizeof( PlocOut ), cudaMemcpyHostToDevice, s ) );
+	// fragments and Morton order
+	const uint32_t* keys = 0;
+	uint32_t key_stride = 0;
+	TRY( fragments_launch( bs, trees, d_base, n, fmin_, fmax_, &keys, &key_stride, sc ) );
+	const uint32_t g = (n + 255) / 256;
+	k_morton<<<g, 256, 0, s>>>( fmin_, fmax_, d_base, trees, keys, key_stride, n, code[0], val[0] ); LAUNCHED();
+	size_t tb = 0, tb2 = 0;
+	CUDA_TRY( cub::DeviceRadixSort::SortPairs( (void*)0, tb, code[0], code[1], val[0], val[1], (int)n, 0, 63, s ) );
+	int tree_bits = 0;
+	while (tree_bits < 32 && (1ull << tree_bits) < trees) tree_bits++;
+	if (trees > 1) CUDA_TRY( cub::DeviceRadixSort::SortPairs( (void*)0, tb2, tkey[0], tkey[1], val[1], val[0], (int)n, 0, tree_bits, s ) );
+	void* temp = 0;
+	TRY( sc.alloc( temp, std::max( tb, tb2 ) ) );
+	TRY( sort_enqueue( s, [&]() { return cub::DeviceRadixSort::SortPairs( temp, tb, code[0], code[1], val[0], val[1], (int)n, 0, 63, s ); } ) );
+	const uint32_t* order = val[1];
+	if (trees > 1)
 	{
-		uint32_t* d_base = 0, * seg[2] = {}, * nn = 0, * flags = 0, * scan = 0, * tile = 0, * pairs = 0, * parent = 0, * arrive = 0, * cnt = 0, * coll = 0, * sub_int = 0, * sub_w = 0, * depth = 0;
-		uint32_t* val[2] = {}, * tkey[2] = {};
-		uint64_t* code[2] = {};
-		float4* fmin_ = 0, * fmax_ = 0, * cl[2] = {}, * pool = 0;
-		float* cost = 0;
-		PlocOut* d_io = 0;
-		DEV_ALLOC( d_base, base.size() * 4 );
-		DEV_ALLOC( fmin_, (size_t)n * 16 ); DEV_ALLOC( fmax_, (size_t)n * 16 );
-		for (int k = 0; k < 2; k++) { DEV_ALLOC( code[k], (size_t)n * 8 ); DEV_ALLOC( val[k], (size_t)n * 4 ); DEV_ALLOC( cl[k], (size_t)n * 32 ); DEV_ALLOC( seg[k], ((size_t)trees + 1) * 4 ); }
-		if (trees > 1) for (int k = 0; k < 2; k++) DEV_ALLOC( tkey[k], (size_t)n * 4 );
-		DEV_ALLOC( nn, (size_t)n * 4 ); DEV_ALLOC( flags, ((size_t)n + 1) * 4 ); DEV_ALLOC( scan, ((size_t)n + 1) * 4 ); DEV_ALLOC( tile, ((size_t)n / 2048 + 2) * 4 );
-		DEV_ALLOC( pairs, 4 ); DEV_ALLOC( pool, (size_t)slots * 32 ); DEV_ALLOC( parent, (size_t)slots * 4 ); DEV_ALLOC( arrive, (size_t)slots * 4 );
-		DEV_ALLOC( cnt, (size_t)slots * 4 ); DEV_ALLOC( coll, (size_t)slots * 4 ); DEV_ALLOC( cost, (size_t)slots * 4 );
-		DEV_ALLOC( sub_int, (size_t)slots * 4 ); DEV_ALLOC( sub_w, (size_t)slots * 4 ); DEV_ALLOC( depth, (size_t)trees * 4 ); DEV_ALLOC( d_io, (size_t)trees * sizeof( PlocOut ) );
-		CUDA_TRY( cudaMallocHost( &h_res, ((size_t)trees * 2 + 2) * 4 ) );
-		CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) );
-		std::vector<PlocOut> io( trees );
-		for (uint32_t t = 0; t < trees; t++) io[t] = PlocOut{ bs[t]->d_nodes, bs[t]->d_prim_idx, base[t] };
-		CUDA_TRY( cudaEventRecord( e0, s ) );
-		CUDA_TRY( cudaMemcpyAsync( d_base, base.data(), base.size() * 4, cudaMemcpyHostToDevice, s ) );
-		CUDA_TRY( cudaMemcpyAsync( d_io, io.data(), io.size() * sizeof( PlocOut ), cudaMemcpyHostToDevice, s ) );
-		// fragments and Morton order
-		const uint32_t* keys = 0;
-		uint32_t key_stride = 0;
-		TRY( fragments_launch( bs, trees, d_base, n, fmin_, fmax_, &keys, &key_stride, scratch, s ) );
-		const uint32_t g = (n + 255) / 256;
-		k_morton<<<g, 256, 0, s>>>( fmin_, fmax_, d_base, trees, keys, key_stride, n, code[0], val[0] ); LAUNCHED();
-		size_t tb = 0, tb2 = 0;
-		CUDA_TRY( cub::DeviceRadixSort::SortPairs( (void*)0, tb, code[0], code[1], val[0], val[1], (int)n, 0, 63, s ) );
-		int tree_bits = 0;
-		while (tree_bits < 32 && (1ull << tree_bits) < trees) tree_bits++;
-		if (trees > 1) CUDA_TRY( cub::DeviceRadixSort::SortPairs( (void*)0, tb2, tkey[0], tkey[1], val[1], val[0], (int)n, 0, tree_bits, s ) );
-		void* temp = 0;
-		DEV_ALLOC( temp, std::max( tb, tb2 ) );
-		TRY( sort_enqueue( s, [&]() { return cub::DeviceRadixSort::SortPairs( temp, tb, code[0], code[1], val[0], val[1], (int)n, 0, 63, s ); } ) );
-		const uint32_t* order = val[1];
-		if (trees > 1)
+		k_tree_keys<<<g, 256, 0, s>>>( val[1], d_base, trees, n, tkey[0] ); LAUNCHED();
+		tb2 = std::max( tb, tb2 );
+		TRY( sort_enqueue( s, [&]() { return cub::DeviceRadixSort::SortPairs( temp, tb2, tkey[0], tkey[1], val[1], val[0], (int)n, 0, tree_bits, s ); } ) );
+		order = val[0];
+	}
+	k_init_clusters<<<(std::max( n, trees + 1 ) + 255) / 256, 256, 0, s>>>( order, fmin_, fmax_, n, cl[0], d_base, seg[0], trees ); LAUNCHED();
+	CUDA_TRY( cudaMemsetAsync( pairs, 0, 4, s ) );
+	// clustering, PLOC_GROUP iterations per host round trip
+	uint32_t live = n, par = 0;
+	while (live > trees)
+	{
+		const uint32_t bound = live, grid = std::min( (bound + 255) / 256, (uint32_t)ctx->sm_count * 8 );
+		for (int it = 0; it < PLOC_GROUP; it++, par ^= 1)
 		{
-			k_tree_keys<<<g, 256, 0, s>>>( val[1], d_base, trees, n, tkey[0] ); LAUNCHED();
-			tb2 = std::max( tb, tb2 );
-			TRY( sort_enqueue( s, [&]() { return cub::DeviceRadixSort::SortPairs( temp, tb2, tkey[0], tkey[1], val[1], val[0], (int)n, 0, tree_bits, s ); } ) );
-			order = val[0];
+			k_nn<<<grid, 256, 0, s>>>( cl[par], seg[par], trees, nn ); LAUNCHED();
+			k_flags<<<grid, 256, 0, s>>>( seg[par], trees, nn, flags, bound ); LAUNCHED();
+			TRY( exclusive_scan( flags, scan, tile, bound, s ) );
+			k_compact<<<grid, 256, 0, s>>>( cl[par], cl[par ^ 1], seg[par], seg[par ^ 1], trees, nn, scan, pool, parent, pairs ); LAUNCHED();
 		}
-		k_init_clusters<<<(std::max( n, trees + 1 ) + 255) / 256, 256, 0, s>>>( order, fmin_, fmax_, n, cl[0], d_base, seg[0], trees ); LAUNCHED();
-		CUDA_TRY( cudaMemsetAsync( pairs, 0, 4, s ) );
-		// clustering, PLOC_GROUP iterations per host round trip
-		uint32_t live = n, par = 0;
-		while (live > trees)
-		{
-			const uint32_t bound = live, grid = std::min( (bound + 255) / 256, (uint32_t)ctx->sm_count * 8 );
-			for (int it = 0; it < PLOC_GROUP; it++, par ^= 1)
-			{
-				k_nn<<<grid, 256, 0, s>>>( cl[par], seg[par], trees, nn ); LAUNCHED();
-				k_flags<<<grid, 256, 0, s>>>( seg[par], trees, nn, flags, bound ); LAUNCHED();
-				TRY( exclusive_scan( flags, scan, tile, bound, s ) );
-				k_compact<<<grid, 256, 0, s>>>( cl[par], cl[par ^ 1], seg[par], seg[par ^ 1], trees, nn, scan, pool, parent, pairs ); LAUNCHED();
-			}
-			CUDA_TRY( cudaMemcpyAsync( h_res, seg[par] + trees, 4, cudaMemcpyDeviceToHost, s ) );
-			CUDA_TRY( cudaStreamSynchronize( s ) );
-			// every iteration over a tree of two or more clusters merges a pair
-			if (h_res[0] >= live) { tbvh_set_error( "build (PLOC): the clustering stopped merging" ); return TBVH_E_LIMIT; }
-			live = h_res[0];
-		}
-		k_roots<<<(trees + 127) / 128, 128, 0, s>>>( cl[par], trees, pool, parent ); LAUNCHED();
-		// collapse, numbering, primIdx
-		const uint32_t gs = (slots + 255) / 256;
-		CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)slots * 4, s ) );
-		k_cost<<<gs, 256, 0, s>>>( pool, parent, arrive, cnt, cost, coll, slots, c_trav, c_int ); LAUNCHED();
-		CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)slots * 4, s ) );
-		k_sizes<<<gs, 256, 0, s>>>( pool, parent, cnt, coll, arrive, sub_int, sub_w, slots, trees ); LAUNCHED();
-		CUDA_TRY( cudaMemsetAsync( depth, 0, (size_t)trees * 4, s ) );
-		k_renumber<<<gs, 256, 0, s>>>( pool, parent, cnt, coll, sub_int, sub_w, order, d_io, depth, slots, trees ); LAUNCHED();
-		CUDA_TRY( cudaMemcpy2DAsync( h_res, 4, sub_int, 8, 4, trees, cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaMemcpyAsync( h_res + trees, depth, (size_t)trees * 4, cudaMemcpyDeviceToHost, s ) );
+		CUDA_TRY( cudaMemcpyAsync( h_res, seg[par] + trees, 4, cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
-		// boxes as BVH::Refit computes them, and the traversal records
-		std::vector<RfTree> T( trees );
-		uint32_t nodes_total = 0;
-		for (uint32_t t = 0; t < trees; t++)
-		{
-			const tbvh_bvh b = bs[t];
-			const uint32_t used = 2 + 2 * h_res[t];
-			T[t] = RfTree{ b->d_nodes, b->d_prim_idx, b->d_verts, b->d_leaf_tris, parent + nodes_total, nodes_total, used, base[t], b->info.prim_count, 1 };
-			b->info.used_nodes = used, b->info.max_depth = h_res[trees + t];
-			nodes_total += used;
-		}
-		RfTree* d_T = 0;
-		uint32_t* roots = 0;
-		DEV_ALLOC( d_T, (size_t)trees * sizeof( RfTree ) ); DEV_ALLOC( roots, (size_t)trees * 32 );
-		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), T.size() * sizeof( RfTree ), cudaMemcpyHostToDevice, s ) );
-		CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)nodes_total * 4, s ) );
-		TRY( refit_enqueue( d_T, trees, nodes_total, arrive, true, s ) );
-		TRY( leaf_tris_enqueue( d_T, trees, n, s ) );
-		CUDA_TRY( cudaEventRecord( e1, s ) );
-		TRY( refit_roots( d_T, trees, roots, s ) );
-		std::vector<uint32_t> rootw( (size_t)trees * 8 );
-		CUDA_TRY( cudaMemcpyAsync( rootw.data(), roots, rootw.size() * 4, cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		float ms = 0;
-		CUDA_TRY( cudaEventElapsedTime( &ms, e0, e1 ) );
-		for (uint32_t t = 0; t < trees; t++)
-		{
-			const tbvh_bvh b = bs[t];
-			const uint32_t* r = rootw.data() + (size_t)t * 8;
-			b->info.build_ms = ms, b->info.idx_count = b->info.prim_count;
-			memcpy( b->info.aabb_min, r, 12 ), memcpy( b->info.aabb_max, r + 4, 12 );
-			b->root_ref = r[3], b->root_count = r[7];
-			b->d_trav = b->d_nodes;
-			b->generation = tbvh_next_generation();
-		}
-		return TBVH_OK;
-	};
-	const int rc = body();
-	cudaStreamSynchronize( s );
-	for (void* p : scratch) cudaFree( p );
-	if (h_res) cudaFreeHost( h_res );
-	if (e0) cudaEventDestroy( e0 );
-	if (e1) cudaEventDestroy( e1 );
-	return rc;
+		// every iteration over a tree of two or more clusters merges a pair
+		if (h_res[0] >= live) { tbvh_set_error( "build (PLOC): the clustering stopped merging" ); return TBVH_E_LIMIT; }
+		live = h_res[0];
+	}
+	k_roots<<<(trees + 127) / 128, 128, 0, s>>>( cl[par], trees, pool, parent ); LAUNCHED();
+	// collapse, numbering, primIdx
+	const uint32_t gs = (slots + 255) / 256;
+	CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)slots * 4, s ) );
+	k_cost<<<gs, 256, 0, s>>>( pool, parent, arrive, cnt, cost, coll, slots, c_trav, c_int ); LAUNCHED();
+	CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)slots * 4, s ) );
+	k_sizes<<<gs, 256, 0, s>>>( pool, parent, cnt, coll, arrive, sub_int, sub_w, slots, trees ); LAUNCHED();
+	CUDA_TRY( cudaMemsetAsync( depth, 0, (size_t)trees * 4, s ) );
+	k_renumber<<<gs, 256, 0, s>>>( pool, parent, cnt, coll, sub_int, sub_w, order, d_io, depth, slots, trees ); LAUNCHED();
+	CUDA_TRY( cudaMemcpy2DAsync( h_res, 4, sub_int, 8, 4, trees, cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaMemcpyAsync( h_res + trees, depth, (size_t)trees * 4, cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	// boxes as BVH::Refit computes them, and the traversal records
+	std::vector<RfTree> T( trees );
+	uint32_t nodes_total = 0;
+	for (uint32_t t = 0; t < trees; t++)
+	{
+		const tbvh_bvh b = bs[t];
+		const uint32_t used = 2 + 2 * h_res[t];
+		T[t] = RfTree{ b->d_nodes, b->d_prim_idx, b->d_verts, b->d_leaf_tris, parent + nodes_total, nodes_total, used, base[t], b->info.prim_count, 1 };
+		out[t].used_nodes = used, out[t].idx_count = b->info.prim_count, out[t].max_depth = h_res[trees + t];
+		nodes_total += used;
+	}
+	RfTree* d_T = 0;
+	uint32_t* roots = 0;
+	TRY( sc.alloc( d_T, (size_t)trees * sizeof( RfTree ) ) ); TRY( sc.alloc( roots, (size_t)trees * 32 ) );
+	CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), T.size() * sizeof( RfTree ), cudaMemcpyHostToDevice, s ) );
+	CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)nodes_total * 4, s ) );
+	TRY( refit_enqueue( d_T, trees, nodes_total, arrive, true, s ) );
+	TRY( leaf_tris_enqueue( d_T, trees, n, s ) );
+	CUDA_TRY( cudaEventRecord( sc.e1, s ) );
+	TRY( refit_roots( d_T, trees, roots, s ) );
+	std::vector<uint32_t> rootw( (size_t)trees * 8 );
+	CUDA_TRY( cudaMemcpyAsync( rootw.data(), roots, rootw.size() * 4, cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	CUDA_TRY( cudaEventElapsedTime( ms, sc.e0, sc.e1 ) );
+	for (uint32_t t = 0; t < trees; t++) memcpy( out[t].root, rootw.data() + (size_t)t * 8, 32 );
+	return TBVH_OK;
 }

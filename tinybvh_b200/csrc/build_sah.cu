@@ -1245,18 +1245,17 @@ int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint3
 	return TBVH_OK;
 }
 
-#define DEV_ALLOC( ptr, bytes ) do { CUDA_TRY( cudaMalloc( (void**)&(ptr), (bytes) ) ); scratch.push_back( (void*)(ptr) ); } while (0)
-
 int fragments_launch( const tbvh_bvh* bs, const uint32_t trees, const uint32_t* d_base, const uint32_t n, float4* frag_min, float4* frag_max,
-	const uint32_t** keys, uint32_t* key_stride, std::vector<void*>& scratch, cudaStream_t s )
+	const uint32_t** keys, uint32_t* key_stride, Scratch& sc )
 {
+	cudaStream_t s = sc.s;
 	BuildArgs A = {};
 	A.trees = trees, A.tree_base = d_base, A.n = n, A.frag_min = frag_min, A.frag_max = frag_max;
 	std::vector<TreeIO> io( trees );
 	for (uint32_t t = 0; t < trees; t++) io[t] = TreeIO{ bs[t]->d_verts, 0, 0, 0 };
 	TreeIO* d_io = 0;
-	DEV_ALLOC( d_io, io.size() * sizeof( TreeIO ) ); DEV_ALLOC( A.ts, (size_t)trees * sizeof( TreeState ) ); DEV_ALLOC( A.ctr, sizeof( Counters ) );
-	DEV_ALLOC( A.idx[0], (size_t)n * 4 );
+	TRY( sc.alloc( d_io, io.size() * sizeof( TreeIO ) ) ); TRY( sc.alloc( A.ts, (size_t)trees * sizeof( TreeState ) ) ); TRY( sc.alloc( A.ctr, sizeof( Counters ) ) );
+	TRY( sc.alloc( A.idx[0], (size_t)n * 4 ) );
 	A.io = d_io;
 	CUDA_TRY( cudaMemcpyAsync( d_io, io.data(), io.size() * sizeof( TreeIO ), cudaMemcpyHostToDevice, s ) );
 	k_init_counters<<<(trees + 255) / 256, 256, 0, s>>>( A, 0 ); LAUNCHED();
@@ -1266,13 +1265,10 @@ int fragments_launch( const tbvh_bvh* bs, const uint32_t trees, const uint32_t* 
 	return TBVH_OK;
 }
 
-// bs[0 .. trees): handles of one context holding their primitives (d_verts, or d_aabbs for a TLAS, which is built alone) and
-// info.prim_count; on success each holds its tree as a build of its own would leave it.  On failure the caller empties them.
-int build_sah_launch( const tbvh_bvh* bs, const uint32_t trees, float c_trav, float c_int, int flavour )
+int build_sah_launch( const tbvh_bvh* bs, const uint32_t trees, float c_trav, float c_int, int flavour, BuiltTree* out, float* ms )
 {
 	const tbvh_ctx ctx = bs[0]->ctx;
 	cudaStream_t s = ctx->stream;
-	std::vector<void*> scratch;
 	BuildArgs A = {};
 	A.aabbs = bs[0]->d_aabbs, A.trees = trees, A.c_trav = c_trav, A.c_int = c_int, A.flavour = (uint32_t)flavour;
 	{
@@ -1294,10 +1290,6 @@ int build_sah_launch( const tbvh_bvh* bs, const uint32_t trees, float c_trav, fl
 	const uint32_t n = base[trees];
 	A.n = n;
 	const size_t max_nodes = (size_t)2 * n + 2 * (size_t)trees, max_large = n / A.small_t + 2;
-	int rc = TBVH_OK;
-	uint32_t* tile_sum = 0;
-	Counters* h_ctr = 0;
-	cudaEvent_t e0 = 0, e1 = 0;
 	// outputs (kept by the handles)
 	std::vector<TreeIO> io( trees );
 	for (uint32_t t = 0; t < trees; t++)
@@ -1310,156 +1302,140 @@ int build_sah_launch( const tbvh_bvh* bs, const uint32_t trees, float c_trav, fl
 		io[t] = TreeIO{ b->d_verts, b->d_nodes, b->d_prim_idx, b->d_leaf_tris };
 	}
 	A.idx_final = bs[0]->d_prim_idx; // one tree: the leaves write the handle's primIdx directly
-	auto body = [&]() -> int
+	Scratch sc( s );
+	uint32_t* d_base = 0, * tile_sum = 0; TreeIO* d_io = 0;
+	Counters* h_ctr = 0;
+	TRY( sc.alloc( d_base, base.size() * 4 ) ); TRY( sc.alloc( d_io, io.size() * sizeof( TreeIO ) ) ); TRY( sc.alloc( A.ts, (size_t)trees * sizeof( TreeState ) ) );
+	A.tree_base = d_base, A.io = d_io;
+	if (trees > 1) TRY( sc.alloc( A.idx_final, (size_t)n * 4 ) ); // global positions, made local by k_tree_outputs
+	TRY( sc.alloc( A.frag_min, (size_t)n * 16 ) ); TRY( sc.alloc( A.frag_max, (size_t)n * 16 ) );
+	TRY( sc.alloc( A.idx[0], (size_t)n * 4 ) ); TRY( sc.alloc( A.idx[1], (size_t)n * 4 ) );
+	TRY( sc.alloc( A.bin_ids, (size_t)n * 2 ) );
+	// chunk space: at most n / CHUNK + (#large nodes) chunks per level
+	const size_t flag_words = (size_t)n + (size_t)CHUNK * (max_large + 1) + 1;
+	TRY( sc.alloc( A.flags, flag_words * 4 ) ); TRY( sc.alloc( A.scan, flag_words * 4 ) ); TRY( sc.alloc( A.pos_bl, ((size_t)n + 1) * 4 ) );
+	TRY( sc.alloc( A.tmp_nodes, max_nodes * 32 ) ); TRY( sc.alloc( A.node_first, max_nodes * 4 ) ); TRY( sc.alloc( A.node_depth, max_nodes * 4 ) );
+	TRY( sc.alloc( A.lvl[0], max_large * sizeof( LargeNode ) ) ); TRY( sc.alloc( A.lvl[1], max_large * sizeof( LargeNode ) ) );
+	TRY( sc.alloc( A.chunk_start, (max_large + 1) * 4 ) ); TRY( sc.alloc( A.chunk_start_next, (max_large + 1) * 4 ) ); TRY( sc.alloc( A.bins, max_large * BIN_STRIDE * 4 ) ); TRY( sc.alloc( A.split, max_large * sizeof( SplitInfo ) ) );
+	TRY( sc.alloc( A.zpos, max_large * ZPOS_WORDS * 4 ) ); // cleared by k_root_zero, with a -0 only
+	TRY( sc.alloc( A.chunk_pre, (flag_words / CHUNK + 2) * 4 ) );
+	TRY( sc.alloc( A.small, ((size_t)n + 1) * sizeof( SmallRoot ) ) );
+	TRY( sc.alloc( A.ctr, sizeof( Counters ) ) );
+	TRY( sc.alloc( tile_sum, (flag_words / SCAN_TILE + 2) * 4 ) );
+	TRY( sc.alloc_host( h_ctr, sizeof( Counters ) ) );
+	TRY( sc.events() );
+	CUDA_TRY( cudaMemcpyAsync( d_base, base.data(), base.size() * 4, cudaMemcpyHostToDevice, s ) );
+	CUDA_TRY( cudaMemcpyAsync( d_io, io.data(), io.size() * sizeof( TreeIO ), cudaMemcpyHostToDevice, s ) );
+	if (!large.empty())
 	{
-		uint32_t* d_base = 0; TreeIO* d_io = 0;
-		DEV_ALLOC( d_base, base.size() * 4 ); DEV_ALLOC( d_io, io.size() * sizeof( TreeIO ) ); DEV_ALLOC( A.ts, (size_t)trees * sizeof( TreeState ) );
-		A.tree_base = d_base, A.io = d_io;
-		if (trees > 1) DEV_ALLOC( A.idx_final, (size_t)n * 4 ); // global positions, made local by k_tree_outputs
-		DEV_ALLOC( A.frag_min, (size_t)n * 16 ); DEV_ALLOC( A.frag_max, (size_t)n * 16 );
-		DEV_ALLOC( A.idx[0], (size_t)n * 4 ); DEV_ALLOC( A.idx[1], (size_t)n * 4 );
-		DEV_ALLOC( A.bin_ids, (size_t)n * 2 );
-		// chunk space: at most n / CHUNK + (#large nodes) chunks per level
-		const size_t flag_words = (size_t)n + (size_t)CHUNK * (max_large + 1) + 1;
-		DEV_ALLOC( A.flags, flag_words * 4 ); DEV_ALLOC( A.scan, flag_words * 4 ); DEV_ALLOC( A.pos_bl, ((size_t)n + 1) * 4 );
-		DEV_ALLOC( A.tmp_nodes, max_nodes * 32 ); DEV_ALLOC( A.node_first, max_nodes * 4 ); DEV_ALLOC( A.node_depth, max_nodes * 4 );
-		DEV_ALLOC( A.lvl[0], max_large * sizeof( LargeNode ) ); DEV_ALLOC( A.lvl[1], max_large * sizeof( LargeNode ) );
-		DEV_ALLOC( A.chunk_start, (max_large + 1) * 4 ); DEV_ALLOC( A.chunk_start_next, (max_large + 1) * 4 ); DEV_ALLOC( A.bins, max_large * BIN_STRIDE * 4 ); DEV_ALLOC( A.split, max_large * sizeof( SplitInfo ) );
-		DEV_ALLOC( A.zpos, max_large * ZPOS_WORDS * 4 ); // cleared by k_root_zero, with a -0 only
-		DEV_ALLOC( A.chunk_pre, (flag_words / CHUNK + 2) * 4 );
-		DEV_ALLOC( A.small, ((size_t)n + 1) * sizeof( SmallRoot ) );
-		DEV_ALLOC( A.ctr, sizeof( Counters ) );
-		DEV_ALLOC( tile_sum, (flag_words / SCAN_TILE + 2) * 4 );
-		CUDA_TRY( cudaMallocHost( &h_ctr, sizeof( Counters ) ) );
-		CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) );
-		CUDA_TRY( cudaMemcpyAsync( d_base, base.data(), base.size() * 4, cudaMemcpyHostToDevice, s ) );
-		CUDA_TRY( cudaMemcpyAsync( d_io, io.data(), io.size() * sizeof( TreeIO ), cudaMemcpyHostToDevice, s ) );
-		if (!large.empty())
+		CUDA_TRY( cudaMemcpyAsync( A.lvl[0], large.data(), large.size() * sizeof( LargeNode ), cudaMemcpyHostToDevice, s ) );
+		CUDA_TRY( cudaMemcpyAsync( A.chunk_start, chunk0.data(), chunk0.size() * 4, cudaMemcpyHostToDevice, s ) );
+	}
+	if (!small.empty()) CUDA_TRY( cudaMemcpyAsync( A.small, small.data(), small.size() * sizeof( SmallRoot ), cudaMemcpyHostToDevice, s ) );
+	CUDA_TRY( cudaEventRecord( sc.e0, s ) );
+	k_init_counters<<<(trees + 255) / 256, 256, 0, s>>>( A, (uint32_t)small.size() ); LAUNCHED();
+	k_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+	k_root_zero<<<ctx->sm_count, 256, 0, s>>>( A, max_large * ZPOS_WORDS ); LAUNCHED();
+	{
+		const size_t work = std::max( (size_t)trees, large.size() * BIN_STRIDE );
+		k_init_root<<<(uint32_t)std::min( (work + 255) / 256, (size_t)ctx->sm_count * 8 ), 256, 0, s>>>( A, (uint32_t)large.size() ); LAUNCHED();
+	}
+	uint32_t num = (uint32_t)large.size(), chunks = chunk0.back(), level = 0;
+	// Large phase.  The first levels of a big scene are bandwidth work over all primitives: one launch per stage, every CTA the
+	// device can hold.  Once a level is down to a few chunks per SM the stages are launch-latency sized, and the rest of the
+	// phase runs inside ONE persistent cooperative launch (k_large_phase) without further host round trips.
+	int per_sm = 0;
+	uint32_t pgrid = 0;
+	if (num && ctx->build_mode == 0)
+	{
+		CUDA_TRY( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &per_sm, k_large_phase, CHUNK, 0 ) );
+		const int want = ctx->build_ctas > 0 ? ctx->build_ctas : 4;
+		if (per_sm > want) per_sm = want;
+		pgrid = (uint32_t)(per_sm > 0 ? per_sm * ctx->sm_count : 0);
+	}
+	const uint32_t persist_chunks = pgrid * 3;
+	while (num)
+	{
+		if (pgrid && chunks <= persist_chunks)
 		{
-			CUDA_TRY( cudaMemcpyAsync( A.lvl[0], large.data(), large.size() * sizeof( LargeNode ), cudaMemcpyHostToDevice, s ) );
-			CUDA_TRY( cudaMemcpyAsync( A.chunk_start, chunk0.data(), chunk0.size() * 4, cudaMemcpyHostToDevice, s ) );
-		}
-		if (!small.empty()) CUDA_TRY( cudaMemcpyAsync( A.small, small.data(), small.size() * sizeof( SmallRoot ), cudaMemcpyHostToDevice, s ) );
-		CUDA_TRY( cudaEventRecord( e0, s ) );
-		k_init_counters<<<(trees + 255) / 256, 256, 0, s>>>( A, (uint32_t)small.size() ); LAUNCHED();
-		k_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
-		k_root_zero<<<ctx->sm_count, 256, 0, s>>>( A, max_large * ZPOS_WORDS ); LAUNCHED();
-		{
-			const size_t work = std::max( (size_t)trees, large.size() * BIN_STRIDE );
-			k_init_root<<<(uint32_t)std::min( (work + 255) / 256, (size_t)ctx->sm_count * 8 ), 256, 0, s>>>( A, (uint32_t)large.size() ); LAUNCHED();
-		}
-		uint32_t num = (uint32_t)large.size(), chunks = chunk0.back(), level = 0;
-		// Large phase.  The first levels of a big scene are bandwidth work over all primitives: one launch per stage, every CTA the
-		// device can hold.  Once a level is down to a few chunks per SM the stages are launch-latency sized, and the rest of the
-		// phase runs inside ONE persistent cooperative launch (k_large_phase) without further host round trips.
-		int per_sm = 0;
-		uint32_t pgrid = 0;
-		if (num && ctx->build_mode == 0)
-		{
-			CUDA_TRY( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &per_sm, k_large_phase, CHUNK, 0 ) );
-			const int want = ctx->build_ctas > 0 ? ctx->build_ctas : 4;
-			if (per_sm > want) per_sm = want;
-			pgrid = (uint32_t)(per_sm > 0 ? per_sm * ctx->sm_count : 0);
-		}
-		const uint32_t persist_chunks = pgrid * 3;
-		while (num)
-		{
-			if (pgrid && chunks <= persist_chunks)
+			const uint32_t state[2] = { num, chunks };
+			CUDA_TRY( cudaMemcpyAsync( &A.ctr->lvl_num[0], &state[0], 4, cudaMemcpyHostToDevice, s ) );
+			CUDA_TRY( cudaMemcpyAsync( &A.ctr->lvl_chunks[0], &state[1], 4, cudaMemcpyHostToDevice, s ) );
+			A.level0 = level;
+			void* params[] = { (void*)&A };
+			const cudaError_t ce = cudaLaunchCooperativeKernel( (const void*)k_large_phase, dim3( pgrid ), dim3( CHUNK ), params, 0, s );
+			if (ce == cudaErrorCooperativeLaunchTooLarge || ce == cudaErrorNotSupported || ce == cudaErrorLaunchOutOfResources)
 			{
-				const uint32_t state[2] = { num, chunks };
-				CUDA_TRY( cudaMemcpyAsync( &A.ctr->lvl_num[0], &state[0], 4, cudaMemcpyHostToDevice, s ) );
-				CUDA_TRY( cudaMemcpyAsync( &A.ctr->lvl_chunks[0], &state[1], 4, cudaMemcpyHostToDevice, s ) );
-				A.level0 = level;
-				void* params[] = { (void*)&A };
-				const cudaError_t ce = cudaLaunchCooperativeKernel( (const void*)k_large_phase, dim3( pgrid ), dim3( CHUNK ), params, 0, s );
-				if (ce == cudaErrorCooperativeLaunchTooLarge || ce == cudaErrorNotSupported || ce == cudaErrorLaunchOutOfResources)
-				{
-					// this device (or partition of it) cannot keep the persistent grid resident: the launch-per-stage path serves every level
-					cudaGetLastError();
-					pgrid = 0;
-					continue;
-				}
-				CUDA_TRY( ce );
-				g_tbvh_launches++;
-				CUDA_TRY( cudaStreamSynchronize( s ) ); // `state` is on this frame
-				break;
+				// this device (or partition of it) cannot keep the persistent grid resident: the launch-per-stage path serves every level
+				cudaGetLastError();
+				pgrid = 0;
+				continue;
 			}
-			const LargeNode* cur = A.lvl[level & 1];
-			LargeNode* next = A.lvl[(level + 1) & 1];
-			const uint32_t* idx_in = A.idx[level & 1];
-			uint32_t* idx_out = A.idx[(level + 1) & 1];
-			k_bin<<<chunks, CHUNK, 0, s>>>( A, cur, num, idx_in ); LAUNCHED();
-			if (level == 0 || h_ctr->negzero) { k_bin_zero<<<min( chunks, (uint32_t)ctx->sm_count ), CHUNK, 0, s>>>( A, cur, num, idx_in, chunks ); LAUNCHED(); }
-			k_sweep<<<(num * 32 + 255) / 256, 256, 0, s>>>( A, cur, next, num, idx_in, (level + 1) & 1 ); LAUNCHED();
-			k_flags<<<chunks, CHUNK, 0, s>>>( A, cur, num ); LAUNCHED();
-			{ const int r = exclusive_scan( A.flags, A.scan, tile_sum, chunks * CHUNK, s ); if (r != TBVH_OK) return r; }
-			k_posbl<<<chunks, CHUNK, 0, s>>>( A, cur, num ); LAUNCHED();
-			k_scatter<<<chunks, CHUNK, 0, s>>>( A, cur, num, idx_in, idx_out ); LAUNCHED();
-			k_prepare_level<<<1, 1024, 0, s>>>( A, next ); LAUNCHED();
-			CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( Counters ), cudaMemcpyDeviceToHost, s ) );
-			CUDA_TRY( cudaStreamSynchronize( s ) );
-			num = h_ctr->next_large, chunks = h_ctr->total_chunks;
-			if (num > max_large) { tbvh_set_error( "build: level list overflow (%u > %zu)", num, max_large ); return TBVH_E_LIMIT; }
-			if (num)
-			{
-				k_bins_init<<<(num * BIN_STRIDE + 255) / 256, 256, 0, s>>>( A.bins, num * BIN_STRIDE ); LAUNCHED();
-				CUDA_TRY( cudaMemsetAsync( &A.ctr->next_large, 0, 4, s ) );
-			}
-			level++;
-			if (level > 4096) { tbvh_set_error( "build: runaway level count" ); return TBVH_E_LIMIT; }
+			CUDA_TRY( ce );
+			g_tbvh_launches++;
+			CUDA_TRY( cudaStreamSynchronize( s ) ); // `state` is on this frame
+			break;
 		}
+		const LargeNode* cur = A.lvl[level & 1];
+		LargeNode* next = A.lvl[(level + 1) & 1];
+		const uint32_t* idx_in = A.idx[level & 1];
+		uint32_t* idx_out = A.idx[(level + 1) & 1];
+		k_bin<<<chunks, CHUNK, 0, s>>>( A, cur, num, idx_in ); LAUNCHED();
+		if (level == 0 || h_ctr->negzero) { k_bin_zero<<<min( chunks, (uint32_t)ctx->sm_count ), CHUNK, 0, s>>>( A, cur, num, idx_in, chunks ); LAUNCHED(); }
+		k_sweep<<<(num * 32 + 255) / 256, 256, 0, s>>>( A, cur, next, num, idx_in, (level + 1) & 1 ); LAUNCHED();
+		k_flags<<<chunks, CHUNK, 0, s>>>( A, cur, num ); LAUNCHED();
+		{ const int r = exclusive_scan( A.flags, A.scan, tile_sum, chunks * CHUNK, s ); if (r != TBVH_OK) return r; }
+		k_posbl<<<chunks, CHUNK, 0, s>>>( A, cur, num ); LAUNCHED();
+		k_scatter<<<chunks, CHUNK, 0, s>>>( A, cur, num, idx_in, idx_out ); LAUNCHED();
+		k_prepare_level<<<1, 1024, 0, s>>>( A, next ); LAUNCHED();
 		CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( Counters ), cudaMemcpyDeviceToHost, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
-		const uint32_t roots = h_ctr->small_roots;
-		if (roots)
+		num = h_ctr->next_large, chunks = h_ctr->total_chunks;
+		if (num > max_large) { tbvh_set_error( "build: level list overflow (%u > %zu)", num, max_large ); return TBVH_E_LIMIT; }
+		if (num)
 		{
-			const uint32_t g = (roots + SMALL_WARPS - 1) / SMALL_WARPS, mode = (uint32_t)ctx->small_mode;
-			// the signed-zero instance also carries the root rule, for trees whose root is a warp subtree
-			#define SMALL( F, G ) do { if (h_ctr->negzero || !small.empty()) k_build_small<F, G, true><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); \
-				else k_build_small<F, G, false><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); } while (0)
-			if (mode == 0) SMALL( false, false );
-			else if (mode == 1) SMALL( true, false );
-			else if (mode == 2) SMALL( false, true );
-			else SMALL( true, true );
-			#undef SMALL
-			LAUNCHED();
+			k_bins_init<<<(num * BIN_STRIDE + 255) / 256, 256, 0, s>>>( A.bins, num * BIN_STRIDE ); LAUNCHED();
+			CUDA_TRY( cudaMemsetAsync( &A.ctr->next_large, 0, 4, s ) );
 		}
-		CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( Counters ), cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		const uint32_t tmp_count = h_ctr->tmp_nodes;
-		if (tmp_count > max_nodes) { tbvh_set_error( "build: node pool overflow" ); return TBVH_E_LIMIT; }
-		// relayout into the reference's numbering: cnt -> flags, prefix -> scan, min depth -> pos_bl
-		CUDA_TRY( cudaMemsetAsync( A.flags, 0, ((size_t)n + 1) * 4, s ) );
-		CUDA_TRY( cudaMemsetAsync( A.pos_bl, 0xff, ((size_t)n + 1) * 4, s ) );
-		k_rank_count<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count, A.flags, A.pos_bl ); LAUNCHED();
-		{ const int r = exclusive_scan( A.flags, A.scan, tile_sum, n, s ); if (r != TBVH_OK) return r; }
-		k_relayout<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count, A.scan, A.pos_bl ); LAUNCHED();
-		CUDA_TRY( cudaEventRecord( e1, s ) );
-		if (trees > 1 || !A.aabbs) { k_tree_outputs<<<(n + 255) / 256, 256, 0, s>>>( A, trees > 1 ); LAUNCHED(); }
-		std::vector<TreeState> ts( trees );
-		CUDA_TRY( cudaMemcpyAsync( ts.data(), A.ts, ts.size() * sizeof( TreeState ), cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		float ms = 0;
-		CUDA_TRY( cudaEventElapsedTime( &ms, e0, e1 ) );
-		for (uint32_t t = 0; t < trees; t++)
-		{
-			const tbvh_bvh b = bs[t];
-			uint32_t rootw[8];
-			memcpy( rootw, ts[t].root, 32 );
-			b->info.build_ms = ms;
-			b->info.used_nodes = ts[t].used_nodes, b->info.idx_count = b->info.prim_count, b->info.max_depth = ts[t].max_depth;
-			memcpy( b->info.aabb_min, rootw, 12 ), memcpy( b->info.aabb_max, rootw + 4, 12 );
-			b->root_ref = rootw[3], b->root_count = rootw[7];
-			b->d_trav = b->d_nodes;
-			b->generation = tbvh_next_generation(); // new arrays: a TLAS built over the old ones must notice (tlas_check)
-		}
-		return TBVH_OK;
-	};
-	rc = body();
-	cudaStreamSynchronize( s );
-	for (void* p : scratch) cudaFree( p );
-	if (h_ctr) cudaFreeHost( h_ctr );
-	if (e0) cudaEventDestroy( e0 );
-	if (e1) cudaEventDestroy( e1 );
-	return rc;
+		level++;
+		if (level > 4096) { tbvh_set_error( "build: runaway level count" ); return TBVH_E_LIMIT; }
+	}
+	CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( Counters ), cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	const uint32_t roots = h_ctr->small_roots;
+	if (roots)
+	{
+		const uint32_t g = (roots + SMALL_WARPS - 1) / SMALL_WARPS, mode = (uint32_t)ctx->small_mode;
+		// the signed-zero instance also carries the root rule, for trees whose root is a warp subtree
+		#define SMALL( F, G ) do { if (h_ctr->negzero || !small.empty()) k_build_small<F, G, true><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); \
+			else k_build_small<F, G, false><<<g, SMALL_WARPS * 32, 0, s>>>( A, roots ); } while (0)
+		if (mode == 0) SMALL( false, false );
+		else if (mode == 1) SMALL( true, false );
+		else if (mode == 2) SMALL( false, true );
+		else SMALL( true, true );
+		#undef SMALL
+		LAUNCHED();
+	}
+	CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( Counters ), cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	const uint32_t tmp_count = h_ctr->tmp_nodes;
+	if (tmp_count > max_nodes) { tbvh_set_error( "build: node pool overflow" ); return TBVH_E_LIMIT; }
+	// relayout into the reference's numbering: cnt -> flags, prefix -> scan, min depth -> pos_bl
+	CUDA_TRY( cudaMemsetAsync( A.flags, 0, ((size_t)n + 1) * 4, s ) );
+	CUDA_TRY( cudaMemsetAsync( A.pos_bl, 0xff, ((size_t)n + 1) * 4, s ) );
+	k_rank_count<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count, A.flags, A.pos_bl ); LAUNCHED();
+	{ const int r = exclusive_scan( A.flags, A.scan, tile_sum, n, s ); if (r != TBVH_OK) return r; }
+	k_relayout<<<(tmp_count + 255) / 256, 256, 0, s>>>( A, tmp_count, A.scan, A.pos_bl ); LAUNCHED();
+	CUDA_TRY( cudaEventRecord( sc.e1, s ) );
+	if (trees > 1 || !A.aabbs) { k_tree_outputs<<<(n + 255) / 256, 256, 0, s>>>( A, trees > 1 ); LAUNCHED(); }
+	std::vector<TreeState> ts( trees );
+	CUDA_TRY( cudaMemcpyAsync( ts.data(), A.ts, ts.size() * sizeof( TreeState ), cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	CUDA_TRY( cudaEventElapsedTime( ms, sc.e0, sc.e1 ) );
+	for (uint32_t t = 0; t < trees; t++)
+	{
+		memcpy( out[t].root, ts[t].root, 32 );
+		out[t].used_nodes = ts[t].used_nodes, out[t].idx_count = bs[t]->info.prim_count, out[t].max_depth = ts[t].max_depth;
+	}
+	return TBVH_OK;
 }

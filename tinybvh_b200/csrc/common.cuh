@@ -24,6 +24,29 @@ extern unsigned long long g_tbvh_launches;
 #define ARG_CHECK( c, msg ) do { if (!(c)) { tbvh_set_error( "%s: %s", __func__, msg ); return TBVH_E_ARG; } } while (0)
 #define TRY( x ) do { int r_ = (x); if (r_ != TBVH_OK) return r_; } while (0)
 
+// ---- the scratch of one host call on stream s: its device allocations (one cudaMalloc each), its page-locked words and its two timing
+// events.  The destructor drains s and then frees them all, on every return path.  Buffers that outlive the call are not scratch.
+struct Scratch
+{
+	cudaStream_t s;
+	cudaEvent_t e0 = 0, e1 = 0;
+	std::vector<void*> dev, pinned;
+	explicit Scratch( cudaStream_t stream ) : s( stream ) {}
+	Scratch( const Scratch& ) = delete;
+	Scratch& operator=( const Scratch& ) = delete;
+	~Scratch()
+	{
+		cudaStreamSynchronize( s );
+		for (void* p : dev) cudaFree( p );
+		for (void* p : pinned) cudaFreeHost( p );
+		if (e0) cudaEventDestroy( e0 );
+		if (e1) cudaEventDestroy( e1 );
+	}
+	template <class T> int alloc( T*& p, size_t bytes ) { void* q = 0; CUDA_TRY( cudaMalloc( &q, bytes ) ); dev.push_back( q ); p = (T*)q; return TBVH_OK; }
+	template <class T> int alloc_host( T*& p, size_t bytes ) { void* q = 0; CUDA_TRY( cudaMallocHost( &q, bytes ) ); pinned.push_back( q ); p = (T*)q; return TBVH_OK; }
+	int events() { CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) ); return TBVH_OK; }
+};
+
 // ---- handles ----------------------------------------------------------------------------------------------
 // one stage buffer set of the host-buffer pipeline (api.cu "host path")
 struct HostSlot
@@ -247,17 +270,23 @@ int cw_make_trav( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
 int cw_expand( const CwTrav* d_T, uint32_t K, uint32_t W, uint32_t* parent, cudaStream_t s );
 float cw_rd_limit_for( uint32_t range );                               // cw_rd_limit of a tree whose expansion found `range`
 unsigned long long* ctx_next_counter( tbvh_ctx c ); // a zero-on-use 8-byte device counter from the context's ring (persistent-warp ray fetch)
-// binned-SAH builds of `trees` handles of one context at once (build_sah.cu); a single build is trees = 1
-int build_sah_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, int flavour );
-// the fragment pass of the binned builder (k_fragments) for the PLOC builder: every triangle's box into frag_min / frag_max at its
-// position of the batch's index space (tree t from d_base[t] on), every tree's root box as six ordered keys (min xyz, max xyz) at
-// (*keys)[key_stride * t ..]; allocations go to scratch
+// A tree a builder has written into a handle's d_nodes / d_prim_idx: the root node's 8 words (aabbMin, leftFirst, aabbMax, triCount)
+// and the counts.  install_tree (api.cu) makes the handle hold it.
+struct BuiltTree { uint32_t root[8]; uint32_t used_nodes, idx_count, max_depth; };
+// The builders of `trees` handles of one context at once; a single build is trees = 1.  Each handle holds its primitives (d_verts, or
+// d_aabbs for a TLAS, which is built alone) and info.prim_count.  The builder allocates the handle's d_nodes, d_prim_idx and (but for a
+// TLAS) d_leaf_tris; on success out[t] describes tree t and *ms is the call's build time.  On failure the caller empties the handles.
+// binned SAH (build_sah.cu)
+int build_sah_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, int flavour, BuiltTree* out, float* ms );
+// the fragment pass of the binned builder (k_fragments) for the PLOC builder, on sc.s: every triangle's box into frag_min / frag_max at
+// its position of the batch's index space (tree t from d_base[t] on), every tree's root box as six ordered keys (min xyz, max xyz) at
+// (*keys)[key_stride * t ..]; its allocations are sc's
 int fragments_launch( const tbvh_bvh* bs, uint32_t trees, const uint32_t* d_base, uint32_t n, float4* frag_min, float4* frag_max,
-	const uint32_t** keys, uint32_t* key_stride, std::vector<void*>& scratch, cudaStream_t s );
-// PLOC builds (TBVH_BUILD_PLOC) of `trees` handles of one context at once (build_ploc.cu); a single build is trees = 1
-int build_ploc_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int );
-// SBVH builds (BuildHQ) of K handles of one context at once (build_hq.cu); a single build is K = 1
-int build_hq_launch( const tbvh_bvh* bs, uint32_t K, float c_trav, float c_int );
+	const uint32_t** keys, uint32_t* key_stride, Scratch& sc );
+// PLOC (TBVH_BUILD_PLOC, build_ploc.cu)
+int build_ploc_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, BuiltTree* out, float* ms );
+// SBVH (BuildHQ, build_hq.cu)
+int build_hq_launch( const tbvh_bvh* bs, uint32_t trees, float c_trav, float c_int, BuiltTree* out, float* ms );
 // BVH::Refit of K trees over one node space of `nodes` nodes; arrive: `nodes` zeroed words; fill: some tree's parents are filled
 int refit_enqueue( const RfTree* d_T, uint32_t K, uint32_t nodes, uint32_t* arrive, bool fill, cudaStream_t s );
 int refit_roots( const RfTree* d_T, uint32_t K, uint32_t* out, cudaStream_t s ); // each tree's root node (8 words) to out[8 t ..]

@@ -557,8 +557,6 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		T[t].nodes = b->d_nodes, T[t].prim_idx = b->d_prim_idx, T[t].verts = b->d_verts, T[t].nbase = N, T[t].used = b->info.used_nodes;
 		N += cw_seg( T[t].used );
 	}
-	std::vector<void*> scratch;
-	#define CW_ALLOC( ptr, bytes ) do { CUDA_TRY( cudaMalloc( (void**)&(ptr), (bytes) ) ); scratch.push_back( (void*)(ptr) ); } while (0)
 	// scratch of one stage carved from one allocation: fewer cudaMalloc / cudaFree pairs per call
 	size_t carve = 0;
 	char* blob = 0;
@@ -571,12 +569,13 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 	float4* ext = 0;
 	auto body = [&]() -> int
 	{
+		Scratch sc( s );
 		// ---- SplitLeafs(3) over every tree, and each tree's first split-tree node
 		{
 			carve = 0;
 			const size_t o_T = take( (size_t)K * sizeof( CwTree ) ), o_extra = take( ((size_t)N + 1) * 4 ), o_base = take( ((size_t)N + 1) * 4 );
 			const size_t o_tile = take( ((size_t)N / 2048 + 2) * 4 ), o_ext = take( ((size_t)K + 1) * 4 );
-			CW_ALLOC( blob, carve );
+			TRY( sc.alloc( blob, carve ) );
 			d_T = (CwTree*)(blob + o_T), extra = (uint32_t*)(blob + o_extra), base = (uint32_t*)(blob + o_base), tile = (uint32_t*)(blob + o_tile);
 			d_ext = (uint32_t*)(blob + o_ext);
 		}
@@ -597,7 +596,7 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 			const size_t o_adopt = take( ((size_t)total + 1) * 32 ), o_ifirst = take( ((size_t)total + 1) * 4 ), o_counts = take( CW_MAX_LEVELS * 4 );
 			const size_t o_groups = K > 1 ? take( ((size_t)total + 1) * 8 ) : 0; // a run per tree and level: at most one per wide node
 			const size_t o_leaf = take( (size_t)K * 4 ), o_tickets = take( (CW_MAX_LEVELS + 1) * 4 ), o_look = take( look_words * 8 );
-			CW_ALLOC( blob, carve );
+			TRY( sc.alloc( blob, carve ) );
 			ext = (float4*)(blob + o_ext), lists = (uint32_t*)(blob + o_lists), wtree = (uint32_t*)(blob + o_wtree), adopt = (uint32_t*)(blob + o_adopt);
 			ifirst = (uint32_t*)(blob + o_ifirst), counts = (uint32_t*)(blob + o_counts), groups = K > 1 ? (uint2*)(blob + o_groups) : 0;
 			leaf = (uint32_t*)(blob + o_leaf), tickets = (uint32_t*)(blob + o_tickets), look = (unsigned long long*)(blob + o_look);
@@ -679,7 +678,7 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		// one allocation: the wide nodes (each tree's slice from its wbase), the runs, the scratch keep blocks
 		carve = 0;
 		const size_t o_wide = take( (size_t)W * sizeof( WideNode ) ), o_runs = take( lv.runs.size() * sizeof( CwRun ) ), o_keep = take( scratch_words * 4 );
-		CW_ALLOC( blob, carve );
+		TRY( sc.alloc( blob, carve ) );
 		const CwRun* d_runs = (const CwRun*)(blob + o_runs);
 		uint32_t* spare = (uint32_t*)(blob + o_keep);
 		for (uint32_t t = 0; t < K; t++)
@@ -699,10 +698,7 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		// the traversal nodes the kernels read and the pending bound of every wide tree (trace_cwbvh.cu); synchronises the stream
 		return cw_make_trav( bs, K, s );
 	};
-	const int rc = body();
-	cudaStreamSynchronize( s );
-	for (void* p : scratch) cudaFree( p );
-	#undef CW_ALLOC
+	const int rc = body(); // the stream is drained and the scratch freed before a failure drops the handles' arrays
 	for (uint32_t t = 0; t < K; t++)
 	{
 		if (rc != TBVH_OK) drop_cwbvh( bs[t] );

@@ -310,9 +310,9 @@ int optimize_tree( tbvh_bvh b, const uint32_t max_rounds, const float c_trav, co
 	// cost floats, key and lock words; then the results and the threshold
 	const size_t nb = (size_t)n * 32, w4 = ((size_t)n * 4 + 255) & ~(size_t)255, w8 = ((size_t)n * 8 + 255) & ~(size_t)255;
 	const size_t bytes = 2 * nb + 9 * w4 + 2 * w8 + 256;
+	Scratch sc( s );
 	char* m = 0;
-	CUDA_TRY( cudaMalloc( &m, bytes ) );
-	struct Free { char* p; ~Free() { cudaFree( p ); } } guard{ m };
+	TRY( sc.alloc( m, bytes ) );
 	float4* cur = (float4*)m, * saved = (float4*)(m + nb);
 	char* q = m + 2 * nb;
 	uint32_t* parent = (uint32_t*)q; q += w4;
@@ -330,11 +330,8 @@ int optimize_tree( tbvh_bvh b, const uint32_t max_rounds, const float c_trav, co
 	unsigned long long* thr = (unsigned long long*)(q + sizeof( OptRes ));
 	const uint32_t g = (n + 255) / 256;
 	OptRes h = {};
-	cudaEvent_t e0, e1;
-	CUDA_TRY( cudaEventCreate( &e0 ) );
-	CUDA_TRY( cudaEventCreate( &e1 ) );
-	struct Ev { cudaEvent_t a, b; ~Ev() { cudaEventDestroy( a ), cudaEventDestroy( b ); } } evs{ e0, e1 };
-	CUDA_TRY( cudaEventRecord( e0, s ) );
+	TRY( sc.events() );
+	CUDA_TRY( cudaEventRecord( sc.e0, s ) );
 	auto settle = [&]() -> int // parents, refold + SAH + depth, and the round's one host synchronisation
 	{
 		k_opt_parents<<<g, 256, 0, s>>>( cur, parent, n ); LAUNCHED();
@@ -400,9 +397,9 @@ int optimize_tree( tbvh_bvh b, const uint32_t max_rounds, const float c_trav, co
 		}
 		*out = o, *used = 2 + 2 * h.interior, *depth = best_depth;
 	}
-	CUDA_TRY( cudaEventRecord( e1, s ) );
-	CUDA_TRY( cudaEventSynchronize( e1 ) );
-	CUDA_TRY( cudaEventElapsedTime( ms, e0, e1 ) );
+	CUDA_TRY( cudaEventRecord( sc.e1, s ) );
+	CUDA_TRY( cudaEventSynchronize( sc.e1 ) );
+	CUDA_TRY( cudaEventElapsedTime( ms, sc.e0, sc.e1 ) );
 	*rounds = accepted, *sah = best;
 	return TBVH_OK;
 }
