@@ -193,7 +193,11 @@ int tbvh_build_batch_hq( tbvh_bvh* bvhs, const tbvh_mesh* meshes, uint32_t count
  * TBVH_E_STATE, and so is walking a TLAS after one of its BLASses was rebuilt, re-converted, re-uploaded or destroyed.
  * The two-level kernel walks a BVH-layout BLAS with a 64-entry stack: a BLAS whose BVH2 has depth 64 or more is refused
  * (TBVH_E_LIMIT) unless it also holds its CWBVH; then the TLAS is built, walks in TBVH_LAYOUT_CWBVH run, and walks in
- * TBVH_LAYOUT_BVH are refused with TBVH_E_LIMIT. */
+ * TBVH_LAYOUT_BVH are refused with TBVH_E_LIMIT.
+ * Refusals (TBVH_E_ARG for bad arguments, a NULL BLAS or one from another context, or an instance naming a BLAS past blas_count;
+ * TBVH_E_STATE / TBVH_E_LIMIT for the BLAS states above) come before the handle is touched: a refused call leaves the handle, and
+ * any TLAS it held, as they were.  Any later failure - a TLAS deeper than the 64-entry stack of IntersectTLAS (TBVH_E_LIMIT), or a
+ * CUDA error - leaves the handle empty, as a failed build does. */
 /* BVH::SAHCost( 0 ) tiny_bvh.h:1889-1897: the tree's SAH cost, host recursion over the (downloaded) 32-byte node array in the
  * reference's own order and rounding - the number the speedtest prints after every build.  _nodes works on a host array. */
 int tbvh_sah_cost( tbvh_bvh bvh, float c_trav, float c_int, float* out );
@@ -250,7 +254,7 @@ int tbvh_build_tlas( tbvh_bvh tlas, const void* instances, uint32_t inst_stride,
  * state decides - handles, counts, stride, the state and limits of the BLASses, and for host records blasIdx < blas_count - is checked
  * before the handle is touched: a refused call leaves a walkable TLAS walkable and the records as they were.  In device records
  * blasIdx is checked by the kernel, which never dereferences an index past the list: TBVH_E_ARG, the handle left empty as after a
- * failed build, the records unspecified.
+ * failed build, the records unspecified.  Every other failure leaves the handle empty too, as for tbvh_build_tlas.
  * A handle that already is a TLAS over the same inst_count and blas_count keeps its instance boxes, instance and BLAS tables and the
  * staging of host records; what a frame still allocates is the builder's own (the node and primIdx arrays and its scratch). */
 int tbvh_build_tlas_update( tbvh_bvh tlas, void* instances, uint32_t inst_stride, uint32_t inst_count, int space, const tbvh_bvh* blasses,

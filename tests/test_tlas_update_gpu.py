@@ -241,13 +241,23 @@ def test_refusals_leave_the_tlas_and_the_records(gpu):
         assert call() == code, f"{what}: {L.tbvh_last_error()}"
         assert rec.tobytes() == fresh.tobytes() and dev.cpu().numpy().tobytes() == fresh.tobytes(), f"{what}: the records changed"
         assert snapshot(t) == before and walks(t, O, D, (api.LAYOUT_BVH,)) == walked, f"{what}: the TLAS on the handle changed"
-    # tbvh_build_tlas gives the same codes
-    scratch = api.TLAS()
+    # tbvh_build_tlas gives the same codes, and it too leaves the TLAS on the handle as it was
     hs2 = lambda h: (C.c_void_p * len(h))(*h)
-    assert L.tbvh_build_tlas(scratch.h, p, 192, n, hs2([blas[0].h, None]), 2, 1.0, 1.0) == _lib.E_ARG
-    assert L.tbvh_build_tlas(scratch.h, p, 192, n, hs2([blas[0].h, other.h]), 2, 1.0, 1.0) == _lib.E_STATE
-    assert L.tbvh_build_tlas(scratch.h, inst.ctypes.data, 192, n, hs2(hs[:1]), 1, 1.0, 1.0) == _lib.E_ARG
-    assert L.tbvh_build_tlas(scratch.h, three.ctypes.data, 192, 3, hs2([deep.h]), 1, 1.0, 1.0) == _lib.E_LIMIT
+    cases = [
+        ("NULL BLAS", lambda: L.tbvh_build_tlas(t.h, p, 192, n, hs2([blas[0].h, None]), 2, 1.0, 1.0), _lib.E_ARG),
+        ("the TLAS as its own BLAS", lambda: L.tbvh_build_tlas(t.h, p, 192, n, hs2([blas[0].h, t.h]), 2, 1.0, 1.0), _lib.E_ARG),
+        ("a TLAS as BLAS", lambda: L.tbvh_build_tlas(t.h, p, 192, n, hs2([blas[0].h, other.h]), 2, 1.0, 1.0), _lib.E_STATE),
+        ("an empty BLAS", lambda: L.tbvh_build_tlas(t.h, p, 192, n, hs2([blas[0].h, empty.h]), 2, 1.0, 1.0), _lib.E_STATE),
+        ("blasIdx past the list", lambda: L.tbvh_build_tlas(t.h, past.ctypes.data, 192, n, hs2(hs), 2, 1.0, 1.0), _lib.E_ARG),
+        ("fewer BLASes than blasIdx names", lambda: L.tbvh_build_tlas(t.h, inst.ctypes.data, 192, n, hs2(hs[:1]), 1, 1.0, 1.0), _lib.E_ARG),
+        ("stride below 160", lambda: L.tbvh_build_tlas(t.h, p, 156, n, hs2(hs), 2, 1.0, 1.0), _lib.E_ARG),
+        ("no instances", lambda: L.tbvh_build_tlas(t.h, p, 192, 0, hs2(hs), 2, 1.0, 1.0), _lib.E_ARG),
+        ("NULL records", lambda: L.tbvh_build_tlas(t.h, None, 192, n, hs2(hs), 2, 1.0, 1.0), _lib.E_ARG),
+        ("deep BLAS without its CWBVH", lambda: L.tbvh_build_tlas(t.h, three.ctypes.data, 192, 3, hs2([deep.h]), 1, 1.0, 1.0), _lib.E_LIMIT),
+    ]
+    for what, call, code in cases:
+        assert call() == code, f"tbvh_build_tlas, {what}: {L.tbvh_last_error()}"
+        assert snapshot(t) == before and walks(t, O, D, (api.LAYOUT_BVH,)) == walked, f"tbvh_build_tlas, {what}: the TLAS on the handle changed"
     # device records: blasIdx is the kernel's to check - reported, never dereferenced, and the handle ends up empty
     bad = torch.from_numpy(past.view(np.uint8).reshape(n, 192)).cuda()
     torch.cuda.synchronize()

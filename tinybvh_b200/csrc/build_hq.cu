@@ -1224,9 +1224,9 @@ int build_hq_launch( const tbvh_bvh* bs, const uint32_t K, float c_trav, float c
 	{
 		const tbvh_bvh b = bs[t];
 		const uint32_t nt = T[t].n, it = nt + (nt >> 1);
-		CUDA_TRY( cudaMalloc( &b->d_nodes, ((size_t)3 * nt + 2) * 32 ) );
-		CUDA_TRY( cudaMalloc( &b->d_prim_idx, (size_t)it * 4 ) );
-		CUDA_TRY( cudaMalloc( &b->d_leaf_tris, (size_t)it * 48 ) ); b->leaf_tris_count = it;
+		TRY( b->d_nodes.alloc( ((size_t)3 * nt + 2) * 32 ) );
+		TRY( b->d_prim_idx.alloc( (size_t)it * 4 ) );
+		TRY( b->d_leaf_tris.alloc( (size_t)it * 48 ) ); b->leaf_tris_count = it;
 		T[t].out_nodes = b->d_nodes, T[t].out_idx = b->d_prim_idx, T[t].leaf_tris = b->d_leaf_tris;
 	}
 	Scratch sc( s );

@@ -287,9 +287,9 @@ int build_ploc_launch( const tbvh_bvh* bs, const uint32_t trees, const float c_t
 	{
 		const tbvh_bvh b = bs[t];
 		const size_t nt = b->info.prim_count;
-		CUDA_TRY( cudaMalloc( &b->d_nodes, (2 * nt + 2) * 32 ) );
-		CUDA_TRY( cudaMalloc( &b->d_prim_idx, nt * 4 ) );
-		CUDA_TRY( cudaMalloc( &b->d_leaf_tris, nt * 48 ) );
+		TRY( b->d_nodes.alloc( (2 * nt + 2) * 32 ) );
+		TRY( b->d_prim_idx.alloc( nt * 4 ) );
+		TRY( b->d_leaf_tris.alloc( nt * 48 ) );
 		b->leaf_tris_count = (uint32_t)nt;
 	}
 	Scratch sc( s );

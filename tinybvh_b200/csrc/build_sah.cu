@@ -1296,9 +1296,9 @@ int build_sah_launch( const tbvh_bvh* bs, const uint32_t trees, float c_trav, fl
 	{
 		const tbvh_bvh b = bs[t];
 		const size_t nt = b->info.prim_count;
-		CUDA_TRY( cudaMalloc( &b->d_nodes, (2 * nt + 2) * 32 ) );
-		CUDA_TRY( cudaMalloc( &b->d_prim_idx, nt * 4 ) );
-		if (!b->d_aabbs) { CUDA_TRY( cudaMalloc( &b->d_leaf_tris, nt * 48 ) ); b->leaf_tris_count = (uint32_t)nt; } // a TLAS has no triangles of its own
+		TRY( b->d_nodes.alloc( (2 * nt + 2) * 32 ) );
+		TRY( b->d_prim_idx.alloc( nt * 4 ) );
+		if (!b->d_aabbs) { TRY( b->d_leaf_tris.alloc( nt * 48 ) ); b->leaf_tris_count = (uint32_t)nt; } // a TLAS has no triangles of its own
 		io[t] = TreeIO{ b->d_verts, b->d_nodes, b->d_prim_idx, b->d_leaf_tris };
 	}
 	A.idx_final = bs[0]->d_prim_idx; // one tree: the leaves write the handle's primIdx directly

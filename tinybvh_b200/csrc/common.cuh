@@ -47,14 +47,41 @@ struct Scratch
 	int events() { CUDA_TRY( cudaEventCreate( &e0 ) ); CUDA_TRY( cudaEventCreate( &e1 ) ); return TBVH_OK; }
 };
 
+// ---- the owner of one allocation that outlives a call: one cudaMalloc (HOST: one page-locked block), freed when the owner is reset,
+// reassigned or destroyed.  It frees on the current device: whoever releases it sets the device first, and drains any stream whose
+// queued work may still read it.  bytes: the size of the block (reserve keeps it while a request fits).
+template <bool HOST> struct Owned
+{
+	void* p = 0;
+	size_t bytes = 0;
+	Owned() = default;
+	Owned( Owned&& o ) noexcept : p( o.p ), bytes( o.bytes ) { o.p = 0, o.bytes = 0; }
+	Owned& operator=( Owned&& o ) noexcept { if (this != &o) { reset(); p = o.p, bytes = o.bytes, o.p = 0, o.bytes = 0; } return *this; }
+	~Owned() { reset(); }
+	void reset() { if (p) { if (HOST) cudaFreeHost( p ); else cudaFree( p ); } p = 0, bytes = 0; }
+	int alloc( size_t n )
+	{
+		reset();
+		void* q = 0;
+		CUDA_TRY( HOST ? cudaMallocHost( &q, n ) : cudaMalloc( &q, n ) );
+		p = q, bytes = n;
+		return TBVH_OK;
+	}
+	int reserve( size_t n ) { return n <= bytes ? TBVH_OK : alloc( n + n / 4 ); } // grown with a quarter of headroom, so a steady state allocates nothing
+	void adopt( void* q, size_t n ) { reset(); p = q, bytes = n; }              // a block allocated elsewhere (HOST: cudaHostAlloc on a NUMA node)
+};
+typedef Owned<false> DevMem;
+typedef Owned<true> HostMem;
+template <class T> struct DevArray : DevMem { T* get() const { return (T*)p; } operator T*() const { return get(); } };
+
 // ---- handles ----------------------------------------------------------------------------------------------
 // one stage buffer set of the host-buffer pipeline (api.cu "host path")
 struct HostSlot
 {
-	void* d_rays = 0;                // chunk of 64-byte device records
-	void* d_hits = 0;                // packed 16-byte hits of the chunk
-	void* d_bits = 0;                // occlusion words of the chunk
-	void* h_hits = 0;                // page-locked staging for the chunk's packed hits (d2h_mode 2: scattered into the records by host threads)
+	DevArray<char> d_rays;           // chunk of 64-byte device records
+	DevArray<float4> d_hits;         // packed 16-byte hits of the chunk
+	DevArray<uint32_t> d_bits;       // occlusion words of the chunk
+	HostMem h_hits;                  // page-locked staging for the chunk's packed hits (d2h_mode 2: scattered into the records by host threads)
 	cudaEvent_t in_done = 0, run_done = 0, out_done = 0;
 };
 #define TBVH_SLOTS 4
@@ -92,17 +119,17 @@ struct tbvh_ctx_t
 	int build_mode = 0;              // BVH::Build large phase: 0 = one persistent cooperative launch (k_large_phase), 1 = one launch per stage and level
 	// ring of 8-byte device counters for kernels that pull work from a counter (one per launch, so launches on different
 	// streams never share one)
-	unsigned long long* d_counters = 0;
+	DevArray<unsigned long long> d_counters;
 	std::atomic<uint32_t> counter_next{ 0 };
 	// refits (convert_cwbvh.cu refit_trees): tables and scratch of one call, kept and grown, so a steady-state frame allocates nothing
 	std::mutex refit_mutex;
-	void* refit_dev = 0; size_t refit_dev_bytes = 0;   // device: tables, arrival counters, parents, BVH_GPU workspace, results
-	void* refit_host = 0; size_t refit_host_bytes = 0; // page-locked: the tables on their way in, the results on their way out
+	DevArray<char> refit_dev;        // device: tables, arrival counters, parents, BVH_GPU workspace, results
+	HostMem refit_host;              // page-locked: the tables on their way in, the results on their way out
 	cudaEvent_t refit_e0 = 0, refit_e1 = 0;
 	// indexed refits (api.cu tbvh_refit_batch_indexed): the new vertices of the call's indexed meshes at a 16-byte pitch and the gather
 	// table, kept and grown; the mutex is held for the whole call (the refit inside it takes refit_mutex)
 	std::mutex ix_mutex;
-	void* ix_dev = 0; size_t ix_dev_bytes = 0;
+	DevArray<char> ix_dev;
 };
 #define TBVH_COUNTERS 256
 
@@ -114,37 +141,39 @@ struct tbvh_bvh_t
 	tbvh_ctx ctx = 0;
 	tbvh_info info = {};
 	// geometry (engine-owned copy, float4 per vertex)
-	float4* d_verts = 0;
+	DevArray<float4> d_verts;
 	// indexed, refittable builds: the 3 * prim_count vertex indices and the vertex count (BVHBase::vertIdx, tiny_bvh.h:806-807), through
 	// which tbvh_refit_batch_indexed writes d_verts from the new positions.  Dropped with the tree (free_layouts); 0 otherwise.
-	uint32_t* d_vert_idx = 0;
+	DevArray<uint32_t> d_vert_idx;
 	uint32_t vert_count = 0;
 	// LAYOUT_BVH: reference node array; children of an interior node are the 64-byte pair at nodes[leftFirst]
-	float4* d_nodes = 0;       // 2 float4 per node
-	uint32_t* d_prim_idx = 0;
-	// traversal view of the BVH2: d_trav aliases d_nodes (LAYOUT_BVH) or is the pair array derived from a BVH_GPU upload
-	float4* d_trav = 0;
+	DevArray<float4> d_nodes;  // 2 float4 per node
+	DevArray<uint32_t> d_prim_idx;
+	// the child-pair array derived from a BVH_GPU upload (convert.cu bvh_gpu_to_bvh); empty otherwise
+	DevArray<float4> d_pairs;
+	// traversal view of the BVH2: the pair array of a BVH_GPU upload, else d_nodes (LAYOUT_BVH)
+	float4* trav() const { return d_pairs.p ? d_pairs : d_nodes; }
 	uint32_t root_ref = 0, root_count = 0; // the root as a child record: count==0 -> pair index, else leaf range
 	// leaf-ordered triangle records for BVH2 traversal: 3 float4 per prim reference
 	//   [0] = (v0.xyz, as_float(primIdx))  [1] = e1 = v1-v0  [2] = e2 = v2-v0
-	float4* d_leaf_tris = 0;
+	DevArray<float4> d_leaf_tris;
 	uint32_t leaf_tris_count = 0; // records d_leaf_tris was allocated for
 	// LAYOUT_BVH_GPU mirror (only materialised on upload / convert / download)
-	float4* d_nodes_gpu = 0;   // 4 float4 per node
+	DevArray<float4> d_nodes_gpu; // 4 float4 per node
 	// LAYOUT_CWBVH
-	float4* d_cw_nodes = 0;    // 5 float4 per node
-	float4* d_cw_tris = 0;     // 3 float4 per triangle
-	float4* d_cw_trav = 0;     // traversal nodes derived from d_cw_nodes (trace_cwbvh.cu cw_make_trav): 10 float4 per node
+	DevArray<float4> d_cw_nodes;  // 5 float4 per node
+	DevArray<float4> d_cw_tris;   // 3 float4 per triangle
+	DevArray<float4> d_cw_trav;   // traversal nodes derived from d_cw_nodes (trace_cwbvh.cu cw_make_trav): 10 float4 per node
 	uint32_t cw_pending = 0;   // most node groups a walk of the wide tree can leave pending (trace_cwbvh.cu k_cw_pending)
 	float cw_rd_limit = -1.0f; // rays with |rD| up to this (and |O| <= 2^126) take the integer-ordered slab test (cw_walk.cuh cw_ray_fits); < 0: none
 	uint32_t generation = 0;   // renewed (tbvh_next_generation) whenever the arrays a TLAS may point at are replaced (build, upload, refit, convert)
 	uint32_t revision = 0;     // counts refits: a refit that drops no layout rewrites the BVH2 arrays in place under the same generation, and a
 	                           // group's scene replicas (multi.cu) must notice that too
 	// TLAS (BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) :2221): nodes / primIdx over instance boxes + device tables
-	float4* d_aabbs = 0;       // instance boxes the TLAS was built over (2 float4 per instance)
-	void* d_inst = 0;          // TlasInst records (inverse transform, BLAS number, mask)
-	void* d_blas = 0;          // BlasRef records (traversal arrays of every BLAS); tbvh_build_tlas_update: then each BLAS's root box and a flag word
-	void* d_inst_stage = 0;    // tbvh_build_tlas_update with host records: bytes 0..159 of every record on their way through the device
+	DevArray<float4> d_aabbs;  // instance boxes the TLAS was built over (2 float4 per instance)
+	DevArray<TlasInst> d_inst; // TlasInst records (inverse transform, BLAS number, mask)
+	DevArray<char> d_blas;     // BlasRef records (traversal arrays of every BLAS); tbvh_build_tlas_update: then each BLAS's root box and a flag word
+	DevArray<char> d_inst_stage; // tbvh_build_tlas_update with host records: bytes 0..159 of every record on their way through the device
 	size_t blas_table_bytes = 0; // bytes of d_blas when tbvh_build_tlas_update made it (0: tbvh_build_tlas's, BlasRef records only)
 	uint32_t inst_count = 0, blas_count = 0;
 	uint32_t tlas_blas_layouts = 0; // TLAS only: layouts EVERY BLAS held at build time (bit TBVH_LAYOUT_BVH / TBVH_LAYOUT_CWBVH)
@@ -156,7 +185,7 @@ struct tbvh_bvh_t
 	struct CwKeep* cw_keep = 0; // refittable trees: the 8-wide collapse of the last tbvh_convert to CWBVH (convert_cwbvh.cu), for tbvh_refit_layouts
 	// statistics
 	int stats = 0;
-	unsigned long long* d_stats = 0; // [0]=steps [1]=tris, accumulated over every launch of one API call
+	DevArray<unsigned long long> d_stats; // [0]=steps [1]=tris, accumulated over every launch of one API call
 };
 
 // any-hit result of a one-ray-per-thread kernel: one ballot word per warp.  blockDim is a multiple of 32 and i is the global thread
@@ -324,8 +353,8 @@ void drop_bvh_gpu( tbvh_bvh b );                  // the BVH_GPU array, its bit 
 int bvh_to_cwbvh( const tbvh_bvh* bs, uint32_t K, cudaStream_t s );
 // the CWBVH arrays, the kept collapse, the bit, the counts and the traversal limits; a TLAS over the arrays becomes stale
 void drop_cwbvh( tbvh_bvh b );
-// tbvh_optimize's rounds over b's BVH-layout tree (optimize.cu).  Writes nothing when *rounds ends 0; else *out is a new allocation
+// tbvh_optimize's rounds over b's BVH-layout tree (optimize.cu).  Writes nothing when *rounds ends 0; else out is a new allocation
 // holding the renumbered tree (*used nodes, depth *depth), *sah its SAHCost and *ms the device time of the call.
-int optimize_tree( tbvh_bvh b, uint32_t max_rounds, float c_trav, float c_int, float4** out, uint32_t* used, uint32_t* depth, uint32_t* rounds, float* sah, float* ms );
+int optimize_tree( tbvh_bvh b, uint32_t max_rounds, float c_trav, float c_int, DevArray<float4>& out, uint32_t* used, uint32_t* depth, uint32_t* rounds, float* sah, float* ms );
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)
 int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint32_t n, cudaStream_t s );

@@ -34,8 +34,9 @@ int leaf_tris_alloc( tbvh_bvh b )
 {
 	const uint32_t n = b->info.idx_count;
 	// a refit keeps the array (same idx_count): a TLAS holding its address stays valid
-	if (b->d_leaf_tris && b->leaf_tris_count != n) { cudaFree( b->d_leaf_tris ); b->d_leaf_tris = 0; }
-	if (!b->d_leaf_tris) { CUDA_TRY( cudaMalloc( &b->d_leaf_tris, (size_t)n * 48 ) ); b->leaf_tris_count = n; b->generation = tbvh_next_generation(); }
+	if (b->d_leaf_tris && b->leaf_tris_count == n) return TBVH_OK;
+	TRY( b->d_leaf_tris.alloc( (size_t)n * 48 ) );
+	b->leaf_tris_count = n, b->generation = tbvh_next_generation();
 	return TBVH_OK;
 }
 
@@ -45,19 +46,13 @@ int make_leaf_tris( tbvh_bvh b, cudaStream_t s )
 	// the tree as a one-entry table; an upload synchronises right after, so the table lives for the call only
 	RfTree entry = {};
 	entry.prim_idx = b->d_prim_idx, entry.verts = b->d_verts, entry.leaf_tris = b->d_leaf_tris;
+	Scratch sc( s );
 	RfTree* d_T = 0;
-	CUDA_TRY( cudaMalloc( &d_T, sizeof( RfTree ) ) );
-	auto body = [&]() -> int
-	{
-		CUDA_TRY( cudaMemcpyAsync( d_T, &entry, sizeof( RfTree ), cudaMemcpyHostToDevice, s ) );
-		TRY( leaf_tris_enqueue( d_T, 1, b->info.idx_count, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		return TBVH_OK;
-	};
-	const int rc = body();
-	cudaStreamSynchronize( s );
-	cudaFree( d_T );
-	return rc;
+	TRY( sc.alloc( d_T, sizeof( RfTree ) ) );
+	CUDA_TRY( cudaMemcpyAsync( d_T, &entry, sizeof( RfTree ), cudaMemcpyHostToDevice, s ) );
+	TRY( leaf_tris_enqueue( d_T, 1, b->info.idx_count, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	return TBVH_OK;
 }
 
 // one thread per Aila-Laine node i; an interior node writes its children as the pair at slots 2i, 2i+1:
@@ -81,11 +76,9 @@ __global__ void k_bvh_gpu_to_pairs( const float4* __restrict__ g, float4* __rest
 
 int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used, cudaStream_t s )
 {
-	float4* pairs = 0;
-	CUDA_TRY( cudaMalloc( &pairs, (size_t)used * 64 ) );
-	k_bvh_gpu_to_pairs<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes_gpu, pairs, used );
+	TRY( b->d_pairs.alloc( (size_t)used * 64 ) );
+	k_bvh_gpu_to_pairs<<<(used + 255) / 256, 256, 0, s>>>( b->d_nodes_gpu, b->d_pairs, used );
 	LAUNCHED();
-	b->d_trav = pairs;
 	return TBVH_OK;
 }
 
@@ -173,8 +166,7 @@ int bvh_gpu_enqueue( const GpuTree* d_T, const uint32_t K, const uint32_t n, uin
 
 void drop_bvh_gpu( tbvh_bvh b )
 {
-	if (b->d_nodes_gpu) cudaFree( b->d_nodes_gpu );
-	b->d_nodes_gpu = 0;
+	b->d_nodes_gpu.reset();
 	b->info.layouts &= ~(1u << TBVH_LAYOUT_BVH_GPU), b->info.used_nodes_gpu = 0;
 }
 
@@ -182,22 +174,22 @@ int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s )
 {
 	const uint32_t used = b->info.used_nodes;
 	drop_bvh_gpu( b );
-	uint32_t* w = 0; // workspace: parent, arrive, sub_int, sub_leaves [used], then the tree as a one-entry table
 	const size_t words = (size_t)used * 4;
 	auto body = [&]() -> int
 	{
-		CUDA_TRY( cudaMalloc( &b->d_nodes_gpu, (size_t)used * 64 ) );
-		CUDA_TRY( cudaMalloc( &w, words * 4 + sizeof( GpuTree ) ) );
-		const GpuTree entry{ b->d_nodes, b->d_nodes_gpu, 0, used };
+		GpuTree entry;
+		Scratch sc( s );
+		TRY( b->d_nodes_gpu.alloc( (size_t)used * 64 ) );
+		uint32_t* w = 0; // workspace: parent, arrive, sub_int, sub_leaves [used], then the tree as a one-entry table
+		TRY( sc.alloc( w, words * 4 + sizeof( GpuTree ) ) );
+		entry = GpuTree{ b->d_nodes, b->d_nodes_gpu, 0, used };
 		GpuTree* const d_T = (GpuTree*)(w + words);
 		CUDA_TRY( cudaMemcpyAsync( d_T, &entry, sizeof( GpuTree ), cudaMemcpyHostToDevice, s ) );
 		TRY( bvh_gpu_enqueue( d_T, 1, used, w, s ) );
 		CUDA_TRY( cudaStreamSynchronize( s ) );
 		return TBVH_OK;
 	};
-	const int rc = body();
-	cudaStreamSynchronize( s );
-	cudaFree( w );
+	const int rc = body(); // the stream is drained and the workspace freed before a failure drops the BVH_GPU array
 	if (rc != TBVH_OK) drop_bvh_gpu( b );
 	else b->info.used_nodes_gpu = used - 1, b->info.layouts |= 1u << TBVH_LAYOUT_BVH_GPU; // node 1 of the Wald layout is unused
 	return rc;

@@ -54,25 +54,15 @@ struct CwKeep
 	bool leaf_root = false;                       // the wide root wraps a leaf root (MBVH<8>::ConvertFrom :5036)
 	std::vector<uint32_t> off;                    // level l holds wide nodes off[l] .. off[l+1]
 	// one allocation, at base, holds the four arrays of the collapse
-	uint32_t* base = 0;                           // used + 1: k_split_count scan, where each split leaf's chain goes
+	DevArray<uint32_t> base;                      // used + 1: k_split_count scan, where each split leaf's chain goes
 	uint32_t* list = 0;                           // wide_count: split-tree node of every wide node
 	uint32_t* adopt = 0;                          // wide_count * 8: its children in ADOPTION order (k_assign breaks ties by it)
 	uint32_t* ifirst = 0;                         // wide_count: wide node of its first interior child; the others follow
 	// refit scratch: allocated by the first refit, alone or in a batch, and kept until the CWBVH is dropped
-	float4* ext = 0;                              // total * 2: the split tree with the refitted boxes
-	WideNode* wide = 0;                           // wide_count
-	uint32_t* parent = 0;                         // used: BVH::Refit's parents (topology only), filled by the first refit
+	DevArray<float4> ext;                         // total * 2: the split tree with the refitted boxes
+	DevArray<WideNode> wide;                      // wide_count
+	DevArray<uint32_t> parent;                    // used: BVH::Refit's parents (topology only), filled by the first refit
 };
-
-static void cw_keep_free( tbvh_bvh b )
-{
-	CwKeep* k = b->cw_keep;
-	if (!k) return;
-	void* p[] = { k->base, k->ext, k->wide, k->parent }; // base also holds list, adopt and ifirst
-	for (void* q : p) if (q) cudaFree( q );
-	delete k;
-	b->cw_keep = 0;
-}
 
 // One tree of a conversion or of a refit that keeps its CWBVH (device table, indexed by tree).  Everything after the collapse works on
 // the tree's own arrays with tree-local numbers.
@@ -534,11 +524,9 @@ static int cw_assign_encode( const CwTree* d_T, const uint32_t K, const CwLevels
 void drop_cwbvh( tbvh_bvh b )
 {
 	if (b->d_cw_trav || b->d_cw_tris) b->generation = tbvh_next_generation(); // a TLAS may hold these addresses (api.cu tlas_check)
-	if (b->d_cw_nodes) cudaFree( b->d_cw_nodes );
-	if (b->d_cw_tris) cudaFree( b->d_cw_tris );
-	if (b->d_cw_trav) cudaFree( b->d_cw_trav );
-	b->d_cw_nodes = 0, b->d_cw_tris = 0, b->d_cw_trav = 0;
-	cw_keep_free( b );
+	b->d_cw_nodes.reset(), b->d_cw_tris.reset(), b->d_cw_trav.reset();
+	delete b->cw_keep; // its arrays free themselves
+	b->cw_keep = 0;
 	b->info.layouts &= ~(1u << TBVH_LAYOUT_CWBVH), b->info.used_blocks = 0, b->info.cwbvh_tri_count = 0;
 	b->cw_pending = 0, b->cw_rd_limit = -1.0f;
 }
@@ -660,8 +648,8 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		{
 			const tbvh_bvh b = bs[t];
 			const uint32_t wc = toff[t].back(), used = b->info.used_nodes;
-			CUDA_TRY( cudaMalloc( &b->d_cw_nodes, (size_t)wc * 80 ) );
-			CUDA_TRY( cudaMalloc( &b->d_cw_tris, (size_t)b->info.idx_count * 48 ) );
+			TRY( b->d_cw_nodes.alloc( (size_t)wc * 80 ) );
+			TRY( b->d_cw_tris.alloc( (size_t)b->info.idx_count * 48 ) );
 			T[t].cw_nodes = b->d_cw_nodes, T[t].cw_tris = b->d_cw_tris, T[t].wbase = wb, T[t].wide_count = wc, T[t].leaf_root = h_leaf[t] != 0;
 			wb += wc;
 			b->info.used_blocks = wc * 5, b->info.cwbvh_tri_count = b->info.idx_count;
@@ -671,7 +659,7 @@ int bvh_to_cwbvh( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 			if (!k) { tbvh_set_error( "CWBVH conversion: out of host memory" ); return TBVH_E_ARG; }
 			b->cw_keep = k;
 			k->used = used, k->total = ext_base[t + 1] - ext_base[t], k->wide_count = wc, k->leaf_root = h_leaf[t] != 0, k->off = toff[t];
-			CUDA_TRY( cudaMalloc( &k->base, ((size_t)used + 1 + (size_t)wc * 10) * 4 ) );
+			TRY( k->base.alloc( ((size_t)used + 1 + (size_t)wc * 10) * 4 ) );
 			k->list = k->base + used + 1, k->adopt = k->list + wc, k->ifirst = k->adopt + (size_t)wc * 8;
 			T[t].keep = k->base;
 		}
@@ -723,20 +711,8 @@ void cw_keep_sizes( tbvh_bvh b, uint32_t* total, uint32_t* wide_count )
 // one upload, one read-back, one host synchronisation.
 static int refit_space( tbvh_ctx c, const size_t dev, const size_t host )
 {
-	if (dev > c->refit_dev_bytes)
-	{
-		if (c->refit_dev) cudaFree( c->refit_dev );
-		c->refit_dev = 0, c->refit_dev_bytes = 0;
-		CUDA_TRY( cudaMalloc( &c->refit_dev, dev + dev / 4 ) );
-		c->refit_dev_bytes = dev + dev / 4;
-	}
-	if (host > c->refit_host_bytes)
-	{
-		if (c->refit_host) cudaFreeHost( c->refit_host );
-		c->refit_host = 0, c->refit_host_bytes = 0;
-		CUDA_TRY( cudaMallocHost( &c->refit_host, host + host / 4 ) );
-		c->refit_host_bytes = host + host / 4;
-	}
+	TRY( c->refit_dev.reserve( dev ) );
+	TRY( c->refit_host.reserve( host ) );
 	if (!c->refit_e0) CUDA_TRY( cudaEventCreate( &c->refit_e0 ) );
 	if (!c->refit_e1) CUDA_TRY( cudaEventCreate( &c->refit_e1 ) );
 	return TBVH_OK;
@@ -770,9 +746,9 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 		{
 			CwKeep* k = bs[t]->cw_keep;
 			fill[t] = !k->parent;
-			if (!k->ext) CUDA_TRY( cudaMalloc( &k->ext, (size_t)k->total * 32 ) );
-			if (!k->wide) CUDA_TRY( cudaMalloc( &k->wide, (size_t)k->wide_count * sizeof( WideNode ) ) );
-			if (!k->parent) CUDA_TRY( cudaMalloc( &k->parent, (size_t)k->used * 4 ) );
+			if (!k->ext) TRY( k->ext.alloc( (size_t)k->total * 32 ) );
+			if (!k->wide) TRY( k->wide.alloc( (size_t)k->wide_count * sizeof( WideNode ) ) );
+			if (!k->parent) TRY( k->parent.alloc( (size_t)k->used * 4 ) );
 		}
 		// the batch levels: each tree's run of every level it reaches
 		std::vector<const std::vector<uint32_t>*> toff( KC );
@@ -787,7 +763,7 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 		const size_t o_arrive = take( (size_t)N * 4 ), res_words = (size_t)K * 8 + KC, o_res = take( res_words * 4 ), zeroed = carve - o_arrive;
 		const size_t o_parent = take( (size_t)N * 4 ), o_gw = take( (size_t)NG * 16 );
 		TRY( refit_space( c, carve, tables + res_words * 4 ) );
-		char* const dev = (char*)c->refit_dev, * const host = (char*)c->refit_host;
+		char* const dev = c->refit_dev, * const host = (char*)c->refit_host.p;
 		uint32_t* const res = (uint32_t*)(dev + o_res), * const h_res = (uint32_t*)(host + tables);
 		RfTree* const rf = (RfTree*)(host + o_rf);
 		CwTree* const cr = (CwTree*)(host + o_cr);
@@ -808,7 +784,7 @@ int refit_trees( const tbvh_bvh* bs, const uint32_t K, const bool keep_layouts, 
 			CwKeep* k = b->cw_keep;
 			cr[i] = CwTree{ b->d_nodes, b->d_prim_idx, b->d_verts, b->d_cw_nodes, b->d_cw_tris, k->ext, k->base, k->list, k->adopt, k->ifirst, k->wide, 0, 0,
 				nb, k->used, wb, k->wide_count, k->leaf_root ? 1u : 0u };
-			ct[i] = CwTrav{ (const uint4*)b->d_cw_nodes, (uint4*)b->d_cw_trav, res + (size_t)K * 8 + i, wb, k->wide_count };
+			ct[i] = CwTrav{ (const uint4*)b->d_cw_nodes.p, (uint4*)b->d_cw_trav.p, res + (size_t)K * 8 + i, wb, k->wide_count };
 			nb += k->used, wb += k->wide_count;
 		}
 		for (uint32_t i = 0, nb = 0; i < KG; i++)

@@ -29,7 +29,7 @@ struct SceneBlas
 };
 
 // what one destination context keeps between calls: the copy kernel's table on the device and its host image
-struct CopyScratch { void* d = 0; size_t d_bytes = 0; std::vector<char> h; };
+struct CopyScratch { DevArray<char> d; std::vector<char> h; };
 
 struct tbvh_group_t
 {
@@ -52,18 +52,18 @@ static void release_replicas( tbvh_group g )
 }
 
 // ---- what a replica carries -------------------------------------------------------------------------------------------------------
-// The device arrays of handle `src` a replica takes, each as (where handle h keeps its address, bytes).  With h = src the list names
-// the source arrays; with h = the replica, the slots to fill, in the same order (presence and sizes come from src alone).
+// The device arrays of handle `src` a replica takes, each as (handle h's owner of it, bytes).  With h = src the list names the source
+// arrays; with h = the replica, the owners to allocate, in the same order (presence and sizes come from src alone).
 //   ARR_TREE      a plain-BVH replica: everything a walk in any layout reads, plus vertices and primIdx
-//   ARR_BLAS_BVH  what the two-level walk reads of a BLAS's BVH2 (its BlasRef trav / tris): the pair array and the leaf triangles
+//   ARR_BLAS_BVH  what the two-level walk reads of a BLAS's BVH2 (its BlasRef trav / tris): trav() and the leaf triangles
 //   ARR_BLAS_CW   ... of its CWBVH (cw_nodes / cw_tris): the traversal nodes and bvh8Tris
 //   ARR_TLAS      a TLAS's own node array, primIdx and instance table (its BLAS table is made for the replica, not copied)
 enum { ARR_TREE = 1, ARR_BLAS_BVH = 2, ARR_BLAS_CW = 4, ARR_TLAS = 8 };
-struct HandleArray { void** at; size_t bytes; };
+struct HandleArray { DevMem* at; size_t bytes; };
 
-template <class T> static void add_array( std::vector<HandleArray>& a, const tbvh_bvh src, tbvh_bvh h, T* tbvh_bvh_t::* m, const size_t bytes )
+template <class M> static void add_array( std::vector<HandleArray>& a, const tbvh_bvh src, tbvh_bvh h, M tbvh_bvh_t::* m, const size_t bytes )
 {
-	if (src->*m && bytes) a.push_back( HandleArray{ (void**)&(h->*m), bytes } );
+	if ((src->*m).p && bytes) a.push_back( HandleArray{ &(h->*m), bytes } );
 }
 
 static std::vector<HandleArray> handle_arrays( const tbvh_bvh src, tbvh_bvh h, const uint32_t what )
@@ -76,14 +76,15 @@ static std::vector<HandleArray> handle_arrays( const tbvh_bvh src, tbvh_bvh h, c
 		add_array( a, src, h, &tbvh_bvh_t::d_verts, (size_t)I.prim_count * 48 );
 		add_array( a, src, h, &tbvh_bvh_t::d_prim_idx, (size_t)I.idx_count * 4 );
 		add_array( a, src, h, &tbvh_bvh_t::d_nodes, nodes_b );
-		if (src->d_trav != src->d_nodes) add_array( a, src, h, &tbvh_bvh_t::d_trav, gpu_b ); // else the replica's d_trav aliases its d_nodes
+		add_array( a, src, h, &tbvh_bvh_t::d_pairs, gpu_b );
 		add_array( a, src, h, &tbvh_bvh_t::d_leaf_tris, (size_t)src->leaf_tris_count * 48 );
 		add_array( a, src, h, &tbvh_bvh_t::d_nodes_gpu, gpu_b );
 		add_array( a, src, h, &tbvh_bvh_t::d_cw_nodes, (size_t)I.used_blocks * 16 );
 	}
 	if (what & ARR_BLAS_BVH)
 	{
-		add_array( a, src, h, &tbvh_bvh_t::d_trav, src->d_trav == src->d_nodes ? nodes_b : gpu_b );
+		if (src->d_pairs.p) add_array( a, src, h, &tbvh_bvh_t::d_pairs, gpu_b );
+		else add_array( a, src, h, &tbvh_bvh_t::d_nodes, nodes_b );
 		add_array( a, src, h, &tbvh_bvh_t::d_leaf_tris, (size_t)src->leaf_tris_count * 48 );
 	}
 	if (what & (ARR_TREE | ARR_BLAS_CW))
@@ -151,13 +152,7 @@ static int copy_to( tbvh_group g, const size_t i, const int src_dev, std::vector
 	// the device image: the segment table, then the host data, which the table's last segment copies to tail_dst
 	CopyScratch& X = g->scratch[i];
 	const size_t K = segs.size() + (tail_bytes ? 1 : 0), tail_at = K * sizeof( CopySeg ), bytes = tail_at + tail_bytes;
-	if (bytes > X.d_bytes)
-	{
-		if (X.d) cudaFree( X.d );
-		X.d = 0, X.d_bytes = 0;
-		CUDA_TRY( cudaMalloc( &X.d, bytes + bytes / 4 ) );
-		X.d_bytes = bytes + bytes / 4;
-	}
+	TRY( X.d.reserve( bytes ) );
 	if (tail_bytes) segs.push_back( CopySeg{ (const char*)X.d + tail_at, (char*)tail_dst, tail_bytes, 0, 0 } );
 	uint32_t first = 0;
 	for (CopySeg& q : segs) q.first = first, first += (uint32_t)((q.bytes + 15) / 16);
@@ -167,7 +162,7 @@ static int copy_to( tbvh_group g, const size_t i, const int src_dev, std::vector
 	if (tail_bytes) memcpy( X.h.data() + tail_at, tail, tail_bytes );
 	CUDA_TRY( cudaMemcpyAsync( X.d, X.h.data(), bytes, cudaMemcpyHostToDevice, s ) );
 	const uint32_t grid = std::min<uint32_t>( (first + 255) / 256, (uint32_t)c->sm_count * 8 );
-	k_copy_segments<<<grid, 256, 0, s>>>( (const CopySeg*)X.d, (uint32_t)K, first );
+	k_copy_segments<<<grid, 256, 0, s>>>( (const CopySeg*)X.d.p, (uint32_t)K, first );
 	LAUNCHED();
 	return TBVH_OK;
 }
@@ -176,7 +171,7 @@ static int copy_to( tbvh_group g, const size_t i, const int src_dev, std::vector
 static void add_segments( std::vector<CopySeg>& segs, const tbvh_bvh src, tbvh_bvh h, const uint32_t what )
 {
 	const std::vector<HandleArray> from = handle_arrays( src, src, what ), to = handle_arrays( src, h, what );
-	for (size_t j = 0; j < from.size(); j++) segs.push_back( CopySeg{ (const char*)*from[j].at, (char*)*to[j].at, from[j].bytes, 0, 0 } );
+	for (size_t j = 0; j < from.size(); j++) segs.push_back( CopySeg{ (const char*)from[j].at->p, (char*)to[j].at->p, from[j].bytes, 0, 0 } );
 }
 
 // run fn( part ) on one worker thread per device, each bound to the CPUs of its device's NUMA node; first error wins
@@ -243,7 +238,7 @@ int tbvh_group_destroy( tbvh_group g )
 {
 	if (!g) return TBVH_OK;
 	release_replicas( g );
-	for (size_t i = 0; i < g->ctx.size(); i++) if (g->scratch[i].d) { cudaSetDevice( g->ctx[i]->device ); cudaFree( g->scratch[i].d ); }
+	for (size_t i = 0; i < g->ctx.size(); i++) if (g->scratch[i].d) { cudaSetDevice( g->ctx[i]->device ); g->scratch[i].d.reset(); }
 	for (auto& b : g->host_blocks) { cudaHostUnregister( b.first ); munmap( b.first, b.second ); }
 	for (tbvh_ctx c : g->ctx) tbvh_ctx_destroy( c );
 	delete g;
@@ -270,8 +265,7 @@ static int replicate_tree( tbvh_group g, tbvh_bvh src, bool& began )
 		g->replica.push_back( r ), g->owned.push_back( 1 );
 		r->info = src->info, r->root_ref = src->root_ref, r->root_count = src->root_count, r->refittable = src->refittable, r->cw_pending = src->cw_pending, r->cw_rd_limit = src->cw_rd_limit;
 		r->leaf_tris_count = src->d_leaf_tris ? src->leaf_tris_count : 0;
-		for (const HandleArray& a : handle_arrays( src, r, ARR_TREE )) CUDA_TRY( cudaMalloc( a.at, a.bytes ) );
-		if (src->d_trav == src->d_nodes) r->d_trav = r->d_nodes;
+		for (const HandleArray& a : handle_arrays( src, r, ARR_TREE )) TRY( a.at->alloc( a.bytes ) );
 		std::vector<CopySeg> segs;
 		add_segments( segs, src, r, ARR_TREE );
 		TRY( copy_to( g, i, src->ctx->device, segs, 0, 0, 0 ) );
@@ -356,7 +350,7 @@ static int replicate_scene( tbvh_group g, tbvh_bvh src, bool& began )
 			{
 				if (r) tbvh_bvh_destroy( r ), r = 0; // a new handle: a new generation for the replica TLAS's links
 				TRY( tbvh_bvh_create( c, &r ) );
-				for (const HandleArray& a : handle_arrays( e.src, r, what )) CUDA_TRY( cudaMalloc( a.at, a.bytes ) );
+				for (const HandleArray& a : handle_arrays( e.src, r, what )) TRY( a.at->alloc( a.bytes ) );
 			}
 			if (!fresh || changed[j]) add_segments( segs, e.src, r, what );
 			const tbvh_bvh b = e.src;
@@ -372,15 +366,15 @@ static int replicate_scene( tbvh_group g, tbvh_bvh src, bool& began )
 			TRY( tbvh_bvh_create( c, &t ) );
 			g->replica[i] = t, g->owned[i] = 1;
 			const size_t cap = src->inst_count;
-			CUDA_TRY( cudaMalloc( &t->d_nodes, (2 * cap + 2) * 32 ) ); // the builder's own allocation (build_sah.cu)
-			CUDA_TRY( cudaMalloc( &t->d_prim_idx, cap * 4 ) );
-			CUDA_TRY( cudaMalloc( &t->d_inst, cap * sizeof( TlasInst ) ) );
-			CUDA_TRY( cudaMalloc( &t->d_blas, (size_t)src->blas_count * sizeof( BlasRef ) ) );
+			TRY( t->d_nodes.alloc( (2 * cap + 2) * 32 ) ); // the builder's own allocation (build_sah.cu)
+			TRY( t->d_prim_idx.alloc( cap * 4 ) );
+			TRY( t->d_inst.alloc( cap * sizeof( TlasInst ) ) );
+			TRY( t->d_blas.alloc( (size_t)src->blas_count * sizeof( BlasRef ) ) );
 			g->tlas_cap[i] = src->inst_count;
 		}
 		g->replica[i] = t, g->owned[i] = 1;
 		add_segments( segs, src, t, ARR_TLAS );
-		t->info = src->info, t->root_ref = src->root_ref, t->root_count = src->root_count, t->d_trav = t->d_nodes, t->refittable = false;
+		t->info = src->info, t->root_ref = src->root_ref, t->root_count = src->root_count, t->refittable = false;
 		t->inst_count = src->inst_count, t->blas_count = src->blas_count;
 		for (uint32_t k = 0; k < nb; k++) hs[k] = g->blas[slot[k]].rep[i];
 		TlasBlasTable B;

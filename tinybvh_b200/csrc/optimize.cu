@@ -300,10 +300,10 @@ __global__ void k_opt_renumber( const float4* __restrict__ nd, const uint32_t* _
 
 // tbvh_optimize's device work (api.cu does the checks and the handle's bookkeeping).  On success with *rounds > 0, *out holds the
 // renumbered tree (*used nodes, depth *depth) in a new allocation the caller takes; with *rounds == 0 nothing was written anywhere.
-int optimize_tree( tbvh_bvh b, const uint32_t max_rounds, const float c_trav, const float c_int, float4** out, uint32_t* used, uint32_t* depth,
+int optimize_tree( tbvh_bvh b, const uint32_t max_rounds, const float c_trav, const float c_int, DevArray<float4>& out, uint32_t* used, uint32_t* depth,
 	uint32_t* rounds, float* sah, float* ms )
 {
-	*out = 0, *rounds = 0;
+	*rounds = 0;
 	const uint32_t n = b->info.used_nodes, L = std::max( b->info.max_depth, 63u );
 	cudaStream_t s = b->ctx->stream;
 	// scratch: the tree and its saved copy, per slot parent / depth / height / arrival / candidate / won / list words, area and
@@ -383,8 +383,8 @@ int optimize_tree( tbvh_bvh b, const uint32_t max_rounds, const float c_trav, co
 		if (restored) { k_opt_parents<<<g, 256, 0, s>>>( cur, parent, n ); LAUNCHED(); }
 		CUDA_TRY( cudaMemsetAsync( arrive, 0, (size_t)n * 4, s ) );
 		k_opt_sizes<<<g, 256, 0, s>>>( cur, parent, arrive, dep, cand, n ); LAUNCHED();
-		float4* o = 0;
-		CUDA_TRY( cudaMalloc( &o, nb ) );
+		DevArray<float4> o;
+		TRY( o.alloc( nb ) );
 		k_opt_renumber<<<g, 256, 0, s>>>( cur, parent, dep, cand, o, res, n );
 		const cudaError_t le = cudaGetLastError();
 		g_tbvh_launches++;
@@ -392,10 +392,9 @@ int optimize_tree( tbvh_bvh b, const uint32_t max_rounds, const float c_trav, co
 		if (le != cudaSuccess || cudaStreamSynchronize( s ) != cudaSuccess)
 		{
 			tbvh_set_error( "tbvh_optimize: write-back -> %s", cudaGetErrorString( le != cudaSuccess ? le : cudaGetLastError() ) );
-			cudaFree( o );
 			return TBVH_E_CUDA;
 		}
-		*out = o, *used = 2 + 2 * h.interior, *depth = best_depth;
+		out = std::move( o ), *used = 2 + 2 * h.interior, *depth = best_depth;
 	}
 	CUDA_TRY( cudaEventRecord( sc.e1, s ) );
 	CUDA_TRY( cudaEventSynchronize( sc.e1 ) );

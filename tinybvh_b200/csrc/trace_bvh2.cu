@@ -111,7 +111,7 @@ unsigned long long* ctx_next_counter( tbvh_ctx c ) { return c->d_counters + (c->
 
 int bvh2_trace_check( tbvh_bvh b, uint64_t n )
 {
-	if (!b->d_trav || !b->d_leaf_tris) { tbvh_set_error( "BVH2 layout not resident" ); return TBVH_E_STATE; }
+	if (!b->trav() || !b->d_leaf_tris) { tbvh_set_error( "BVH2 layout not resident" ); return TBVH_E_STATE; }
 	if (n == 0) return TBVH_OK;
 	if (b->info.max_depth + 1 > TBVH_STACK_DEEP) { tbvh_set_error( "BVH depth %u exceeds the %d-entry traversal stack (the reference's own, tiny_bvh.h:3249)", b->info.max_depth, TBVH_STACK_DEEP ); return TBVH_E_LIMIT; }
 	return TBVH_OK;
@@ -128,7 +128,7 @@ int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_
 	const uint64_t grid = (n + block - 1) / block;
 	if (grid > 0x7fffffffull) { tbvh_set_error( "ray batch too large for one launch" ); return TBVH_E_ARG; }
 	const int variant = b->ctx->trace_variant;
-	#define LAUNCH( A, S, O, D ) k_trace_bvh2<A, S, O, D><<<(uint32_t)grid, block, 0, s>>>( b->d_trav, b->d_leaf_tris, (const char*)d_rays, stride, \
+	#define LAUNCH( A, S, O, D ) k_trace_bvh2<A, S, O, D><<<(uint32_t)grid, block, 0, s>>>( b->trav(), b->d_leaf_tris, (const char*)d_rays, stride, \
 		(char*)d_hits, hit_stride, d_bits, n, root_ref, root_count, d_stats )
 	if (deep)
 	{
@@ -145,8 +145,8 @@ int bvh2_trace_launch( tbvh_bvh b, const void* d_rays, uint32_t stride, void* d_
 		CUDA_TRY( cudaMemsetAsync( next, 0, 8, s ) );
 		if (anyhit) CUDA_TRY( cudaMemsetAsync( d_bits, 0, ((n + 31) / 32) * 4, s ) );
 		const uint32_t pgrid = (uint32_t)b->ctx->sm_count * 10u;
-		if (anyhit) k_trace_bvh2_persist<true><<<pgrid, 128, 0, s>>>( b->d_trav, b->d_leaf_tris, (const char*)d_rays, stride, (char*)d_hits, hit_stride, d_bits, n, root_ref, root_count, next );
-		else k_trace_bvh2_persist<false><<<pgrid, 128, 0, s>>>( b->d_trav, b->d_leaf_tris, (const char*)d_rays, stride, (char*)d_hits, hit_stride, d_bits, n, root_ref, root_count, next );
+		if (anyhit) k_trace_bvh2_persist<true><<<pgrid, 128, 0, s>>>( b->trav(), b->d_leaf_tris, (const char*)d_rays, stride, (char*)d_hits, hit_stride, d_bits, n, root_ref, root_count, next );
+		else k_trace_bvh2_persist<false><<<pgrid, 128, 0, s>>>( b->trav(), b->d_leaf_tris, (const char*)d_rays, stride, (char*)d_hits, hit_stride, d_bits, n, root_ref, root_count, next );
 		LAUNCHED();
 		return TBVH_OK;
 	}

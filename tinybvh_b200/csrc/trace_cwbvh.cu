@@ -174,44 +174,37 @@ int cw_make_trav( const tbvh_bvh* bs, const uint32_t K, cudaStream_t s )
 		b->cw_pending = 0xffffffffu, b->cw_rd_limit = -1.0f;
 		const uint32_t count = b->info.used_blocks / 5;
 		if (count == 0) { tbvh_set_error( "cw_make_trav: no CWBVH nodes" ); return TBVH_E_STATE; }
-		T[t] = CwTrav{ (const uint4*)b->d_cw_nodes, 0, 0, W, count };
+		T[t] = CwTrav{ (const uint4*)b->d_cw_nodes.p, 0, 0, W, count };
 		W += count, most = max( most, count );
 	}
 	for (uint32_t t = 0; t < K; t++)
 	{
-		CUDA_TRY( cudaMalloc( &bs[t]->d_cw_trav, (size_t)T[t].count * CW_NODE_F4 * 16 ) );
-		T[t].dst = (uint4*)bs[t]->d_cw_trav;
+		TRY( bs[t]->d_cw_trav.alloc( (size_t)T[t].count * CW_NODE_F4 * 16 ) );
+		T[t].dst = (uint4*)bs[t]->d_cw_trav.p;
 	}
-	CwTrav* d_T = 0;
-	uint32_t* d_parent = 0;
 	std::vector<uint32_t> res( (size_t)K * 2 ); // range, pending bound per tree
-	auto body = [&]() -> int
-	{
-		// every node notes its parent, then the counts of ancestors that leave node groups pending are summed up to the root
-		const size_t words = (((size_t)W * 5 + (size_t)K * 2) + 63) & ~(size_t)63; // the tree table follows, 256-byte aligned
-		CUDA_TRY( cudaMalloc( &d_parent, words * 4 + (size_t)K * sizeof( CwTrav ) ) );
-		d_T = (CwTrav*)(d_parent + words);
-		uint32_t* const anc[2] = { d_parent + W, d_parent + 2 * (size_t)W }, * const cnt[2] = { d_parent + 3 * (size_t)W, d_parent + 4 * (size_t)W };
-		uint32_t* const d_res = d_parent + 5 * (size_t)W;
-		for (uint32_t t = 0; t < K; t++) T[t].res = d_res + 2 * (size_t)t;
-		CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTrav ), cudaMemcpyHostToDevice, s ) );
-		CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)W * 4, s ) );
-		CUDA_TRY( cudaMemsetAsync( d_res, 0, (size_t)K * 8, s ) );
-		TRY( cw_expand( d_T, K, W, d_parent, s ) );
-		const uint32_t g = (W + 127) / 128;
-		k_cw_jump_init<<<g, 128, 0, s>>>( d_T, K, d_parent, W, anc[0], cnt[0] ); LAUNCHED();
-		int cur = 0;
-		for (uint32_t reach = 1; reach < 2 * most; reach *= 2, cur ^= 1) { k_cw_jump<<<g, 128, 0, s>>>( W, anc[cur], cnt[cur], anc[cur ^ 1], cnt[cur ^ 1] ); LAUNCHED(); }
-		k_cw_pending<<<g, 128, 0, s>>>( d_T, K, W, anc[cur], cnt[cur] ); LAUNCHED();
-		CUDA_TRY( cudaMemcpyAsync( res.data(), d_res, (size_t)K * 8, cudaMemcpyDeviceToHost, s ) );
-		CUDA_TRY( cudaStreamSynchronize( s ) );
-		return TBVH_OK;
-	};
-	const int rc = body();
-	cudaStreamSynchronize( s );
-	if (d_parent) cudaFree( d_parent );
-	if (rc == TBVH_OK) for (uint32_t t = 0; t < K; t++) bs[t]->cw_pending = res[2 * (size_t)t + 1], bs[t]->cw_rd_limit = cw_rd_limit_for( res[2 * (size_t)t] );
-	return rc;
+	Scratch sc( s );
+	// every node notes its parent, then the counts of ancestors that leave node groups pending are summed up to the root
+	const size_t words = (((size_t)W * 5 + (size_t)K * 2) + 63) & ~(size_t)63; // the tree table follows, 256-byte aligned
+	uint32_t* d_parent = 0;
+	TRY( sc.alloc( d_parent, words * 4 + (size_t)K * sizeof( CwTrav ) ) );
+	CwTrav* const d_T = (CwTrav*)(d_parent + words);
+	uint32_t* const anc[2] = { d_parent + W, d_parent + 2 * (size_t)W }, * const cnt[2] = { d_parent + 3 * (size_t)W, d_parent + 4 * (size_t)W };
+	uint32_t* const d_res = d_parent + 5 * (size_t)W;
+	for (uint32_t t = 0; t < K; t++) T[t].res = d_res + 2 * (size_t)t;
+	CUDA_TRY( cudaMemcpyAsync( d_T, T.data(), (size_t)K * sizeof( CwTrav ), cudaMemcpyHostToDevice, s ) );
+	CUDA_TRY( cudaMemsetAsync( d_parent, 0xff, (size_t)W * 4, s ) );
+	CUDA_TRY( cudaMemsetAsync( d_res, 0, (size_t)K * 8, s ) );
+	TRY( cw_expand( d_T, K, W, d_parent, s ) );
+	const uint32_t g = (W + 127) / 128;
+	k_cw_jump_init<<<g, 128, 0, s>>>( d_T, K, d_parent, W, anc[0], cnt[0] ); LAUNCHED();
+	int cur = 0;
+	for (uint32_t reach = 1; reach < 2 * most; reach *= 2, cur ^= 1) { k_cw_jump<<<g, 128, 0, s>>>( W, anc[cur], cnt[cur], anc[cur ^ 1], cnt[cur ^ 1] ); LAUNCHED(); }
+	k_cw_pending<<<g, 128, 0, s>>>( d_T, K, W, anc[cur], cnt[cur] ); LAUNCHED();
+	CUDA_TRY( cudaMemcpyAsync( res.data(), d_res, (size_t)K * 8, cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	for (uint32_t t = 0; t < K; t++) bs[t]->cw_pending = res[2 * (size_t)t + 1], bs[t]->cw_rd_limit = cw_rd_limit_for( res[2 * (size_t)t] );
+	return TBVH_OK;
 }
 
 // ---- traversal ------------------------------------------------------------------------------------------------------

@@ -69,7 +69,7 @@ int tlas_trace_launch( tbvh_bvh b, int layout, const void* d_rays, uint32_t stri
 	const uint64_t grid = (n + 127) / 128;
 	if (grid > 0x7fffffffull) { tbvh_set_error( "ray batch too large for one launch" ); return TBVH_E_ARG; }
 	const uint32_t shift = tlas_inst_shift( b );
-	#define LAUNCH( A, C ) k_trace_tlas<A, C><<<(uint32_t)grid, 128, 0, s>>>( b->d_nodes, b->d_prim_idx, (const TlasInst*)b->d_inst, (const BlasRef*)b->d_blas, \
+	#define LAUNCH( A, C ) k_trace_tlas<A, C><<<(uint32_t)grid, 128, 0, s>>>( b->d_nodes, b->d_prim_idx, b->d_inst, (const BlasRef*)b->d_blas.p, \
 		(char*)d_rays, stride, d_bits, n, b->root_ref, b->root_count, shift )
 	if (anyhit) { if (cw) LAUNCH( true, true ); else LAUNCH( true, false ); }
 	else { if (cw) LAUNCH( false, true ); else LAUNCH( false, false ); }
