@@ -384,6 +384,26 @@ int tbvh_occluded( tbvh_bvh bvh, int layout, const void* rays, uint32_t stride, 
 int tbvh_intersect_device( tbvh_bvh bvh, int layout, void* d_rays, uint32_t stride, void* d_hits, uint64_t n, void* stream );
 int tbvh_occluded_device( tbvh_bvh bvh, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, void* stream );
 
+/* ---- proximity queries ---------------------------------------------------------------------------------- */
+/* Nearest surface point and sphere overlap of query points over the BVH-layout tree of `bvh` (the arrays the BVH2 walk reads): builds of
+ * every flavour, flat, indexed and batched; BVH_GPU and CWBVH objects built or converted by the library; tbvh_upload_bvh /
+ * tbvh_upload_bvh_gpu trees; refitted and optimised trees; group replicas.  The engine's own definition (DESIGN.md 4.9), not bit for
+ * bit the reference's BVH::IntersectSphere (tiny_bvh.h:3140-3200), whose separating-axis test may decide otherwise where a sphere only
+ * touches a triangle: a reference (leaf, triangle) is worth d2 = max( |p - closest point|^2, P ), P the squared distance bound of the
+ * boxes on its leaf's path, and results are the smallest ( d2, prim ), whatever the tree's visiting order.
+ *  tbvh_closest_point  queries: n float4 { x, y, z, r_max } (r_max = INFINITY: unbounded); results: n 16-byte records { d, u, v, prim }:
+ *                      d = the distance to the nearest triangle within r_max, its closest point v0 + u (v1 - v0) + v (v2 - v0) (the
+ *                      u, v of a Moeller-Trumbore hit; u, v >= 0, u + v <= 1); nothing within r_max, a NaN coordinate or an r_max
+ *                      not >= 0: { r_max, 0, 0, 0xffffffff }.
+ *  tbvh_sphere_overlap queries: n float4 { x, y, z, r }; bits[i>>5] bit (i&31) = some triangle lies within r of the centre, exactly
+ *                      when tbvh_closest_point with r_max = r finds one; (n+31)/32 words are written, bits past n are 0.
+ * TBVH_DEVICE: asynchronous on `stream` (a cudaStream_t, 0 = default), pointers 16-byte aligned.  TBVH_HOST: staged through the
+ * device and complete on return (`stream` unused).  n = 0 does nothing.  Refusals, before any launch: TBVH_E_ARG for NULL arguments,
+ * an unknown space, a misaligned device pointer or a batch too large for one launch; TBVH_E_STATE for a handle without a BVH-layout
+ * tree (empty, or a CWBVH-only upload); TBVH_E_UNSUPPORTED for a TLAS; TBVH_E_LIMIT for a tree deeper than 255. */
+int tbvh_closest_point( tbvh_bvh bvh, const void* queries, void* results, uint64_t n, int space, void* stream );
+int tbvh_sphere_overlap( tbvh_bvh bvh, const void* queries, uint32_t* bits, uint64_t n, int space, void* stream );
+
 /* Traversal from the caller's own kernels (include/tinybvh_b200_device.cuh): the traversal functions of the reference's GPU code
  * (traverse_cwbvh / isoccluded_cwbvh, traverse_ailalaine, traverse_tlas / isoccluded_tlas, SURVEY.md 2.3) as device functions over a
  * view of a resident tree.  A view holds what the matching tbvh_intersect_device / tbvh_occluded_device launch passes its kernel:

@@ -141,6 +141,29 @@ public:
 	// per-ray forms with the reference's signatures (correct, but one PCIe round trip each: use the batch forms)
 	template <class RayT> int32_t Intersect( RayT& ray ) const { return (int32_t)Intersect( &ray, 1 ); }
 	template <class RayT> bool IsOccluded( const RayT& ray ) const { uint32_t b = 0; IsOccluded( &ray, 1, &b ); return b & 1; }
+	// proximity queries over the BVH-layout tree (tbvh_closest_point / tbvh_sphere_overlap), host batches of 16-byte { x, y, z, r }
+	// records (bvhvec4 or any float4-like type).  ClosestPoint: results16[i] = { d, u, v, prim } of the nearest triangle within r, the
+	// point v0 + u (v1 - v0) + v (v2 - v0); { r, 0, 0, 0xffffffff } when none.  IntersectSphere: bit i of bits = some triangle lies within r.
+	template <class Vec4> void ClosestPoint( const Vec4* q, uint64_t n, void* results16 ) const
+	{
+		static_assert( sizeof( Vec4 ) == 16, "queries are 16-byte { x, y, z, r } records" );
+		TBVH_FATAL_IF( tbvh_closest_point( h, q, results16, n, TBVH_HOST, 0 ), "ClosestPoint" );
+	}
+	template <class Vec4> void IntersectSphere( const Vec4* q, uint64_t n, uint32_t* bits ) const
+	{
+		static_assert( sizeof( Vec4 ) == 16, "queries are 16-byte { x, y, z, r } records" );
+		TBVH_FATAL_IF( tbvh_sphere_overlap( h, q, bits, n, TBVH_HOST, 0 ), "IntersectSphere" );
+	}
+	// BVH::IntersectSphere( pos, r ) tiny_bvh.h:3140 with its signature, one query (a PCIe round trip: batch where you can).  It answers
+	// under this library's definition (DESIGN.md 4.9: some triangle within r by exact closest-point distance), not the reference's
+	// separating-axis test, which may decide otherwise where the sphere only touches a triangle.
+	template <class Vec3> bool IntersectSphere( const Vec3& pos, const float r ) const
+	{
+		const float q[4] = { pos.x, pos.y, pos.z, r };
+		uint32_t bits = 0;
+		TBVH_FATAL_IF( tbvh_sphere_overlap( h, q, &bits, 1, TBVH_HOST, 0 ), "IntersectSphere" );
+		return bits & 1;
+	}
 protected:
 	BVHBase( int l ) : layout( l ) { TBVH_FATAL_IF( tbvh_bvh_create( context(), &h ), "BVHBase" ); }
 	~BVHBase() { if (own) tbvh_bvh_destroy( h ); }

@@ -1,4 +1,4 @@
-// include/tinybvh_b200_device.cuh - ray traversal from the caller's own CUDA kernels (sm_90a).
+// include/tinybvh_b200_device.cuh - ray traversal and proximity queries from the caller's own CUDA kernels (sm_90a).
 //
 // The reference's GPU code traces from inside the application's kernels: traverse_cwbvh / isoccluded_cwbvh, traverse_ailalaine and
 // traverse_tlas / isoccluded_tlas are device functions that wavefront.cl's Extend / Connect call.  This header gives the same shape
@@ -8,6 +8,11 @@
 //     tbvh::intersect_bvh( view, ray )             tbvh::isoccluded_bvh( view, ray )              BVH / BVH_GPU layout
 //     tbvh::intersect_cwbvh( view, ray )           tbvh::isoccluded_cwbvh( view, ray )            BVH8_CWBVH
 //     tbvh::intersect_tlas<LAYOUT>( view, ray )    tbvh::isoccluded_tlas<LAYOUT>( view, ray )     TLAS, BLASses walked in LAYOUT
+//
+//     tbvh::closest_point_bvh( view, q )           tbvh::sphere_overlaps_bvh( view, q )           BVH / BVH_GPU layout, q = { x, y, z, r }
+//
+// The proximity functions return what tbvh_closest_point / tbvh_sphere_overlap write for the same query, bit for bit; they take no warp
+// vote, so any subset of lanes may call them.
 //
 // The ray is the 64-byte device record in registers (tbvh::Ray: O | mask, D | instIdx, rD | hit.inst, t u v prim).  intersect_*
 // updates ray.hit - and for a TLAS with INST_IDX_BITS 32 the hit.inst word, byte 44 - exactly as tbvh_intersect_device writes those
@@ -29,6 +34,7 @@
 #include "tinybvh_b200_device/base.cuh"
 #include "tinybvh_b200_device/bvh2_walk.cuh"
 #include "tinybvh_b200_device/cw_walk.cuh"
+#include "tinybvh_b200_device/closest_walk.cuh"
 
 namespace tbvh
 {
@@ -277,6 +283,24 @@ template <int BLAS_LAYOUT> __device__ __forceinline__ bool isoccluded_tlas( cons
 	if (v.kind != tlas_view_kind<BLAS_LAYOUT>()) return false;
 	Ray c = r;
 	return tlas_view_trace<true, BLAS_LAYOUT>( v, c );
+}
+
+// tbvh_closest_point of one query { x, y, z, r_max } over a view of kind TBVH_VIEW_BVH: the record { d, u, v, prim } the batch call writes,
+// bit for bit; { r_max, 0, 0, 0xffffffff } when nothing lies within r_max, and for a view of another kind
+__device__ __forceinline__ float4 closest_point_bvh( const tbvh_view& v, const float4& q )
+{
+	if (v.kind != TBVH_VIEW_BVH) return make_float4( q.w, 0.0f, 0.0f, __uint_as_float( CP_NO_PRIM ) );
+	const float4* nodes = (const float4*)v.nodes, * tris = (const float4*)v.tris;
+	if (v.stack > TBVH_STACK) return cp_closest<TBVH_STACK_DEEP>( nodes, tris, v.root_ref, v.root_count, q );
+	return cp_closest<TBVH_STACK>( nodes, tris, v.root_ref, v.root_count, q );
+}
+// tbvh_sphere_overlap of one sphere { x, y, z, r }: the bit the batch call writes (false for a view of another kind)
+__device__ __forceinline__ bool sphere_overlaps_bvh( const tbvh_view& v, const float4& q )
+{
+	if (v.kind != TBVH_VIEW_BVH) return false;
+	const float4* nodes = (const float4*)v.nodes, * tris = (const float4*)v.tris;
+	if (v.stack > TBVH_STACK) return cp_overlaps<TBVH_STACK_DEEP>( nodes, tris, v.root_ref, v.root_count, q );
+	return cp_overlaps<TBVH_STACK>( nodes, tris, v.root_ref, v.root_count, q );
 }
 
 } // namespace tbvh

@@ -83,6 +83,41 @@ def _verts_arg(verts):
     return _np_ptr(v), 16, v.shape[0], HOST, v
 
 
+def _query_radius(points, r):
+    """(n, 4) rows are {x, y, z, r} records whose fourth column is the radius; (n, 3) points take the radius from r (a scalar or one per
+    point).  Giving both, or neither, is an error."""
+    assert points.ndim == 2 and points.shape[1] in (3, 4), "points must be (n, 3) or (n, 4)"
+    if points.shape[1] == 4 and r is not None:
+        raise TbvhError("(n, 4) queries carry their radius in the fourth column: pass no radius argument")
+    if points.shape[1] == 3 and r is None:
+        raise TbvhError("(n, 3) points need a radius argument (np.inf: unbounded)")
+
+
+def _np_queries(points, r):
+    """-> contiguous float32 {x, y, z, r} rows (_query_radius's rules)"""
+    p = np.asarray(points, np.float32)
+    _query_radius(p, r)
+    if p.shape[1] == 4:
+        return np.ascontiguousarray(p)
+    q = np.empty((p.shape[0], 4), np.float32)
+    q[:, :3] = p
+    q[:, 3] = np.asarray(r, np.float32)
+    return q
+
+
+def _torch_queries(points, r):
+    """_np_queries for a CUDA tensor, made on torch's current stream"""
+    import torch
+    assert points.is_cuda, "points must be a CUDA tensor"
+    _query_radius(points, r)
+    if points.shape[1] == 4:
+        return points.to(torch.float32).contiguous()
+    q = torch.empty((points.shape[0], 4), dtype=torch.float32, device=points.device)
+    q[:, :3] = points
+    q[:, 3] = torch.as_tensor(r, dtype=torch.float32, device=points.device)
+    return q
+
+
 class _Base:
     layout = LAYOUT_BVH
     build_flavour = _lib.BUILD_AVX   # derived layouts build through BuildDefault; set to _lib.BUILD_REFERENCE for BVH::Build's tree
@@ -176,6 +211,46 @@ class _Base:
             bits = np.zeros((n + 31) // 32, np.uint32)
         check(L.tbvh_occluded(self.h, self.layout, _np_ptr(rays), rays.dtype.itemsize, n, _np_ptr(bits)))
         return bits
+
+    # -- proximity queries over the BVH-layout tree (tbvh_closest_point / tbvh_sphere_overlap, DESIGN.md §4.9)
+    def closest_point(self, points, r_max=None, stream=None):
+        """Nearest triangle within r_max of every point -> (d, u, v, prim): the closest point is v0 + u (v1 - v0) + v (v2 - v0) of
+        triangle prim; prim 0xffffffff and d = r_max where nothing lies within r_max.  points: (n, 3) with r_max a scalar or one per
+        point (np.inf: unbounded), or (n, 4) {x, y, z, r_max} records, the C-ABI's own, with r_max left out (TbvhError otherwise).  numpy -> host path, numpy arrays (prim uint32); torch CUDA tensor -> device path, everything queued
+        on `stream` (default: torch's current stream), tensors (prim as int32 bits).  No autograd."""
+        L = _lib.lib()
+        if _is_torch(points):
+            import torch
+            st = _stream_arg(stream, points.device)
+            with torch.cuda.stream(torch.cuda.ExternalStream(st, device=points.device)):
+                q = _torch_queries(points, r_max)
+                rec = torch.empty((q.shape[0], 4), dtype=torch.float32, device=q.device)
+                check(L.tbvh_closest_point(self.h, C.c_void_p(q.data_ptr()), C.c_void_p(rec.data_ptr()), q.shape[0], DEVICE, C.c_void_p(st)))
+            return rec[:, 0], rec[:, 1], rec[:, 2], rec[:, 3].view(torch.int32)
+        q = _np_queries(points, r_max)
+        rec = np.empty((q.shape[0], 4), np.float32)
+        check(L.tbvh_closest_point(self.h, _np_ptr(q), _np_ptr(rec), q.shape[0], HOST, None))
+        return rec[:, 0].copy(), rec[:, 1].copy(), rec[:, 2].copy(), rec[:, 3].view(np.uint32).copy()
+
+    def sphere_overlap(self, centers, radii=None, stream=None):
+        """The batched BVH::IntersectSphere under the engine's definition: True where some triangle lies within the radius of the centre.
+        centers: (n, 3) with radii a scalar or one per centre, or (n, 4) {x, y, z, r} records with radii left out, as closest_point.  numpy -> bool array; torch CUDA tensor -> bool tensor queued on `stream`."""
+        L = _lib.lib()
+        if _is_torch(centers):
+            import torch
+            st = _stream_arg(stream, centers.device)
+            with torch.cuda.stream(torch.cuda.ExternalStream(st, device=centers.device)):
+                q = _torch_queries(centers, radii)
+                n = q.shape[0]
+                words = torch.empty(max((n + 31) // 32, 1), dtype=torch.int32, device=q.device)
+                check(L.tbvh_sphere_overlap(self.h, C.c_void_p(q.data_ptr()), C.c_void_p(words.data_ptr()), n, DEVICE, C.c_void_p(st)))
+                shifts = torch.arange(32, dtype=torch.int32, device=q.device)
+                return ((words[:, None] >> shifts) & 1).reshape(-1)[:n].bool()
+        q = _np_queries(centers, radii)
+        n = q.shape[0]
+        words = np.zeros(max((n + 31) // 32, 1), np.uint32)
+        check(L.tbvh_sphere_overlap(self.h, _np_ptr(q), _np_ptr(words), n, HOST, None))
+        return np.unpackbits(words.view(np.uint8), bitorder="little")[:n].astype(bool)
 
     def device_view(self, layout: int = None) -> _lib.DeviceView:
         """tbvh_device_view: the view a kernel of the caller's passes to the device functions of include/tinybvh_b200_device.cuh, for
