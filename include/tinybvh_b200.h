@@ -404,6 +404,27 @@ int tbvh_occluded_device( tbvh_bvh bvh, int layout, const void* d_rays, uint32_t
 int tbvh_closest_point( tbvh_bvh bvh, const void* queries, void* results, uint64_t n, int space, void* stream );
 int tbvh_sphere_overlap( tbvh_bvh bvh, const void* queries, uint32_t* bits, uint64_t n, int space, void* stream );
 
+/* ---- signed distances ----------------------------------------------------------------------------------- */
+/* Signed distance of query points to the triangles of `bvh` (DESIGN.md 4.10): the closest-point query above, signed by the angle-weighted
+ * pseudonormal (Baerentzen & Aanaes 2005) of the feature - face, edge or vertex - the closest point lies on.  Topology comes from
+ * positions, not indices: corners whose x, y and z are equal as values (-0 equals +0) are one vertex, a corner with a NaN coordinate welds
+ * to nothing, so a flat soup, an indexed build and its V[I] soup get the same pseudonormals.
+ * The sign is meaningful only on closed, consistently oriented, manifold surfaces whose normals by the right-hand rule on (v0, v1, v2)
+ * point outward: then sd < 0 exactly inside.  Boundary and non-manifold edges get the same sums, and no claim is made about the sign there.
+ *  tbvh_signed_distance_prepare  builds the handle's pseudonormal table on the engine stream (7 x 16 bytes per triangle) and returns when
+ *                      it is complete.  The table is tied to the tree and vertices it was made from: any later build, upload,
+ *                      tbvh_optimize that changes the tree, or refit makes it stale, and it must be prepared again.  Refusals:
+ *                      TBVH_E_ARG for NULL; TBVH_E_UNSUPPORTED for a TLAS; TBVH_E_STATE without a BVH-layout tree; TBVH_E_LIMIT above
+ *                      2^30 triangles.  A failure after the device work began leaves the tree untouched and no table.
+ *  tbvh_signed_distance  queries: n float4 { x, y, z, r_max } as tbvh_closest_point; results: n 16-byte records { sd, u, v, prim }:
+ *                      u, v and prim are tbvh_closest_point's, |sd| is its d, and sd < 0 exactly when ( p - c ) . N < 0, c the
+ *                      closest point and N the feature's pseudonormal (a point on the surface gives +0).  A miss, a NaN coordinate
+ *                      or an r_max not >= 0 gives the closest-point miss record { r_max, 0, 0, 0xffffffff }: there the sign is unknown.
+ *                      Space, stream and refusals as tbvh_closest_point, in the same order; after them TBVH_E_STATE when no table was
+ *                      prepared or the table is stale.  Every refusal comes before any launch. */
+int tbvh_signed_distance_prepare( tbvh_bvh bvh );
+int tbvh_signed_distance( tbvh_bvh bvh, const void* queries, void* results, uint64_t n, int space, void* stream );
+
 /* Traversal from the caller's own kernels (include/tinybvh_b200_device.cuh): the traversal functions of the reference's GPU code
  * (traverse_cwbvh / isoccluded_cwbvh, traverse_ailalaine, traverse_tlas / isoccluded_tlas, SURVEY.md 2.3) as device functions over a
  * view of a resident tree.  A view holds what the matching tbvh_intersect_device / tbvh_occluded_device launch passes its kernel:

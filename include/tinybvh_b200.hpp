@@ -154,6 +154,15 @@ public:
 		static_assert( sizeof( Vec4 ) == 16, "queries are 16-byte { x, y, z, r } records" );
 		TBVH_FATAL_IF( tbvh_sphere_overlap( h, q, bits, n, TBVH_HOST, 0 ), "IntersectSphere" );
 	}
+	// signed distances (tbvh_signed_distance_prepare / tbvh_signed_distance): PrepareSignedDistance builds the pseudonormal table once per
+	// tree and vertex set (again after any rebuild or refit); SignedDistance: results16[i] = { sd, u, v, prim }, ClosestPoint's record with
+	// the distance negative inside a closed, outward-oriented mesh.
+	void PrepareSignedDistance() { TBVH_FATAL_IF( tbvh_signed_distance_prepare( h ), "PrepareSignedDistance" ); }
+	template <class Vec4> void SignedDistance( const Vec4* q, uint64_t n, void* results16 ) const
+	{
+		static_assert( sizeof( Vec4 ) == 16, "queries are 16-byte { x, y, z, r } records" );
+		TBVH_FATAL_IF( tbvh_signed_distance( h, q, results16, n, TBVH_HOST, 0 ), "SignedDistance" );
+	}
 	// BVH::IntersectSphere( pos, r ) tiny_bvh.h:3140 with its signature, one query (a PCIe round trip: batch where you can).  It answers
 	// under this library's definition (DESIGN.md 4.9: some triangle within r by exact closest-point distance), not the reference's
 	// separating-axis test, which may decide otherwise where the sphere only touches a triangle.

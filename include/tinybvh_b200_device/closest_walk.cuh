@@ -41,15 +41,23 @@ __device__ __forceinline__ float cp_dist2( const float apx, const float apy, con
 	return __fmaf_rn( dz, dz, __fmaf_rn( dy, dy, __fmul_rn( dx, dx ) ) );
 }
 
+// The feature of the triangle a closest point lies on (DESIGN.md 4.10), decided by the branch and the clamp of cp_triangle_feature that
+// produced (u, v), never by comparing floats afterwards: the face, a vertex (v0, v1, v2) or an edge (AB = v0v1, AC = v0v2, BC = v1v2).
+// The values index a signed-distance table record (signed_distance.cu): face normal, three vertex and three edge pseudonormals.
+enum CpFeature : uint32_t { CP_FACE = 0, CP_V0 = 1, CP_V1 = 2, CP_V2 = 3, CP_AB = 4, CP_AC = 5, CP_BC = 6 };
+// an edge from vertex a to vertex b at the clamped parameter t: its end vertex where t is exactly 0 or 1, else the edge
+__device__ __forceinline__ uint32_t cp_edge_feature( const float t, const uint32_t a, const uint32_t b, const uint32_t e ) { return t == 0.0f ? a : t == 1.0f ? b : e; }
+
 // ClosestPtPointTriangle of p against the leaf record (v0 | prim, e1, e2): the closest point is v0 + u e1 + v e2, u, v >= 0, u + v <= 1.
-// Returns d2_raw.  Regions in Ericson's order: A, B, AB, C, AC, BC, face; the face region takes the nearest of its face point (when the
-// triangle's normal is not 0) and the three clamped edge points, ties to the face, then AB, AC, BC.
-__device__ __forceinline__ float cp_triangle( const float px, const float py, const float pz, const float4& v0, const float4& e1, const float4& e2,
-	float& u, float& v )
+// Returns d2_raw; f: the feature of the closest point.  Regions in Ericson's order: A, B, AB, C, AC, BC, face; the face region takes the
+// nearest of its face point (when the triangle's normal is not 0) and the three clamped edge points, ties to the face, then AB, AC, BC.
+// A face point clamped onto an edge gives that edge (uf == 0: AC, vf == 0: AB, vf limited by 1 - uf: BC), two clamps their vertex.
+__device__ __forceinline__ float cp_triangle_feature( const float px, const float py, const float pz, const float4& v0, const float4& e1, const float4& e2,
+	float& u, float& v, uint32_t& f )
 {
 	const float apx = __fsub_rn( px, v0.x ), apy = __fsub_rn( py, v0.y ), apz = __fsub_rn( pz, v0.z );
 	const float d1 = cp_dot( e1.x, e1.y, e1.z, apx, apy, apz ), d2 = cp_dot( e2.x, e2.y, e2.z, apx, apy, apz );
-	if (d1 <= 0.0f && d2 <= 0.0f) u = 0.0f, v = 0.0f;                                             // A
+	if (d1 <= 0.0f && d2 <= 0.0f) u = 0.0f, v = 0.0f, f = CP_V0;                                 // A
 	else
 	{
 		const float bpx = __fsub_rn( apx, e1.x ), bpy = __fsub_rn( apy, e1.y ), bpz = __fsub_rn( apz, e1.z );
@@ -60,14 +68,16 @@ __device__ __forceinline__ float cp_triangle( const float px, const float py, co
 		const float vb = __fsub_rn( __fmul_rn( d5, d2 ), __fmul_rn( d1, d6 ) );
 		const float va = __fsub_rn( __fmul_rn( d3, d6 ), __fmul_rn( d5, d4 ) );
 		const float x = __fsub_rn( d4, d3 ), y = __fsub_rn( d5, d6 );
-		if (d3 >= 0.0f && d4 <= d3) u = 1.0f, v = 0.0f;                                             // B
-		else if (vc <= 0.0f && d1 >= 0.0f && d3 <= 0.0f) u = cp_edge( d1, __fsub_rn( d1, d3 ) ), v = 0.0f; // AB
-		else if (d6 >= 0.0f && d5 <= d6) u = 0.0f, v = 1.0f;                                        // C
-		else if (vb <= 0.0f && d2 >= 0.0f && d6 <= 0.0f) u = 0.0f, v = cp_edge( d2, __fsub_rn( d2, d6 ) ); // AC
+		if (d3 >= 0.0f && d4 <= d3) u = 1.0f, v = 0.0f, f = CP_V1;                                 // B
+		else if (vc <= 0.0f && d1 >= 0.0f && d3 <= 0.0f)                                            // AB
+			u = cp_edge( d1, __fsub_rn( d1, d3 ) ), v = 0.0f, f = cp_edge_feature( u, CP_V0, CP_V1, CP_AB );
+		else if (d6 >= 0.0f && d5 <= d6) u = 0.0f, v = 1.0f, f = CP_V2;                            // C
+		else if (vb <= 0.0f && d2 >= 0.0f && d6 <= 0.0f)                                            // AC
+			u = 0.0f, v = cp_edge( d2, __fsub_rn( d2, d6 ) ), f = cp_edge_feature( v, CP_V0, CP_V2, CP_AC );
 		else if (va <= 0.0f && x >= 0.0f && y >= 0.0f)                                              // BC
 		{
 			const float w = cp_edge( x, __fadd_rn( x, y ) );
-			u = __fsub_rn( 1.0f, w ), v = w;
+			u = __fsub_rn( 1.0f, w ), v = w, f = cp_edge_feature( w, CP_V1, CP_V2, CP_BC );
 		}
 		else
 		{
@@ -84,7 +94,7 @@ __device__ __forceinline__ float cp_triangle( const float px, const float py, co
 			const float nn = cp_dot( nx, ny, nz, nx, ny, nz );
 			const float dab = cp_dist2( apx, apy, apz, e1, e2, tab, 0.0f );
 			float dm = dab;
-			u = tab, v = 0.0f;
+			u = tab, v = 0.0f, f = cp_edge_feature( tab, CP_V0, CP_V1, CP_AB );
 			if (nn > 0.0f)
 			{
 				cp_cross( apx, apy, apz, e2.x, e2.y, e2.z, ax, ay, az );
@@ -93,15 +103,27 @@ __device__ __forceinline__ float cp_triangle( const float px, const float py, co
 				const float uf = cp_unit( __fmul_rn( cp_dot( ax, ay, az, nx, ny, nz ), inv ) );
 				const float vmax = __fsub_rn( 1.0f, uf ), w = cp_unit( __fmul_rn( cp_dot( bx, by, bz, nx, ny, nz ), inv ) );
 				const float vf = w < vmax ? w : vmax, df = cp_dist2( apx, apy, apz, e1, e2, uf, vf );
-				if (df <= dab) u = uf, v = vf, dm = df;
+				if (df <= dab)
+				{
+					const bool cu = uf == 0.0f, cv = vf == 0.0f, cl = !(w < vmax);
+					u = uf, v = vf, dm = df;
+					f = cu ? (cv ? CP_V0 : cl ? CP_V2 : CP_AC) : cv ? (cl ? CP_V1 : CP_AB) : cl ? CP_BC : CP_FACE;
+				}
 			}
 			const float dac = cp_dist2( apx, apy, apz, e1, e2, 0.0f, tac );
-			if (dac < dm) u = 0.0f, v = tac, dm = dac;
+			if (dac < dm) u = 0.0f, v = tac, dm = dac, f = cp_edge_feature( tac, CP_V0, CP_V2, CP_AC );
 			const float ubc = __fsub_rn( 1.0f, tbc ), dbc = cp_dist2( apx, apy, apz, e1, e2, ubc, tbc );
-			if (dbc < dm) u = ubc, v = tbc;
+			if (dbc < dm) u = ubc, v = tbc, f = cp_edge_feature( tbc, CP_V1, CP_V2, CP_BC );
 		}
 	}
 	return cp_dist2( apx, apy, apz, e1, e2, u, v );
+}
+// the form the walk calls: no feature
+__device__ __forceinline__ float cp_triangle( const float px, const float py, const float pz, const float4& v0, const float4& e1, const float4& e2,
+	float& u, float& v )
+{
+	uint32_t f;
+	return cp_triangle_feature( px, py, pz, v0, e1, e2, u, v, f );
 }
 
 // squared distance from p to the box [bmin, bmax] (0 inside): each operation is monotone in the box and in the distance

@@ -88,6 +88,8 @@ SYMBOLS = {
     "tbvh_occluded_device": (i32, [vp, i32, vp, u32, vp, u64, vp]),
     "tbvh_closest_point": (i32, [vp, vp, vp, u64, i32, vp]),
     "tbvh_sphere_overlap": (i32, [vp, vp, vp, u64, i32, vp]),
+    "tbvh_signed_distance_prepare": (i32, [vp]),
+    "tbvh_signed_distance": (i32, [vp, vp, vp, u64, i32, vp]),
     "tbvh_device_view": (i32, [vp, i32, C.POINTER(DeviceView)]),
     "tbvh_set_stats": (i32, [vp, i32]),
     "tbvh_get_stats": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),

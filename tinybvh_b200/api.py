@@ -252,6 +252,31 @@ class _Base:
         check(L.tbvh_sphere_overlap(self.h, _np_ptr(q), _np_ptr(words), n, HOST, None))
         return np.unpackbits(words.view(np.uint8), bitorder="little")[:n].astype(bool)
 
+    # -- signed distances (tbvh_signed_distance_prepare / tbvh_signed_distance, DESIGN.md §4.10)
+    def prepare_signed_distance(self):
+        """Build the pseudonormal table the signed-distance query reads (on the device; returns when done).  Any later build, upload,
+        conversion, optimize or refit makes it stale: call this again before the next signed_distance."""
+        check(_lib.lib().tbvh_signed_distance_prepare(self.h))
+        return self
+
+    def signed_distance(self, points, r_max=None, stream=None):
+        """closest_point with the distance signed: negative inside a closed, consistently oriented mesh (outward normals by the
+        right-hand rule on v0, v1, v2) -> (sd, u, v, prim).  Where nothing lies within r_max, sd = r_max and prim 0xffffffff (no sign is
+        known).  points and r_max follow closest_point's rules; numpy -> host path, torch CUDA tensor -> queued on `stream`."""
+        L = _lib.lib()
+        if _is_torch(points):
+            import torch
+            st = _stream_arg(stream, points.device)
+            with torch.cuda.stream(torch.cuda.ExternalStream(st, device=points.device)):
+                q = _torch_queries(points, r_max)
+                rec = torch.empty((q.shape[0], 4), dtype=torch.float32, device=q.device)
+                check(L.tbvh_signed_distance(self.h, C.c_void_p(q.data_ptr()), C.c_void_p(rec.data_ptr()), q.shape[0], DEVICE, C.c_void_p(st)))
+            return rec[:, 0], rec[:, 1], rec[:, 2], rec[:, 3].view(torch.int32)
+        q = _np_queries(points, r_max)
+        rec = np.empty((q.shape[0], 4), np.float32)
+        check(L.tbvh_signed_distance(self.h, _np_ptr(q), _np_ptr(rec), q.shape[0], HOST, None))
+        return rec[:, 0].copy(), rec[:, 1].copy(), rec[:, 2].copy(), rec[:, 3].view(np.uint32).copy()
+
     def device_view(self, layout: int = None) -> _lib.DeviceView:
         """tbvh_device_view: the view a kernel of the caller's passes to the device functions of include/tinybvh_b200_device.cuh, for
         `layout` (default: the layout Intersect walks).  Host work only; valid until the handle's arrays change (include/tinybvh_b200.h)."""

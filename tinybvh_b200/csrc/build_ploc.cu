@@ -254,28 +254,6 @@ __global__ void __launch_bounds__( 256 ) k_renumber( const float4* __restrict__ 
 }
 } // namespace
 
-// A CUB radix sort on s.  Its kernel launches are counted exactly (g_tbvh_launches): the same call is first captured into a graph
-// that is never launched, and its kernel nodes are counted; then it is enqueued.
-template <class Sort> static int sort_enqueue( cudaStream_t s, Sort sort )
-{
-	cudaGraph_t g = 0;
-	CUDA_TRY( cudaStreamBeginCapture( s, cudaStreamCaptureModeRelaxed ) );
-	const cudaError_t e = sort(), e2 = cudaStreamEndCapture( s, &g );
-	size_t count = 0, kernels = 0;
-	if (e == cudaSuccess && e2 == cudaSuccess && cudaGraphGetNodes( g, 0, &count ) == cudaSuccess)
-	{
-		std::vector<cudaGraphNode_t> nodes( count );
-		cudaGraphGetNodes( g, nodes.data(), &count );
-		for (cudaGraphNode_t x : nodes) { cudaGraphNodeType t; if (cudaGraphNodeGetType( x, &t ) == cudaSuccess && t == cudaGraphNodeTypeKernel) kernels++; }
-	}
-	if (g) cudaGraphDestroy( g );
-	CUDA_TRY( e );
-	CUDA_TRY( e2 );
-	CUDA_TRY( sort() );
-	g_tbvh_launches += kernels;
-	return TBVH_OK;
-}
-
 int build_ploc_launch( const tbvh_bvh* bs, const uint32_t trees, const float c_trav, const float c_int, BuiltTree* out, float* ms )
 {
 	const tbvh_ctx ctx = bs[0]->ctx;

@@ -43,17 +43,23 @@ static int closest_launch( tbvh_bvh b, const float4* d_queries, float4* d_result
 	return TBVH_OK;
 }
 
-// tbvh_closest_point / tbvh_sphere_overlap: every refusal before any launch; TBVH_HOST stages through the call's scratch
-static int closest_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, bool any )
+// tbvh_closest_point / tbvh_sphere_overlap / tbvh_signed_distance: every refusal before any launch; TBVH_HOST stages through the call's
+// scratch
+int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, int kind )
 {
+	const bool any = kind == PROX_ANY;
 	if (!b || !queries || !out) { tbvh_set_error( "%s: NULL argument", fn ); return TBVH_E_ARG; }
 	if (space != TBVH_HOST && space != TBVH_DEVICE) { tbvh_set_error( "%s: unknown space %d", fn, space ); return TBVH_E_ARG; }
 	if (space == TBVH_DEVICE && (((uintptr_t)queries & 15) || ((uintptr_t)out & 15))) { tbvh_set_error( "%s: device pointers must be 16-byte aligned", fn ); return TBVH_E_ARG; }
 	TRY( closest_check( b, n ) );
+	if (kind == PROX_SIGNED) TRY( sd_table_check( b ) );
 	if (n == 0) return TBVH_OK;
 	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
-	if (space == TBVH_DEVICE)
-		return closest_launch( b, (const float4*)queries, any ? 0 : (float4*)out, any ? (uint32_t*)out : 0, n, (cudaStream_t)stream );
+	auto launch = [&]( const float4* q, void* o, cudaStream_t s )
+	{
+		return kind == PROX_SIGNED ? sd_launch( b, q, (float4*)o, n, s ) : closest_launch( b, q, any ? 0 : (float4*)o, any ? (uint32_t*)o : 0, n, s );
+	};
+	if (space == TBVH_DEVICE) return launch( (const float4*)queries, out, (cudaStream_t)stream );
 	const size_t out_bytes = any ? ((n + 31) / 32) * 4 : n * 16;
 	Scratch sc( b->ctx->stream );
 	float4* d_q = 0;
@@ -61,7 +67,7 @@ static int closest_query( const char* fn, tbvh_bvh b, const void* queries, void*
 	TRY( sc.alloc( d_q, n * 16 ) );
 	TRY( sc.alloc( d_out, out_bytes ) );
 	CUDA_TRY( cudaMemcpyAsync( d_q, queries, n * 16, cudaMemcpyHostToDevice, sc.s ) );
-	TRY( closest_launch( b, d_q, any ? 0 : (float4*)d_out, any ? (uint32_t*)d_out : 0, n, sc.s ) );
+	TRY( launch( d_q, d_out, sc.s ) );
 	CUDA_TRY( cudaMemcpyAsync( out, d_out, out_bytes, cudaMemcpyDeviceToHost, sc.s ) );
 	CUDA_TRY( cudaStreamSynchronize( sc.s ) );
 	return TBVH_OK;
@@ -71,12 +77,12 @@ extern "C" {
 
 int tbvh_closest_point( tbvh_bvh b, const void* queries, void* results, uint64_t n, int space, void* stream )
 {
-	return closest_query( __func__, b, queries, results, n, space, stream, false );
+	return proximity_query( __func__, b, queries, results, n, space, stream, PROX_CLOSEST );
 }
 
 int tbvh_sphere_overlap( tbvh_bvh b, const void* queries, uint32_t* bits, uint64_t n, int space, void* stream )
 {
-	return closest_query( __func__, b, queries, bits, n, space, stream, true );
+	return proximity_query( __func__, b, queries, bits, n, space, stream, PROX_ANY );
 }
 
 } // extern "C"

@@ -74,6 +74,28 @@ typedef Owned<false> DevMem;
 typedef Owned<true> HostMem;
 template <class T> struct DevArray : DevMem { T* get() const { return (T*)p; } operator T*() const { return get(); } };
 
+// ---- a CUB radix sort on s (build_ploc.cu, signed_distance.cu).  Its kernel launches are counted exactly (g_tbvh_launches): the same call is first captured into a graph
+// that is never launched, and its kernel nodes are counted; then it is enqueued.
+template <class Sort> int sort_enqueue( cudaStream_t s, Sort sort )
+{
+	cudaGraph_t g = 0;
+	CUDA_TRY( cudaStreamBeginCapture( s, cudaStreamCaptureModeRelaxed ) );
+	const cudaError_t e = sort(), e2 = cudaStreamEndCapture( s, &g );
+	size_t count = 0, kernels = 0;
+	if (e == cudaSuccess && e2 == cudaSuccess && cudaGraphGetNodes( g, 0, &count ) == cudaSuccess)
+	{
+		std::vector<cudaGraphNode_t> nodes( count );
+		cudaGraphGetNodes( g, nodes.data(), &count );
+		for (cudaGraphNode_t x : nodes) { cudaGraphNodeType t; if (cudaGraphNodeGetType( x, &t ) == cudaSuccess && t == cudaGraphNodeTypeKernel) kernels++; }
+	}
+	if (g) cudaGraphDestroy( g );
+	CUDA_TRY( e );
+	CUDA_TRY( e2 );
+	CUDA_TRY( sort() );
+	g_tbvh_launches += kernels;
+	return TBVH_OK;
+}
+
 // ---- handles ----------------------------------------------------------------------------------------------
 // one stage buffer set of the host-buffer pipeline (api.cu "host path")
 struct HostSlot
@@ -182,6 +204,10 @@ struct tbvh_bvh_t
 	bool refittable = true;    // BVHBase::refittable (:811): false after BuildHQ ("can't refit an SBVH", :3027)
 	bool stray_slots = false;  // tbvh_upload_bvh: a slot other than node 1 is outside the tree, or the tree reaches node 1 or a slot past
 	                           // used_nodes, or reaches a slot twice (builders never leave such a tree; tbvh_optimize refuses it)
+	// signed-distance table (signed_distance.cu): 7 float4 per primitive, valid while the handle's generation and revision equal the
+	// stamp taken by tbvh_signed_distance_prepare (every build, upload, conversion, optimisation and refit changes one of them)
+	DevArray<float4> d_sdf;
+	uint32_t sdf_generation = 0, sdf_revision = 0;
 	struct CwKeep* cw_keep = 0; // refittable trees: the 8-wide collapse of the last tbvh_convert to CWBVH (convert_cwbvh.cu), for tbvh_refit_layouts
 	// statistics
 	int stats = 0;
@@ -358,3 +384,10 @@ void drop_cwbvh( tbvh_bvh b );
 int optimize_tree( tbvh_bvh b, uint32_t max_rounds, float c_trav, float c_int, DevArray<float4>& out, uint32_t* used, uint32_t* depth, uint32_t* rounds, float* sah, float* ms );
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)
 int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint32_t n, cudaStream_t s );
+// batched proximity queries (closest_point.cu): the argument checks, the staging of TBVH_HOST batches and the launch of one kind
+enum { PROX_CLOSEST = 0, PROX_ANY = 1, PROX_SIGNED = 2 };
+int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, int kind );
+// signed distances (signed_distance.cu): TBVH_E_STATE without a table prepared for the handle's current tree and vertices; the launch
+// of n > 0 device-space queries after proximity_query's checks
+int sd_table_check( tbvh_bvh b );
+int sd_launch( tbvh_bvh b, const float4* d_queries, float4* d_results, uint64_t n, cudaStream_t s );
