@@ -425,6 +425,27 @@ int tbvh_sphere_overlap( tbvh_bvh bvh, const void* queries, uint32_t* bits, uint
 int tbvh_signed_distance_prepare( tbvh_bvh bvh );
 int tbvh_signed_distance( tbvh_bvh bvh, const void* queries, void* results, uint64_t n, int space, void* stream );
 
+/* ---- generalized winding numbers ------------------------------------------------------------------------ */
+/* The generalized winding number w(q) of the triangles `bvh` references (DESIGN.md 4.11; Jacobson et al. 2013, Barill et al. 2018): 1
+ * inside and 0 outside a closed mesh whose normals by the right-hand rule on (v0, v1, v2) point outward, 2 where two such solids overlap,
+ * and a smooth value across holes, so "w > 0.5" is an inside test for open, self-intersecting and non-manifold meshes too.  No topology
+ * is needed.  Each triangle counts once: a triangle an SBVH references from several leaves belongs to its first reached reference.
+ * Subtrees far from the query (|p - q| > beta r, p and r the centre and half diagonal of the box of their triangles) contribute a
+ * second-order expansion; the others are summed exactly.  beta = +inf gives the exact sum.
+ * For an inside/outside sign on an open mesh: |d| from tbvh_closest_point, negative where the winding number is > 0.5.
+ *  tbvh_winding_number_prepare  builds the handle's table on the engine stream (64 bytes per node slot plus 4 bytes per primitive
+ *                      reference) and returns when it is complete.  Stale after the same calls as the signed-distance table.
+ *                      Refusals: TBVH_E_ARG for NULL; TBVH_E_UNSUPPORTED for a TLAS; TBVH_E_STATE without a BVH-layout tree, or for a
+ *                      tree that reaches a node on two paths (a DAG); TBVH_E_LIMIT for a tree deeper than 255.  A refused prepare
+ *                      leaves the tree untouched and no table.
+ *  tbvh_winding_number  queries: n float4 { x, y, z, ignored } (16-byte aligned); results: n floats (4-byte aligned).  A NaN coordinate
+ *                      gives NaN.  beta must be > 1 (+inf allowed).  Space and stream as tbvh_closest_point.  Refusals, before any
+ *                      launch, in this order: TBVH_E_ARG (NULL, space, alignment, beta not > 1, NaN included), TBVH_E_UNSUPPORTED for a
+ *                      TLAS, TBVH_E_STATE / TBVH_E_LIMIT as tbvh_closest_point, then TBVH_E_STATE when no table was prepared or it is
+ *                      stale. */
+int tbvh_winding_number_prepare( tbvh_bvh bvh );
+int tbvh_winding_number( tbvh_bvh bvh, const void* queries, float* results, uint64_t n, float beta, int space, void* stream );
+
 /* Traversal from the caller's own kernels (include/tinybvh_b200_device.cuh): the traversal functions of the reference's GPU code
  * (traverse_cwbvh / isoccluded_cwbvh, traverse_ailalaine, traverse_tlas / isoccluded_tlas, SURVEY.md 2.3) as device functions over a
  * view of a resident tree.  A view holds what the matching tbvh_intersect_device / tbvh_occluded_device launch passes its kernel:

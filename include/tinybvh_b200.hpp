@@ -163,6 +163,15 @@ public:
 		static_assert( sizeof( Vec4 ) == 16, "queries are 16-byte { x, y, z, r } records" );
 		TBVH_FATAL_IF( tbvh_signed_distance( h, q, results16, n, TBVH_HOST, 0 ), "SignedDistance" );
 	}
+	// generalized winding numbers (tbvh_winding_number_prepare / tbvh_winding_number): PrepareWindingNumber builds the moment table once
+	// per tree and vertex set (again after any rebuild or refit); WindingNumber: w[i] = the winding number at q[i] (its w ignored), 1 inside
+	// and 0 outside a closed, outward-oriented mesh, also meaningful on open and self-intersecting ones; beta = INFINITY: the exact sum.
+	void PrepareWindingNumber() { TBVH_FATAL_IF( tbvh_winding_number_prepare( h ), "PrepareWindingNumber" ); }
+	template <class Vec4> void WindingNumber( const Vec4* q, uint64_t n, float* w, float beta = 2.0f ) const
+	{
+		static_assert( sizeof( Vec4 ) == 16, "queries are 16-byte { x, y, z, ignored } records" );
+		TBVH_FATAL_IF( tbvh_winding_number( h, q, w, n, beta, TBVH_HOST, 0 ), "WindingNumber" );
+	}
 	// BVH::IntersectSphere( pos, r ) tiny_bvh.h:3140 with its signature, one query (a PCIe round trip: batch where you can).  It answers
 	// under this library's definition (DESIGN.md 4.9: some triangle within r by exact closest-point distance), not the reference's
 	// separating-axis test, which may decide otherwise where the sphere only touches a triangle.

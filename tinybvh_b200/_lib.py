@@ -90,6 +90,8 @@ SYMBOLS = {
     "tbvh_sphere_overlap": (i32, [vp, vp, vp, u64, i32, vp]),
     "tbvh_signed_distance_prepare": (i32, [vp]),
     "tbvh_signed_distance": (i32, [vp, vp, vp, u64, i32, vp]),
+    "tbvh_winding_number_prepare": (i32, [vp]),
+    "tbvh_winding_number": (i32, [vp, vp, vp, u64, C.c_float, i32, vp]),
     "tbvh_device_view": (i32, [vp, i32, C.POINTER(DeviceView)]),
     "tbvh_set_stats": (i32, [vp, i32]),
     "tbvh_get_stats": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),

@@ -277,6 +277,39 @@ class _Base:
         check(L.tbvh_signed_distance(self.h, _np_ptr(q), _np_ptr(rec), q.shape[0], HOST, None))
         return rec[:, 0].copy(), rec[:, 1].copy(), rec[:, 2].copy(), rec[:, 3].view(np.uint32).copy()
 
+    # -- generalized winding numbers (tbvh_winding_number_prepare / tbvh_winding_number, DESIGN.md §4.11)
+    def prepare_winding_number(self):
+        """Build the table of subtree moments the winding-number query reads (on the device; returns when done).  Any later build,
+        upload, conversion, optimize or refit makes it stale: call this again before the next winding_number."""
+        check(_lib.lib().tbvh_winding_number_prepare(self.h))
+        return self
+
+    def winding_number(self, points, beta=2.0, stream=None):
+        """The generalized winding number of every point -> w: 1 inside and 0 outside a closed mesh with outward normals (right-hand
+        rule on v0, v1, v2), 2 where two such solids overlap, smooth across holes; NaN for a NaN coordinate.  Subtrees farther than
+        beta times their radius take a second-order expansion (beta > 1; 2 as Barill et al. recommend; np.inf: the exact sum).
+        points: (n, 3), or (n, 4) with the fourth column ignored.  numpy -> host path, float32 array; torch CUDA tensor -> float32
+        tensor queued on `stream` (default: torch's current stream).
+        An inside/outside sign that works on open meshes: d from closest_point, negative where winding_number(...) > 0.5."""
+        L = _lib.lib()
+        assert points.ndim == 2 and points.shape[1] in (3, 4), "points must be (n, 3) or (n, 4)"
+        if _is_torch(points):
+            import torch
+            assert points.is_cuda, "points must be a CUDA tensor"
+            st = _stream_arg(stream, points.device)
+            with torch.cuda.stream(torch.cuda.ExternalStream(st, device=points.device)):
+                q = torch.zeros((points.shape[0], 4), dtype=torch.float32, device=points.device)
+                q[:, :3] = points[:, :3]
+                w = torch.empty(q.shape[0], dtype=torch.float32, device=q.device)
+                check(L.tbvh_winding_number(self.h, C.c_void_p(q.data_ptr()), C.c_void_p(w.data_ptr()), q.shape[0], float(beta), DEVICE, C.c_void_p(st)))
+            return w
+        p = np.asarray(points, np.float32)
+        q = np.zeros((p.shape[0], 4), np.float32)
+        q[:, :3] = p[:, :3]
+        w = np.empty(q.shape[0], np.float32)
+        check(L.tbvh_winding_number(self.h, _np_ptr(q), _np_ptr(w), q.shape[0], float(beta), HOST, None))
+        return w
+
     def device_view(self, layout: int = None) -> _lib.DeviceView:
         """tbvh_device_view: the view a kernel of the caller's passes to the device functions of include/tinybvh_b200_device.cuh, for
         `layout` (default: the layout Intersect walks).  Host work only; valid until the handle's arrays change (include/tinybvh_b200.h)."""

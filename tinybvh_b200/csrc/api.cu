@@ -370,7 +370,7 @@ static void free_layouts( tbvh_bvh b )
 {
 	drop_bvh_gpu( b );
 	drop_cwbvh( b );
-	DevMem* const arrays[] = { &b->d_verts, &b->d_vert_idx, &b->d_nodes, &b->d_prim_idx, &b->d_pairs, &b->d_leaf_tris, &b->d_aabbs, &b->d_inst, &b->d_blas, &b->d_inst_stage, &b->d_sdf };
+	DevMem* const arrays[] = { &b->d_verts, &b->d_vert_idx, &b->d_nodes, &b->d_prim_idx, &b->d_pairs, &b->d_leaf_tris, &b->d_aabbs, &b->d_inst, &b->d_blas, &b->d_inst_stage, &b->d_sdf, &b->d_wn, &b->d_wn_own };
 	for (DevMem* a : arrays) a->reset();
 	b->vert_count = 0, b->leaf_tris_count = 0;
 	b->blas_table_bytes = 0, b->inst_count = 0, b->blas_count = 0, b->tlas_blas_layouts = 0;

@@ -43,24 +43,28 @@ static int closest_launch( tbvh_bvh b, const float4* d_queries, float4* d_result
 	return TBVH_OK;
 }
 
-// tbvh_closest_point / tbvh_sphere_overlap / tbvh_signed_distance: every refusal before any launch; TBVH_HOST stages through the call's
-// scratch
-int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, int kind )
+// tbvh_closest_point / tbvh_sphere_overlap / tbvh_signed_distance / tbvh_winding_number: every refusal before any launch; TBVH_HOST
+// stages through the call's scratch
+int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, int kind, float beta )
 {
-	const bool any = kind == PROX_ANY;
+	const bool any = kind == PROX_ANY, wn = kind == PROX_WINDING;
 	if (!b || !queries || !out) { tbvh_set_error( "%s: NULL argument", fn ); return TBVH_E_ARG; }
 	if (space != TBVH_HOST && space != TBVH_DEVICE) { tbvh_set_error( "%s: unknown space %d", fn, space ); return TBVH_E_ARG; }
-	if (space == TBVH_DEVICE && (((uintptr_t)queries & 15) || ((uintptr_t)out & 15))) { tbvh_set_error( "%s: device pointers must be 16-byte aligned", fn ); return TBVH_E_ARG; }
+	if (space == TBVH_DEVICE && (((uintptr_t)queries & 15) || ((uintptr_t)out & (wn ? 3 : 15))))
+	{ tbvh_set_error( wn ? "%s: device queries must be 16-byte and results 4-byte aligned" : "%s: device pointers must be 16-byte aligned", fn ); return TBVH_E_ARG; }
+	if (wn && !(beta > 1.0f)) { tbvh_set_error( "%s: beta must be > 1 (the expansion needs the query outside the ball)", fn ); return TBVH_E_ARG; }
 	TRY( closest_check( b, n ) );
 	if (kind == PROX_SIGNED) TRY( sd_table_check( b ) );
+	if (wn) TRY( wn_table_check( b ) );
 	if (n == 0) return TBVH_OK;
 	CUDA_TRY( cudaSetDevice( b->ctx->device ) );
 	auto launch = [&]( const float4* q, void* o, cudaStream_t s )
 	{
+		if (wn) return wn_launch( b, q, (float*)o, n, beta, s );
 		return kind == PROX_SIGNED ? sd_launch( b, q, (float4*)o, n, s ) : closest_launch( b, q, any ? 0 : (float4*)o, any ? (uint32_t*)o : 0, n, s );
 	};
 	if (space == TBVH_DEVICE) return launch( (const float4*)queries, out, (cudaStream_t)stream );
-	const size_t out_bytes = any ? ((n + 31) / 32) * 4 : n * 16;
+	const size_t out_bytes = any ? ((n + 31) / 32) * 4 : wn ? n * 4 : n * 16;
 	Scratch sc( b->ctx->stream );
 	float4* d_q = 0;
 	char* d_out = 0;

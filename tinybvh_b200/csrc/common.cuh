@@ -208,6 +208,11 @@ struct tbvh_bvh_t
 	// stamp taken by tbvh_signed_distance_prepare (every build, upload, conversion, optimisation and refit changes one of them)
 	DevArray<float4> d_sdf;
 	uint32_t sdf_generation = 0, sdf_revision = 0;
+	// winding-number table (winding_number.cu): 4 float4 per slot of trav() plus the root's, and per primitive reference the prim it
+	// owns (0xffffffff: none); stamped and made stale exactly as d_sdf
+	DevArray<float4> d_wn;
+	DevArray<uint32_t> d_wn_own;
+	uint32_t wn_generation = 0, wn_revision = 0;
 	struct CwKeep* cw_keep = 0; // refittable trees: the 8-wide collapse of the last tbvh_convert to CWBVH (convert_cwbvh.cu), for tbvh_refit_layouts
 	// statistics
 	int stats = 0;
@@ -385,9 +390,13 @@ int optimize_tree( tbvh_bvh b, uint32_t max_rounds, float c_trav, float c_int, D
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)
 int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint32_t n, cudaStream_t s );
 // batched proximity queries (closest_point.cu): the argument checks, the staging of TBVH_HOST batches and the launch of one kind
-enum { PROX_CLOSEST = 0, PROX_ANY = 1, PROX_SIGNED = 2 };
-int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, int kind );
+// PROX_WINDING: 4-byte results and the expansion's beta (unused by the other kinds)
+enum { PROX_CLOSEST = 0, PROX_ANY = 1, PROX_SIGNED = 2, PROX_WINDING = 3 };
+int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, int kind, float beta = 0.0f );
 // signed distances (signed_distance.cu): TBVH_E_STATE without a table prepared for the handle's current tree and vertices; the launch
 // of n > 0 device-space queries after proximity_query's checks
 int sd_table_check( tbvh_bvh b );
 int sd_launch( tbvh_bvh b, const float4* d_queries, float4* d_results, uint64_t n, cudaStream_t s );
+// winding numbers (winding_number.cu): the same pair for the winding-number table
+int wn_table_check( tbvh_bvh b );
+int wn_launch( tbvh_bvh b, const float4* d_queries, float* d_results, uint64_t n, float beta, cudaStream_t s );
