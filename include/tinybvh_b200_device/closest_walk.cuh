@@ -48,14 +48,35 @@ enum CpFeature : uint32_t { CP_FACE = 0, CP_V0 = 1, CP_V1 = 2, CP_V2 = 3, CP_AB 
 // an edge from vertex a to vertex b at the clamped parameter t: its end vertex where t is exactly 0 or 1, else the edge
 __device__ __forceinline__ uint32_t cp_edge_feature( const float t, const uint32_t a, const uint32_t b, const uint32_t e ) { return t == 0.0f ? a : t == 1.0f ? b : e; }
 
+// The power of two that brings m (a largest magnitude, >= 0) into [1, 2): 2^-e for m in [2^e, 2^(e+1)), e clamped to [-126, 126] so that
+// both it and its inverse (*inv = 2^e) are normal; 1 when m is 0 or not finite.  Multiplying by it is exact wherever nothing over- or
+// underflows, so a quantity of degree k in lengths comes out scaled by exactly its k-th power.
+__device__ __forceinline__ float cp_pow2( const float m, float& inv )
+{
+	const uint32_t f = __float_as_uint( m ) >> 23;
+	if (!(m > 0.0f) || f == 255u) { inv = 1.0f; return 1.0f; }
+	const uint32_t c = f < 1u ? 1u : f > 253u ? 253u : f;
+	inv = __uint_as_float( c << 23 );
+	return __uint_as_float( (254u - c) << 23 );
+}
+
 // ClosestPtPointTriangle of p against the leaf record (v0 | prim, e1, e2): the closest point is v0 + u e1 + v e2, u, v >= 0, u + v <= 1.
 // Returns d2_raw; f: the feature of the closest point.  Regions in Ericson's order: A, B, AB, C, AC, BC, face; the face region takes the
 // nearest of its face point (when the triangle's normal is not 0) and the three clamped edge points, ties to the face, then AB, AC, BC.
 // A face point clamped onto an edge gives that edge (uf == 0: AC, vf == 0: AB, vf limited by 1 - uf: BC), two clamps their vertex.
-__device__ __forceinline__ float cp_triangle_feature( const float px, const float py, const float pz, const float4& v0, const float4& e1, const float4& e2,
+// ap, e1 and e2 are first scaled by the power of two of their largest component (cp_pow2): the region products (vc, vb, va) and |n|^2
+// are of degree 4 in lengths and would over- or underflow from about 2^32 and below 2^-31; d2_raw is scaled back at the end.
+__device__ __forceinline__ float cp_triangle_feature( const float px, const float py, const float pz, const float4& v0, const float4& e1r, const float4& e2r,
 	float& u, float& v, uint32_t& f )
 {
-	const float apx = __fsub_rn( px, v0.x ), apy = __fsub_rn( py, v0.y ), apz = __fsub_rn( pz, v0.z );
+	const float rx = __fsub_rn( px, v0.x ), ry = __fsub_rn( py, v0.y ), rz = __fsub_rn( pz, v0.z );
+	const float m = fmaxf( fmaxf( fmaxf( fmaxf( fabsf( rx ), fabsf( ry ) ), fmaxf( fabsf( rz ), fabsf( e1r.x ) ) ), fmaxf( fmaxf( fabsf( e1r.y ), fabsf( e1r.z ) ),
+		fmaxf( fabsf( e2r.x ), fabsf( e2r.y ) ) ) ), fabsf( e2r.z ) );
+	float inv;
+	const float s = cp_pow2( m, inv );
+	const float apx = __fmul_rn( rx, s ), apy = __fmul_rn( ry, s ), apz = __fmul_rn( rz, s );
+	const float4 e1 = make_float4( __fmul_rn( e1r.x, s ), __fmul_rn( e1r.y, s ), __fmul_rn( e1r.z, s ), 0.0f );
+	const float4 e2 = make_float4( __fmul_rn( e2r.x, s ), __fmul_rn( e2r.y, s ), __fmul_rn( e2r.z, s ), 0.0f );
 	const float d1 = cp_dot( e1.x, e1.y, e1.z, apx, apy, apz ), d2 = cp_dot( e2.x, e2.y, e2.z, apx, apy, apz );
 	if (d1 <= 0.0f && d2 <= 0.0f) u = 0.0f, v = 0.0f, f = CP_V0;                                 // A
 	else
@@ -116,7 +137,7 @@ __device__ __forceinline__ float cp_triangle_feature( const float px, const floa
 			if (dbc < dm) u = ubc, v = tbc, f = cp_edge_feature( tbc, CP_V1, CP_V2, CP_BC );
 		}
 	}
-	return cp_dist2( apx, apy, apz, e1, e2, u, v );
+	return __fmul_rn( __fmul_rn( cp_dist2( apx, apy, apz, e1, e2, u, v ), inv ), inv );
 }
 // the form the walk calls: no feature
 __device__ __forceinline__ float cp_triangle( const float px, const float py, const float pz, const float4& v0, const float4& e1, const float4& e2,

@@ -29,10 +29,29 @@ static float dist2( const float* ap, const float* e1, const float* e2, const flo
 	return fmaf( d[2], d[2], fmaf( d[1], d[1], d[0] * d[0] ) );
 }
 
-float orc_cp_triangle( const float* p, const float* v0, const float* e1, const float* e2, float* uo, float* vo )
+/* closest_walk.cuh cp_pow2: 2^-e bringing m >= 0 into [1, 2), e clamped to [-126, 126], *inv = 2^e; 1 when m is 0 or not finite */
+static float pow2( const float m, float* inv )
 {
-	float ap[3], bp[3], cp[3], u, v;
-	for (int k = 0; k < 3; k++) ap[k] = p[k] - v0[k];
+	uint32_t f, c;
+	memcpy( &f, &m, 4 );
+	f >>= 23;
+	if (!(m > 0.0f) || f == 255u) { *inv = 1.0f; return 1.0f; }
+	c = f < 1u ? 1u : f > 253u ? 253u : f;
+	const uint32_t ib = c << 23, sb = (254u - c) << 23;
+	float s;
+	memcpy( inv, &ib, 4 ), memcpy( &s, &sb, 4 );
+	return s;
+}
+
+/* ap, e1, e2 scaled by the power of two of their largest component, d2_raw scaled back (closest_walk.cuh cp_triangle_feature) */
+float orc_cp_triangle( const float* p, const float* v0, const float* e1r, const float* e2r, float* uo, float* vo )
+{
+	float ap[3], bp[3], cp[3], e1[3], e2[3], r[3], u, v, inv;
+	for (int k = 0; k < 3; k++) r[k] = p[k] - v0[k];
+	const float m = fmaxf( fmaxf( fmaxf( fmaxf( fabsf( r[0] ), fabsf( r[1] ) ), fmaxf( fabsf( r[2] ), fabsf( e1r[0] ) ) ),
+		fmaxf( fmaxf( fabsf( e1r[1] ), fabsf( e1r[2] ) ), fmaxf( fabsf( e2r[0] ), fabsf( e2r[1] ) ) ) ), fabsf( e2r[2] ) );
+	const float s = pow2( m, &inv );
+	for (int k = 0; k < 3; k++) ap[k] = r[k] * s, e1[k] = e1r[k] * s, e2[k] = e2r[k] * s;
 	const float d1 = dot3( e1, ap ), d2 = dot3( e2, ap );
 	if (d1 <= 0.0f && d2 <= 0.0f) u = 0.0f, v = 0.0f; /* A */
 	else
@@ -74,7 +93,7 @@ float orc_cp_triangle( const float* p, const float* v0, const float* e1, const f
 		}
 	}
 	*uo = u, *vo = v;
-	return dist2( ap, e1, e2, u, v );
+	return (dist2( ap, e1, e2, u, v ) * inv) * inv;
 }
 
 static float box_bound( const float* p, const node32* n )

@@ -15,11 +15,15 @@ enum { F_FACE = 0, F_V0 = 1, F_V1 = 2, F_V2 = 3, F_AB = 4, F_AC = 5, F_BC = 6 };
 
 static uint32_t efeat( const float t, const uint32_t a, const uint32_t b, const uint32_t e ) { return t == 0.0f ? a : t == 1.0f ? b : e; }
 
-float orc_sd_triangle( const float* p, const float* v0, const float* e1, const float* e2, float* uo, float* vo, uint32_t* fo )
+float orc_sd_triangle( const float* p, const float* v0, const float* e1r, const float* e2r, float* uo, float* vo, uint32_t* fo )
 {
-	float ap[3], bp[3], cp[3], u, v;
+	float ap[3], bp[3], cp[3], e1[3], e2[3], r[3], u, v, inv;
 	uint32_t f;
-	for (int k = 0; k < 3; k++) ap[k] = p[k] - v0[k];
+	for (int k = 0; k < 3; k++) r[k] = p[k] - v0[k];
+	const float m = fmaxf( fmaxf( fmaxf( fmaxf( fabsf( r[0] ), fabsf( r[1] ) ), fmaxf( fabsf( r[2] ), fabsf( e1r[0] ) ) ),
+		fmaxf( fmaxf( fabsf( e1r[1] ), fabsf( e1r[2] ) ), fmaxf( fabsf( e2r[0] ), fabsf( e2r[1] ) ) ) ), fabsf( e2r[2] ) );
+	const float s = pow2( m, &inv );
+	for (int k = 0; k < 3; k++) ap[k] = r[k] * s, e1[k] = e1r[k] * s, e2[k] = e2r[k] * s;
 	const float d1 = dot3( e1, ap ), d2 = dot3( e2, ap );
 	if (d1 <= 0.0f && d2 <= 0.0f) u = 0.0f, v = 0.0f, f = F_V0; /* A */
 	else
@@ -66,7 +70,7 @@ float orc_sd_triangle( const float* p, const float* v0, const float* e1, const f
 		}
 	}
 	*uo = u, *vo = v, *fo = f;
-	return dist2( ap, e1, e2, u, v );
+	return (dist2( ap, e1, e2, u, v ) * inv) * inv;
 }
 
 /* A&S 4.4.46 */
@@ -132,8 +136,12 @@ void orc_sd_prepare( const float* verts, const uint32_t prims, float* table )
 		const float* v[3] = { verts + (size_t)p * 12, verts + (size_t)p * 12 + 4, verts + (size_t)p * 12 + 8 };
 		float e[3][3], g[3][3]; /* e[k]: corner k to corner k+1, g[k]: corner k to corner k+2 */
 		for (int k = 0; k < 3; k++) for (int a = 0; a < 3; a++) e[k][a] = v[(k + 1) % 3][a] - v[k][a], g[k][a] = v[(k + 2) % 3][a] - v[k][a];
-		/* e1 = v1 - v0 = e[0], e2 = v2 - v0 = g[0] */
-		const float nx = e[0][1] * g[0][2] - e[0][2] * g[0][1], ny = e[0][2] * g[0][0] - e[0][0] * g[0][2], nz = e[0][0] * g[0][1] - e[0][1] * g[0][0];
+		/* e1 = v1 - v0 = e[0], e2 = v2 - v0 = g[0], scaled by the power of two of their largest component before the cross product */
+		float a[3], b[3], inv;
+		const float m = fmaxf( fmaxf( fmaxf( fabsf( e[0][0] ), fabsf( e[0][1] ) ), fmaxf( fabsf( e[0][2] ), fabsf( g[0][0] ) ) ), fmaxf( fabsf( g[0][1] ), fabsf( g[0][2] ) ) );
+		const float sc = pow2( m, &inv );
+		for (int k = 0; k < 3; k++) a[k] = e[0][k] * sc, b[k] = g[0][k] * sc;
+		const float nx = a[1] * b[2] - a[2] * b[1], ny = a[2] * b[0] - a[0] * b[2], nz = a[0] * b[1] - a[1] * b[0];
 		const float nn = fmaf( nz, nz, fmaf( ny, ny, nx * nx ) );
 		float* n = table + (size_t)p * SD_REC * 4;
 		if (nn > 0.0f && nn <= SD_FLT_MAX) { const float l = sqrtf( nn ); n[0] = nx / l, n[1] = ny / l, n[2] = nz / l; }

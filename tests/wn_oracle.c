@@ -52,11 +52,24 @@ void orc_wn_atan2v( const float* y, const float* x, uint64_t n, float* out )
 	for (uint64_t i = 0; i < n; i++) out[i] = orc_wn_atan2( y[i], x[i] );
 }
 
+// 2^-e bringing m >= 0 into [1, 2), e clamped to [-126, 126]; 1 when m is 0 or not finite (closest_walk.cuh cp_pow2)
+static float pow2( float m )
+{
+	const uint32_t f = f2u( m ) >> 23;
+	if (!(m > 0.0f) || f == 255u) return 1.0f;
+	const uint32_t c = f < 1u ? 1u : f > 253u ? 253u : f;
+	return u2f( (254u - c) << 23 );
+}
+
+// a, b, c scaled by the power of two of their largest component, as winding_number.cu wn_triangle
 static float wn_triangle( float qx, float qy, float qz, const float* v0, const float* v1, const float* v2 )
 {
-	const float ax = v0[0] - qx, ay = v0[1] - qy, az = v0[2] - qz;
-	const float bx = v1[0] - qx, by = v1[1] - qy, bz = v1[2] - qz;
-	const float cx = v2[0] - qx, cy = v2[1] - qy, cz = v2[2] - qz;
+	const float rax = v0[0] - qx, ray = v0[1] - qy, raz = v0[2] - qz;
+	const float rbx = v1[0] - qx, rby = v1[1] - qy, rbz = v1[2] - qz;
+	const float rcx = v2[0] - qx, rcy = v2[1] - qy, rcz = v2[2] - qz;
+	const float s = pow2( fmaxf( fmaxf( fmaxf( fmaxf( fabsf( rax ), fabsf( ray ) ), fmaxf( fabsf( raz ), fabsf( rbx ) ) ),
+		fmaxf( fmaxf( fabsf( rby ), fabsf( rbz ) ), fmaxf( fabsf( rcx ), fabsf( rcy ) ) ) ), fabsf( rcz ) ) );
+	const float ax = rax * s, ay = ray * s, az = raz * s, bx = rbx * s, by = rby * s, bz = rbz * s, cx = rcx * s, cy = rcy * s, cz = rcz * s;
 	float nx, ny, nz;
 	cross3( bx, by, bz, cx, cy, cz, &nx, &ny, &nz );
 	const float det = dot3( ax, ay, az, nx, ny, nz );
@@ -68,16 +81,27 @@ static float wn_triangle( float qx, float qy, float qz, const float* v0, const f
 	return orc_wn_atan2( det, den ) / WN_TWO_PI;
 }
 
-// r: 16 floats { p, r, N, M00, M01 .. M22 }
+// 2^-h for 2^2h <= dd < 2^(2h+2) (h in [-63, 63]); 1 when dd is not finite
+static float wn_scale( float dd )
+{
+	const uint32_t f = f2u( dd ) >> 23;
+	if (f >= 255u) return 1.0f;
+	const int h = ((int)(f < 1u ? 1u : f) - 127) >> 1;
+	return u2f( (uint32_t)(127 - h) << 23 );
+}
+
+// r: 16 floats { p, r, N, M00, M01 .. M22 }; every term scaled by s^3, s = wn_scale( dd ), as winding_number.cu wn_far
 static float wn_far( float dx, float dy, float dz, float dd, const float* r )
 {
 	const float* M = r + 7; // M[0] = M00 .. M[8] = M22
-	const float dN = dot3( dx, dy, dz, r[4], r[5], r[6] );
-	const float tr = (M[0] + M[4]) + M[8];
-	const float m0 = dot3( M[0], M[1], M[2], dx, dy, dz ), m1 = dot3( M[3], M[4], M[5], dx, dy, dz ), m2 = dot3( M[6], M[7], M[8], dx, dy, dz );
-	const float dMd = dot3( dx, dy, dz, m0, m1, m2 );
-	const float num = (dN + tr) - (3.0f * dMd) / dd;
-	return num / ((WN_FOUR_PI * dd) * sqrtf( dd ));
+	const float s = wn_scale( dd ), s2 = s * s;
+	const float ex = dx * s, ey = dy * s, ez = dz * s, ee = dd * s2;
+	const float dN = dot3( ex, ey, ez, r[4] * s2, r[5] * s2, r[6] * s2 );
+	const float tr = (((M[0] + M[4]) + M[8]) * s2) * s;
+	const float m0 = dot3( M[0], M[1], M[2], ex, ey, ez ), m1 = dot3( M[3], M[4], M[5], ex, ey, ez ), m2 = dot3( M[6], M[7], M[8], ex, ey, ez );
+	const float dMd = dot3( ex, ey, ez, (m0 * s2) * s, (m1 * s2) * s, (m2 * s2) * s );
+	const float num = (dN + tr) - (3.0f * dMd) / ee;
+	return num / ((WN_FOUR_PI * ee) * sqrtf( ee ));
 }
 
 typedef struct { const Node32* nodes; uint32_t S, root_ref, root_count, refs, prims; const uint32_t* prim_idx; } Tree;

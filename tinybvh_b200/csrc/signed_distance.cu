@@ -73,8 +73,12 @@ __global__ void k_sd_faces( const float4* __restrict__ verts, const uint32_t pri
 	if (p >= prims) return;
 	const float4 v0 = __ldg( verts + (size_t)p * 3 ), v1 = __ldg( verts + (size_t)p * 3 + 1 ), v2 = __ldg( verts + (size_t)p * 3 + 2 );
 	const float4 e1 = f4sub( v1, v0 ), e2 = f4sub( v2, v0 ), e3 = f4sub( v2, v1 ), f1 = f4sub( v0, v1 ), g0 = f4sub( v0, v2 ), g1 = f4sub( v1, v2 );
+	// |n|^2 is of degree 4 in lengths: e1 and e2 are scaled by the power of two of their largest component first, which leaves n's
+	// direction exact and keeps |n|^2 from over- or underflowing (from about 2^32 and below 2^-31 it would, and the normal would be 0)
+	float inv;
+	const float sc = tbvh::cp_pow2( fmaxf( fmaxf( fmaxf( fabsf( e1.x ), fabsf( e1.y ) ), fmaxf( fabsf( e1.z ), fabsf( e2.x ) ) ), fmaxf( fabsf( e2.y ), fabsf( e2.z ) ) ), inv );
 	float nx, ny, nz;
-	cp_cross( e1.x, e1.y, e1.z, e2.x, e2.y, e2.z, nx, ny, nz );
+	cp_cross( __fmul_rn( e1.x, sc ), __fmul_rn( e1.y, sc ), __fmul_rn( e1.z, sc ), __fmul_rn( e2.x, sc ), __fmul_rn( e2.y, sc ), __fmul_rn( e2.z, sc ), nx, ny, nz );
 	const float nn = cp_dot( nx, ny, nz, nx, ny, nz );
 	float4 n = make_float4( 0.0f, 0.0f, 0.0f, 0.0f );
 	if (nn > 0.0f && nn <= SD_FLT_MAX)

@@ -51,12 +51,20 @@ __device__ __forceinline__ float wn_atan2( const float y, const float x )
 	return y < 0.0f ? -a : a;
 }
 
-// the solid angle of triangle (v0, v1, v2) seen from q over 4 pi: atan2( det, den ) / 2 pi (Van Oosterom & Strackee)
+// the solid angle of triangle (v0, v1, v2) seen from q over 4 pi: atan2( det, den ) / 2 pi (Van Oosterom & Strackee).  det and den are
+// of degree 3 in lengths: a, b, c are first scaled by the power of two of their largest component (tbvh::cp_pow2), which leaves the
+// angle's bits as they are wherever nothing over- or underflows and keeps det from underflowing near small triangles
 __device__ __forceinline__ float wn_triangle( const float qx, const float qy, const float qz, const float4& v0, const float4& v1, const float4& v2 )
 {
-	const float ax = __fsub_rn( v0.x, qx ), ay = __fsub_rn( v0.y, qy ), az = __fsub_rn( v0.z, qz );
-	const float bx = __fsub_rn( v1.x, qx ), by = __fsub_rn( v1.y, qy ), bz = __fsub_rn( v1.z, qz );
-	const float cx = __fsub_rn( v2.x, qx ), cy = __fsub_rn( v2.y, qy ), cz = __fsub_rn( v2.z, qz );
+	const float rax = __fsub_rn( v0.x, qx ), ray = __fsub_rn( v0.y, qy ), raz = __fsub_rn( v0.z, qz );
+	const float rbx = __fsub_rn( v1.x, qx ), rby = __fsub_rn( v1.y, qy ), rbz = __fsub_rn( v1.z, qz );
+	const float rcx = __fsub_rn( v2.x, qx ), rcy = __fsub_rn( v2.y, qy ), rcz = __fsub_rn( v2.z, qz );
+	float inv;
+	const float s = tbvh::cp_pow2( fmaxf( fmaxf( fmaxf( fmaxf( fabsf( rax ), fabsf( ray ) ), fmaxf( fabsf( raz ), fabsf( rbx ) ) ),
+		fmaxf( fmaxf( fabsf( rby ), fabsf( rbz ) ), fmaxf( fabsf( rcx ), fabsf( rcy ) ) ) ), fabsf( rcz ) ), inv );
+	const float ax = __fmul_rn( rax, s ), ay = __fmul_rn( ray, s ), az = __fmul_rn( raz, s );
+	const float bx = __fmul_rn( rbx, s ), by = __fmul_rn( rby, s ), bz = __fmul_rn( rbz, s );
+	const float cx = __fmul_rn( rcx, s ), cy = __fmul_rn( rcy, s ), cz = __fmul_rn( rcz, s );
 	float nx, ny, nz;
 	cp_cross( bx, by, bz, cx, cy, cz, nx, ny, nz );
 	const float det = cp_dot( ax, ay, az, nx, ny, nz );
@@ -68,15 +76,29 @@ __device__ __forceinline__ float wn_triangle( const float qx, const float qy, co
 	return __fdiv_rn( wn_atan2( det, den ), WN_TWO_PI );
 }
 
-// the far-field term of a record, d = p - q: ( d.N + tr M - 3 d^T M d / |d|^2 ) / ( 4 pi |d|^3 )
+// 2^-h for 2^2h <= dd < 2^(2h+2) (h in [-63, 63]), so that |d| 2^-h lies in [1, 2); 1 when dd is not finite
+__device__ __forceinline__ float wn_scale( const float dd )
+{
+	const uint32_t f = __float_as_uint( dd ) >> 23;
+	if (f >= 255u) return 1.0f;
+	const int h = ((int)(f < 1u ? 1u : f) - 127) >> 1;
+	return __uint_as_float( (uint32_t)(127 - h) << 23 );
+}
+
+// the far-field term of a record, d = p - q: ( d.N + tr M - 3 d^T M d / |d|^2 ) / ( 4 pi |d|^3 ).  Numerator and denominator are of
+// degree 3 and d^T M d of degree 5 in lengths, so every term is evaluated scaled by s^3, s = wn_scale( dd ): d by s, N by s^2, tr M and
+// M d by s^3 (M d s^4 before the last dot), |d|^2 by s^2.  The quotient is the unscaled one bit for bit wherever the unscaled terms
+// neither over- nor underflow, and it stays finite where they would (a mesh more than about 2^25 units across, or less than 2^-26).
 __device__ __forceinline__ float wn_far( const float dx, const float dy, const float dz, const float dd, const float4& r1, const float4& r2, const float4& r3 )
 {
-	const float dN = cp_dot( dx, dy, dz, r1.x, r1.y, r1.z );
-	const float tr = __fadd_rn( __fadd_rn( r1.w, r2.w ), r3.w );
-	const float m0 = cp_dot( r1.w, r2.x, r2.y, dx, dy, dz ), m1 = cp_dot( r2.z, r2.w, r3.x, dx, dy, dz ), m2 = cp_dot( r3.y, r3.z, r3.w, dx, dy, dz );
-	const float dMd = cp_dot( dx, dy, dz, m0, m1, m2 );
-	const float num = __fsub_rn( __fadd_rn( dN, tr ), __fdiv_rn( __fmul_rn( 3.0f, dMd ), dd ) );
-	return __fdiv_rn( num, __fmul_rn( __fmul_rn( WN_FOUR_PI, dd ), __fsqrt_rn( dd ) ) );
+	const float s = wn_scale( dd ), s2 = __fmul_rn( s, s );
+	const float ex = __fmul_rn( dx, s ), ey = __fmul_rn( dy, s ), ez = __fmul_rn( dz, s ), ee = __fmul_rn( dd, s2 );
+	const float dN = cp_dot( ex, ey, ez, __fmul_rn( r1.x, s2 ), __fmul_rn( r1.y, s2 ), __fmul_rn( r1.z, s2 ) );
+	const float tr = __fmul_rn( __fmul_rn( __fadd_rn( __fadd_rn( r1.w, r2.w ), r3.w ), s2 ), s );
+	const float m0 = cp_dot( r1.w, r2.x, r2.y, ex, ey, ez ), m1 = cp_dot( r2.z, r2.w, r3.x, ex, ey, ez ), m2 = cp_dot( r3.y, r3.z, r3.w, ex, ey, ez );
+	const float dMd = cp_dot( ex, ey, ez, __fmul_rn( __fmul_rn( m0, s2 ), s ), __fmul_rn( __fmul_rn( m1, s2 ), s ), __fmul_rn( __fmul_rn( m2, s2 ), s ) );
+	const float num = __fsub_rn( __fadd_rn( dN, tr ), __fdiv_rn( __fmul_rn( 3.0f, dMd ), ee ) );
+	return __fdiv_rn( num, __fmul_rn( __fmul_rn( WN_FOUR_PI, ee ), __fsqrt_rn( ee ) ) );
 }
 
 __device__ __forceinline__ float tmin( const float a, const float b ) { return a < b ? a : b; }
