@@ -446,6 +446,38 @@ int tbvh_signed_distance( tbvh_bvh bvh, const void* queries, void* results, uint
 int tbvh_winding_number_prepare( tbvh_bvh bvh );
 int tbvh_winding_number( tbvh_bvh bvh, const void* queries, float* results, uint64_t n, float beta, int space, void* stream );
 
+/* ---- intersecting triangle pairs ------------------------------------------------------------------------ */
+/* Which triangles of mesh a cross which triangles of mesh b, and (b == a) which triangles of one mesh cross each other (DESIGN.md 4.12).
+ * Both handles hold a BVH-layout tree as for tbvh_closest_point; their vertices are taken as they are, in one space (no transforms).
+ * The pair test tt_overlap( T, U ) is on closed triangles, so touching counts, and uses orientation predicates only (after Guigue &
+ * Devillers 2003), in fp32 in a fixed order: the triangle whose nine coordinates are lexicographically smaller as ordered keys is T,
+ * T's v0 is subtracted from all six corners and the differences are scaled by the power of two of their largest magnitude.  So the test
+ * is symmetric bit for bit, scaling both meshes by 2^k (k in [-40, 40]) gives the same pairs, and on integer coordinates in [-16, 16]
+ * every predicate is exact.  A triangle of zero scaled normal (zero area) or with a NaN or infinite coordinate is never reported.
+ * Triangles are the input corners of each handle (the vertices it was built, uploaded or refitted with).
+ *  two meshes: the pairs (i, j), i a triangle of a and j of b, such that some reference of j in b's tree is reached (every box on its
+ *              path but the root's overlaps the box of triangle i: closed boxes compared in fp32) and tt_overlap holds.  With boxes that
+ *              hold their triangles, as every builder's, that is every intersecting pair.
+ *  b == a:     the pairs i < j of one mesh.  Corners at equal positions (as values: -0 equals +0, NaN equals nothing) are shared, and a
+ *              pair sharing none is reported by tt_overlap; sharing one, when the edge opposite the shared corner in either triangle
+ *              meets the other triangle; sharing two (an edge), only when both lie in one plane with their third corners on the same side
+ *              of the shared edge (a face folded onto its neighbour); sharing three (a duplicate face), always.
+ *  tbvh_mesh_overlap_pairs  pairs: capacity pairs of two uint32 { i, j } (8-byte aligned in device space; NULL allowed when capacity
+ *              is 0), sorted by (i, j) without repeats (a triangle an SBVH references from several leaves, or a leaf a DAG reaches twice,
+ *              still gives one pair).  *count (a host word) = the number of pairs, even when it exceeds capacity: the first
+ *              min( count, capacity ) are written and a caller can call again with a larger buffer.  Synchronous: its scratch is sized
+ *              from a counting pass; in TBVH_DEVICE its device work is ordered after `stream`'s work so far, in TBVH_HOST `stream` is
+ *              unused.  After the counting pass, TBVH_E_LIMIT when the raw pairs (repeats included) exceed 2^31: *count is then that
+ *              raw total, and no pair is written.
+ *  tbvh_mesh_overlap_bits   bits: (n + 31) / 32 words (4-byte aligned in device space), n the triangles of a; bit (i & 31) of word
+ *              i >> 5 = triangle i of a is a member of some pair (b == a: either member, so every j != i is tested); bits past n are 0.
+ *              TBVH_DEVICE: one launch, asynchronous on `stream`.  TBVH_HOST: complete on return (`stream` unused).
+ * Refusals, before any launch, leaving the outputs untouched, in this order: TBVH_E_ARG for NULL arguments, an unknown space, a
+ * misaligned device output or handles of different contexts; TBVH_E_UNSUPPORTED for a TLAS on either side; TBVH_E_STATE when either
+ * handle holds no BVH-layout tree (empty, or a CWBVH-only upload); TBVH_E_LIMIT when b's tree is deeper than 255. */
+int tbvh_mesh_overlap_pairs( tbvh_bvh a, tbvh_bvh b, uint32_t* pairs, uint64_t capacity, uint64_t* count, int space, void* stream );
+int tbvh_mesh_overlap_bits( tbvh_bvh a, tbvh_bvh b, uint32_t* bits, int space, void* stream );
+
 /* Traversal from the caller's own kernels (include/tinybvh_b200_device.cuh): the traversal functions of the reference's GPU code
  * (traverse_cwbvh / isoccluded_cwbvh, traverse_ailalaine, traverse_tlas / isoccluded_tlas, SURVEY.md 2.3) as device functions over a
  * view of a resident tree.  A view holds what the matching tbvh_intersect_device / tbvh_occluded_device launch passes its kernel:

@@ -16,6 +16,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <array>
+#include <vector>
 
 namespace tinybvh_b200 {
 
@@ -172,6 +174,24 @@ public:
 		static_assert( sizeof( Vec4 ) == 16, "queries are 16-byte { x, y, z, ignored } records" );
 		TBVH_FATAL_IF( tbvh_winding_number( h, q, w, n, beta, TBVH_HOST, 0 ), "WindingNumber" );
 	}
+	// intersecting triangle pairs (tbvh_mesh_overlap_pairs / tbvh_mesh_overlap_bits, DESIGN.md 4.12), both meshes' vertices in one space.
+	// OverlapPairs: every (i, j), i a triangle of this mesh and j of other, that intersect, sorted by (i, j); SelfIntersections: the pairs
+	// i < j of this mesh that intersect, apart from neighbours that only share corners or an edge; OverlapBits( other, bits ): bit i of
+	// (triCount + 31) / 32 words = triangle i intersects some triangle of other (other = *this: some other triangle of this mesh).
+	void OverlapPairs( const BVHBase& other, std::vector<std::array<uint32_t, 2>>& pairs ) const
+	{
+		uint64_t count = 0;
+		pairs.resize( Info().prim_count );
+		TBVH_FATAL_IF( tbvh_mesh_overlap_pairs( h, other.h, pairs.empty() ? 0 : pairs[0].data(), pairs.size(), &count, TBVH_HOST, 0 ), "OverlapPairs" );
+		if (count > pairs.size())
+		{
+			pairs.resize( count );
+			TBVH_FATAL_IF( tbvh_mesh_overlap_pairs( h, other.h, pairs[0].data(), pairs.size(), &count, TBVH_HOST, 0 ), "OverlapPairs" );
+		}
+		pairs.resize( count );
+	}
+	void SelfIntersections( std::vector<std::array<uint32_t, 2>>& pairs ) const { OverlapPairs( *this, pairs ); }
+	void OverlapBits( const BVHBase& other, uint32_t* bits ) const { TBVH_FATAL_IF( tbvh_mesh_overlap_bits( h, other.h, bits, TBVH_HOST, 0 ), "OverlapBits" ); }
 	// BVH::IntersectSphere( pos, r ) tiny_bvh.h:3140 with its signature, one query (a PCIe round trip: batch where you can).  It answers
 	// under this library's definition (DESIGN.md 4.9: some triangle within r by exact closest-point distance), not the reference's
 	// separating-axis test, which may decide otherwise where the sphere only touches a triangle.

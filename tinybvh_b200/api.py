@@ -310,6 +310,54 @@ class _Base:
         check(L.tbvh_winding_number(self.h, _np_ptr(q), _np_ptr(w), q.shape[0], float(beta), HOST, None))
         return w
 
+    # -- intersecting triangle pairs (tbvh_mesh_overlap_pairs / tbvh_mesh_overlap_bits, DESIGN.md §4.12)
+    def overlap_pairs(self, other=None, stream=None):
+        """The pairs (i, j) of a triangle i of self and a triangle j of other that intersect (closed triangles: touching counts), sorted
+        by (i, j) -> (m, 2).  other=None: the self-intersections of this mesh, pairs i < j, where neighbours that only share corners or an
+        edge are not reported (DESIGN.md §4.12).  Both handles' vertices are in one space.  stream=None -> uint32 numpy array;
+        a torch.cuda.Stream (or raw cudaStream_t) -> int32 CUDA tensor holding the bits of the uint32 values, the work ordered after
+        that stream's.  The call returns when done; it starts with a capacity guess and repeats once with the returned count."""
+        L = _lib.lib()
+        o = self if other is None else other
+        n = self.triCount
+        count = C.c_uint64()
+        if stream is None:
+            out = np.zeros((max(n, 1), 2), np.uint32)
+            check(L.tbvh_mesh_overlap_pairs(self.h, o.h, _np_ptr(out), out.shape[0], C.byref(count), HOST, None))
+            if count.value > out.shape[0]:
+                out = np.zeros((count.value, 2), np.uint32)
+                check(L.tbvh_mesh_overlap_pairs(self.h, o.h, _np_ptr(out), out.shape[0], C.byref(count), HOST, None))
+            return out[: count.value].copy()
+        import torch
+        st = getattr(stream, "cuda_stream", stream)
+        dev = torch.device("cuda", self.device)
+        out = torch.empty((max(n, 1), 2), dtype=torch.int32, device=dev)
+        check(L.tbvh_mesh_overlap_pairs(self.h, o.h, C.c_void_p(out.data_ptr()), out.shape[0], C.byref(count), DEVICE, C.c_void_p(st)))
+        if count.value > out.shape[0]:
+            out = torch.empty((count.value, 2), dtype=torch.int32, device=dev)
+            check(L.tbvh_mesh_overlap_pairs(self.h, o.h, C.c_void_p(out.data_ptr()), out.shape[0], C.byref(count), DEVICE, C.c_void_p(st)))
+        return out[: count.value]
+
+    def overlapping(self, other=None, stream=None):
+        """Per triangle of self: True where it intersects some triangle of other (other=None: some other triangle of this mesh, under
+        overlap_pairs' rules for neighbours).  stream=None -> numpy bool array; a torch.cuda.Stream (or raw cudaStream_t) -> bool CUDA
+        tensor queued on that stream."""
+        L = _lib.lib()
+        o = self if other is None else other
+        n = self.triCount
+        if stream is None:
+            words = np.zeros(max((n + 31) // 32, 1), np.uint32)
+            check(L.tbvh_mesh_overlap_bits(self.h, o.h, _np_ptr(words), HOST, None))
+            return np.unpackbits(words.view(np.uint8), bitorder="little")[:n].astype(bool)
+        import torch
+        st = getattr(stream, "cuda_stream", stream)
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.stream(torch.cuda.ExternalStream(st, device=dev)):
+            words = torch.empty(max((n + 31) // 32, 1), dtype=torch.int32, device=dev)
+            check(L.tbvh_mesh_overlap_bits(self.h, o.h, C.c_void_p(words.data_ptr()), DEVICE, C.c_void_p(st)))
+            shifts = torch.arange(32, dtype=torch.int32, device=dev)
+            return ((words[:, None] >> shifts) & 1).reshape(-1)[:n].bool()
+
     def device_view(self, layout: int = None) -> _lib.DeviceView:
         """tbvh_device_view: the view a kernel of the caller's passes to the device functions of include/tinybvh_b200_device.cuh, for
         `layout` (default: the layout Intersect walks).  Host work only; valid until the handle's arrays change (include/tinybvh_b200.h)."""
