@@ -478,6 +478,32 @@ int tbvh_winding_number( tbvh_bvh bvh, const void* queries, float* results, uint
 int tbvh_mesh_overlap_pairs( tbvh_bvh a, tbvh_bvh b, uint32_t* pairs, uint64_t capacity, uint64_t* count, int space, void* stream );
 int tbvh_mesh_overlap_bits( tbvh_bvh a, tbvh_bvh b, uint32_t* bits, int space, void* stream );
 
+/* ---- distances between meshes --------------------------------------------------------------------------- */
+/* How far each triangle of mesh a lies from mesh b, and which pairs lie within a distance (DESIGN.md 4.13): contact candidates within a
+ * margin, clearance between bodies, and (b == a) thin walls and near-touching sheets of one mesh.  Handles, trees and vertices as for
+ * tbvh_mesh_overlap_pairs (a BVH-layout tree on each, vertices in one space, the input corners of each handle).
+ * The pair distance tt_dist2( T, U ) is the engine's own, fp32 in a fixed order: a pair with a NaN or infinite coordinate is skipped (never
+ * a candidate, not even at r = +inf); a pair that tt_overlap reports (tbvh_mesh_overlap_pairs' test) is at 0; otherwise it is the least of
+ * six vertex-triangle distances (the per-triangle function of tbvh_closest_point) and the nine edge-edge distances at interior solutions,
+ * on the canonical pair moved to T's v0 and scaled by a power of two.  So it is symmetric bit for bit, and scaling both meshes by 2^k
+ * (k in [-40, 40]) scales every distance by exactly 2^k.  A zero-area triangle is never at 0 unless a vertex or edge candidate is.
+ * The value of a reference (leaf, j) of b's tree for triangle i of a is max( tt_dist2, LBtri, P ): LBtri the squared gap of the two
+ * triangles' boxes, P the largest squared gap between i's box and a box on the path to the leaf (the root's excepted; the least over
+ * several paths).  Where boxes hold their triangles that is tt_dist2 up to rounding.
+ *  b == a:  the self query: pairs i != j that share no corner (corners equal as values: -0 equals +0, NaN equals nothing).  Neighbours
+ *           are at distance 0 by construction; a face folded onto its neighbour is tbvh_mesh_overlap_pairs' to find.
+ *  tbvh_mesh_distance        results: n 8-byte records { float d, uint32 j } (8-byte aligned in device space), n the triangles of a: the
+ *           smallest ( value, j ) with value <= r_max^2, d = sqrt( value ); { r_max, 0xffffffff } when nothing is found or triangle i has
+ *           a non-finite coordinate.  r_max = +INFINITY: unbounded.  The separation of the meshes is the least d.  TBVH_DEVICE: one
+ *           launch, asynchronous on `stream`.  TBVH_HOST: complete on return (`stream` unused).
+ *  tbvh_mesh_distance_pairs  pairs: every (i, j) with some reference of j reached at value <= r^2 (r = 0: touching and crossing pairs;
+ *           b == a: i < j only), as tbvh_mesh_overlap_pairs returns them: capacity pairs of two uint32, sorted without repeats, *count
+ *           the exact number even above capacity, synchronous, ordered after `stream` in TBVH_DEVICE, TBVH_E_LIMIT above 2^31 raw pairs.
+ * Refusals, before any launch, leaving the outputs untouched, in this order: TBVH_E_ARG for r_max / r NaN or negative, then
+ * tbvh_mesh_overlap_pairs' refusals in their order (TBVH_E_ARG, TBVH_E_UNSUPPORTED, TBVH_E_STATE, TBVH_E_LIMIT). */
+int tbvh_mesh_distance( tbvh_bvh a, tbvh_bvh b, float r_max, void* results, int space, void* stream );
+int tbvh_mesh_distance_pairs( tbvh_bvh a, tbvh_bvh b, float r, uint32_t* pairs, uint64_t capacity, uint64_t* count, int space, void* stream );
+
 /* Traversal from the caller's own kernels (include/tinybvh_b200_device.cuh): the traversal functions of the reference's GPU code
  * (traverse_cwbvh / isoccluded_cwbvh, traverse_ailalaine, traverse_tlas / isoccluded_tlas, SURVEY.md 2.3) as device functions over a
  * view of a resident tree.  A view holds what the matching tbvh_intersect_device / tbvh_occluded_device launch passes its kernel:

@@ -192,6 +192,26 @@ public:
 	}
 	void SelfIntersections( std::vector<std::array<uint32_t, 2>>& pairs ) const { OverlapPairs( *this, pairs ); }
 	void OverlapBits( const BVHBase& other, uint32_t* bits ) const { TBVH_FATAL_IF( tbvh_mesh_overlap_bits( h, other.h, bits, TBVH_HOST, 0 ), "OverlapBits" ); }
+	// distances between meshes (tbvh_mesh_distance / tbvh_mesh_distance_pairs, DESIGN.md 4.13), both meshes' vertices in one space.
+	// NearestTriangles: results8[i] = { float d, uint32 j } of the nearest triangle j of other within r_max of triangle i (r_max = INFINITY:
+	// unbounded), { r_max, 0xffffffff } when none; other = *this: the nearest triangle sharing no corner.  DistancePairs: every (i, j) within
+	// distance r, sorted by (i, j) (other = *this: i < j, sharing no corner).
+	void NearestTriangles( const BVHBase& other, const float r_max, void* results8 ) const
+	{
+		TBVH_FATAL_IF( tbvh_mesh_distance( h, other.h, r_max, results8, TBVH_HOST, 0 ), "NearestTriangles" );
+	}
+	void DistancePairs( const BVHBase& other, const float r, std::vector<std::array<uint32_t, 2>>& pairs ) const
+	{
+		uint64_t count = 0;
+		pairs.resize( Info().prim_count );
+		TBVH_FATAL_IF( tbvh_mesh_distance_pairs( h, other.h, r, pairs.empty() ? 0 : pairs[0].data(), pairs.size(), &count, TBVH_HOST, 0 ), "DistancePairs" );
+		if (count > pairs.size())
+		{
+			pairs.resize( count );
+			TBVH_FATAL_IF( tbvh_mesh_distance_pairs( h, other.h, r, pairs[0].data(), pairs.size(), &count, TBVH_HOST, 0 ), "DistancePairs" );
+		}
+		pairs.resize( count );
+	}
 	// BVH::IntersectSphere( pos, r ) tiny_bvh.h:3140 with its signature, one query (a PCIe round trip: batch where you can).  It answers
 	// under this library's definition (DESIGN.md 4.9: some triangle within r by exact closest-point distance), not the reference's
 	// separating-axis test, which may decide otherwise where the sphere only touches a triangle.

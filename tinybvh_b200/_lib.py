@@ -94,6 +94,8 @@ SYMBOLS = {
     "tbvh_winding_number": (i32, [vp, vp, vp, u64, C.c_float, i32, vp]),
     "tbvh_mesh_overlap_pairs": (i32, [vp, vp, vp, u64, vp, i32, vp]),
     "tbvh_mesh_overlap_bits": (i32, [vp, vp, vp, i32, vp]),
+    "tbvh_mesh_distance": (i32, [vp, vp, f32, vp, i32, vp]),
+    "tbvh_mesh_distance_pairs": (i32, [vp, vp, f32, vp, u64, vp, i32, vp]),
     "tbvh_device_view": (i32, [vp, i32, C.POINTER(DeviceView)]),
     "tbvh_set_stats": (i32, [vp, i32]),
     "tbvh_get_stats": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),

@@ -358,6 +358,55 @@ class _Base:
             shifts = torch.arange(32, dtype=torch.int32, device=dev)
             return ((words[:, None] >> shifts) & 1).reshape(-1)[:n].bool()
 
+    # -- distances between meshes (tbvh_mesh_distance / tbvh_mesh_distance_pairs, DESIGN.md §4.13)
+    def nearest_triangles(self, other=None, r_max=np.inf, stream=None):
+        """The nearest triangle of other within r_max of every triangle of self -> (d, j): j 0xffffffff and d = r_max where there is none
+        (or the triangle has a non-finite coordinate).  other=None: the nearest triangle of this mesh that shares no corner with it (thin
+        walls, near-touching sheets).  Both handles' vertices are in one space; the separation of the meshes is d.min().
+        stream=None -> numpy arrays (d float32, j uint32); a torch.cuda.Stream (or raw cudaStream_t) -> CUDA tensors (j as int32 bits)
+        queued on that stream."""
+        L = _lib.lib()
+        o = self if other is None else other
+        n = self.triCount
+        if stream is None:
+            rec = np.zeros((n, 2), np.float32)
+            check(L.tbvh_mesh_distance(self.h, o.h, float(r_max), _np_ptr(rec), HOST, None))
+            return rec[:, 0].copy(), rec[:, 1].view(np.uint32).copy()
+        import torch
+        st = getattr(stream, "cuda_stream", stream)
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.stream(torch.cuda.ExternalStream(st, device=dev)):
+            rec = torch.empty((max(n, 1), 2), dtype=torch.float32, device=dev)
+            check(L.tbvh_mesh_distance(self.h, o.h, float(r_max), C.c_void_p(rec.data_ptr()), DEVICE, C.c_void_p(st)))
+        return rec[:n, 0], rec[:n, 1].view(torch.int32)
+
+    def distance_pairs(self, other=None, r=None, stream=None):
+        """The pairs (i, j) of a triangle i of self and a triangle j of other within distance r of each other (r = 0: touching and
+        crossing pairs), sorted by (i, j) -> (m, 2).  other=None: pairs i < j of this mesh that share no corner.  stream and the
+        capacity retry as overlap_pairs."""
+        if r is None:
+            raise TbvhError("distance_pairs needs a distance r")
+        L = _lib.lib()
+        o = self if other is None else other
+        n = self.triCount
+        count = C.c_uint64()
+        if stream is None:
+            out = np.zeros((max(n, 1), 2), np.uint32)
+            check(L.tbvh_mesh_distance_pairs(self.h, o.h, float(r), _np_ptr(out), out.shape[0], C.byref(count), HOST, None))
+            if count.value > out.shape[0]:
+                out = np.zeros((count.value, 2), np.uint32)
+                check(L.tbvh_mesh_distance_pairs(self.h, o.h, float(r), _np_ptr(out), out.shape[0], C.byref(count), HOST, None))
+            return out[: count.value].copy()
+        import torch
+        st = getattr(stream, "cuda_stream", stream)
+        dev = torch.device("cuda", self.device)
+        out = torch.empty((max(n, 1), 2), dtype=torch.int32, device=dev)
+        check(L.tbvh_mesh_distance_pairs(self.h, o.h, float(r), C.c_void_p(out.data_ptr()), out.shape[0], C.byref(count), DEVICE, C.c_void_p(st)))
+        if count.value > out.shape[0]:
+            out = torch.empty((count.value, 2), dtype=torch.int32, device=dev)
+            check(L.tbvh_mesh_distance_pairs(self.h, o.h, float(r), C.c_void_p(out.data_ptr()), out.shape[0], C.byref(count), DEVICE, C.c_void_p(st)))
+        return out[: count.value]
+
     def device_view(self, layout: int = None) -> _lib.DeviceView:
         """tbvh_device_view: the view a kernel of the caller's passes to the device functions of include/tinybvh_b200_device.cuh, for
         `layout` (default: the layout Intersect walks).  Host work only; valid until the handle's arrays change (include/tinybvh_b200.h)."""
