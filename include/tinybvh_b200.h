@@ -412,8 +412,9 @@ int tbvh_sphere_overlap( tbvh_bvh bvh, const void* queries, uint32_t* bits, uint
  * The sign is meaningful only on closed, consistently oriented, manifold surfaces whose normals by the right-hand rule on (v0, v1, v2)
  * point outward: then sd < 0 exactly inside.  Boundary and non-manifold edges get the same sums, and no claim is made about the sign there.
  *  tbvh_signed_distance_prepare  builds the handle's pseudonormal table on the engine stream (7 x 16 bytes per triangle) and returns when
- *                      it is complete.  The table is tied to the tree and vertices it was made from: any later build, upload,
- *                      tbvh_optimize that changes the tree, or refit makes it stale, and it must be prepared again.  Refusals:
+ *                      it is complete.  The table is tied to the tree and vertices it was made from: any later build, upload of a
+ *                      BVH or BVH_GPU, tbvh_optimize that changes the tree, or refit makes it stale, and it must be prepared again.
+ *                      A conversion (tbvh_convert, tbvh_convert_batch) or a CWBVH upload changes neither and keeps it.  Refusals:
  *                      TBVH_E_ARG for NULL; TBVH_E_UNSUPPORTED for a TLAS; TBVH_E_STATE without a BVH-layout tree; TBVH_E_LIMIT above
  *                      2^30 triangles.  A failure after the device work began leaves the tree untouched and no table.
  *  tbvh_signed_distance  queries: n float4 { x, y, z, r_max } as tbvh_closest_point; results: n 16-byte records { sd, u, v, prim }:

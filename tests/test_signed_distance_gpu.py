@@ -323,3 +323,28 @@ def test_refusals(gpu):
         assert fn(e.h, qp, op, 4, _lib.DEVICE, None) == _lib.E_STATE, f"stale after {name}"
         assert api.launch_count() == n1
     assert api.launch_count() > n0
+
+
+def test_conversions_keep_the_table(gpu):
+    """A conversion leaves the tree and its vertices as they were, so a prepared table stays valid through it: converting a handle that
+    already holds a CWBVH again (single and batched), converting to BVH_GPU, and uploading a CWBVH over it.  Every query after them gives
+    the records it gave before."""
+    V, F = icosphere(3)
+    v = soup(V, F)
+    e = api.BVH8_CWBVH().Build(v)
+    other = api.BVH().Build(scene(500, 23))
+    q = qrows(sample_queries(V, F, np.random.default_rng(24), n=500))
+    L = _lib.lib()
+    _lib.check(L.tbvh_signed_distance_prepare(e.h))
+    before = sd_device(e.h, q)
+    same_bits(before, so.brute(*api.BVH.download(e), v, q), "prepared")
+    data, tris = e.download()
+    calls = {
+        "convert CWBVH again": lambda: L.tbvh_convert(e.h, api.LAYOUT_CWBVH),
+        "convert_batch": lambda: L.tbvh_convert_batch((C.c_void_p * 2)(e.h.value, other.h.value), 2, api.LAYOUT_CWBVH),
+        "convert BVH_GPU": lambda: L.tbvh_convert(e.h, api.LAYOUT_BVH_GPU),
+        "upload_cwbvh": lambda: L.tbvh_upload_cwbvh(e.h, C.c_void_p(data.ctypes.data), data.shape[0], C.c_void_p(tris.ctypes.data), tris.shape[0] // 3, _lib.HOST),
+    }
+    for name, call in calls.items():
+        assert call() == _lib.OK, name
+        same_bits(sd_device(e.h, q), before, f"after {name}")

@@ -306,3 +306,29 @@ def test_refusals_and_launch_counts(gpu):
         n1 = api.launch_count()
         assert fn(e.h, qp, op, 4) == _lib.E_STATE, f"stale after {name}"
         assert api.launch_count() == n1
+
+
+def test_conversions_keep_the_table(gpu):
+    """A conversion leaves the tree and its vertices as they were, so a prepared table stays valid through it: converting a handle that
+    already holds a CWBVH again (single and batched) and converting to BVH_GPU.  Every query after them gives the numbers it gave
+    before, at beta 2 and inf."""
+    V, F = icosphere(3)
+    v = soup(V, F)
+    e = api.BVH8_CWBVH().Build(v)
+    other = api.BVH().Build(scene(500, 23))
+    q = soup_queries(v, np.random.default_rng(25), n=500)
+    L = _lib.lib()
+    _lib.check(L.tbvh_winding_number_prepare(e.h))
+    nodes, idx = api.BVH.download(e)
+    before = {beta: wn_device(e.h, q, beta) for beta in (2.0, np.inf)}
+    for beta, w in before.items():
+        same_bits(w, wo.winding(nodes, idx, v, q, beta), f"prepared, beta {beta}")
+    calls = {
+        "convert CWBVH again": lambda: L.tbvh_convert(e.h, api.LAYOUT_CWBVH),
+        "convert_batch": lambda: L.tbvh_convert_batch((C.c_void_p * 2)(e.h.value, other.h.value), 2, api.LAYOUT_CWBVH),
+        "convert BVH_GPU": lambda: L.tbvh_convert(e.h, api.LAYOUT_BVH_GPU),
+    }
+    for name, call in calls.items():
+        assert call() == _lib.OK, name
+        for beta, w in before.items():
+            same_bits(wn_device(e.h, q, beta), w, f"after {name}, beta {beta}")

@@ -254,8 +254,8 @@ class _Base:
 
     # -- signed distances (tbvh_signed_distance_prepare / tbvh_signed_distance, DESIGN.md §4.10)
     def prepare_signed_distance(self):
-        """Build the pseudonormal table the signed-distance query reads (on the device; returns when done).  Any later build, upload,
-        conversion, optimize or refit makes it stale: call this again before the next signed_distance."""
+        """Build the pseudonormal table the signed-distance query reads (on the device; returns when done).  Any later build, upload
+        of a tree, optimize or refit makes it stale: call this again before the next signed_distance.  Conversions keep it."""
         check(_lib.lib().tbvh_signed_distance_prepare(self.h))
         return self
 
@@ -280,7 +280,7 @@ class _Base:
     # -- generalized winding numbers (tbvh_winding_number_prepare / tbvh_winding_number, DESIGN.md §4.11)
     def prepare_winding_number(self):
         """Build the table of subtree moments the winding-number query reads (on the device; returns when done).  Any later build,
-        upload, conversion, optimize or refit makes it stale: call this again before the next winding_number."""
+        upload of a tree, optimize or refit makes it stale: call this again before the next winding_number.  Conversions keep it."""
         check(_lib.lib().tbvh_winding_number_prepare(self.h))
         return self
 

@@ -377,6 +377,7 @@ static void free_layouts( tbvh_bvh b )
 	b->tlas_deep_blas = 0, b->tlas_deep_depth = 0;
 	b->links.clear();
 	b->generation = tbvh_next_generation(); // a TLAS built over the old arrays must notice (tlas_check)
+	b->tree_stamp = tbvh_next_generation();
 	memset( &b->info, 0, sizeof( b->info ) );
 	b->refittable = true, b->stray_slots = false;
 }
@@ -390,6 +391,7 @@ static void install_tree( tbvh_bvh b, const BuiltTree& r, const float ms )
 	b->root_ref = r.root[3], b->root_count = r.root[7];
 	b->d_pairs.reset(); // walked through its own nodes (trav)
 	b->generation = tbvh_next_generation(); // new arrays: a TLAS built over the old ones must notice (tlas_check)
+	b->tree_stamp = tbvh_next_generation(); // a new tree: the signed-distance and winding-number tables are stale
 }
 
 int tbvh_bvh_destroy( tbvh_bvh b )

@@ -191,6 +191,8 @@ struct tbvh_bvh_t
 	uint32_t generation = 0;   // renewed (tbvh_next_generation) whenever the arrays a TLAS may point at are replaced (build, upload, refit, convert)
 	uint32_t revision = 0;     // counts refits: a refit that drops no layout rewrites the BVH2 arrays in place under the same generation, and a
 	                           // group's scene replicas (multi.cu) must notice that too
+	uint32_t tree_stamp = 0;   // renewed (tbvh_next_generation) whenever the BVH2 or its vertices are replaced (build, upload, changing optimize);
+	                           // unlike the generation, not by a conversion, which leaves both as they were
 	// TLAS (BVH::Build( BLASInstance*, instCount, BVHBase**, blasCount ) :2221): nodes / primIdx over instance boxes + device tables
 	DevArray<float4> d_aabbs;  // instance boxes the TLAS was built over (2 float4 per instance)
 	DevArray<TlasInst> d_inst; // TlasInst records (inverse transform, BLAS number, mask)
@@ -204,15 +206,15 @@ struct tbvh_bvh_t
 	bool refittable = true;    // BVHBase::refittable (:811): false after BuildHQ ("can't refit an SBVH", :3027)
 	bool stray_slots = false;  // tbvh_upload_bvh: a slot other than node 1 is outside the tree, or the tree reaches node 1 or a slot past
 	                           // used_nodes, or reaches a slot twice (builders never leave such a tree; tbvh_optimize refuses it)
-	// signed-distance table (signed_distance.cu): 7 float4 per primitive, valid while the handle's generation and revision equal the
-	// stamp taken by tbvh_signed_distance_prepare (every build, upload, conversion, optimisation and refit changes one of them)
+	// signed-distance table (signed_distance.cu): 7 float4 per primitive, valid while the handle's tree_stamp and revision equal the
+	// stamp taken by tbvh_signed_distance_prepare (every build, upload, changing optimisation and refit changes one of them)
 	DevArray<float4> d_sdf;
-	uint32_t sdf_generation = 0, sdf_revision = 0;
+	uint32_t sdf_tree_stamp = 0, sdf_revision = 0;
 	// winding-number table (winding_number.cu): 4 float4 per slot of trav() plus the root's, and per primitive reference the prim it
 	// owns (0xffffffff: none); stamped and made stale exactly as d_sdf
 	DevArray<float4> d_wn;
 	DevArray<uint32_t> d_wn_own;
-	uint32_t wn_generation = 0, wn_revision = 0;
+	uint32_t wn_tree_stamp = 0, wn_revision = 0;
 	struct CwKeep* cw_keep = 0; // refittable trees: the 8-wide collapse of the last tbvh_convert to CWBVH (convert_cwbvh.cu), for tbvh_refit_layouts
 	// statistics
 	int stats = 0;

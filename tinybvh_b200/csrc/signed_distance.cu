@@ -219,7 +219,7 @@ __global__ void __launch_bounds__( 128 ) k_signed_distance( const float4* __rest
 int sd_table_check( tbvh_bvh b )
 {
 	if (!b->d_sdf) { tbvh_set_error( "no signed-distance table: call tbvh_signed_distance_prepare first" ); return TBVH_E_STATE; }
-	if (b->sdf_generation != b->generation || b->sdf_revision != b->revision)
+	if (b->sdf_tree_stamp != b->tree_stamp || b->sdf_revision != b->revision)
 	{
 		tbvh_set_error( "the signed-distance table is stale: the tree or its vertices changed since tbvh_signed_distance_prepare" );
 		return TBVH_E_STATE;
@@ -303,7 +303,7 @@ int tbvh_signed_distance_prepare( tbvh_bvh b )
 	const int rc = sd_prepare( b, table, b->ctx->stream );
 	if (rc != TBVH_OK) return rc;
 	b->d_sdf = std::move( table );
-	b->sdf_generation = b->generation, b->sdf_revision = b->revision;
+	b->sdf_tree_stamp = b->tree_stamp, b->sdf_revision = b->revision;
 	return TBVH_OK;
 }
 

@@ -321,7 +321,7 @@ static uint32_t wn_slots( tbvh_bvh b )
 int wn_table_check( tbvh_bvh b )
 {
 	if (!b->d_wn) { tbvh_set_error( "no winding-number table: call tbvh_winding_number_prepare first" ); return TBVH_E_STATE; }
-	if (b->wn_generation != b->generation || b->wn_revision != b->revision)
+	if (b->wn_tree_stamp != b->tree_stamp || b->wn_revision != b->revision)
 	{
 		tbvh_set_error( "the winding-number table is stale: the tree or its vertices changed since tbvh_winding_number_prepare" );
 		return TBVH_E_STATE;
@@ -387,7 +387,7 @@ int tbvh_winding_number_prepare( tbvh_bvh b )
 	if (flag & WN_DAG) { tbvh_set_error( "%s: the tree reaches a slot on two paths (a DAG): its triangles would count twice", __func__ ); return TBVH_E_STATE; }
 	if (flag) { tbvh_set_error( "%s: a reached node names a child, leaf range or triangle outside the tree's arrays", __func__ ); return TBVH_E_STATE; }
 	b->d_wn = std::move( table ), b->d_wn_own = std::move( own );
-	b->wn_generation = b->generation, b->wn_revision = b->revision;
+	b->wn_tree_stamp = b->tree_stamp, b->wn_revision = b->revision;
 	return TBVH_OK;
 }
 
