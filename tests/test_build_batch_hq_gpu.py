@@ -142,14 +142,15 @@ def test_offatrium_inputs_next_to_plain_meshes(gpu):
 
 
 def test_signed_zero_families_match_separate_builds(gpu):
-    """BuildHQ's handling of -0 inside its bins is a known gap against the reference: here the batch only has to equal the separate
-    GPU builds, and the plain neighbours a batch of their own."""
+    """Meshes with -0 coordinates next to plain ones: every tree is the reference's and equals its separate GPU build, and the plain
+    neighbours equal a batch of their own."""
     base = mesh(3000, 71)
     named = [("plain", mesh(1500, 72))] + [(f"signed zero {m}", util.signed_zero(base, m, seed=5)) for m in ("pos", "neg", "random", "order")]
     named += [("signed zero small", util.signed_zero(mesh(100, 73), "neg", seed=6)), ("plain after", mesh(700, 74))]
     meshes = [v for _, v in named]
     got = hq_batch(meshes)
     for k, (label, _) in enumerate(named):
+        assert_oracle(got[k], meshes[k], label)
         assert_same([got[k]], separate([meshes[k]]), label)
     assert_same([got[0], got[-1]], hq_batch([meshes[0], meshes[-1]]), "plain meshes next to signed zeros")
 

@@ -51,7 +51,7 @@ def fail_scene_hq(name):
 @pytest.mark.parametrize("name", list(FAIL_SCENES))
 def test_scene_fails_splits_without_negative_zero(name):
     v = fail_scene(name)
-    # BuildHQ's -0 tie rule is a known difference (tests/test_offatrium_gpu.py HQ_SIGNED_ZERO), not what these scenes test
+    # signed zeros are tests/test_build_hq_signed_zero.py's: these scenes stay on the path without the sign pass
     assert util.count_neg_zero(v[:, :3]) == 0
     _, _, _, failed, stale, largest = fail_scene_hq(name)
     assert failed > 0 and stale > 0, f"{name}: {failed} failed splits, {stale} stale"

@@ -20,15 +20,6 @@ ZERO = ["zero:pos", "zero:neg", "zero:random", "zero:order"]
 SCALE = ["scale:%d" % k for k in (-126, -100, -60, -6, -4, 8, 16, 24, 30, 40, 90)]
 SHIFT = ["shift:1048576", "shift:-12582912"]   # +2^20, -3 * 2^22
 BUILDERS = {"Build": 0, "BuildAVX": 1, "BuildHQ": 2}
-# BuildHQ resolves the sign of tied zero bounds only for the root box; its object bins, spatial bins and refolded child boxes
-# still take the ordered keys' -0 (DESIGN 4.3b).  Every BuildHQ case of a family with -0 coordinates is marked; whether a given
-# tree happens to come out right depends on the seed, so the mark is not strict.
-HQ_SIGNED_ZERO = pytest.mark.xfail(strict=False, reason="BuildHQ's bins and child boxes do not follow the reference's tie rule for signed zeros")
-
-
-def hq_signed_zero(request, builder, fam):
-    if builder == "BuildHQ" and fam in ("zero:neg", "zero:random", "zero:order"):
-        request.applymarker(HQ_SIGNED_ZERO)
 
 
 def family(fam, ntris, seed=5):
@@ -74,8 +65,7 @@ def assert_tree(e, v, builder, label):
 @pytest.mark.parametrize("ntris", [1, 3, 40, 2000])
 @pytest.mark.parametrize("fam", ZERO + SCALE + SHIFT)
 @pytest.mark.parametrize("builder", list(BUILDERS))
-def test_tree_matches_oracle(gpu, request, builder, fam, ntris):
-    hq_signed_zero(request, builder, fam)
+def test_tree_matches_oracle(gpu, builder, fam, ntris):
     v = family(fam, ntris)
     if fam.startswith("zero") and fam != "zero:pos" and ntris >= 40:
         assert util.count_neg_zero(v[:, :3]) > 0
@@ -85,9 +75,8 @@ def test_tree_matches_oracle(gpu, request, builder, fam, ntris):
 @pytest.mark.parametrize("fam", ["zero:random", "zero:order", "scale:-126", "scale:40", "shift:1048576"])
 @pytest.mark.parametrize("build_mode", [0, 1])
 @pytest.mark.parametrize("builder", list(BUILDERS))
-def test_tree_matches_oracle_large(gpu, request, builder, build_mode, fam):
+def test_tree_matches_oracle_large(gpu, builder, build_mode, fam):
     """70k triangles: the large phase (nodes above small_t) runs over several levels, in both drivers of the SAH build."""
-    hq_signed_zero(request, builder, fam)
     v = family(fam, 70000)
     api.set_option("build_mode", build_mode)
     try:

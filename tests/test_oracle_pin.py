@@ -411,14 +411,23 @@ def test_reference_layouts_disagree_on_a_pinned_set_of_rays(ntris, seed, res, pr
 
 
 @pytest.mark.skipif(not refpy.available(), reason="oracle/_ref not built (needs /root/reference)")
-@pytest.mark.parametrize("fam", ["zero:random", "zero:order", "scale:-126", "scale:-6", "scale:24", "scale:40", "scale:90", "shift:1048576", "shift:-12582912"])
+@pytest.mark.parametrize("fam", ["zero:random", "zero:order", "scale:-126", "scale:-6", "scale:24", "scale:40", "scale:90", "shift:1048576", "shift:-12582912"]
+                         + ["hq:" + f for f in ("zero:neg", "mirror:xyz", "mirror:x", "flat", "straddle")])
 @pytest.mark.parametrize("mode", [0, 1, 2])
 def test_port_matches_reference_on_offatrium_families(mode, fam):
     """The restatement against the compiled reference on the off-atrium families (tests/test_offatrium_gpu.py): signed zeros,
     power-of-two scales on both sides of the scale-invariance window, large translations.  Trees byte for byte, BVH and CWBVH walks
-    bit for bit on camera, axis (+-0 directions, rD = +-inf) and all-octant rays."""
+    bit for bit on camera, axis (+-0 directions, rD = +-inf) and all-octant rays.  "hq:" families are BuildHQ's signed-zero inputs
+    (tests/test_build_hq_signed_zero.py), held in mode 2."""
     from tests.test_offatrium_gpu import family, unit_rays
-    v = family(fam, 2000)
+    if fam.startswith("hq:"):
+        if mode != 2:
+            pytest.skip("a BuildHQ input family")
+        from tests import test_build_hq_signed_zero as hq
+        v = hq.family(fam[3:], 2000)
+        unit_rays = lambda *_: hq.family_rays(v)  # noqa: E731
+    else:
+        v = family(fam, 2000)
     ref = refpy.RefBVH(v, mode=mode, threaded=False)
     if mode == 2:
         nodes, idx, ic = portpy.build_hq(v)

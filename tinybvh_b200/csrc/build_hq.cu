@@ -41,6 +41,10 @@ namespace
 #define HQ_BIG_THREADS 256
 #define HQ_SMALL_WARPS 4
 #define HQ_STACK 64
+// NEGZERO instances only: position words (common.cuh zpos_word) of zero bounds, [axis][bin][bmin xyz, bmax xyz] for the bins, then
+// the 12 of the refolded child boxes in GroupSmem::ckey order
+#define HQ_ZBINS (3 * HQBINS * 6)
+#define HQ_ZW (HQ_ZBINS + 12)
 
 struct HQTask { uint32_t node, sliceStart, sliceEnd, depth; };
 struct HQCounters
@@ -321,6 +325,7 @@ struct Grp
 	uint32_t rank, nct;       // CTA rank in the cluster, cluster size
 	GroupSmem* S; GroupSmem* S0;
 	uint32_t* job;            // 3 * HQ_MLP * G words of this CTA's (warp's) shared memory: clip jobs of one item tile (spatial binning)
+	uint32_t* Z; uint32_t* Z0; // NEGZERO: HQ_ZW position words of zero bounds, this CTA's (warp's) and the leader's (merged)
 };
 template <int G> __device__ __forceinline__ void lsync() { if (G == 32) __syncwarp(); else __syncthreads(); }
 template <int G> __device__ __forceinline__ void gsync( const Grp& g )
@@ -364,13 +369,14 @@ template <int G> __device__ __forceinline__ uint32_t gscan( const Grp& g, const 
 	return base;
 }
 
-__device__ __forceinline__ void bins_reset( GroupSmem& S, const int tid, const int G )
+template <bool NEGZERO> __device__ __forceinline__ void bins_reset( const Grp& g, GroupSmem& S, const int tid, const int G )
 {
 	for (int k = tid; k < 3 * HQBINS * 3; k += G) (&S.kmin[0][0][0])[k] = f2key( BVH_FAR ), (&S.kmax[0][0][0])[k] = f2key( -BVH_FAR );
 	for (int k = tid; k < 3 * HQBINS; k += G) (&S.cntA[0][0])[k] = 0, (&S.cntB[0][0])[k] = 0;
+	if (NEGZERO) for (int k = tid; k < HQ_ZBINS; k += G) g.Z[k] = 0;
 }
 // cluster: fold this CTA's tables into the leader's (distributed shared memory atomics)
-template <int G> __device__ __forceinline__ void bins_merge( const Grp& g )
+template <int G, bool NEGZERO> __device__ __forceinline__ void bins_merge( const Grp& g )
 {
 	if (G == 32 || g.nct == 1) return;
 	__syncthreads();
@@ -381,6 +387,20 @@ template <int G> __device__ __forceinline__ void bins_merge( const Grp& g )
 			atomicMin( &(&D.kmin[0][0][0])[k], (&S.kmin[0][0][0])[k] ), atomicMax( &(&D.kmax[0][0][0])[k], (&S.kmax[0][0][0])[k] );
 		for (int k = g.tid; k < 3 * HQBINS; k += G)
 			atomicAdd( &(&D.cntA[0][0])[k], (&S.cntA[0][0])[k] ), atomicAdd( &(&D.cntB[0][0])[k], (&S.cntB[0][0])[k] );
+		if (NEGZERO) for (int k = g.tid; k < HQ_ZBINS; k += G) if (g.Z[k]) atomicMax( &g.Z0[k], g.Z[k] );
+	}
+}
+// Signed zeros (NEGZERO): the reference folds a bin's bounds over the node's fragments in slice order, so of several zero bounds the
+// one of the last fragment gives the bin bound its sign.  Fragment `pos` of the node offers its zero bounds to bin (a, b); the sweep
+// resolves the bin's zero keys with the highest offer (common.cuh zero_resolve).
+__device__ __forceinline__ void bin_zero( uint32_t* Z, const uint32_t a, const uint32_t b, const uint32_t pos, const float* mn, const float* mx )
+{
+	uint32_t* z = Z + (a * HQBINS + b) * 6;
+	#pragma unroll
+	for (int k = 0; k < 3; k++)
+	{
+		if (mn[k] == 0) atomicMax( z + k, zpos_word( pos, mn[k] ) );
+		if (mx[k] == 0) atomicMax( z + 3 + k, zpos_word( pos, mx[k] ) );
 	}
 }
 // Shared atomics are the scarce resource of the binning loops (8192 of them per 256-thread trip), and after the first few
@@ -403,7 +423,9 @@ __device__ __forceinline__ void bin_grow( GroupSmem& S, const uint32_t a, const 
 //   spatial split (:2847-2870, countIn / countOut): the same among candidates with NL + NR < budget, NL * NR > 0 and
 //                 C < 0.985 * splitCost.
 // The winner lane stores the child boxes in S.best.  Returns the candidate index (-1: none) and its cost, on every lane.
-__device__ __noinline__ int sweep_select( GroupSmem& S, const bool spatial, const float rSAV, const float c_trav, const float c_int,
+// NEGZERO: the bins' zero bounds take their signs from Z, and the unions fold in the reference's order: upward for the left side
+// and downward for the right, each bin the second operand, so the last tied zero wins.
+template <bool NEGZERO> __device__ __noinline__ int sweep_select( GroupSmem& S, const uint32_t* Z, const bool spatial, const float rSAV, const float c_trav, const float c_int,
 	const bool ok0, const bool ok1, const bool ok2, const float limit, const int budget, float& bestCost, int& bestNL, int& bestNR )
 {
 	// lane = axis * 8 + bin: each lane decodes its own bin, then segmented (width 8) prefix and suffix unions by shuffles;
@@ -413,7 +435,12 @@ __device__ __noinline__ int sweep_select( GroupSmem& S, const bool spatial, cons
 	const uint32_t a = lane < 24 ? lane >> 3 : 0, i = lane & 7;
 	float l1[3], l2[3], r1[3], r2[3];
 	#pragma unroll
-	for (int k = 0; k < 3; k++) l1[k] = r1[k] = key2f( S.kmin[a][i][k] ), l2[k] = r2[k] = key2f( S.kmax[a][i][k] );
+	for (int k = 0; k < 3; k++)
+	{
+		uint32_t lo = S.kmin[a][i][k], hi = S.kmax[a][i][k];
+		if (NEGZERO) lo = zero_resolve( lo, Z[(a * HQBINS + i) * 6 + k] ), hi = zero_resolve( hi, Z[(a * HQBINS + i) * 6 + 3 + k] );
+		l1[k] = r1[k] = key2f( lo ), l2[k] = r2[k] = key2f( hi );
+	}
 	uint32_t lN = S.cntA[a][i], rN = spatial ? S.cntB[a][i] : lN;
 	#pragma unroll
 	for (int d = 1; d < 8; d <<= 1)
@@ -424,8 +451,9 @@ __device__ __noinline__ int sweep_select( GroupSmem& S, const bool spatial, cons
 		{
 			const float a1 = __shfl_up_sync( 0xffffffffu, l1[k], d, 8 ), a2 = __shfl_up_sync( 0xffffffffu, l2[k], d, 8 );
 			const float b1 = __shfl_down_sync( 0xffffffffu, r1[k], d, 8 ), b2 = __shfl_down_sync( 0xffffffffu, r2[k], d, 8 );
-			if (up) l1[k] = tmin( l1[k], a1 ), l2[k] = tmax( l2[k], a2 );
-			if (dn) r1[k] = tmin( r1[k], b1 ), r2[k] = tmax( r2[k], b2 );
+			// a1 / a2 cover the bins below this lane's run, b1 / b2 those above it
+			if (up) { if (NEGZERO) l1[k] = tmin( a1, l1[k] ), l2[k] = tmax( a2, l2[k] ); else l1[k] = tmin( l1[k], a1 ), l2[k] = tmax( l2[k], a2 ); }
+			if (dn) { if (NEGZERO) r1[k] = tmin( b1, r1[k] ), r2[k] = tmax( b2, r2[k] ); else r1[k] = tmin( r1[k], b1 ), r2[k] = tmax( r2[k], b2 ); }
 		}
 		const uint32_t an = __shfl_up_sync( 0xffffffffu, lN, d, 8 ), bn = __shfl_down_sync( 0xffffffffu, rN, d, 8 );
 		if (up) lN += an;
@@ -486,7 +514,7 @@ __device__ __noinline__ int sweep_select( GroupSmem& S, const bool spatial, cons
 
 // One node, start to finish, by a group of G threads (G = 32: a warp, G = 256: a CTA).  Returns true and the two child
 // tasks when the node was split.
-template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp& g, const HQTask t, HQTask& outL, HQTask& outR )
+template <int G, bool BATCH, bool NEGZERO> __device__ bool hq_node( const HQArgs& A, const Grp& g, const HQTask t, HQTask& outL, HQTask& outR )
 {
 	GroupSmem& S = *g.S;            // this CTA's (warp's) tables
 	GroupSmem& S0 = *g.S0;          // the leader's: merged tables, decisions
@@ -521,7 +549,7 @@ template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp
 	const uint32_t* primIdx = A.prim_idx;
 
 	// ---- object split: bins :2758-2775
-	bins_reset( S, tid, G );
+	bins_reset<NEGZERO>( g, S, tid, G );
 	gsync<G>( g );
 	if (BATCH) tree_limits();
 	// HQ_MLP fragments per thread and trip: the index -> fragment loads of a trip are issued together
@@ -542,18 +570,19 @@ template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp
 			{
 				const int bi = clampi( cvtt( __fmul_rn( __fmaf_rn( __fadd_rn( mn[a], mx[a] ), 0.5f, -nmin3[a] ), rpd3[a] ) ), 0, HQBINS - 1 );
 				bin_grow( S, a, bi, mn, mx );
+				if (NEGZERO) bin_zero( g.Z, a, bi, i0 + u * GT, mn, mx );
 				atomicAdd( &S.cntA[a][bi], 1u );
 			}
 		}
 	}
-	bins_merge<G>( g );
+	bins_merge<G, NEGZERO>( g );
 	gsync<G>( g );
 	PH( 0 );
 	if (lead && tid < 32)
 	{
 		float splitCost = noSplitCost;
 		int nl = 0, nr = 0;
-		const int best = sweep_select( S, false, rSAV, A.c_trav, A.c_int, axisOK[0], axisOK[1], axisOK[2], noSplitCost, budget, splitCost, nl, nr );
+		const int best = sweep_select<NEGZERO>( S, g.Z, false, rSAV, A.c_trav, A.c_int, axisOK[0], axisOK[1], axisOK[2], noSplitCost, budget, splitCost, nl, nr );
 		if (tid == 0)
 		{
 			S.hasObj = best >= 0, S.spatial = 0, S.bestNL = S.bestNR = 0;
@@ -576,7 +605,7 @@ template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp
 	// ---- spatial split candidate :2808-2872
 	if (S0.trySpatial)
 	{
-		bins_reset( S, tid, G );
+		bins_reset<NEGZERO>( g, S, tid, G );
 		gsync<G>( g );
 		const float planeDist3[3] = { __fdiv_rn( ext[0], __fmul_rn( (float)HQBINS, 0.9999f ) ), __fdiv_rn( ext[1], __fmul_rn( (float)HQBINS, 0.9999f ) ), __fdiv_rn( ext[2], __fmul_rn( (float)HQBINS, 0.9999f ) ) };
 		// items are (fragment, axis) pairs; an item that spans several bins becomes one clip job per bin (:2831-2845).  The
@@ -610,6 +639,7 @@ template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp
 				{
 					const float mn[3] = { fa[u].x, fa[u].y, fa[u].z }, mx[3] = { fb[u].x, fb[u].y, fb[u].z };
 					bin_grow( S, a, bin1, mn, mx );
+					if (NEGZERO) bin_zero( g.Z, a, bin1, (base + gtid * kpp + u) / 3, mn, mx );
 				}
 				else nb[u] = (uint32_t)(bin2 - bin1 + 1), ab[u] = a | ((uint32_t)bin1 << 2);
 				nbsum += nb[u];
@@ -639,17 +669,18 @@ template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp
 				if (a == 0) bmin[0] = lo_a, bmax[0] = hi_a; else if (a == 1) bmin[1] = lo_a, bmax[1] = hi_a; else bmin[2] = lo_a, bmax[2] = hi_a;
 				if (!clip_frag<BATCH>( A, BATCH ? S0.tree : 0u, f, nbmin, nbmax, bmin, bmax, minDim, a )) continue;
 				bin_grow( S, a, (uint32_t)j, nbmin, nbmax );
+				if (NEGZERO) bin_zero( g.Z, a, (uint32_t)j, (base + (gtid - tid + lo / HQ_MLP) * kpp + lo % HQ_MLP) / 3, nbmin, nbmax ); // the job's item
 			}
 			lsync<G>();
 		}
-		bins_merge<G>( g );
+		bins_merge<G, NEGZERO>( g );
 		gsync<G>( g );
 		PH( 2 );
 		if (lead && tid < 32)
 		{
 			float splitCost = S.splitCost;
 			int nl = 0, nr = 0;
-			const int best = sweep_select( S, true, rSAV, A.c_trav, A.c_int, axisOK[0], axisOK[1], axisOK[2], __fmul_rn( splitCost, 0.985f ), budget, splitCost, nl, nr );
+			const int best = sweep_select<NEGZERO>( S, g.Z, true, rSAV, A.c_trav, A.c_int, axisOK[0], axisOK[1], axisOK[2], __fmul_rn( splitCost, 0.985f ), budget, splitCost, nl, nr );
 			if (best >= 0 && tid == 0)
 			{
 				const uint32_t a = best / 7;
@@ -866,14 +897,19 @@ template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp
 			Apos += tot & 0xffffu, Bpos -= tot >> 16;
 		}
 		// child bounds are refreshed from the fragments :2943-2950
-		for (int k = tid; k < 12; k += G) S.ckey[k] = ((k / 3) & 1) ? f2key( -BVH_FAR ) : f2key( BVH_FAR );
+		for (int k = tid; k < 12; k += G)
+		{
+			S.ckey[k] = ((k / 3) & 1) ? f2key( -BVH_FAR ) : f2key( BVH_FAR );
+			if (NEGZERO) g.Z[HQ_ZBINS + k] = 0;
+		}
 		gsync<G>( g );
 		const uint32_t nl = Apos - t.sliceStart, nr = t.sliceEnd - Bpos;
 		{
 			// per-thread boxes over its fragments, one redux per word and warp, one shared atomic per word and warp
-			uint32_t bk[12];
+			// NEGZERO: and the highest position word of a zero per word, the fold being in idxTmp order on either side
+			uint32_t bk[12], bz[12];
 			#pragma unroll
-			for (int k = 0; k < 12; k++) bk[k] = ((k / 3) & 1) ? f2key( -BVH_FAR ) : f2key( BVH_FAR );
+			for (int k = 0; k < 12; k++) bk[k] = ((k / 3) & 1) ? f2key( -BVH_FAR ) : f2key( BVH_FAR ), bz[k] = 0;
 			for (uint32_t base = 0; base < nl + nr; base += GT * HQ_MLP)
 			{
 				uint32_t fr[HQ_MLP];
@@ -888,15 +924,23 @@ template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp
 				{
 					const float4 fa = A.frag_min[fr[u]], fb = A.frag_max[fr[u]];
 					const uint32_t ka[6] = { f2key( fa.x ), f2key( fa.y ), f2key( fa.z ), f2key( fb.x ), f2key( fb.y ), f2key( fb.z ) };
-					if (base + gtid + u * GT >= nl)
+					const uint32_t i = base + gtid + u * GT;
+					const float f[6] = { fa.x, fa.y, fa.z, fb.x, fb.y, fb.z };
+					if (i >= nl)
 					{
 						#pragma unroll
 						for (int q = 0; q < 3; q++) bk[6 + q] = min( bk[6 + q], ka[q] ), bk[9 + q] = max( bk[9 + q], ka[3 + q] );
+						if (NEGZERO)
+							#pragma unroll
+							for (int q = 0; q < 6; q++) if (f[q] == 0) bz[6 + q] = max( bz[6 + q], zpos_word( i, f[q] ) );
 					}
 					else
 					{
 						#pragma unroll
 						for (int q = 0; q < 3; q++) bk[q] = min( bk[q], ka[q] ), bk[3 + q] = max( bk[3 + q], ka[3 + q] );
+						if (NEGZERO)
+							#pragma unroll
+							for (int q = 0; q < 6; q++) if (f[q] == 0) bz[q] = max( bz[q], zpos_word( i, f[q] ) );
 					}
 				}
 			}
@@ -906,15 +950,21 @@ template <int G, bool BATCH> __device__ bool hq_node( const HQArgs& A, const Grp
 			{
 				const uint32_t r = ((k / 3) & 1) ? __reduce_max_sync( 0xffffffffu, bk[k] ) : __reduce_min_sync( 0xffffffffu, bk[k] );
 				if ((tid & 31) == 0) { if ((k / 3) & 1) atomicMax( &S.ckey[k], r ); else atomicMin( &S.ckey[k], r ); }
+				if (NEGZERO)
+				{
+					const uint32_t z = __reduce_max_sync( 0xffffffffu, bz[k] );
+					if ((tid & 31) == 0 && z) atomicMax( &g.Z[HQ_ZBINS + k], z );
+				}
 			}
 		}
 		if (G != 32 && g.nct > 1)
 		{
 			__syncthreads();
 			if (!lead && tid < 12) { if ((tid / 3) & 1) atomicMax( &S0.ckey[tid], S.ckey[tid] ); else atomicMin( &S0.ckey[tid], S.ckey[tid] ); }
+			if (NEGZERO && !lead && tid < 12 && g.Z[HQ_ZBINS + tid]) atomicMax( &g.Z0[HQ_ZBINS + tid], g.Z[HQ_ZBINS + tid] );
 		}
 		gsync<G>( g );
-		if (lead && tid < 12) S.best[tid] = key2f( S.ckey[tid] );
+		if (lead && tid < 12) S.best[tid] = key2f( NEGZERO ? zero_resolve( S.ckey[tid], g.Z[HQ_ZBINS + tid] ) : S.ckey[tid] );
 		PH( 8 );
 	}
 	gsync<G>( g );
@@ -1093,39 +1143,43 @@ __device__ __forceinline__ void hq_enqueue( const HQArgs& A, HQTask* next, const
 	else A.small[atomicAdd( &A.ctr->small_roots, 1u )] = c;
 }
 
-// level-synchronous phase: one cluster of nct CTAs (run-time cluster dimension, 1..16) per node
-template <bool BATCH> __global__ void __launch_bounds__( HQ_BIG_THREADS, 3 ) k_hq_level( HQArgs A, const HQTask* cur, HQTask* next, const uint32_t nct )
+// level-synchronous phase: one cluster of nct CTAs (run-time cluster dimension, 1..16) per node.  NEGZERO: some fragment bound is
+// -0 (HQCounters::negzero), and bins and child boxes take the signs of their zero bounds as the reference's folds give them.
+template <bool BATCH, bool NEGZERO> __global__ void __launch_bounds__( HQ_BIG_THREADS, 3 ) k_hq_level( HQArgs A, const HQTask* cur, HQTask* next, const uint32_t nct )
 {
 	__shared__ GroupSmem S;
 	__shared__ uint32_t job[3 * HQ_MLP * HQ_BIG_THREADS];
+	__shared__ uint32_t Z[NEGZERO ? HQ_ZW : 1];
 	Grp g;
-	g.tid = (int)threadIdx.x, g.nct = nct, g.rank = 0, g.S = g.S0 = &S, g.job = job;
+	g.tid = (int)threadIdx.x, g.nct = nct, g.rank = 0, g.S = g.S0 = &S, g.job = job, g.Z = g.Z0 = Z;
 	if (nct > 1)
 	{
 		cg::cluster_group cl = cg::this_cluster();
 		g.rank = cl.block_rank(), g.S0 = cl.map_shared_rank( &S, 0 );
+		if (NEGZERO) g.Z0 = cl.map_shared_rank( Z, 0 );
 	}
 	g.gtid = (int)(g.rank * HQ_BIG_THREADS + threadIdx.x), g.GT = (int)(nct * HQ_BIG_THREADS);
 	HQTask l, r;
-	const bool split = hq_node<HQ_BIG_THREADS, BATCH>( A, g, cur[blockIdx.x / nct], l, r );
+	const bool split = hq_node<HQ_BIG_THREADS, BATCH, NEGZERO>( A, g, cur[blockIdx.x / nct], l, r );
 	if (split && g.rank == 0 && threadIdx.x == 0) hq_enqueue( A, next, l ), hq_enqueue( A, next, r );
 }
 
-template <bool BATCH> __global__ void __launch_bounds__( HQ_SMALL_WARPS * 32, 6 ) k_hq_subtrees( HQArgs A, const uint32_t roots )
+template <bool BATCH, bool NEGZERO> __global__ void __launch_bounds__( HQ_SMALL_WARPS * 32, 6 ) k_hq_subtrees( HQArgs A, const uint32_t roots )
 {
 	__shared__ GroupSmem Ss[HQ_SMALL_WARPS];
 	__shared__ HQTask stack[HQ_SMALL_WARPS][HQ_STACK];
 	__shared__ uint32_t job[HQ_SMALL_WARPS][3 * HQ_MLP * 32];
+	__shared__ uint32_t Z[HQ_SMALL_WARPS][NEGZERO ? HQ_ZW : 1];
 	const uint32_t w = threadIdx.x >> 5, lane = threadIdx.x & 31, id = blockIdx.x * HQ_SMALL_WARPS + w;
 	if (id >= roots) return;
 	Grp g;
-	g.tid = g.gtid = (int)lane, g.GT = 32, g.rank = 0, g.nct = 1, g.S = g.S0 = &Ss[w], g.job = job[w];
+	g.tid = g.gtid = (int)lane, g.GT = 32, g.rank = 0, g.nct = 1, g.S = g.S0 = &Ss[w], g.job = job[w], g.Z = g.Z0 = Z[w];
 	HQTask t = A.small[id];
 	uint32_t sp = 0;
 	for (;;)
 	{
 		HQTask l, r;
-		if (hq_node<32, BATCH>( A, g, t, l, r ))
+		if (hq_node<32, BATCH, NEGZERO>( A, g, t, l, r ))
 		{
 			// continue with the child that holds fewer fragments, park the other: the stack stays logarithmic
 			const uint32_t cl = __float_as_uint( A.tmp_nodes[(size_t)l.node * 2 + 1].w ), cr = __float_as_uint( A.tmp_nodes[(size_t)r.node * 2 + 1].w );
@@ -1253,12 +1307,18 @@ int build_hq_launch( const tbvh_bvh* bs, const uint32_t K, float c_trav, float c
 	k_hq_fragments<<<(n + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
 	k_hq_root_zero<<<ctx->sm_count, 256, 0, s>>>( A ); LAUNCHED();
 	k_hq_root<<<(K + 255) / 256, 256, 0, s>>>( A ); LAUNCHED();
+	// with a -0 fragment bound anywhere in the batch, the node kernels' instances that give zero bounds their signs (NEGZERO); a tree
+	// without one comes out the same from either
+	CUDA_TRY( cudaMemcpyAsync( &h_ctr->negzero, &A.ctr->negzero, 4, cudaMemcpyDeviceToHost, s ) );
+	CUDA_TRY( cudaStreamSynchronize( s ) );
+	const bool negzero = h_ctr->negzero != 0;
 	uint32_t level = 0;
 	uint32_t max_cluster = (uint32_t)(ctx->hq_cluster < 1 ? 1 : ctx->hq_cluster > HQ_MAX_CLUSTER ? HQ_MAX_CLUSTER : ctx->hq_cluster);
 	// tuning knobs of the cluster sizing rule, read from the environment: fragments per CTA, CTAs per SM in flight
 	const char* env_cf = getenv( "TBVH_HQ_CTA_FRAGS" ); const char* env_cc = getenv( "TBVH_HQ_CTA_CAP" );
 	const size_t cta_frags = env_cf && atoi( env_cf ) > 0 ? (size_t)atoi( env_cf ) : 512, cta_cap = env_cc && atoi( env_cc ) > 0 ? (size_t)atoi( env_cc ) : 16;
-	void (*level_kernel)( HQArgs, const HQTask*, HQTask*, uint32_t ) = K > 1 ? k_hq_level<true> : k_hq_level<false>;
+	void (*level_kernel)( HQArgs, const HQTask*, HQTask*, uint32_t ) = K > 1 ? (negzero ? k_hq_level<true, true> : k_hq_level<true, false>)
+		: (negzero ? k_hq_level<false, true> : k_hq_level<false, false>);
 	if (max_cluster > 8) CUDA_TRY( cudaFuncSetAttribute( level_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1 ) );
 	// one level list for every tree: the cluster size follows the level's largest node, whichever tree holds it
 	while (num)
@@ -1301,8 +1361,9 @@ int build_hq_launch( const tbvh_bvh* bs, const uint32_t K, float c_trav, float c
 	if (roots)
 	{
 		const uint32_t grid = (roots + HQ_SMALL_WARPS - 1) / HQ_SMALL_WARPS;
-		if (K > 1) k_hq_subtrees<true><<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots ); else k_hq_subtrees<false><<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots );
-		LAUNCHED();
+		void (*subtree_kernel)( HQArgs, uint32_t ) = K > 1 ? (negzero ? k_hq_subtrees<true, true> : k_hq_subtrees<true, false>)
+			: (negzero ? k_hq_subtrees<false, true> : k_hq_subtrees<false, false>);
+		subtree_kernel<<<grid, HQ_SMALL_WARPS * 32, 0, s>>>( A, roots ); LAUNCHED();
 	}
 	CUDA_TRY( cudaMemcpyAsync( h_ctr, A.ctr, sizeof( HQCounters ), cudaMemcpyDeviceToHost, s ) );
 	CUDA_TRY( cudaStreamSynchronize( s ) );
