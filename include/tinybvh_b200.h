@@ -384,6 +384,30 @@ int tbvh_occluded( tbvh_bvh bvh, int layout, const void* rays, uint32_t stride, 
 int tbvh_intersect_device( tbvh_bvh bvh, int layout, void* d_rays, uint32_t stride, void* d_hits, uint64_t n, void* stream );
 int tbvh_occluded_device( tbvh_bvh bvh, int layout, const void* d_rays, uint32_t stride, uint32_t* d_bits, uint64_t n, void* stream );
 
+/* ---- multi-hit rays ------------------------------------------------------------------------------------- */
+/* Every surface a ray crosses, nearest first (DESIGN.md 4.14): the k nearest distinct triangles along each ray and how many it crosses, for
+ * layered transparency and alpha-tested geometry (take the first opaque record), thickness and penetration depth, multi-return sensors and
+ * ray-parity inside tests.  Over the BVH-layout tree of `bvh`, the same handles as tbvh_closest_point.  Rays are the 64-byte device records
+ * (O, D, rD, hit) at `stride` bytes (a multiple of 16, at least 64); hit.t is the ray's tmax, and the rays are not modified.
+ * A child box is reached when its parent is and the slab test of the BVH2 walk passes with the ray's tmax (the root's box is not tested);
+ * its path bound is P = max( P( parent ), the box's entry distance ), P( root ) = 0.  A reference (leaf, triangle) is accepted when the
+ * Moeller-Trumbore test of tbvh_intersect accepts it on [0, tmax] with a t that is not NaN; its key is max( t, P ), which is t wherever
+ * boxes hold their triangles, up to rounding.  Each distinct prim takes its least key (a triangle an SBVH references from several leaves, or
+ * a leaf a DAG reaches twice, counts once), and the result is the k smallest ( key, prim ), ties to the lower prim, whatever the tree's
+ * visiting order.  With k = 1, record 0's t is tbvh_intersect_device's wherever key == t; count > 0 is tbvh_occluded_device's bit, except
+ * for a ray whose tmax is NaN or whose only hits have a NaN t, which that call reports and this one does not.
+ *  tbvh_intersect_all  k in 1 .. TBVH_INTERSECT_ALL_MAX_K (64).  hits: row i at hits + i * k * 16, k records { t, u, v, prim } (the
+ *                      Moeller-Trumbore values) ordered by ( key, prim ), slots past the count { tmax, 0, 0, 0xffffffff }.  counts[i] = the
+ *                      number of distinct prims accepted, saturated at k + 1 (count > k: more than k hits).  A ray whose tmax is NaN or
+ *                      negative gets count 0 and empty slots.
+ * TBVH_DEVICE: asynchronous on `stream` (a cudaStream_t, 0 = default); rays and hits 16-byte aligned, counts 4-byte aligned.  TBVH_HOST:
+ * staged through the device and complete on return (`stream` unused).  n = 0 does nothing.  Refusals, before any launch, leaving the
+ * outputs untouched, in this order: TBVH_E_ARG for NULL arguments, an unknown space, a bad stride, a misaligned device pointer, k outside
+ * 1 .. 64 or a batch too large for one launch; TBVH_E_UNSUPPORTED for a TLAS; TBVH_E_STATE for a handle without a BVH-layout tree (empty,
+ * or a CWBVH-only upload); TBVH_E_LIMIT for a tree deeper than 255. */
+#define TBVH_INTERSECT_ALL_MAX_K 64
+int tbvh_intersect_all( tbvh_bvh bvh, const void* rays, uint32_t stride, uint64_t n, uint32_t k, void* hits, uint32_t* counts, int space, void* stream );
+
 /* ---- proximity queries ---------------------------------------------------------------------------------- */
 /* Nearest surface point and sphere overlap of query points over the BVH-layout tree of `bvh` (the arrays the BVH2 walk reads): builds of
  * every flavour, flat, indexed and batched; BVH_GPU and CWBVH objects built or converted by the library; tbvh_upload_bvh /

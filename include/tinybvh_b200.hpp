@@ -143,6 +143,13 @@ public:
 	// per-ray forms with the reference's signatures (correct, but one PCIe round trip each: use the batch forms)
 	template <class RayT> int32_t Intersect( RayT& ray ) const { return (int32_t)Intersect( &ray, 1 ); }
 	template <class RayT> bool IsOccluded( const RayT& ray ) const { uint32_t b = 0; IsOccluded( &ray, 1, &b ); return b & 1; }
+	// multi-hit rays over the BVH-layout tree (tbvh_intersect_all): hits16 + i * k * 16 holds ray i's k nearest distinct hits { t, u, v,
+	// prim }, nearest first, slots past the count { tmax, 0, 0, 0xffffffff }; counts[i] = the triangles it crosses, saturated at k + 1
+	template <class RayT> void IntersectAll( const RayT* rays, uint64_t n, uint32_t k, void* hits16, uint32_t* counts ) const
+	{
+		static_assert( sizeof( RayT ) == 64 || sizeof( RayT ) == 128, "ray record must be the 64- or 128-byte layout" );
+		TBVH_FATAL_IF( tbvh_intersect_all( h, rays, (uint32_t)sizeof( RayT ), n, k, hits16, counts, TBVH_HOST, 0 ), "IntersectAll" );
+	}
 	// proximity queries over the BVH-layout tree (tbvh_closest_point / tbvh_sphere_overlap), host batches of 16-byte { x, y, z, r }
 	// records (bvhvec4 or any float4-like type).  ClosestPoint: results16[i] = { d, u, v, prim } of the nearest triangle within r, the
 	// point v0 + u (v1 - v0) + v (v2 - v0); { r, 0, 0, 0xffffffff } when none.  IntersectSphere: bit i of bits = some triangle lies within r.

@@ -11,8 +11,10 @@
 //
 //     tbvh::closest_point_bvh( view, q )           tbvh::sphere_overlaps_bvh( view, q )           BVH / BVH_GPU layout, q = { x, y, z, r }
 //
-// The proximity functions return what tbvh_closest_point / tbvh_sphere_overlap write for the same query, bit for bit; they take no warp
-// vote, so any subset of lanes may call them.
+//     tbvh::intersect_all_bvh( view, ray, k, hits )                                               BVH / BVH_GPU layout, multi-hit
+//
+// The proximity functions return what tbvh_closest_point / tbvh_sphere_overlap write for the same query, bit for bit, and intersect_all_bvh
+// what tbvh_intersect_all writes for the same ray; they take no warp vote, so any subset of lanes may call them.
 //
 // The ray is the 64-byte device record in registers (tbvh::Ray: O | mask, D | instIdx, rD | hit.inst, t u v prim).  intersect_*
 // updates ray.hit - and for a TLAS with INST_IDX_BITS 32 the hit.inst word, byte 44 - exactly as tbvh_intersect_device writes those
@@ -35,6 +37,7 @@
 #include "tinybvh_b200_device/bvh2_walk.cuh"
 #include "tinybvh_b200_device/cw_walk.cuh"
 #include "tinybvh_b200_device/closest_walk.cuh"
+#include "tinybvh_b200_device/all_hits_walk.cuh"
 
 namespace tbvh
 {
@@ -301,6 +304,18 @@ __device__ __forceinline__ bool sphere_overlaps_bvh( const tbvh_view& v, const f
 	const float4* nodes = (const float4*)v.nodes, * tris = (const float4*)v.tris;
 	if (v.stack > TBVH_STACK) return cp_overlaps<TBVH_STACK_DEEP>( nodes, tris, v.root_ref, v.root_count, q );
 	return cp_overlaps<TBVH_STACK>( nodes, tris, v.root_ref, v.root_count, q );
+}
+
+// tbvh_intersect_all of one ray over a view of kind TBVH_VIEW_BVH: writes the k records { t, u, v, prim } the batch call writes for the
+// same ray, bit for bit, to hits[0 .. k-1] and returns the count (saturated at k + 1).  A view of another kind gets k empty records
+// { tmax, 0, 0, 0xffffffff } and 0; a k outside 1 .. TBVH_INTERSECT_ALL_MAX_K writes nothing and returns 0.  The ray is not modified.
+__device__ __forceinline__ uint32_t intersect_all_bvh( const tbvh_view& v, const Ray& r, const uint32_t k, float4* hits )
+{
+	if (k < 1 || k > TBVH_INTERSECT_ALL_MAX_K) return 0;
+	if (v.kind != TBVH_VIEW_BVH) { ah_store_empty( hits, k, r.hit.x ); return 0; }
+	const float4* nodes = (const float4*)v.nodes, * tris = (const float4*)v.tris;
+	if (v.stack > TBVH_STACK) return ah_intersect_all<TBVH_STACK_DEEP>( nodes, tris, v.root_ref, v.root_count, r.O, r.D, r.rD, r.hit.x, k, hits );
+	return ah_intersect_all<TBVH_STACK>( nodes, tris, v.root_ref, v.root_count, r.O, r.D, r.rD, r.hit.x, k, hits );
 }
 
 } // namespace tbvh

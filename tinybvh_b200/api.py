@@ -212,6 +212,32 @@ class _Base:
         check(L.tbvh_occluded(self.h, self.layout, _np_ptr(rays), rays.dtype.itemsize, n, _np_ptr(bits)))
         return bits
 
+    # -- multi-hit rays over the BVH-layout tree (tbvh_intersect_all, DESIGN.md §4.14)
+    def intersect_all(self, rays, k, stream=None):
+        """The k nearest distinct triangles along every ray, nearest first, and how many the ray crosses -> (hits, counts).  rays: 64- or
+        128-byte records (hit.t is the ray's tmax; the rays are not modified).  hits (n, k, 4): { t, u, v, prim } records, slots past the
+        count { tmax, 0, 0, 0xffffffff }; counts: the number of distinct triangles crossed, saturated at k + 1 (count > k: more than k).
+        numpy -> host path, hits float32 with prim as uint32 bits in column 3, counts uint32; torch CUDA tensor ([n, 64|128 bytes]) ->
+        queued on `stream` (default: torch's current stream), tensors (counts as int32)."""
+        L = _lib.lib()
+        if _is_torch(rays):
+            import torch
+            assert rays.is_cuda and rays.is_contiguous()
+            stride = rays.stride(0) * rays.element_size()
+            n = rays.shape[0]
+            st = _stream_arg(stream, rays.device)
+            hits = torch.empty((n, k, 4), dtype=torch.float32, device=rays.device)
+            counts = torch.empty(n, dtype=torch.int32, device=rays.device)
+            check(L.tbvh_intersect_all(self.h, C.c_void_p(rays.data_ptr()), stride, n, k, C.c_void_p(hits.data_ptr()),
+                                       C.c_void_p(counts.data_ptr()), DEVICE, C.c_void_p(st)))
+            return hits, counts
+        assert rays.dtype.itemsize in (64, 128) and rays.flags.c_contiguous
+        n = rays.shape[0]
+        hits = np.empty((n, k, 4), np.float32)
+        counts = np.empty(n, np.uint32)
+        check(L.tbvh_intersect_all(self.h, _np_ptr(rays), rays.dtype.itemsize, n, k, _np_ptr(hits), _np_ptr(counts), HOST, None))
+        return hits, counts
+
     # -- proximity queries over the BVH-layout tree (tbvh_closest_point / tbvh_sphere_overlap, DESIGN.md §4.9)
     def closest_point(self, points, r_max=None, stream=None):
         """Nearest triangle within r_max of every point -> (d, u, v, prim): the closest point is v0 + u (v1 - v0) + v (v2 - v0) of
