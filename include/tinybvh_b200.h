@@ -403,10 +403,26 @@ int tbvh_occluded_device( tbvh_bvh bvh, int layout, const void* d_rays, uint32_t
  * TBVH_DEVICE: asynchronous on `stream` (a cudaStream_t, 0 = default); rays and hits 16-byte aligned, counts 4-byte aligned.  TBVH_HOST:
  * staged through the device and complete on return (`stream` unused).  n = 0 does nothing.  Refusals, before any launch, leaving the
  * outputs untouched, in this order: TBVH_E_ARG for NULL arguments, an unknown space, a bad stride, a misaligned device pointer, k outside
- * 1 .. 64 or a batch too large for one launch; TBVH_E_UNSUPPORTED for a TLAS; TBVH_E_STATE for a handle without a BVH-layout tree (empty,
+ * 1 .. 64 or a batch too large for one launch; TBVH_E_UNSUPPORTED for a TLAS (tbvh_intersect_all_tlas); TBVH_E_STATE for a handle without a BVH-layout tree (empty,
  * or a CWBVH-only upload); TBVH_E_LIMIT for a tree deeper than 255. */
 #define TBVH_INTERSECT_ALL_MAX_K 64
 int tbvh_intersect_all( tbvh_bvh bvh, const void* rays, uint32_t stride, uint64_t n, uint32_t k, void* hits, uint32_t* counts, int space, void* stream );
+/* Multi-hit rays through a TLAS over BVH-layout BLASses (DESIGN.md 4.14, two levels): the rules above applied to the TLAS with the world
+ * ray's stored rD, then inside every instance of a reached TLAS leaf whose mask shares a bit with the ray's - the ray transformed into BLAS
+ * space as tbvh_intersect_device does it (rD' = safercp( D' )), the BLAS root reached with the TLAS leaf's path bound and not tested, the
+ * same tmax.  t is shared between world and BLAS space (the direction is not re-normalised), so scaled, mirrored and projective instances
+ * need no other notion of distance.  A hit is an ( instance, prim ) pair: each pair takes its least key (a split triangle or a DAG leaf
+ * counts once per instance), two instances of one BLAS give two hits, and the result is the k smallest ( key, instance, prim ).
+ *  tbvh_intersect_all_tlas  hits as tbvh_intersect_all, prim the BLAS's own triangle number (the context's inst_idx_bits does not apply);
+ *                           insts: row i at insts + i * k, the k instance numbers, 0xffffffff past the count.  counts as tbvh_intersect_all.
+ *                           With k = 1, record 0's t is tbvh_intersect_device's ( TBVH_LAYOUT_BVH ) wherever key == t and count > 0 is
+ *                           tbvh_occluded_device's bit, with the same NaN exceptions.
+ * Spaces as tbvh_intersect_all; device insts 4-byte aligned.  Refusals, before any launch, leaving the outputs untouched, in this order:
+ * TBVH_E_ARG as tbvh_intersect_all and for a NULL or misaligned insts; TBVH_E_UNSUPPORTED for a handle that holds no TLAS; then what
+ * tbvh_intersect_device( tlas, TBVH_LAYOUT_BVH, .. ) refuses: TBVH_E_LIMIT for a BLAS too deep for the two-level walk's 64-entry stack,
+ * TBVH_E_STATE for BLASses without a BVH-layout tree (a TLAS over CWBVH-only BLASses) or a stale TLAS. */
+int tbvh_intersect_all_tlas( tbvh_bvh tlas, const void* rays, uint32_t stride, uint64_t n, uint32_t k, void* hits, uint32_t* insts, uint32_t* counts,
+	int space, void* stream );
 
 /* ---- proximity queries ---------------------------------------------------------------------------------- */
 /* Nearest surface point and sphere overlap of query points over the BVH-layout tree of `bvh` (the arrays the BVH2 walk reads): builds of

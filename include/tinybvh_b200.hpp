@@ -150,6 +150,13 @@ public:
 		static_assert( sizeof( RayT ) == 64 || sizeof( RayT ) == 128, "ray record must be the 64- or 128-byte layout" );
 		TBVH_FATAL_IF( tbvh_intersect_all( h, rays, (uint32_t)sizeof( RayT ), n, k, hits16, counts, TBVH_HOST, 0 ), "IntersectAll" );
 	}
+	// the same over a TLAS (tbvh_intersect_all_tlas): hits16 as above with prim the BLAS's own triangle, insts + i * k the k instances
+	// (0xffffffff past the count)
+	template <class RayT> void IntersectAll( const RayT* rays, uint64_t n, uint32_t k, void* hits16, uint32_t* insts, uint32_t* counts ) const
+	{
+		static_assert( sizeof( RayT ) == 64 || sizeof( RayT ) == 128, "ray record must be the 64- or 128-byte layout" );
+		TBVH_FATAL_IF( tbvh_intersect_all_tlas( h, rays, (uint32_t)sizeof( RayT ), n, k, hits16, insts, counts, TBVH_HOST, 0 ), "IntersectAll (TLAS)" );
+	}
 	// proximity queries over the BVH-layout tree (tbvh_closest_point / tbvh_sphere_overlap), host batches of 16-byte { x, y, z, r }
 	// records (bvhvec4 or any float4-like type).  ClosestPoint: results16[i] = { d, u, v, prim } of the nearest triangle within r, the
 	// point v0 + u (v1 - v0) + v (v2 - v0); { r, 0, 0, 0xffffffff } when none.  IntersectSphere: bit i of bits = some triangle lies within r.

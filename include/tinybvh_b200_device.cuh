@@ -12,9 +12,11 @@
 //     tbvh::closest_point_bvh( view, q )           tbvh::sphere_overlaps_bvh( view, q )           BVH / BVH_GPU layout, q = { x, y, z, r }
 //
 //     tbvh::intersect_all_bvh( view, ray, k, hits )                                               BVH / BVH_GPU layout, multi-hit
+//     tbvh::intersect_all_tlas( view, ray, k, hits, insts )                                       TLAS, BLASses walked in TBVH_LAYOUT_BVH
 //
-// The proximity functions return what tbvh_closest_point / tbvh_sphere_overlap write for the same query, bit for bit, and intersect_all_bvh
-// what tbvh_intersect_all writes for the same ray; they take no warp vote, so any subset of lanes may call them.
+// The proximity functions return what tbvh_closest_point / tbvh_sphere_overlap write for the same query, bit for bit, intersect_all_bvh
+// what tbvh_intersect_all and intersect_all_tlas what tbvh_intersect_all_tlas writes for the same ray; they take no warp vote, so any
+// subset of lanes may call them.
 //
 // The ray is the 64-byte device record in registers (tbvh::Ray: O | mask, D | instIdx, rD | hit.inst, t u v prim).  intersect_*
 // updates ray.hit - and for a TLAS with INST_IDX_BITS 32 the hit.inst word, byte 44 - exactly as tbvh_intersect_device writes those
@@ -150,14 +152,8 @@ template <bool ANYHIT, bool CW> __device__ __forceinline__ bool tlas_trace( cons
 				const float4 r0 = __ldg( ip ), r1 = __ldg( ip + 1 ), r2 = __ldg( ip + 2 ), r3 = __ldg( ip + 3 ), meta = __ldg( ip + 4 );
 				if (!(__float_as_uint( meta.y ) & rmask)) continue;
 				// tinybvh_transform_point / _vector (:513-527) in the reference build's pairing
-				float tox = __fadd_rn( __fmaf_rn( r0.z, oz, __fmaf_rn( r0.x, ox, __fmul_rn( r0.y, oy ) ) ), r0.w );
-				float toy = __fadd_rn( __fmaf_rn( r1.z, oz, __fmaf_rn( r1.x, ox, __fmul_rn( r1.y, oy ) ) ), r1.w );
-				float toz = __fadd_rn( __fmaf_rn( r2.z, oz, __fmaf_rn( r2.x, ox, __fmul_rn( r2.y, oy ) ) ), r2.w );
-				const float w = __fadd_rn( __fmaf_rn( oz, r3.z, __fmaf_rn( ox, r3.x, __fmul_rn( oy, r3.y ) ) ), r3.w );
-				if (!(w == 1.0f)) { const float rw = __fdiv_rn( 1.0f, w ); tox = __fmul_rn( tox, rw ), toy = __fmul_rn( toy, rw ), toz = __fmul_rn( toz, rw ); }
-				const float tdx = __fmaf_rn( r0.z, dz, __fmaf_rn( r0.x, dx, __fmul_rn( r0.y, dy ) ) );
-				const float tdy = __fmaf_rn( r1.z, dz, __fmaf_rn( r1.x, dx, __fmul_rn( r1.y, dy ) ) );
-				const float tdz = __fmaf_rn( r2.z, dz, __fmaf_rn( r2.x, dx, __fmul_rn( r2.y, dy ) ) );
+				float tox, toy, toz, tdx, tdy, tdz;
+				inst_transform( r0, r1, r2, r3, ox, oy, oz, dx, dy, dz, tox, toy, toz, tdx, tdy, tdz );
 				const BlasRef B = blas[__float_as_uint( meta.x )];
 				const float trdx = safercp( tdx ), trdy = safercp( tdy ), trdz = safercp( tdz );
 				bool hit; // any-hit: the ray is occluded; closest hit: the BLAS gave a nearer hit
@@ -316,6 +312,25 @@ __device__ __forceinline__ uint32_t intersect_all_bvh( const tbvh_view& v, const
 	const float4* nodes = (const float4*)v.nodes, * tris = (const float4*)v.tris;
 	if (v.stack > TBVH_STACK) return ah_intersect_all<TBVH_STACK_DEEP>( nodes, tris, v.root_ref, v.root_count, r.O, r.D, r.rD, r.hit.x, k, hits );
 	return ah_intersect_all<TBVH_STACK>( nodes, tris, v.root_ref, v.root_count, r.O, r.D, r.rD, r.hit.x, k, hits );
+}
+
+// tbvh_intersect_all_tlas of one ray over a view of kind TBVH_VIEW_TLAS_BVH (a TLAS view taken for TBVH_LAYOUT_BVH): writes the k records
+// { t, u, v, prim } to hits[0 .. k-1] and the k instances to insts[0 .. k-1] that the batch call writes for the same ray, bit for bit, and
+// returns the count (saturated at k + 1).  A view of another kind - a TLAS view taken for TBVH_LAYOUT_CWBVH included - gets k empty records
+// { tmax, 0, 0, 0xffffffff }, instances 0xffffffff and 0; a k outside 1 .. TBVH_INTERSECT_ALL_MAX_K writes nothing and returns 0.  The ray is
+// not modified.
+__device__ __forceinline__ uint32_t intersect_all_tlas( const tbvh_view& v, const Ray& r, const uint32_t k, float4* hits, uint32_t* insts )
+{
+	if (k < 1 || k > TBVH_INTERSECT_ALL_MAX_K) return 0;
+	if (v.kind != TBVH_VIEW_TLAS_BVH) { ah_store_empty( hits, insts, k, r.hit.x ); return 0; }
+	CpEntry stack[TLAS_STACK], bstack[TBVH_STACK];
+	const float4* nodes = (const float4*)v.nodes;
+	const uint32_t* prim_idx = (const uint32_t*)v.prim_idx;
+	const TlasInst* inst = (const TlasInst*)v.inst;
+	const BlasRef* blas = (const BlasRef*)v.blas;
+	if (k <= TBVH_INTERSECT_ALL_REG_K)
+		return ah_walk_tlas<TBVH_INTERSECT_ALL_REG_K + 1, true>( nodes, prim_idx, inst, blas, v.root_ref, v.root_count, r.O, r.D, r.rD, r.hit.x, k, hits, insts, stack, bstack );
+	return ah_walk_tlas<TBVH_INTERSECT_ALL_MAX_K + 1, false>( nodes, prim_idx, inst, blas, v.root_ref, v.root_count, r.O, r.D, r.rD, r.hit.x, k, hits, insts, stack, bstack );
 }
 
 } // namespace tbvh

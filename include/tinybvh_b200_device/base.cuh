@@ -61,4 +61,20 @@ __device__ __forceinline__ void load_ray( const char* rays, const uint64_t i, co
 struct TlasInst { float inv[16]; uint32_t blasIdx, mask, pad0, pad1; };                                  // 80 bytes
 struct BlasRef { const float4* trav; const float4* tris; uint32_t root_ref, root_count; float cw_rd_limit; uint32_t pad1; const float4* cw_nodes; const float4* cw_tris; }; // 48 bytes: BVH-layout arrays, CWBVH traversal nodes + bvh8Tris (0 when absent) and their rD limit
 
+// A ray in a BLAS's space: O' = transform_point( O, T ), D' = transform_vector( D, T ) for rows r0 .. r3 of an instance's inverse transform
+// (tiny_bvh.h:513-527 in the reference build's pairing: fma( Tz, z, fma( Tx, x, Ty*y ) ) + Tw per row, the point divided by w only when
+// w != 1).  The two-level walks (tlas_trace, ah_walk_tlas) take rD' = safercp( D' ) from it.
+__device__ __forceinline__ void inst_transform( const float4& r0, const float4& r1, const float4& r2, const float4& r3, const float ox, const float oy,
+	const float oz, const float dx, const float dy, const float dz, float& tox, float& toy, float& toz, float& tdx, float& tdy, float& tdz )
+{
+	tox = __fadd_rn( __fmaf_rn( r0.z, oz, __fmaf_rn( r0.x, ox, __fmul_rn( r0.y, oy ) ) ), r0.w );
+	toy = __fadd_rn( __fmaf_rn( r1.z, oz, __fmaf_rn( r1.x, ox, __fmul_rn( r1.y, oy ) ) ), r1.w );
+	toz = __fadd_rn( __fmaf_rn( r2.z, oz, __fmaf_rn( r2.x, ox, __fmul_rn( r2.y, oy ) ) ), r2.w );
+	const float w = __fadd_rn( __fmaf_rn( oz, r3.z, __fmaf_rn( ox, r3.x, __fmul_rn( oy, r3.y ) ) ), r3.w );
+	if (!(w == 1.0f)) { const float rw = __fdiv_rn( 1.0f, w ); tox = __fmul_rn( tox, rw ), toy = __fmul_rn( toy, rw ), toz = __fmul_rn( toz, rw ); }
+	tdx = __fmaf_rn( r0.z, dz, __fmaf_rn( r0.x, dx, __fmul_rn( r0.y, dy ) ) );
+	tdy = __fmaf_rn( r1.z, dz, __fmaf_rn( r1.x, dx, __fmul_rn( r1.y, dy ) ) );
+	tdz = __fmaf_rn( r2.z, dz, __fmaf_rn( r2.x, dx, __fmul_rn( r2.y, dy ) ) );
+}
+
 } // namespace tbvh

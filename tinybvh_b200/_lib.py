@@ -87,6 +87,7 @@ SYMBOLS = {
     "tbvh_intersect_device": (i32, [vp, i32, vp, u32, vp, u64, vp]),
     "tbvh_occluded_device": (i32, [vp, i32, vp, u32, vp, u64, vp]),
     "tbvh_intersect_all": (i32, [vp, vp, u32, u64, u32, vp, vp, i32, vp]),
+    "tbvh_intersect_all_tlas": (i32, [vp, vp, u32, u64, u32, vp, vp, vp, i32, vp]),
     "tbvh_closest_point": (i32, [vp, vp, vp, u64, i32, vp]),
     "tbvh_sphere_overlap": (i32, [vp, vp, vp, u64, i32, vp]),
     "tbvh_signed_distance_prepare": (i32, [vp]),

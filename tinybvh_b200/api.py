@@ -568,6 +568,33 @@ class TLAS(BVH):
         check(_lib.lib().tbvh_build_tlas_update(self.h, p, stride, n, space, hs, len(self.blasses), self.c_trav, self.c_int))
         return self
 
+    def intersect_all(self, rays, k, stream=None):
+        """Multi-hit rays through the TLAS (tbvh_intersect_all_tlas, DESIGN.md §4.14): the k nearest distinct instance hits along every ray,
+        nearest first, and how many the ray crosses -> (hits, insts, counts).  The BLASses are walked in their BVH layout.  hits as
+        BVH.intersect_all with prim the BLAS's own triangle; insts (n, k): the instance of every record, 0xffffffff past the count; counts:
+        the distinct ( instance, prim ) pairs crossed, saturated at k + 1.  numpy -> host path (insts uint32); torch CUDA tensor -> queued on
+        `stream` (default: torch's current stream), tensors (insts and counts as int32)."""
+        L = _lib.lib()
+        if _is_torch(rays):
+            import torch
+            assert rays.is_cuda and rays.is_contiguous()
+            stride = rays.stride(0) * rays.element_size()
+            n = rays.shape[0]
+            st = _stream_arg(stream, rays.device)
+            hits = torch.empty((n, k, 4), dtype=torch.float32, device=rays.device)
+            insts = torch.empty((n, k), dtype=torch.int32, device=rays.device)
+            counts = torch.empty(n, dtype=torch.int32, device=rays.device)
+            check(L.tbvh_intersect_all_tlas(self.h, C.c_void_p(rays.data_ptr()), stride, n, k, C.c_void_p(hits.data_ptr()), C.c_void_p(insts.data_ptr()),
+                                            C.c_void_p(counts.data_ptr()), DEVICE, C.c_void_p(st)))
+            return hits, insts, counts
+        assert rays.dtype.itemsize in (64, 128) and rays.flags.c_contiguous
+        n = rays.shape[0]
+        hits = np.empty((n, k, 4), np.float32)
+        insts = np.empty((n, k), np.uint32)
+        counts = np.empty(n, np.uint32)
+        check(L.tbvh_intersect_all_tlas(self.h, _np_ptr(rays), rays.dtype.itemsize, n, k, _np_ptr(hits), _np_ptr(insts), _np_ptr(counts), HOST, None))
+        return hits, insts, counts
+
 
 def _optimize(obj, max_rounds, c_trav, c_int, layout=LAYOUT_BVH):
     rounds, sah = C.c_uint32(), C.c_float()

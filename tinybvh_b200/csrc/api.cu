@@ -1216,7 +1216,7 @@ static void live_add( tbvh_bvh b ) { std::lock_guard<std::mutex> lk( g_live_mute
 static void live_remove( tbvh_bvh b ) { std::lock_guard<std::mutex> lk( g_live_mutex ); for (size_t i = 0; i < g_live.size(); i++) if (g_live[i] == b) { g_live[i] = g_live.back(); g_live.pop_back(); break; } }
 
 // a TLAS points at the arrays of its BLASses: refuse to walk it once one of them was rebuilt, re-uploaded or destroyed
-static int tlas_check( tbvh_bvh t, int layout )
+extern "C++" int tlas_check( tbvh_bvh t, int layout )
 {
 	// the layout argument of a traversal call on a TLAS names the layout the BLASses are walked in (trace_tlas.cu)
 	const uint32_t want = layout == TBVH_LAYOUT_CWBVH ? 1u << TBVH_LAYOUT_CWBVH : 1u << TBVH_LAYOUT_BVH;

@@ -373,6 +373,9 @@ uint32_t tlas_inst_shift( tbvh_bvh b ); // 32 - INST_IDX_BITS of the context's i
 // the two-level kernel's BVH-layout walk (1 + its number; 0: none).  Reads host state only and touches no handle.
 struct TlasBlasTable { std::vector<BlasRef> refs; uint32_t layouts, deep_blas, deep_depth; };
 int tlas_blas_table( const tbvh_bvh t, const tbvh_bvh* blasses, const uint32_t blas_count, TlasBlasTable& T );
+// the refusals of a traversal call on TLAS t for BLASses walked in `layout` (api.cu): TBVH_E_LIMIT for a BLAS too deep for the BVH-layout
+// walk, TBVH_E_STATE for a BLAS without the layout or a stale TLAS
+int tlas_check( tbvh_bvh t, int layout );
 int tlas_stale_check( tbvh_bvh t ); // TBVH_E_STATE once a BLAS the TLAS was built over has been rebuilt, re-uploaded or destroyed
 // BLASInstance::Update of n records `stride` bytes apart (instance_update.cu): invTransform and world box into the records, the TlasInst
 // entries and the builder's boxes in one pass; *d_bad_blas is set when a record names a BLAS past blas_count
