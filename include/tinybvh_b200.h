@@ -491,10 +491,10 @@ int tbvh_winding_number( tbvh_bvh bvh, const void* queries, float* results, uint
 /* Which triangles of mesh a cross which triangles of mesh b, and (b == a) which triangles of one mesh cross each other (DESIGN.md 4.12).
  * Both handles hold a BVH-layout tree as for tbvh_closest_point; their vertices are taken as they are, in one space (no transforms).
  * The pair test tt_overlap( T, U ) is on closed triangles, so touching counts, and uses orientation predicates only (after Guigue &
- * Devillers 2003), in fp32 in a fixed order: the triangle whose nine coordinates are lexicographically smaller as ordered keys is T,
- * T's v0 is subtracted from all six corners and the differences are scaled by the power of two of their largest magnitude.  So the test
- * is symmetric bit for bit, scaling both meshes by 2^k (k in [-40, 40]) gives the same pairs, and on integer coordinates in [-16, 16]
- * every predicate is exact.  A triangle of zero scaled normal (zero area) or with a NaN or infinite coordinate is never reported.
+ * Devillers 2003), in fp32 in a fixed order: every corner is read as x + 0 (-0 is +0), the triangle whose nine coordinates are then
+ * lexicographically smaller as ordered keys is T, T's v0 is subtracted from all six corners and the differences are scaled by the power
+ * of two of their largest magnitude.  So the test is symmetric bit for bit, a mesh whose zeros are -0 gives the same pairs as with +0,
+ * scaling both meshes by 2^k (k in [-40, 40]) gives the same pairs, and on integer coordinates in [-16, 16] every predicate is exact.  A triangle of zero scaled normal (zero area) or with a NaN or infinite coordinate is never reported.
  * Triangles are the input corners of each handle (the vertices it was built, uploaded or refitted with).
  *  two meshes: the pairs (i, j), i a triangle of a and j of b, such that some reference of j in b's tree is reached (every box on its
  *              path but the root's overlaps the box of triangle i: closed boxes compared in fp32) and tt_overlap holds.  With boxes that
@@ -526,8 +526,9 @@ int tbvh_mesh_overlap_bits( tbvh_bvh a, tbvh_bvh b, uint32_t* bits, int space, v
  * The pair distance tt_dist2( T, U ) is the engine's own, fp32 in a fixed order: a pair with a NaN or infinite coordinate is skipped (never
  * a candidate, not even at r = +inf); a pair that tt_overlap reports (tbvh_mesh_overlap_pairs' test) is at 0; otherwise it is the least of
  * six vertex-triangle distances (the per-triangle function of tbvh_closest_point) and the nine edge-edge distances at interior solutions,
- * on the canonical pair moved to T's v0 and scaled by a power of two.  So it is symmetric bit for bit, and scaling both meshes by 2^k
- * (k in [-40, 40]) scales every distance by exactly 2^k.  A zero-area triangle is never at 0 unless a vertex or edge candidate is.
+ * on the canonical pair (corners read as x + 0, as tt_overlap reads them) moved to T's v0 and scaled by a power of two.  So it is
+ * symmetric bit for bit, -0 and +0 give the same distance bit for bit, and scaling both meshes by 2^k (k in [-40, 40]) scales every
+ * distance by exactly 2^k.  A zero-area triangle is never at 0 unless a vertex or edge candidate is.
  * The value of a reference (leaf, j) of b's tree for triangle i of a is max( tt_dist2, LBtri, P ): LBtri the squared gap of the two
  * triangles' boxes, P the largest squared gap between i's box and a box on the path to the leaf (the root's excepted; the least over
  * several paths).  Where boxes hold their triangles that is tt_dist2 up to rounding.

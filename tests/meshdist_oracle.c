@@ -57,9 +57,11 @@ static float md_seg( const float* p, const float* q, const float* q1 )
 	return tt_dot3( w, w );
 }
 
-/* mesh_distance.cu tt_dist2: a and b are three corners (9 floats) each; NaN when either has a non-finite coordinate */
-float orc_tt_dist2( const float* a, const float* b )
+/* mesh_distance.cu tt_dist2: a and b are three corners (9 floats) each, read as x + 0; NaN when either has a non-finite coordinate */
+float orc_tt_dist2( const float* a_in, const float* b_in )
 {
+	float a[9], b[9];
+	pos9( a_in, a ), pos9( b_in, b );
 	if (!finite9( a ) || !finite9( b )) return NAN;
 	if (orc_tt( a, b, 0 )) return 0.0f;
 	int swap = 0;

@@ -103,9 +103,14 @@ static float pow2( const float m )
 	return s;
 }
 
-/* mesh_overlap.cu mo_test: a and b are three corners (9 floats) each; self = 1 applies the self rules */
-int orc_tt( const float* a, const float* b, const int self )
+/* tri_pair.cuh mo_pos: the corners read as x + 0 (-0 becomes +0, every other value keeps its bits) */
+static void pos9( const float* x, float* r ) { for (int k = 0; k < 9; k++) r[k] = x[k] + 0.0f; }
+
+/* tri_pair.cuh mo_test: a and b are three corners (9 floats) each; self = 1 applies the self rules */
+int orc_tt( const float* a_in, const float* b_in, const int self )
 {
+	float a[9], b[9];
+	pos9( a_in, a ), pos9( b_in, b );
 	for (int k = 0; k < 9; k++) if (!(fabsf( a[k] ) <= FLT_MAX) || !(fabsf( b[k] ) <= FLT_MAX)) return 0;
 	/* the closed boxes of the input corners */
 	for (int k = 0; k < 3; k++)

@@ -141,7 +141,8 @@ class _Track:
 
 
 def _key(f):
-    u = int(np.float32(f).view(np.uint32))
+    """the ordered key of f read as f + 0, as mo_test reads its corners (-0 and +0 one key)"""
+    u = int((np.float32(f) + np.float32(0)).view(np.uint32))
     return (~u) & 0xFFFFFFFF if u & 0x80000000 else u | 0x80000000
 
 

@@ -51,9 +51,10 @@ __device__ __forceinline__ bool md_finite3( const V3* a ) { return mo_finite( a[
 	mo_finite( a[1].x ) && mo_finite( a[1].y ) && mo_finite( a[1].z ) && mo_finite( a[2].x ) && mo_finite( a[2].y ) && mo_finite( a[2].z ); }
 
 // tt_dist2( a, b ), DESIGN.md 4.13, of two finite triangles: 0 when tt_overlap holds, else the least of six vertex-triangle, nine
-// edge-edge and eighteen vertex-edge candidates on the canonical, scaled corners, scaled back
-__device__ __forceinline__ float tt_dist2( const V3* a, const V3* b )
+// edge-edge and eighteen vertex-edge candidates on the canonical, scaled corners, scaled back; the corners read as x + 0 as in mo_test
+__device__ __forceinline__ float tt_dist2( const V3* a_in, const V3* b_in )
 {
+	const V3 a[3] = { mo_pos( a_in[0] ), mo_pos( a_in[1] ), mo_pos( a_in[2] ) }, b[3] = { mo_pos( b_in[0] ), mo_pos( b_in[1] ), mo_pos( b_in[2] ) };
 	if (mo_test<false>( a, b )) return 0.0f;
 	bool swap = false, done = false;
 	#pragma unroll

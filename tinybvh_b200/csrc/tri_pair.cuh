@@ -75,10 +75,14 @@ __device__ __forceinline__ bool mo_seg_tri( const V3& a, const V3& b, const floa
 }
 __device__ __forceinline__ bool mo_finite( const float f ) { return fabsf( f ) <= 3.402823466e38f; }
 __device__ __forceinline__ bool mo_eq( const V3& a, const V3& b ) { return a.x == b.x && a.y == b.y && a.z == b.z; }
+// a corner read as x + 0: -0 becomes +0 and every other value keeps its bits
+__device__ __forceinline__ V3 mo_pos( const V3& a ) { return V3{ __fadd_rn( a.x, 0.0f ), __fadd_rn( a.y, 0.0f ), __fadd_rn( a.z, 0.0f ) }; }
 
-// The pair test of triangles a and b (three corners each), DESIGN.md 4.12; SELF applies the self rules of shared corners.
-template <bool SELF> __device__ __forceinline__ bool mo_test( const V3* a, const V3* b )
+// The pair test of triangles a and b (three corners each), DESIGN.md 4.12; SELF applies the self rules of shared corners.  The corners are
+// read as x + 0, so the canonical order and every step after it are those of the +0 twin: the result does not depend on the sign of zero.
+template <bool SELF> __device__ __forceinline__ bool mo_test( const V3* a_in, const V3* b_in )
 {
+	const V3 a[3] = { mo_pos( a_in[0] ), mo_pos( a_in[1] ), mo_pos( a_in[2] ) }, b[3] = { mo_pos( b_in[0] ), mo_pos( b_in[1] ), mo_pos( b_in[2] ) };
 	#pragma unroll
 	for (int c = 0; c < 3; c++)
 		if (!(mo_finite( a[c].x ) && mo_finite( a[c].y ) && mo_finite( a[c].z ) && mo_finite( b[c].x ) && mo_finite( b[c].y ) && mo_finite( b[c].z ))) return false;
