@@ -20,11 +20,12 @@ def lib():
     global _lib
     if _lib is None:
         portpy.build_lib()   # orc_tlas_walk1, which the included file calls, comes from the oracle library
-        key = hashlib.sha256(b"".join(open(s, "rb").read() for s in _SRCS)).hexdigest()[:16]
+        odir = os.path.dirname(portpy.PORT_SO)
+        # the library's directory is in the key: the object's runpath names it, so another checkout's copy would load that checkout's library
+        key = hashlib.sha256(odir.encode() + b"".join(open(s, "rb").read() for s in _SRCS)).hexdigest()[:16]
         so = os.path.join(tempfile.gettempdir(), f"tbvh_cwbvh_refit_oracle_{os.getuid()}_{key}.so")
         if not os.path.isfile(so):
             tmp = f"{so}.{os.getpid()}.tmp"
-            odir = os.path.dirname(portpy.PORT_SO)
             subprocess.check_call(["gcc", "-std=c11", "-O3", "-mavx2", "-mfma", "-ffp-contract=off", "-fPIC", "-shared", _SRCS[0], "-o", tmp,
                                    "-L" + odir, "-l:" + os.path.basename(portpy.PORT_SO), "-Wl,-rpath," + odir, "-lm"])
             os.replace(tmp, so)

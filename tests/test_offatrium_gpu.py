@@ -13,6 +13,7 @@ from tests.test_build_gpu import assert_same_tree
 from tests.test_build_hq_gpu import assert_same_hq_tree
 from tests.test_convert_gpu import diff_blob, diff_nodes
 from tests.test_tlas_gpu import _CW, words
+from tests.util import family, unit_rays  # noqa: F401 (other test modules import them from here)
 
 pytestmark = pytest.mark.gpu
 
@@ -20,31 +21,6 @@ ZERO = ["zero:pos", "zero:neg", "zero:random", "zero:order"]
 SCALE = ["scale:%d" % k for k in (-126, -100, -60, -6, -4, 8, 16, 24, 30, 40, 90)]
 SHIFT = ["shift:1048576", "shift:-12582912"]   # +2^20, -3 * 2^22
 BUILDERS = {"Build": 0, "BuildAVX": 1, "BuildHQ": 2}
-
-
-def family(fam, ntris, seed=5):
-    kind, arg = fam.split(":")
-    base = scenes.procedural_scene(ntris, seed)
-    if kind == "zero":
-        return util.signed_zero(base, arg, seed)
-    if kind == "scale":
-        return util.scaled(base, int(arg))
-    return util.translated(base, float(arg))
-
-
-def unit_rays(fam, ntris, seed=5, res=24):
-    """Camera rays, axis rays and rays of every octant made at unit scale (moved to 2^k for a scaled family), octant-blocked."""
-    base = scenes.procedural_scene(ntris, seed)
-    kind, arg = fam.split(":")
-    lo, hi = scenes.scene_bounds(base)
-    cam = util.ray_sets(base, res=res)[0]["primary"]
-    ax = util.axis_rays(lo, hi, per_axis=8, seed=seed)
-    r = util.octant_blocks(np.concatenate([cam, ax, util.with_inf_rd(ax), util.octant_rays(lo, hi, 40, seed)]), seed)
-    if kind == "scale":
-        return util.scaled_rays(r, int(arg))
-    if kind == "shift":
-        r["O"] += np.float32(float(arg))
-    return r
 
 
 def engine_tree(v, builder):

@@ -510,6 +510,33 @@ def translated(v, shift):
     return v
 
 
+def family(fam, ntris, seed=5):
+    """The seeded scene of `ntris` triangles in an off-atrium family: "zero:<mode>" (signed_zero), "scale:<k>" (scaled by 2^k) or
+    "shift:<s>" (translated by s)."""
+    kind, arg = fam.split(":")
+    base = scenes.procedural_scene(ntris, seed)
+    if kind == "zero":
+        return signed_zero(base, arg, seed)
+    if kind == "scale":
+        return scaled(base, int(arg))
+    return translated(base, float(arg))
+
+
+def unit_rays(fam, ntris, seed=5, res=24):
+    """Camera rays, axis rays and rays of every octant made at unit scale (moved to 2^k for a scaled family), octant-blocked."""
+    base = scenes.procedural_scene(ntris, seed)
+    kind, arg = fam.split(":")
+    lo, hi = scenes.scene_bounds(base)
+    cam = ray_sets(base, res=res)[0]["primary"]
+    ax = axis_rays(lo, hi, per_axis=8, seed=seed)
+    r = octant_blocks(np.concatenate([cam, ax, with_inf_rd(ax), octant_rays(lo, hi, 40, seed)]), seed)
+    if kind == "scale":
+        return scaled_rays(r, int(arg))
+    if kind == "shift":
+        r["O"] += np.float32(float(arg))
+    return r
+
+
 def snapped(v, q):
     """Positions rounded to multiples of 1 / q, with no -0 left (the + 0.0 turns -0 into +0).  Many fragment bounds then sit on
     the same planes, so BuildHQ's spatial splits often fail (every fragment on one side, tiny_bvh.h:2939), in big nodes too."""
