@@ -546,6 +546,42 @@ int tbvh_mesh_overlap_bits( tbvh_bvh a, tbvh_bvh b, uint32_t* bits, int space, v
 int tbvh_mesh_distance( tbvh_bvh a, tbvh_bvh b, float r_max, void* results, int space, void* stream );
 int tbvh_mesh_distance_pairs( tbvh_bvh a, tbvh_bvh b, float r, uint32_t* pairs, uint64_t capacity, uint64_t* count, int space, void* stream );
 
+/* ---- times of impact between moving meshes ---------------------------------------------------------------- */
+/* When moving meshes first come within a separation (DESIGN.md 4.15): the continuous counterpart of tbvh_mesh_distance for cloth and
+ * IPC-style solvers, motion checks and animated scenes, which a check at the two ends of a step misses when thin or fast geometry passes
+ * through other geometry within it.  Handles and trees as for tbvh_mesh_distance.  Each handle's vertices (as built, uploaded or refitted)
+ * are the start frame; a_end / b_end hold the end frame, the same triangles flat (three vertices per triangle, `stride` bytes apart:
+ * >= 12 and a multiple of 4) in `space`; exactly 3 x prim_count rows of each are read, so a frame must hold them all (after an indexed
+ * build, the vertices through the indices).  Every corner moves linearly over t in [0, 1]: x( t ) = fma( t, x1, fma( -t, x0, x0 ) ).
+ * For one pair the time of contact is found by conservative advancement on tt_dist2 (tbvh_mesh_distance's pair distance) at the
+ * positions at t: starting at t = 0, contact when the distance is <= eta + xi (compared squared), else a step of ( d - eta ) / L, L the
+ * largest |dT_a - dU_b| over the nine corner pairs (d = x1 - x0) rounded up by 2^-16 of itself; no contact when L = 0 or the step
+ * passes t = 1; a step that does not move t, or the step after max_iters of them, ends unresolved with contact at the current t and
+ * iters = max_iters (so a relative displacement above about 1.8e19, whose square overflows L to +inf, ends unresolved at t = 0).  A
+ * resolved t lies between the first times at eta + xi and at eta in exact arithmetic, an unresolved t before the
+ * first time at eta.  The result of a pair is symmetric in its triangles, equal for -0 and +0 corners, and scaling both meshes, eta and
+ * xi by 2^k (k in [-40, 40]) keeps t, j and iters and scales d by 2^k.  A pair with a NaN or infinite corner in either frame is skipped.
+ * A reference (leaf, j) of b's tree is reached for triangle i of a when the squared box-box gap of i's swept box (the box of its six
+ * corners) to every swept box on the path (the box of both frames of every triangle below; the root's excepted), and to j's own swept
+ * box, is <= ( eta + xi )^2.  The swept boxes are built per call from the tree's topology, so every tree tbvh_mesh_distance walks (SBVHs,
+ * uploads whose boxes stick out, DAGs) works and the handles are not modified.
+ *  b == a:  pairs i != j that share no corner (equal as values in both frames); b_end and b_stride must be a_end and a_stride.
+ *  tbvh_mesh_toi        results: n 16-byte records { float t, float d, uint32 j, uint32 iters } (16-byte aligned in device space), n the
+ *           triangles of a: the smallest ( t, j ) over the reached references in contact, d the distance at t; { +inf, +inf, 0xffffffff,
+ *           0 } when there is none or triangle i has a non-finite corner.  TBVH_DEVICE: asynchronous on `stream` (the end frames are read
+ *           in its order).  TBVH_HOST: complete on return (`stream` unused).
+ *  tbvh_mesh_toi_pairs  pairs: every reached (i, j) in contact within the step (b == a: i < j), as tbvh_mesh_distance_pairs returns them
+ *           (capacity pairs, sorted without repeats, *count exact above capacity, synchronous, ordered after `stream` in TBVH_DEVICE,
+ *           TBVH_E_LIMIT above 2^31 raw pairs).  times: NULL, or min( count, capacity ) floats (4-byte aligned in device space), the
+ *           contact time of each pair written.
+ * Refusals, before any launch, leaving the outputs untouched, in this order: TBVH_E_ARG for eta NaN, infinite or negative, xi NaN,
+ * infinite or <= 0, max_iters 0 or above 65536, a NULL end frame, a bad stride, a self query with another end frame, (pairs) misaligned
+ * device times; then tbvh_mesh_overlap_pairs' refusals in their order (TBVH_E_ARG, TBVH_E_UNSUPPORTED, TBVH_E_STATE, TBVH_E_LIMIT). */
+int tbvh_mesh_toi( tbvh_bvh a, const void* a_end, uint32_t a_stride, tbvh_bvh b, const void* b_end, uint32_t b_stride, float eta, float xi, uint32_t max_iters,
+	void* results, int space, void* stream );
+int tbvh_mesh_toi_pairs( tbvh_bvh a, const void* a_end, uint32_t a_stride, tbvh_bvh b, const void* b_end, uint32_t b_stride, float eta, float xi, uint32_t max_iters,
+	uint32_t* pairs, float* times, uint64_t capacity, uint64_t* count, int space, void* stream );
+
 /* Traversal from the caller's own kernels (include/tinybvh_b200_device.cuh): the traversal functions of the reference's GPU code
  * (traverse_cwbvh / isoccluded_cwbvh, traverse_ailalaine, traverse_tlas / isoccluded_tlas, SURVEY.md 2.3) as device functions over a
  * view of a resident tree.  A view holds what the matching tbvh_intersect_device / tbvh_occluded_device launch passes its kernel:

@@ -226,6 +226,31 @@ public:
 		}
 		pairs.resize( count );
 	}
+	// times of impact between moving meshes (tbvh_mesh_toi / tbvh_mesh_toi_pairs, DESIGN.md 4.15): every vertex moves linearly from the
+	// handle's vertices to the host end frames `end` / `other_end` (16-byte rows, the same triangles; other = *this: pass end twice).
+	// TimeOfImpact: results16[i] = { float t, float d, uint32 j, uint32 iters } of the first triangle j of other within eta + xi of triangle i
+	// during the step, { inf, inf, 0xffffffff, 0 } when none.  ImpactPairs: every (i, j) in contact within the step, sorted by (i, j), and
+	// each pair's contact time.
+	template <class Vec4> void TimeOfImpact( const Vec4* end, const BVHBase& other, const Vec4* other_end, const float eta, const float xi,
+		const uint32_t max_iters, void* results16 ) const
+	{
+		TBVH_FATAL_IF( tbvh_mesh_toi( h, end, sizeof( Vec4 ), other.h, other_end, sizeof( Vec4 ), eta, xi, max_iters, results16, TBVH_HOST, 0 ), "TimeOfImpact" );
+	}
+	template <class Vec4> void ImpactPairs( const Vec4* end, const BVHBase& other, const Vec4* other_end, const float eta, const float xi,
+		const uint32_t max_iters, std::vector<std::array<uint32_t, 2>>& pairs, std::vector<float>& times ) const
+	{
+		uint64_t count = 0;
+		pairs.resize( Info().prim_count ), times.resize( pairs.size() );
+		TBVH_FATAL_IF( tbvh_mesh_toi_pairs( h, end, sizeof( Vec4 ), other.h, other_end, sizeof( Vec4 ), eta, xi, max_iters, pairs.empty() ? 0 : pairs[0].data(),
+			times.empty() ? 0 : times.data(), pairs.size(), &count, TBVH_HOST, 0 ), "ImpactPairs" );
+		if (count > pairs.size())
+		{
+			pairs.resize( count ), times.resize( count );
+			TBVH_FATAL_IF( tbvh_mesh_toi_pairs( h, end, sizeof( Vec4 ), other.h, other_end, sizeof( Vec4 ), eta, xi, max_iters, pairs[0].data(), times.data(),
+				pairs.size(), &count, TBVH_HOST, 0 ), "ImpactPairs" );
+		}
+		pairs.resize( count ), times.resize( count );
+	}
 	// BVH::IntersectSphere( pos, r ) tiny_bvh.h:3140 with its signature, one query (a PCIe round trip: batch where you can).  It answers
 	// under this library's definition (DESIGN.md 4.9: some triangle within r by exact closest-point distance), not the reference's
 	// separating-axis test, which may decide otherwise where the sphere only touches a triangle.

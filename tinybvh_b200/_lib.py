@@ -98,6 +98,8 @@ SYMBOLS = {
     "tbvh_mesh_overlap_bits": (i32, [vp, vp, vp, i32, vp]),
     "tbvh_mesh_distance": (i32, [vp, vp, f32, vp, i32, vp]),
     "tbvh_mesh_distance_pairs": (i32, [vp, vp, f32, vp, u64, vp, i32, vp]),
+    "tbvh_mesh_toi": (i32, [vp, vp, u32, vp, vp, u32, f32, f32, u32, vp, i32, vp]),
+    "tbvh_mesh_toi_pairs": (i32, [vp, vp, u32, vp, vp, u32, f32, f32, u32, vp, vp, u64, vp, i32, vp]),
     "tbvh_device_view": (i32, [vp, i32, C.POINTER(DeviceView)]),
     "tbvh_set_stats": (i32, [vp, i32]),
     "tbvh_get_stats": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),

@@ -433,6 +433,93 @@ class _Base:
             check(L.tbvh_mesh_distance_pairs(self.h, o.h, float(r), C.c_void_p(out.data_ptr()), out.shape[0], C.byref(count), DEVICE, C.c_void_p(st)))
         return out[: count.value]
 
+    # -- times of impact between moving meshes (tbvh_mesh_toi / tbvh_mesh_toi_pairs, DESIGN.md §4.15)
+    def _toi_args(self, end, other, other_end, eta, xi, max_iters, stream):
+        """-> (L, o, argument tuple up to max_iters, device or None, keepalive).  Each end frame is (3 * triangles, 3) or (3 * triangles,
+        4) rows of the same mesh's flat vertices (after an indexed build, V1[I]): the C-ABI reads exactly that many rows, so any other
+        shape is refused here.  stream=None: the frames as float32 numpy (host space); else as float32 CUDA tensors on self's device,
+        numpy and CPU tensors copied over on that stream."""
+        if xi is None:
+            raise TbvhError("the resolution xi has no scale-free default: pass it")
+        o = self if other is None else other
+        if o is self:
+            if other_end is not None and other_end is not end:
+                raise TbvhError("a self query takes one end frame: pass end only")
+            frames = [(end, self, "end")]
+        else:
+            if other_end is None:
+                raise TbvhError("the other mesh needs its end frame (other_end)")
+            frames = [(end, self, "end"), (other_end, o, "other_end")]
+        for e, mesh, name in frames:
+            shape = tuple(e.shape) if hasattr(e, "shape") else np.shape(e)
+            rows = 3 * mesh.triCount
+            if len(shape) != 2 or shape[1] not in (3, 4) or shape[0] != rows:
+                raise TbvhError(f"{name} must be ({rows}, 3) or ({rows}, 4): three vertices per triangle of its mesh, not {shape}")
+        dev, keep, ptrs = None, [], []
+        if stream is not None:
+            import torch
+            dev = torch.device("cuda", self.device)
+            with torch.cuda.stream(torch.cuda.ExternalStream(_stream_arg(stream, dev), device=dev)):
+                for e, _, _ in frames:
+                    t = e if _is_torch(e) else torch.as_tensor(np.asarray(e, np.float32))
+                    keep.append(t.to(device=dev, dtype=torch.float32).contiguous())
+            ptrs = [(C.c_void_p(t.data_ptr()), 4 * t.shape[1]) for t in keep]
+        else:
+            for e, _, _ in frames:
+                keep.append(np.ascontiguousarray(e.detach().cpu().numpy() if _is_torch(e) else e, np.float32))
+            ptrs = [(C.c_void_p(a.ctypes.data), 4 * a.shape[1]) for a in keep]
+        pa, sa = ptrs[0]
+        pb, sb = ptrs[-1]
+        return _lib.lib(), o, (self.h, pa, sa, o.h, pb, sb, float(eta), float(xi), int(max_iters)), dev, keep
+
+    def time_of_impact(self, end, other=None, other_end=None, eta=0.0, xi=None, max_iters=64, stream=None):
+        """The first time within the step that a triangle of other comes within eta + xi of each triangle of self -> (t, d, j, iters).
+        Every vertex moves linearly from the handle's current vertices (t = 0) to `end` (t = 1): end holds self's 3 * triCount flat
+        vertices at the end of the step as (3 * triCount, 3) or (3 * triCount, 4) rows (after an indexed build, V1[I]), other_end
+        other's (other=None: the self query of this mesh, pairs that share no corner; other_end, if given, must be end).  Frames of
+        another shape raise TbvhError before any work.  A resolved t lies
+        between the first times at eta + xi and at eta; iters == max_iters marks a pair the advancement did not resolve (t still
+        before the first time at eta).  No contact: t = d = inf, j = 0xffffffff.  xi, the resolution, has no scale-free default.
+        stream=None -> numpy arrays (t, d float32, j, iters uint32); a torch.cuda.Stream (or raw cudaStream_t) -> CUDA tensors (j and
+        iters as int32 bits) queued on that stream, the end frames read in its order."""
+        L, o, args, dev, keep = self._toi_args(end, other, other_end, eta, xi, max_iters, stream)
+        n = self.triCount
+        if dev is None:
+            rec = np.zeros((n, 4), np.float32)
+            check(L.tbvh_mesh_toi(*args, _np_ptr(rec), HOST, None))
+            return rec[:, 0].copy(), rec[:, 1].copy(), rec[:, 2].view(np.uint32).copy(), rec[:, 3].view(np.uint32).copy()
+        import torch
+        st = _stream_arg(stream, dev)
+        with torch.cuda.stream(torch.cuda.ExternalStream(st, device=dev)):
+            rec = torch.empty((max(n, 1), 4), dtype=torch.float32, device=dev)
+            check(L.tbvh_mesh_toi(*args, C.c_void_p(rec.data_ptr()), DEVICE, C.c_void_p(st)))
+        return rec[:n, 0], rec[:n, 1], rec[:n, 2].view(torch.int32), rec[:n, 3].view(torch.int32)
+
+    def impact_pairs(self, end, other=None, other_end=None, eta=0.0, xi=None, max_iters=64, stream=None):
+        """Every pair (i, j) of a triangle of self and a triangle of other that comes within eta + xi during the step, sorted by
+        (i, j), and each pair's contact time -> (pairs (m, 2), times (m,)).  Arguments as time_of_impact; stream and the capacity
+        retry as distance_pairs."""
+        L, o, args, dev, keep = self._toi_args(end, other, other_end, eta, xi, max_iters, stream)
+        n = self.triCount
+        count = C.c_uint64()
+        if dev is None:
+            out, times = np.zeros((max(n, 1), 2), np.uint32), np.zeros(max(n, 1), np.float32)
+            check(L.tbvh_mesh_toi_pairs(*args, _np_ptr(out), _np_ptr(times), out.shape[0], C.byref(count), HOST, None))
+            if count.value > out.shape[0]:
+                out, times = np.zeros((count.value, 2), np.uint32), np.zeros(count.value, np.float32)
+                check(L.tbvh_mesh_toi_pairs(*args, _np_ptr(out), _np_ptr(times), out.shape[0], C.byref(count), HOST, None))
+            return out[: count.value].copy(), times[: count.value].copy()
+        import torch
+        st = _stream_arg(stream, dev)
+        out = torch.empty((max(n, 1), 2), dtype=torch.int32, device=dev)
+        times = torch.empty(max(n, 1), dtype=torch.float32, device=dev)
+        check(L.tbvh_mesh_toi_pairs(*args, C.c_void_p(out.data_ptr()), C.c_void_p(times.data_ptr()), out.shape[0], C.byref(count), DEVICE, C.c_void_p(st)))
+        if count.value > out.shape[0]:
+            out = torch.empty((count.value, 2), dtype=torch.int32, device=dev)
+            times = torch.empty(count.value, dtype=torch.float32, device=dev)
+            check(L.tbvh_mesh_toi_pairs(*args, C.c_void_p(out.data_ptr()), C.c_void_p(times.data_ptr()), out.shape[0], C.byref(count), DEVICE, C.c_void_p(st)))
+        return out[: count.value], times[: count.value]
+
     def device_view(self, layout: int = None) -> _lib.DeviceView:
         """tbvh_device_view: the view a kernel of the caller's passes to the device functions of include/tinybvh_b200_device.cuh, for
         `layout` (default: the layout Intersect walks).  Host work only; valid until the handle's arrays change (include/tinybvh_b200.h)."""

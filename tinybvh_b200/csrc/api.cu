@@ -432,7 +432,7 @@ int tbvh_get_stats_ex( tbvh_bvh b, uint64_t out[4] )
 
 // nv vertices `stride` bytes apart -> rows of a 16-byte-pitch array: the first min( stride, 16 ) bytes of each, so below stride 16
 // the w lane of dst is left as it was
-static int copy_rows( float4* dst, const void* verts, uint32_t stride, size_t nv, int space, cudaStream_t s )
+int copy_rows( float4* dst, const void* verts, uint32_t stride, size_t nv, int space, cudaStream_t s )
 {
 	const cudaMemcpyKind kind = space == TBVH_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
 	if (stride == 16) CUDA_TRY( cudaMemcpyAsync( dst, verts, nv * 16, kind, s ) );

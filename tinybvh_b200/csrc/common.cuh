@@ -381,6 +381,9 @@ int tlas_stale_check( tbvh_bvh t ); // TBVH_E_STATE once a BLAS the TLAS was bui
 // entries and the builder's boxes in one pass; *d_bad_blas is set when a record names a BLAS past blas_count
 int instance_update_launch( void* d_records, uint32_t stride, uint32_t n, const float4* d_blas_box, uint32_t blas_count, void* d_tlas_inst, float4* d_aabbs,
 	uint32_t* d_bad_blas, cudaStream_t s );
+int copy_rows( float4* dst, const void* verts, uint32_t stride, size_t nv, int space, cudaStream_t s ); // vertex rows at a 16-byte pitch (api.cu)
+// the slots of trav() (winding_number.cu): the pair array of a BVH_GPU upload, else the node array up to used_nodes
+uint32_t trav_slots( tbvh_bvh b );
 int make_leaf_tris( tbvh_bvh b, cudaStream_t s );
 int bvh_gpu_to_bvh( tbvh_bvh b, uint32_t used_nodes_gpu, cudaStream_t s );
 int bvh_to_bvh_gpu( tbvh_bvh b, cudaStream_t s ); // sets the BVH_GPU bit on success; on failure the handle holds no BVH_GPU

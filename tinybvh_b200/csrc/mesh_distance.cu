@@ -12,114 +12,6 @@ namespace
 enum { MD_NEAREST = 0, MD_COUNT = 1, MD_FILL = 2 };
 
 struct MdRec { float d; uint32_t j; }; // the 8-byte result record of one triangle of A
-
-__device__ __forceinline__ float4 md_f4( const V3& a ) { return make_float4( a.x, a.y, a.z, 0.0f ); }
-
-// the squared distance between a point and the triangle (v0, v1, v2): the 4.9 per-triangle function on (v0, v1 - v0, v2 - v0)
-__device__ __forceinline__ float md_point( const V3& p, const V3& v0, const V3& v1, const V3& v2 )
-{
-	float u, v;
-	return tbvh::cp_triangle( p.x, p.y, p.z, md_f4( v0 ), md_f4( v3sub( v1, v0 ) ), md_f4( v3sub( v2, v0 ) ), u, v );
-}
-
-// the edge-edge candidate of (p, p + d1) and (q, q + d2): |r + s d1 - t d2|^2, r = p - q, at the unclamped solution s = ((q - p) x d2) . n /
-// |n|^2, t = ((q - p) x d1) . n / |n|^2, n = d1 x d2, when |n|^2 > 0 and s, t lie in [0, 1]; +inf (no candidate) otherwise.  The cross
-// products keep s and t accurate on nearly parallel edges, where Ericson's a e - b b loses its digits.
-__device__ __forceinline__ float md_edges( const V3& p, const V3& p1, const V3& q, const V3& q1 )
-{
-	const V3 d1 = v3sub( p1, p ), d2 = v3sub( q1, q ), r = v3sub( p, q ), w = v3sub( q, p );
-	const V3 n = v3cross( d1, d2 );
-	const float nn = v3dot( n, n );
-	if (!(nn > 0.0f)) return __int_as_float( 0x7f800000 );
-	const float s = __fdiv_rn( v3dot( v3cross( w, d2 ), n ), nn ), t = __fdiv_rn( v3dot( v3cross( w, d1 ), n ), nn );
-	if (!(s >= 0.0f && s <= 1.0f && t >= 0.0f && t <= 1.0f)) return __int_as_float( 0x7f800000 );
-	const V3 x{ __fsub_rn( __fmaf_rn( s, d1.x, r.x ), __fmul_rn( t, d2.x ) ), __fsub_rn( __fmaf_rn( s, d1.y, r.y ), __fmul_rn( t, d2.y ) ),
-		__fsub_rn( __fmaf_rn( s, d1.z, r.z ), __fmul_rn( t, d2.z ) ) };
-	return v3dot( x, x );
-}
-
-// the squared distance from p to the segment (q, q + d), d = q1 - q: the projection parameter clamped to [0, 1] (0 / 0 gives q)
-__device__ __forceinline__ float md_seg( const V3& p, const V3& q, const V3& q1 )
-{
-	const V3 d = v3sub( q1, q ), r = v3sub( p, q );
-	const float t = tbvh::cp_edge( v3dot( r, d ), v3dot( d, d ) );
-	const V3 w{ __fsub_rn( r.x, __fmul_rn( t, d.x ) ), __fsub_rn( r.y, __fmul_rn( t, d.y ) ), __fsub_rn( r.z, __fmul_rn( t, d.z ) ) };
-	return v3dot( w, w );
-}
-
-__device__ __forceinline__ bool md_finite3( const V3* a ) { return mo_finite( a[0].x ) && mo_finite( a[0].y ) && mo_finite( a[0].z ) &&
-	mo_finite( a[1].x ) && mo_finite( a[1].y ) && mo_finite( a[1].z ) && mo_finite( a[2].x ) && mo_finite( a[2].y ) && mo_finite( a[2].z ); }
-
-// tt_dist2( a, b ), DESIGN.md 4.13, of two finite triangles: 0 when tt_overlap holds, else the least of six vertex-triangle, nine
-// edge-edge and eighteen vertex-edge candidates on the canonical, scaled corners, scaled back; the corners read as x + 0 as in mo_test
-__device__ __forceinline__ float tt_dist2( const V3* a_in, const V3* b_in )
-{
-	const V3 a[3] = { mo_pos( a_in[0] ), mo_pos( a_in[1] ), mo_pos( a_in[2] ) }, b[3] = { mo_pos( b_in[0] ), mo_pos( b_in[1] ), mo_pos( b_in[2] ) };
-	if (mo_test<false>( a, b )) return 0.0f;
-	bool swap = false, done = false;
-	#pragma unroll
-	for (int k = 0; k < 9; k++)
-	{
-		const uint32_t ka = f2key( v3c( a[k / 3], k % 3 ) ), kb = f2key( v3c( b[k / 3], k % 3 ) );
-		if (!done && ka != kb) swap = kb < ka, done = true;
-	}
-	const V3* rt = swap ? b : a, * ru = swap ? a : b;
-	V3 T[3], U[3];
-	float m = 0.0f;
-	#pragma unroll
-	for (int c = 0; c < 3; c++)
-	{
-		T[c] = v3sub( rt[c], rt[0] );
-		m = fmaxf( m, fabsf( T[c].x ) ), m = fmaxf( m, fabsf( T[c].y ) ), m = fmaxf( m, fabsf( T[c].z ) );
-	}
-	#pragma unroll
-	for (int c = 0; c < 3; c++)
-	{
-		U[c] = v3sub( ru[c], rt[0] );
-		m = fmaxf( m, fabsf( U[c].x ) ), m = fmaxf( m, fabsf( U[c].y ) ), m = fmaxf( m, fabsf( U[c].z ) );
-	}
-	float inv;
-	const float s = tbvh::cp_pow2( m, inv );
-	#pragma unroll
-	for (int c = 0; c < 3; c++)
-	{
-		T[c] = V3{ __fmul_rn( T[c].x, s ), __fmul_rn( T[c].y, s ), __fmul_rn( T[c].z, s ) };
-		U[c] = V3{ __fmul_rn( U[c].x, s ), __fmul_rn( U[c].y, s ), __fmul_rn( U[c].z, s ) };
-	}
-	// U's corners against T, then T's against U, then the edges (T's edge k from corner k to k + 1) against U's
-	float d = md_point( U[0], T[0], T[1], T[2] );
-	d = fminf( d, md_point( U[1], T[0], T[1], T[2] ) );
-	d = fminf( d, md_point( U[2], T[0], T[1], T[2] ) );
-	d = fminf( d, md_point( T[0], U[0], U[1], U[2] ) );
-	d = fminf( d, md_point( T[1], U[0], U[1], U[2] ) );
-	d = fminf( d, md_point( T[2], U[0], U[1], U[2] ) );
-	#pragma unroll
-	for (int k = 0; k < 3; k++)
-		#pragma unroll
-		for (int l = 0; l < 3; l++) d = fminf( d, md_edges( T[k], T[(k + 1) % 3], U[l], U[(l + 1) % 3] ) );
-	// every corner against every edge of the other: exact where the per-triangle function's regions misplace the point (an edge of zero
-	// length), and the endpoint cases of the edge pairs
-	#pragma unroll
-	for (int k = 0; k < 3; k++)
-		#pragma unroll
-		for (int l = 0; l < 3; l++) d = fminf( fminf( d, md_seg( U[k], T[l], T[(l + 1) % 3] ) ), md_seg( T[k], U[l], U[(l + 1) % 3] ) );
-	return __fmul_rn( __fmul_rn( d, inv ), inv );
-}
-
-// the box-box bound of the box [mn, mx] against [bmin, bmax]: per axis g = max( bmin - mx, mn - bmax, 0 ), then fma( gz, gz, fma( gy, gy,
-// gx gx ) ); every step is monotone in both boxes
-__device__ __forceinline__ float md_box_bound( const V3& mn, const V3& mx, const float bminx, const float bminy, const float bminz,
-	const float bmaxx, const float bmaxy, const float bmaxz )
-{
-	const float gx = fmaxf( fmaxf( __fsub_rn( bminx, mx.x ), __fsub_rn( mn.x, bmaxx ) ), 0.0f );
-	const float gy = fmaxf( fmaxf( __fsub_rn( bminy, mx.y ), __fsub_rn( mn.y, bmaxy ) ), 0.0f );
-	const float gz = fmaxf( fmaxf( __fsub_rn( bminz, mx.z ), __fsub_rn( mn.z, bmaxz ) ), 0.0f );
-	return __fmaf_rn( gz, gz, __fmaf_rn( gy, gy, __fmul_rn( gx, gx ) ) );
-}
-__device__ __forceinline__ float md_node_bound( const V3& mn, const V3& mx, const float4& bmin, const float4& bmax )
-{
-	return md_box_bound( mn, mx, bmin.x, bmin.y, bmin.z, bmax.x, bmax.y, bmax.z );
-}
 } // namespace
 
 // One thread per triangle i of A in 128-thread CTAs; B's BVH2 walked as cp_walk walks it, with the box-box bound of i's box against each

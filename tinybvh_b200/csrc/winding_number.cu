@@ -311,8 +311,7 @@ __global__ void __launch_bounds__( 128 ) k_winding_number( const float4* __restr
 	results[i] = r == r ? r : __uint_as_float( WN_NAN );
 }
 
-// the slots of trav(): the pair array of a BVH_GPU upload, else the node array up to used_nodes
-static uint32_t wn_slots( tbvh_bvh b )
+uint32_t trav_slots( tbvh_bvh b )
 {
 	if (b->d_pairs.p) return (uint32_t)(b->d_pairs.bytes / 32);
 	return (uint32_t)std::min<size_t>( std::max( b->info.used_nodes, 2u ), b->d_nodes.bytes / 32 );
@@ -331,7 +330,7 @@ int wn_table_check( tbvh_bvh b )
 
 int wn_launch( tbvh_bvh b, const float4* d_queries, float* d_results, uint64_t n, float beta, cudaStream_t s )
 {
-	const uint32_t grid = (uint32_t)((n + 127) / 128), S = wn_slots( b );
+	const uint32_t grid = (uint32_t)((n + 127) / 128), S = trav_slots( b );
 	if (b->info.max_depth + 1 > TBVH_STACK)
 		k_winding_number<TBVH_STACK_DEEP><<<grid, 128, 0, s>>>( b->trav(), b->d_wn_own, b->d_verts, b->d_wn, d_queries, d_results, n, beta, b->root_ref, b->root_count, S );
 	else k_winding_number<TBVH_STACK><<<grid, 128, 0, s>>>( b->trav(), b->d_wn_own, b->d_verts, b->d_wn, d_queries, d_results, n, beta, b->root_ref, b->root_count, S );
@@ -342,7 +341,7 @@ int wn_launch( tbvh_bvh b, const float4* d_queries, float* d_results, uint64_t n
 // the records and ownership of b's tree into table / own (allocated here), on s; *flag: WN_DAG / WN_RANGE
 static int wn_prepare( tbvh_bvh b, DevArray<float4>& table, DevArray<uint32_t>& own, uint32_t* flag, cudaStream_t s )
 {
-	const uint32_t S = wn_slots( b ), refs = b->info.idx_count, prims = b->info.prim_count, depth = b->info.max_depth;
+	const uint32_t S = trav_slots( b ), refs = b->info.idx_count, prims = b->info.prim_count, depth = b->info.max_depth;
 	const WnTree T = { b->trav(), b->d_leaf_tris, S, b->root_ref, b->root_count, b->d_pairs.p ? 0u : 1u, refs, prims };
 	TRY( table.alloc( ((size_t)S + 1) * WN_REC * 16 ) );
 	TRY( own.alloc( (size_t)std::max( refs, 1u ) * 4 ) );
