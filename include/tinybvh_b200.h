@@ -444,6 +444,33 @@ int tbvh_intersect_all_tlas( tbvh_bvh tlas, const void* rays, uint32_t stride, u
 int tbvh_closest_point( tbvh_bvh bvh, const void* queries, void* results, uint64_t n, int space, void* stream );
 int tbvh_sphere_overlap( tbvh_bvh bvh, const void* queries, uint32_t* bits, uint64_t n, int space, void* stream );
 
+/* ---- sphere casts --------------------------------------------------------------------------------------- */
+/* The first time a sphere moving along a line touches a triangle (DESIGN.md 4.16), over the BVH-layout tree of `bvh`: the same handles as
+ * tbvh_closest_point.  A query is 32 bytes, { cx, cy, cz, r }, { dx, dy, dz, tmax }: the centre at t is c + t D, t in [0, tmax], D not
+ * normalised (a unit D with tmax a distance, or a displacement with tmax = 1).  The sphere touches a triangle at t when the distance from
+ * c + t D to the closed, two-sided triangle is <= r.  Per triangle: t = 0 with tbvh_closest_point's (u, v) when the sphere already
+ * touches it (the sphere-overlap test); else the least time in [0, tmax] at which it meets the face (the sphere's touching point inside
+ * the triangle), an edge (AB, AC, BC: the cylinder around it, at an edge parameter in [0, 1]) or a vertex (A, B, C), ties in that order,
+ * with the contact point's (u, v): the face's barycentrics, (s, 0) / (0, s) / (1 - s, s) on an edge, (0, 0) / (1, 0) / (0, 1) at a
+ * vertex.  fp32 in a fixed order, on c - v0, e1, e2 and r scaled by one power of two and D by another: scaling the mesh and the query by
+ * 2^k (k in [-40, 40]) gives the same records, and D by 2^m with tmax by 2^-m gives t times 2^-m, bit for bit.
+ * Over the tree: a child is reached when its parent is and the line c + t D on [0, tmax] meets its box inflated by r (rounded outward;
+ * the root box is not tested), its path bound P is the larger of its parent's and its entry time, and a reference (leaf, triangle) in
+ * contact at t_tri has key max( t_tri, P( leaf ) ).  Results are the smallest ( key, prim ), whatever the tree's visiting order.
+ *  tbvh_sphere_cast           results: n 16-byte records { t, u, v, prim } (t = t_tri); nothing touched in [0, tmax]: { tmax, 0, 0,
+ *                             0xffffffff }.
+ *  tbvh_sphere_cast_occluded  bits[i>>5] bit (i&31) = some reached triangle is touched in [0, tmax]; (n+31)/32 words are written, bits
+ *                             past n are 0.
+ * A query with a NaN or infinite coordinate of c or D, an r not finite or below 0, or a tmax NaN or below 0 gets the miss record and
+ * bit 0 without a walk (tmax = INFINITY is allowed).  A contact normal is normalize( c + t D - p(u, v) ).
+ * TBVH_DEVICE: asynchronous on `stream` (a cudaStream_t, 0 = default), queries and results 16-byte aligned.  TBVH_HOST: staged through
+ * the device and complete on return (`stream` unused).  n = 0 does nothing.  Refusals, before any launch and leaving the outputs
+ * untouched, in this order: TBVH_E_ARG for NULL arguments, an unknown space, a misaligned device pointer or a batch too large for one
+ * launch; TBVH_E_UNSUPPORTED for a TLAS (a sphere does not survive non-rigid instance transforms); TBVH_E_STATE for a handle without a
+ * BVH-layout tree (empty, or a CWBVH-only upload); TBVH_E_LIMIT for a tree deeper than 255. */
+int tbvh_sphere_cast( tbvh_bvh bvh, const void* queries, void* results, uint64_t n, int space, void* stream );
+int tbvh_sphere_cast_occluded( tbvh_bvh bvh, const void* queries, uint32_t* bits, uint64_t n, int space, void* stream );
+
 /* ---- signed distances ----------------------------------------------------------------------------------- */
 /* Signed distance of query points to the triangles of `bvh` (DESIGN.md 4.10): the closest-point query above, signed by the angle-weighted
  * pseudonormal (Baerentzen & Aanaes 2005) of the feature - face, edge or vertex - the closest point lies on.  Topology comes from

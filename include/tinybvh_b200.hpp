@@ -170,6 +170,19 @@ public:
 		static_assert( sizeof( Vec4 ) == 16, "queries are 16-byte { x, y, z, r } records" );
 		TBVH_FATAL_IF( tbvh_sphere_overlap( h, q, bits, n, TBVH_HOST, 0 ), "IntersectSphere" );
 	}
+	// sphere casts (tbvh_sphere_cast / tbvh_sphere_cast_occluded), host batches of 32-byte { cx, cy, cz, r, dx, dy, dz, tmax } records: the
+	// sphere's centre moves along c + t D, t in [0, tmax].  SphereCast: results16[i] = { t, u, v, prim } of the first triangle it touches,
+	// at the point v0 + u (v1 - v0) + v (v2 - v0); { tmax, 0, 0, 0xffffffff } when none.  SphereCastOccluded: bit i of bits = it touches one.
+	template <class Query> void SphereCast( const Query* q, uint64_t n, void* results16 ) const
+	{
+		static_assert( sizeof( Query ) == 32, "queries are 32-byte { cx, cy, cz, r, dx, dy, dz, tmax } records" );
+		TBVH_FATAL_IF( tbvh_sphere_cast( h, q, results16, n, TBVH_HOST, 0 ), "SphereCast" );
+	}
+	template <class Query> void SphereCastOccluded( const Query* q, uint64_t n, uint32_t* bits ) const
+	{
+		static_assert( sizeof( Query ) == 32, "queries are 32-byte { cx, cy, cz, r, dx, dy, dz, tmax } records" );
+		TBVH_FATAL_IF( tbvh_sphere_cast_occluded( h, q, bits, n, TBVH_HOST, 0 ), "SphereCastOccluded" );
+	}
 	// signed distances (tbvh_signed_distance_prepare / tbvh_signed_distance): PrepareSignedDistance builds the pseudonormal table once per
 	// tree and vertex set (again after any rebuild or refit); SignedDistance: results16[i] = { sd, u, v, prim }, ClosestPoint's record with
 	// the distance negative inside a closed, outward-oriented mesh.

@@ -10,11 +10,13 @@
 //     tbvh::intersect_tlas<LAYOUT>( view, ray )    tbvh::isoccluded_tlas<LAYOUT>( view, ray )     TLAS, BLASses walked in LAYOUT
 //
 //     tbvh::closest_point_bvh( view, q )           tbvh::sphere_overlaps_bvh( view, q )           BVH / BVH_GPU layout, q = { x, y, z, r }
+//     tbvh::sphere_cast_bvh( view, q0, q1 )        tbvh::sphere_cast_occluded_bvh( view, q0, q1 ) BVH / BVH_GPU layout, sphere cast
 //
 //     tbvh::intersect_all_bvh( view, ray, k, hits )                                               BVH / BVH_GPU layout, multi-hit
 //     tbvh::intersect_all_tlas( view, ray, k, hits, insts )                                       TLAS, BLASses walked in TBVH_LAYOUT_BVH
 //
-// The proximity functions return what tbvh_closest_point / tbvh_sphere_overlap write for the same query, bit for bit, intersect_all_bvh
+// The proximity functions return what tbvh_closest_point / tbvh_sphere_overlap write for the same query, bit for bit, the sphere casts
+// what tbvh_sphere_cast / tbvh_sphere_cast_occluded write, intersect_all_bvh
 // what tbvh_intersect_all and intersect_all_tlas what tbvh_intersect_all_tlas writes for the same ray; they take no warp vote, so any
 // subset of lanes may call them.
 //
@@ -39,6 +41,7 @@
 #include "tinybvh_b200_device/bvh2_walk.cuh"
 #include "tinybvh_b200_device/cw_walk.cuh"
 #include "tinybvh_b200_device/closest_walk.cuh"
+#include "tinybvh_b200_device/sweep_walk.cuh"
 #include "tinybvh_b200_device/all_hits_walk.cuh"
 
 namespace tbvh
@@ -300,6 +303,24 @@ __device__ __forceinline__ bool sphere_overlaps_bvh( const tbvh_view& v, const f
 	const float4* nodes = (const float4*)v.nodes, * tris = (const float4*)v.tris;
 	if (v.stack > TBVH_STACK) return cp_overlaps<TBVH_STACK_DEEP>( nodes, tris, v.root_ref, v.root_count, q );
 	return cp_overlaps<TBVH_STACK>( nodes, tris, v.root_ref, v.root_count, q );
+}
+
+// tbvh_sphere_cast of one query q0 = { cx, cy, cz, r }, q1 = { dx, dy, dz, tmax } over a view of kind TBVH_VIEW_BVH: the record
+// { t, u, v, prim } the batch call writes, bit for bit; { tmax, 0, 0, 0xffffffff } when nothing is touched, and for a view of another kind
+__device__ __forceinline__ float4 sphere_cast_bvh( const tbvh_view& v, const float4& q0, const float4& q1 )
+{
+	if (v.kind != TBVH_VIEW_BVH) return make_float4( q1.w, 0.0f, 0.0f, __uint_as_float( CP_NO_PRIM ) );
+	const float4* nodes = (const float4*)v.nodes, * tris = (const float4*)v.tris;
+	if (v.stack > TBVH_STACK) return sc_cast<TBVH_STACK_DEEP>( nodes, tris, v.root_ref, v.root_count, q0, q1 );
+	return sc_cast<TBVH_STACK>( nodes, tris, v.root_ref, v.root_count, q0, q1 );
+}
+// tbvh_sphere_cast_occluded of one query: the bit the batch call writes (false for a view of another kind)
+__device__ __forceinline__ bool sphere_cast_occluded_bvh( const tbvh_view& v, const float4& q0, const float4& q1 )
+{
+	if (v.kind != TBVH_VIEW_BVH) return false;
+	const float4* nodes = (const float4*)v.nodes, * tris = (const float4*)v.tris;
+	if (v.stack > TBVH_STACK) return sc_blocked<TBVH_STACK_DEEP>( nodes, tris, v.root_ref, v.root_count, q0, q1 );
+	return sc_blocked<TBVH_STACK>( nodes, tris, v.root_ref, v.root_count, q0, q1 );
 }
 
 // tbvh_intersect_all of one ray over a view of kind TBVH_VIEW_BVH: writes the k records { t, u, v, prim } the batch call writes for the

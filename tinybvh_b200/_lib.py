@@ -90,6 +90,8 @@ SYMBOLS = {
     "tbvh_intersect_all_tlas": (i32, [vp, vp, u32, u64, u32, vp, vp, vp, i32, vp]),
     "tbvh_closest_point": (i32, [vp, vp, vp, u64, i32, vp]),
     "tbvh_sphere_overlap": (i32, [vp, vp, vp, u64, i32, vp]),
+    "tbvh_sphere_cast": (i32, [vp, vp, vp, u64, i32, vp]),
+    "tbvh_sphere_cast_occluded": (i32, [vp, vp, vp, u64, i32, vp]),
     "tbvh_signed_distance_prepare": (i32, [vp]),
     "tbvh_signed_distance": (i32, [vp, vp, vp, u64, i32, vp]),
     "tbvh_winding_number_prepare": (i32, [vp]),

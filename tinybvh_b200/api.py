@@ -118,6 +118,75 @@ def _torch_queries(points, r):
     return q
 
 
+def _torch_stream(stream, device):
+    """the torch stream object of a `stream` argument: torch's current stream on `device` for None, a torch.cuda.Stream as it is, a raw
+    cudaStream_t wrapped.  The current stream is used as the object torch holds, not re-wrapped from its handle: torch does not order an
+    ExternalStream made from the default stream's handle 0 after work on that stream."""
+    import torch
+    if stream is None:
+        return torch.cuda.current_stream(device)
+    if isinstance(stream, torch.cuda.Stream):
+        return stream
+    return torch.cuda.ExternalStream(stream, device=device)
+
+
+def _sweep_rows(centers, directions, radii, tmax):
+    """The checks of a sphere-cast batch, before any native call: (n, 8) records alone, or centres (n, 3) with radii (a scalar or one per
+    row) or (n, 4) {x, y, z, r} rows, and directions (n, 3) with tmax (a scalar or one per row; default inf) or (n, 4) {dx, dy, dz, tmax}
+    rows.  Raises TbvhError on anything else."""
+    if centers.ndim != 2 or centers.shape[1] not in (3, 4, 8):
+        raise TbvhError("centers must be (n, 3), (n, 4) or (n, 8) records")
+    n = centers.shape[0]
+    if centers.shape[1] == 8:
+        if directions is not None or radii is not None or tmax is not None:
+            raise TbvhError("(n, 8) records carry the radius, the direction and tmax: pass nothing else")
+        return
+    if directions is None or directions.ndim != 2 or directions.shape[0] != n or directions.shape[1] not in (3, 4):
+        raise TbvhError("directions must be (n, 3) or (n, 4) with one row per centre")
+    for a, name, cols in ((radii, "radii", centers.shape[1]), (tmax, "tmax", directions.shape[1])):
+        if cols == 4 and a is not None:
+            raise TbvhError(f"(n, 4) rows carry {name} in their fourth column: pass no {name} argument")
+        if a is not None and np.ndim(a) not in (0,) and tuple(np.shape(a)) != (n,):
+            raise TbvhError(f"{name} must be a scalar or one value per row")
+    if centers.shape[1] == 3 and radii is None:
+        raise TbvhError("(n, 3) centres need a radius argument")
+
+
+def _np_sweeps(centers, directions, radii, tmax):
+    """-> contiguous float32 (n, 8) records { cx, cy, cz, r, dx, dy, dz, tmax } (_sweep_rows's rules)"""
+    c = np.asarray(centers, np.float32)
+    d = None if directions is None else np.asarray(directions, np.float32)
+    _sweep_rows(c, d, radii, tmax)
+    if c.shape[1] == 8:
+        return np.ascontiguousarray(c)
+    q = np.empty((c.shape[0], 8), np.float32)
+    q[:, :4] = c if c.shape[1] == 4 else 0
+    q[:, 4:8] = d if d.shape[1] == 4 else 0
+    if c.shape[1] == 3:
+        q[:, :3], q[:, 3] = c, np.asarray(radii, np.float32)
+    if d.shape[1] == 3:
+        q[:, 4:7], q[:, 7] = d, np.asarray(np.inf if tmax is None else tmax, np.float32)
+    return q
+
+
+def _torch_sweeps(centers, directions, radii, tmax):
+    """_np_sweeps for CUDA tensors, made on torch's current stream"""
+    import torch
+    assert centers.is_cuda and (directions is None or directions.is_cuda), "centers and directions must be CUDA tensors"
+    _sweep_rows(centers, directions, None if radii is None else torch.as_tensor(radii).cpu() if _is_torch(radii) else radii,
+                None if tmax is None else torch.as_tensor(tmax).cpu() if _is_torch(tmax) else tmax)
+    if centers.shape[1] == 8:
+        return centers.to(torch.float32).contiguous()
+    q = torch.empty((centers.shape[0], 8), dtype=torch.float32, device=centers.device)
+    q[:, : centers.shape[1]] = centers
+    q[:, 4: 4 + directions.shape[1]] = directions
+    if centers.shape[1] == 3:
+        q[:, 3] = torch.as_tensor(radii, dtype=torch.float32, device=centers.device)
+    if directions.shape[1] == 3:
+        q[:, 7] = torch.as_tensor(np.inf if tmax is None else tmax, dtype=torch.float32, device=centers.device)
+    return q
+
+
 class _Base:
     layout = LAYOUT_BVH
     build_flavour = _lib.BUILD_AVX   # derived layouts build through BuildDefault; set to _lib.BUILD_REFERENCE for BVH::Build's tree
@@ -276,6 +345,51 @@ class _Base:
         n = q.shape[0]
         words = np.zeros(max((n + 31) // 32, 1), np.uint32)
         check(L.tbvh_sphere_overlap(self.h, _np_ptr(q), _np_ptr(words), n, HOST, None))
+        return np.unpackbits(words.view(np.uint8), bitorder="little")[:n].astype(bool)
+
+    # -- sphere casts over the BVH-layout tree (tbvh_sphere_cast / tbvh_sphere_cast_occluded, DESIGN.md §4.16)
+    def sphere_cast(self, centers, directions=None, radii=None, tmax=None, stream=None):
+        """The first contact of a sphere moving from each centre along c + t D, t in [0, tmax] -> (t, u, v, prim): the sphere first touches
+        triangle prim at t, at its point v0 + u (v1 - v0) + v (v2 - v0); t = 0 when it already touches; prim 0xffffffff and t = tmax when it
+        touches nothing.  D need not be unit: a unit D with tmax a distance, or a displacement with tmax = 1.  centers: (n, 3) with radii a
+        scalar or one per row, or (n, 4) {x, y, z, r}; directions: (n, 3) with tmax a scalar or one per row (default inf), or (n, 4)
+        {dx, dy, dz, tmax}; or centers alone as the C-ABI's (n, 8) records.  TbvhError on mismatched shapes.  numpy -> host path, numpy
+        arrays (prim uint32); torch CUDA tensors -> everything queued on `stream` (default: torch's current stream), tensors (prim as int32
+        bits).  The contact normal is normalize( c + t D - p(u, v) )."""
+        L = _lib.lib()
+        if _is_torch(centers):
+            import torch
+            ts = _torch_stream(stream, centers.device)
+            st = ts.cuda_stream
+            with torch.cuda.stream(ts):
+                q = _torch_sweeps(centers, directions, radii, tmax)
+                rec = torch.empty((q.shape[0], 4), dtype=torch.float32, device=q.device)
+                check(L.tbvh_sphere_cast(self.h, C.c_void_p(q.data_ptr()), C.c_void_p(rec.data_ptr()), q.shape[0], DEVICE, C.c_void_p(st)))
+            return rec[:, 0], rec[:, 1], rec[:, 2], rec[:, 3].view(torch.int32)
+        q = _np_sweeps(centers, directions, radii, tmax)
+        rec = np.empty((q.shape[0], 4), np.float32)
+        check(L.tbvh_sphere_cast(self.h, _np_ptr(q), _np_ptr(rec), q.shape[0], HOST, None))
+        return rec[:, 0].copy(), rec[:, 1].copy(), rec[:, 2].copy(), rec[:, 3].view(np.uint32).copy()
+
+    def sphere_cast_occluded(self, centers, directions=None, radii=None, tmax=None, stream=None):
+        """True where the moving sphere touches some triangle for t in [0, tmax] (sphere_cast finds a contact).  Arguments as sphere_cast;
+        numpy -> bool array; torch CUDA tensors -> bool tensor queued on `stream`."""
+        L = _lib.lib()
+        if _is_torch(centers):
+            import torch
+            ts = _torch_stream(stream, centers.device)
+            st = ts.cuda_stream
+            with torch.cuda.stream(ts):
+                q = _torch_sweeps(centers, directions, radii, tmax)
+                n = q.shape[0]
+                words = torch.empty(max((n + 31) // 32, 1), dtype=torch.int32, device=q.device)
+                check(L.tbvh_sphere_cast_occluded(self.h, C.c_void_p(q.data_ptr()), C.c_void_p(words.data_ptr()), n, DEVICE, C.c_void_p(st)))
+                shifts = torch.arange(32, dtype=torch.int32, device=q.device)
+                return ((words[:, None] >> shifts) & 1).reshape(-1)[:n].bool()
+        q = _np_sweeps(centers, directions, radii, tmax)
+        n = q.shape[0]
+        words = np.zeros(max((n + 31) // 32, 1), np.uint32)
+        check(L.tbvh_sphere_cast_occluded(self.h, _np_ptr(q), _np_ptr(words), n, HOST, None))
         return np.unpackbits(words.view(np.uint8), bitorder="little")[:n].astype(bool)
 
     # -- signed distances (tbvh_signed_distance_prepare / tbvh_signed_distance, DESIGN.md §4.10)

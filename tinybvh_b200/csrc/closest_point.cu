@@ -43,11 +43,12 @@ static int closest_launch( tbvh_bvh b, const float4* d_queries, float4* d_result
 	return TBVH_OK;
 }
 
-// tbvh_closest_point / tbvh_sphere_overlap / tbvh_signed_distance / tbvh_winding_number: every refusal before any launch; TBVH_HOST
-// stages through the call's scratch
+// tbvh_closest_point / tbvh_sphere_overlap / tbvh_signed_distance / tbvh_winding_number / tbvh_sphere_cast(_occluded): every refusal
+// before any launch; TBVH_HOST stages through the call's scratch
 int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, int kind, float beta )
 {
-	const bool any = kind == PROX_ANY, wn = kind == PROX_WINDING;
+	const bool any = kind == PROX_ANY || kind == PROX_SWEEP_ANY, wn = kind == PROX_WINDING, sweep = kind == PROX_SWEEP || kind == PROX_SWEEP_ANY;
+	const size_t q_bytes = sweep ? 32 : 16;
 	if (!b || !queries || !out) { tbvh_set_error( "%s: NULL argument", fn ); return TBVH_E_ARG; }
 	if (space != TBVH_HOST && space != TBVH_DEVICE) { tbvh_set_error( "%s: unknown space %d", fn, space ); return TBVH_E_ARG; }
 	if (space == TBVH_DEVICE && (((uintptr_t)queries & 15) || ((uintptr_t)out & (wn ? 3 : 15))))
@@ -61,6 +62,7 @@ int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out,
 	auto launch = [&]( const float4* q, void* o, cudaStream_t s )
 	{
 		if (wn) return wn_launch( b, q, (float*)o, n, beta, s );
+		if (sweep) return sc_launch( b, q, any ? 0 : (float4*)o, any ? (uint32_t*)o : 0, n, s );
 		return kind == PROX_SIGNED ? sd_launch( b, q, (float4*)o, n, s ) : closest_launch( b, q, any ? 0 : (float4*)o, any ? (uint32_t*)o : 0, n, s );
 	};
 	if (space == TBVH_DEVICE) return launch( (const float4*)queries, out, (cudaStream_t)stream );
@@ -68,9 +70,9 @@ int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out,
 	Scratch sc( b->ctx->stream );
 	float4* d_q = 0;
 	char* d_out = 0;
-	TRY( sc.alloc( d_q, n * 16 ) );
+	TRY( sc.alloc( d_q, n * q_bytes ) );
 	TRY( sc.alloc( d_out, out_bytes ) );
-	CUDA_TRY( cudaMemcpyAsync( d_q, queries, n * 16, cudaMemcpyHostToDevice, sc.s ) );
+	CUDA_TRY( cudaMemcpyAsync( d_q, queries, n * q_bytes, cudaMemcpyHostToDevice, sc.s ) );
 	TRY( launch( d_q, d_out, sc.s ) );
 	CUDA_TRY( cudaMemcpyAsync( out, d_out, out_bytes, cudaMemcpyDeviceToHost, sc.s ) );
 	CUDA_TRY( cudaStreamSynchronize( sc.s ) );

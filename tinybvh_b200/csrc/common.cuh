@@ -398,8 +398,8 @@ int optimize_tree( tbvh_bvh b, uint32_t max_rounds, float c_trav, float c_int, D
 // exclusive scan of in[0..n) into out[0..n] (out[n] = total); tile_sum needs n/2048 + 2 words (build_sah.cu)
 int exclusive_scan( const uint32_t* in, uint32_t* out, uint32_t* tile_sum, uint32_t n, cudaStream_t s );
 // batched proximity queries (closest_point.cu): the argument checks, the staging of TBVH_HOST batches and the launch of one kind
-// PROX_WINDING: 4-byte results and the expansion's beta (unused by the other kinds)
-enum { PROX_CLOSEST = 0, PROX_ANY = 1, PROX_SIGNED = 2, PROX_WINDING = 3 };
+// PROX_WINDING: 4-byte results and the expansion's beta (unused by the other kinds); PROX_SWEEP / PROX_SWEEP_ANY: 32-byte queries
+enum { PROX_CLOSEST = 0, PROX_ANY = 1, PROX_SIGNED = 2, PROX_WINDING = 3, PROX_SWEEP = 4, PROX_SWEEP_ANY = 5 };
 int proximity_query( const char* fn, tbvh_bvh b, const void* queries, void* out, uint64_t n, int space, void* stream, int kind, float beta = 0.0f );
 // signed distances (signed_distance.cu): TBVH_E_STATE without a table prepared for the handle's current tree and vertices; the launch
 // of n > 0 device-space queries after proximity_query's checks
@@ -408,3 +408,5 @@ int sd_launch( tbvh_bvh b, const float4* d_queries, float4* d_results, uint64_t 
 // winding numbers (winding_number.cu): the same pair for the winding-number table
 int wn_table_check( tbvh_bvh b );
 int wn_launch( tbvh_bvh b, const float4* d_queries, float* d_results, uint64_t n, float beta, cudaStream_t s );
+// sphere casts (sphere_cast.cu): the launch of n > 0 device-space 32-byte queries after proximity_query's checks; d_bits != 0: one bit each
+int sc_launch( tbvh_bvh b, const float4* d_queries, float4* d_results, uint32_t* d_bits, uint64_t n, cudaStream_t s );
